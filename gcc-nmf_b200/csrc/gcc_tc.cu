@@ -756,7 +756,7 @@ int gccnmf_masked_recon_planes(gccnmf_handle* h, const float* masks, const float
     const int waste = (F + widths[i] - 1) / widths[i] * widths[i] - F;
     if (waste < best) { best = waste; bn = widths[i]; }
   }
-  return plane_gemm<true, false>(h, bn, Amn, Wk, M, F, K, 1, false, epi, nullptr, stream, false);
+  return plane_gemm<true, false>(h, bn, Amn, Wk, M, F, K, 1, false, epi, nullptr, stream, false, bn > tgemm::kBM);   // pairs for wide tiles
 }
 
 }  // extern "C"

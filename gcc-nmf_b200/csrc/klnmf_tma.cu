@@ -804,7 +804,7 @@ bool wh_split2(gccnmf_handle* h, int F, int T2, int K) {
 int launch_wh(gccnmf_handle* h, const Plan& p, const Operand& Wk, const Operand& HTk, int F, int T2, int K, const EpiRatioPlanes& e, void* stream) {
   if (wh_split2(h, F, T2, K))
     return plane_gemm_z_reduce<false, false>(h, kWhSplitTile, Wk, HTk, F, T2, K, 2, e, nullptr, stream, nullptr, nullptr, true);
-  return plane_gemm<false, false>(h, p.bn_wh, Wk, HTk, F, T2, K, 1, true, e, nullptr, stream, false, true);
+  return plane_gemm<false, false>(h, p.bn_wh, Wk, HTk, F, T2, K, 1, true, e, nullptr, stream);
 }
 
 // Whether the W-update numerator contraction sums its k-splits inside (1, 1, splits) clusters through distributed shared memory

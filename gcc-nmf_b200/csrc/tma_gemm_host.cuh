@@ -308,13 +308,12 @@ int launch_plane_gemm(gccnmf_handle* h, const Operand& A, const Operand& B, int 
   g.n_tiles = (N + BN - 1) / BN;
   const int ctas = g.n_tiles * g.m_tiles * splits;
   // CTA pairs (option gemm_pair: -1 where the call site asks for them, 1 wherever the shape allows, 0 never): two m tiles share
-  // the B tile through a 1 x 2 cluster, each CTA loading half of it and multicasting it to both.  Without them, a 1 x 2 cluster
-  // is tried for wide K-major B tiles of a contraction without k-splits (the H update's 208-row tiles).
+  // the B tile through a 1 x 2 cluster, each CTA loading half of it and multicasting it to both.  The KL-NMF contractions do not
+  // ask for them: on an H100 SXM their main loops run faster alone (tools/nmf_phases.py, DESIGN.md 4.1).
   const bool pair = h->gemm_pair > 0 || (h->gemm_pair < 0 && prefer_pair);
   const int order_share_b[4][2] = {{1, 2}, {1, 1}, {1, 1}, {1, 1}}, order_none[4][2] = {{1, 1}, {1, 1}, {1, 1}, {1, 1}};
   const int order_forced[4][2] = {{2, 2}, {1, 2}, {2, 1}, {1, 1}};
-  const int (*order)[2] = h->gemm_cluster >= 0 ? order_forced
-                          : ((pair || (BN > tgemm::kBM && !B_MN && splits == 1)) ? order_share_b : order_none);
+  const int (*order)[2] = h->gemm_cluster >= 0 ? order_forced : (pair ? order_share_b : order_none);
   for (int i = 0; i < 4; ++i) {
     const int cn = order[i][0], cm = order[i][1];
     if (h->gemm_cluster >= 0 && h->gemm_cluster != 10 * cn + cm && !(cn == 1 && cm == 1)) continue;
