@@ -50,7 +50,8 @@ constexpr int kApplyTile = 32;
 struct EpiStoreT {   // DT[z][n][m] = acc.  G4 partials (m = atom, n = f) and the test entry.
   struct State {};
   struct Loaded {};
-  static constexpr bool kDualN = true;       // (takes effect for K-major B tiles of <= 128 columns: the test entry covers the dual-N loop)
+  static constexpr bool kDualN = true;       // (takes effect for K-major B tiles of <= 128 columns: the test entry covers the dual-N loop,
+                                             // whose products are the plain loop's three)
   static constexpr bool kRowReduce = false;
   static constexpr int kRowValues = 0;
   static constexpr bool kPrefetch = false;
@@ -76,7 +77,7 @@ struct EpiRatioPlanes {   // RT[n][m] = split(VT[n][m] / acc)     G1 / G3 (m = f
   static constexpr bool kRowReduce = false;
   static constexpr int kRowValues = 0;
   static constexpr bool kPrefetch = false;   // V^T is read twice per iteration and stays in L2 (96 % hit rate measured)
-  static constexpr bool kDualN = true;       // 2 MMAs of N = 2 BN per k-step (all four hi / lo products), see tma_gemm.cuh
+  static constexpr bool kDualN = true;       // 2 MMAs per k-step, N = BN and N = 2 BN (the three hi / lo products), see tma_gemm.cuh
   static constexpr bool kPreloadOperands = true;   // V^T of the thread's columns is fetched while the main loop runs
   const float* __restrict__ VT; bf16* __restrict__ RT; int64_t ld, plane; int M, N; bool vec;
   __device__ void prefetch(int, int) const {}
@@ -692,12 +693,16 @@ __global__ void tma_reduce_pull_kernel(PeerSet peers, float* reduced_local, int6
 }
 
 // ------------------------------------------------------------------------------------------------ tile plan
-// Cost model of the planner, in cycles per 16-deep k-step of one 128-row CTA: the dual-N loop issues 2 MMAs of N = 2 bn per k-step,
-// the plain loop 3 of N = bn, and an MMA of N > 208 costs more than a narrower one.  The constants are relative weights that pick
-// between tile widths and wave counts; they have not been measured on H100.
-double mma_cycles(int n) { return n <= 208 ? 128.0 : 168.0; }
-double kstep_cycles(int bn, bool dual) { return (dual && 2 * bn <= 256) ? 2.0 * mma_cycles(2 * bn) : 3.0 * mma_cycles(bn); }
-double epilogue_cycles(int bn) { return 1500.0 + 20.0 * bn; }
+// Cost model of the planner, in SM cycles of one 128-row CTA, from the per-CTA phase stamps of tools/nmf_phases.py at the benchmark
+// shape (H100 SXM, DESIGN.md 4.1).  Per 16-deep k-step the dual-N loop issues MMAs of N = bn and N = 2 bn, the plain loop three of
+// N = bn; an MMA costs 1.1 - 1.2 cycles per column of N (both warpgroups; G1 - G4 main loops at widths 120 - 256).  The epilogue
+// costs about 100 cycles per column for the ratio (G1 / G3) and the H update (G2), 42 for the plain store of the W-update numerator
+// (G4); the fill, the launch and the gaps about 8 k cycles per wave.
+constexpr double kEpiRatioCycles = 100.0, kEpiUpdateHCycles = 100.0, kEpiStoreCycles = 42.0;
+double mma_cycles(int n) { return 1.2 * n; }
+double kstep_cycles(int bn, bool dual) { return (dual && 2 * bn <= 256) ? mma_cycles(2 * bn) + mma_cycles(bn) : 3.0 * mma_cycles(bn); }
+double epilogue_cycles(int bn, double per_column) { return per_column * bn; }
+constexpr double kWaveCycles = 8000.0;
 
 int m_tiles_of(int M, bool simt_tail) {
   const int tail = M % tgemm::kBM;
@@ -707,7 +712,8 @@ int m_tiles_of(int M, bool simt_tail) {
 struct TilePlan { int bn, splits; };
 
 // Picks the tile width (and k-split count when `allow_split`) with the smallest estimated time.
-TilePlan plan_tiles(int sm_count, int m_tiles, int N, int Kc, bool allow_split, const int* widths, int n_widths, bool dual = false) {
+TilePlan plan_tiles(int sm_count, int m_tiles, int N, int Kc, bool allow_split, const int* widths, int n_widths, double epi_per_column,
+                    bool dual = false) {
   TilePlan best{128, 1};
   double best_cost = 1e300;
   const int total_kb = (Kc + kKB - 1) / kKB;
@@ -718,14 +724,14 @@ TilePlan plan_tiles(int sm_count, int m_tiles, int N, int Kc, bool allow_split, 
     if (allow_split) splits = std::max(1, std::min(std::min(kMaxSplits, sm_count / std::max(1, tiles)), total_kb / 4));
     const int kb = (total_kb + splits - 1) / splits;
     const int waves = (tiles * splits + sm_count - 1) / sm_count;
-    const double cost = waves * (kb * (kKB / 16) * kstep_cycles(bn, dual) + epilogue_cycles(bn) + 3000.0);
+    const double cost = waves * (kb * (kKB / 16) * kstep_cycles(bn, dual) + epilogue_cycles(bn, epi_per_column) + kWaveCycles);
     if (cost < best_cost) { best_cost = cost; best = TilePlan{bn, splits}; }
   }
   return best;
 }
 
-const int kWidthsWH[] = {104, 128, 256};          // K-major B: the dual-N loop applies up to 128 columns (112: wh_tile option)
-const int kWidthsAll[] = {128, 176, 208, 256};
+const int kWidthsWH[] = {104, 120, 128, 256};     // K-major B: the dual-N loop applies up to 128 columns (112: wh_tile option)
+const int kWidthsAll[] = {128, 176, 208, 240, 256};
 
 struct Plan {
   int bn_wh;            // G1 / G3
@@ -736,9 +742,9 @@ struct Plan {
 
 Plan make_plan(const gccnmf_handle* h, int F, int T2, int K) {
   Plan p;
-  p.bn_wh = h->wh_tile ? h->wh_tile : plan_tiles(h->sm_count, m_tiles_of(F, true), T2, K, false, kWidthsWH, 3, true).bn;
-  p.bn_h = plan_tiles(h->sm_count, m_tiles_of(K, false), T2, F, false, kWidthsAll, 4).bn;
-  p.w = plan_tiles(h->sm_count, m_tiles_of(K, false), F, T2, true, kWidthsAll, 4);
+  p.bn_wh = h->wh_tile ? h->wh_tile : plan_tiles(h->sm_count, m_tiles_of(F, true), T2, K, false, kWidthsWH, 4, kEpiRatioCycles, true).bn;
+  p.bn_h = plan_tiles(h->sm_count, m_tiles_of(K, false), T2, F, false, kWidthsAll, 5, kEpiUpdateHCycles).bn;
+  p.w = plan_tiles(h->sm_count, m_tiles_of(K, false), F, T2, true, kWidthsAll, 5, kEpiStoreCycles);
   p.rowsum_slots = (T2 + p.bn_h - 1) / p.bn_h;
   return p;
 }
@@ -1169,7 +1175,7 @@ size_t gccnmf_gemm_planes_workspace_bytes(int M, int N, int Kc) {
 
 // Test / diagnostics entry of the TMA plane GEMM: DT (N, M) row-major = (A . B^T)^T.
 //   a_mn_major = 0: A is (M, Kc) row-major;  1: A is (Kc, M) row-major (m contiguous).  Same for B with N.
-// The float32 operands are split into bf16 hi/lo planes in the workspace first.  tile_n in {128, 176, 208, 256};
+// The float32 operands are split into bf16 hi/lo planes in the workspace first.  tile_n: see plane_gemm (tma_gemm_host.cuh);
 // splits > 1 writes `splits` partial slabs DT[z] (N * M floats each).  timing: 6 clock64 stamps per CTA, or NULL.
 int gccnmf_gemm_planes(gccnmf_handle* h, const float* A, int a_mn_major, const float* B, int b_mn_major, float* DT, int M, int N, int Kc,
                        int tile_n, int splits, void* workspace, size_t workspace_bytes, unsigned long long* timing, void* stream) {

@@ -8,8 +8,8 @@
 //   MN-major : element (r, k) at rows k, r contiguous        TMA boxes {64, KB, 2 planes} = 64-wide atoms, SWIZZLE_128B
 // so no matrix is ever transposed or re-split inside the loop.
 // Per 16-deep k-step the products lo.hi + hi.lo + hi.hi accumulate in float32 registers: three wgmma of width BN, or -- dual-N
-// loop, K-major B with 2 BN <= 256 -- two of width 2 BN against the adjacent [B_hi; B_lo] planes of the stage, which also yields
-// lo.lo; the epilogue adds the two accumulator halves.
+// loop, K-major B with 2 BN <= 256 -- A_lo . B_hi of width BN and A_hi . [B_hi; B_lo] of width 2 BN over the adjacent hi and lo
+// planes of the stage; the epilogue adds the two accumulator halves.
 //
 // CTA = one 128 x BN accumulator tile, three warpgroups (12 warps):
 //   warpgroup 0  warp 0 lane 0 is the TMA producer: waits empty[s], arms full[s] with the stage's byte count, issues the boxes;
@@ -164,7 +164,7 @@ struct Config {
 
 // One k-block (KB deep) of the 3xBF16 contraction for the 64 accumulator rows of one warpgroup, issued asynchronously.
 //   a_base: this warpgroup's rows of the A hi plane in the stage; b_base: the B hi plane; b_lo_off: B lo plane - B hi plane
-// Products in the order lo.hi, hi.lo, hi.hi (dual-N: A_lo . [B_hi; B_lo], then A_hi . [B_hi; B_lo]).  The k tail needs no
+// Products in the order lo.hi, hi.lo, hi.hi (dual-N: A_lo . B_hi, then A_hi . [B_hi; B_lo]).  The k tail needs no
 // special case: TMA zero-fills the k-rows past the end of both operands, so their products add exact zeros (and an issue that
 // depends on the data would make ptxas serialise the wgmma).
 template <int N, int KB, bool A_MN, bool B_MN, bool DUAL>
@@ -183,8 +183,16 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[N / 2], uint32_t a_base,
     const uint64_t a_hi = desc(a_addr, A_MN), a_lo = desc(a_addr + a_lo_off, A_MN);
     const uint64_t b_hi = desc(b_addr, B_MN), b_lo = desc(b_addr + b_lo_off, B_MN);
     if constexpr (DUAL) {
+      // N = BN into the first half of the accumulator: the column of a fragment element depends on its register index and the
+      // lane only, so acc[0 .. N / 4) of the N = 2 BN fragment are exactly the N = BN fragment.  lo.lo is not computed: it is
+      // below 2^-18 |a| |b|, under the 2^-17 to which each plane pair represents its value.
+      // Ordering: the PTX ISA orders accumulator accesses of successive wgmma.mma_async by default only when they have the same
+      // shape.  These two MMAs differ in N and share registers, so each is preceded by wgmma.fence (for kk = 0 the caller's
+      // fence before the k-block is the first one).
+      if (kk > 0) gmma::wgmma_fence();
+      gmma::Wgmma<N / 2>::template mma<A_MN, B_MN>(reinterpret_cast<float(&)[N / 4]>(acc), a_lo, b_hi);
+      gmma::wgmma_fence();
       // N = 2 BN: the descriptor at b_hi walks the BN rows of the hi plane and on into the lo plane behind it
-      gmma::Wgmma<N>::template mma<A_MN, B_MN>(acc, a_lo, b_hi);
       gmma::Wgmma<N>::template mma<A_MN, B_MN>(acc, a_hi, b_hi);
       (void)b_lo;
     } else {
@@ -203,9 +211,9 @@ template <class E>
 struct has_tile_epilogue<E, decltype((void)E::kTileEpilogue)> { static constexpr bool value = E::kTileEpilogue; };
 
 // Epilogues with `static constexpr bool kDualN = true` ask for the dual-N main loop where the shape allows it (K-major B, 2 BN <= 256).
-// The hi and lo planes of a K-major B tile are adjacent in the stage, so ONE MMA with N = 2 BN multiplies an A plane with
-// [B_hi ; B_lo] into two accumulator halves: 2 MMAs per k-step (A_lo, then A_hi) compute all FOUR products hi.hi + lo.hi | hi.lo + lo.lo
-// instead of three products in three MMAs, and the epilogue adds the two halves.
+// The hi and lo planes of a K-major B tile are adjacent in the stage, so ONE MMA with N = 2 BN multiplies A_hi with [B_hi ; B_lo]
+// into two accumulator halves, and one of N = BN adds A_lo . B_hi to the first half: 2 MMAs per k-step compute the three products
+// lo.hi + hi.hi | hi.lo over 3 BN columns, as the plain loop does in three MMAs of BN, and the epilogue adds the two halves.
 // Epilogues with `static constexpr bool kPreloadOperands = true` have their by-column global operands fetched into registers while
 // the main loop runs (opt-in: measured to pay for the ratio epilogue of the W.H contractions, to cost for the H update).
 template <class E, class = void>
@@ -458,7 +466,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     for (int j = 0; j < BN / 2; ++j) {
       const int col = 8 * (j >> 2) + c0 + (j & 1), row = r0 + 8 * ((j >> 1) & 1);
       float v = acc[j];
-      if constexpr (DUAL) v += acc[j + BN / 2];        // + the [hi ; lo] . B_lo half: columns BN .. 2 BN - 1
+      if constexpr (DUAL) v += acc[j + BN / 2];        // + the A_hi . B_lo half: columns BN .. 2 BN - 1
       tile[(size_t)col * kBM + row] = v;
     }
     preload();

@@ -341,17 +341,22 @@ template <bool A_MN, bool B_MN, class Epi>
 int plane_gemm(gccnmf_handle* h, int bn, const Operand& A, const Operand& B, int M, int N, int Kc, int splits, bool simt_tail, const Epi& epi,
                unsigned long long* timing, void* stream, bool m_fastest = false, bool prefer_pair = false) {
   switch (bn) {
-    case 104:      // only as a dual-N tile (2 x 104 = 208 columns per MMA; 104 alone is not a multiple of 16)
+    case 104:      // only as a dual-N tile (MMAs of 104 + 208 columns per k-step; 104 alone is not a multiple of 16)
       if constexpr (tgemm::wants_dual_n<Epi>::value && !B_MN)
         return launch_plane_gemm<104, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, timing, stream, m_fastest, prefer_pair);
+      break;
+    case 120:      // only as a dual-N tile (MMAs of 120 + 240 columns per k-step): the planner offers it to the W.H contractions only
+      if constexpr (tgemm::wants_dual_n<Epi>::value && !B_MN)
+        return launch_plane_gemm<120, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, timing, stream, m_fastest, prefer_pair);
       break;
     case 112: return launch_plane_gemm<112, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, timing, stream, m_fastest, prefer_pair);
     case 128: return launch_plane_gemm<128, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, timing, stream, m_fastest, prefer_pair);
     case 176: return launch_plane_gemm<176, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, timing, stream, m_fastest, prefer_pair);
     case 208: return launch_plane_gemm<208, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, timing, stream, m_fastest, prefer_pair);
+    case 240: return launch_plane_gemm<240, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, timing, stream, m_fastest, prefer_pair);
     case 256: return launch_plane_gemm<256, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, timing, stream, m_fastest, prefer_pair);
   }
-  return gccnmf_fail(h, GCCNMF_ERR_UNSUPPORTED, "plane gemm: tile width %d (supported: 104, 112, 128, 176, 208, 256)", bn);
+  return gccnmf_fail(h, GCCNMF_ERR_UNSUPPORTED, "plane gemm: tile width %d (supported: 104, 112, 120, 128, 176, 208, 240, 256)", bn);
 }
 
 // k-splits reduced inside (1, 1, splits) clusters (no slabs): query how many such clusters are resident at once / launch.

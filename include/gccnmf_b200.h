@@ -64,7 +64,7 @@ GCCNMF_API int64_t gccnmf_launch_count(const gccnmf_handle* h);
  *   "gemm_cluster" [-1]         plane GEMM cluster shape 10 CN + CM (11, 12, 21, 22) instead of the automatic choice
  *   "argmax_refine_shared" [1]  float64 refinement of near-tie argmax decisions with E staged in shared memory
  *   "argmax_persistent" [1]     all-TDOA argmax GEMM as one persistent CTA per SM (epilogue from registers); 0 = one CTA per tile
- *   "wh_tile" [0]               tile width of the W.H contractions (104 / 112 / 128 / 256) instead of the planned one
+ *   "wh_tile" [0]               tile width of the W.H contractions (104 / 112 / 120 / 128 / 256) instead of the planned one
  *   "gemm_pair" [-1]            plane GEMM on CTA pairs (1 x 2 clusters sharing the B tile): -1 where a call site prefers it, 0 never, 1 wherever possible
  *                               (bit-identical results either way)
  *   "l2_persist" [0]            KL-NMF loop: persisting L2 access-policy window over G^T (1 = float32 master, 2 = master + planes)
@@ -373,7 +373,8 @@ GCCNMF_API int gccnmf_rt_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, v
  * non-contiguous dimension is consumed MN-major.  Test / diagnostics entry: splits the float32 operands into planes
  * in the workspace, then DT (N, M) row-major = (A . B^T)^T.
  *   a_mn_major = 0: A is (M, Kc) row-major;  1: A is (Kc, M) row-major.   b_mn_major likewise with N.
- *   tile_n in {128, 176, 208, 256};  splits > 1: `splits` partial slabs DT[z] over k ranges (N * M floats each).
+ *   tile_n in {112, 128, 176, 208, 240, 256}, and 104 / 120 with a K-major B (dual-N tiles);  splits > 1: `splits` partial slabs
+ *   DT[z] over k ranges (N * M floats each).
  *   timing: device uint64[8 x CTAs] stamps (layout: gccnmf_debug_timing) or NULL.
  */
 /* Tile plan of the KL-NMF loop on a device with sm_count SMs (host logic only; callable without a GPU):

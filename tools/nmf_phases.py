@@ -1,6 +1,6 @@
 """Where one KL-NMF iteration spends its time, contraction by contraction, at the benchmark shape on one GPU.
 
-  python tools/nmf_phases.py [--iterations 100] [--gemm-cluster 10CN+CM] [--gemm-pair -1|0|1] [--out FILE.json]
+  python tools/nmf_phases.py [--iterations 100] [--gemm-cluster 10CN+CM] [--gemm-pair -1|0|1] [--wh-tile BN] [--out FILE.json]
 
 Runs the KL-NMF loop (F = 513, T2 = 3744, K = 1024) with the plane GEMM's timing records on (gccnmf_debug_timing: 8 uint64 per
 CTA; see csrc/tma_gemm.cuh) and prints for G1 - G4 and the W update: the exclusive time of each launch (end of the previous
@@ -36,6 +36,7 @@ def main():
     ap.add_argument('--iterations', type=int, default=100)
     ap.add_argument('--gemm-cluster', type=int, default=-1, help='option gemm_cluster (10 CN + CM; -1: automatic)')
     ap.add_argument('--gemm-pair', type=int, default=-1, help='option gemm_pair (-1: where a call site prefers CTA pairs)')
+    ap.add_argument('--wh-tile', type=int, default=0, help='option wh_tile: tile width of G1 / G3 (0: planned)')
     ap.add_argument('--out', default=None)
     args = ap.parse_args()
     import torch
@@ -43,10 +44,13 @@ def main():
     h = default_handle()
     h.set_option('gemm_cluster', args.gemm_cluster)
     h.set_option('gemm_pair', args.gemm_pair)
+    h.set_option('wh_tile', args.wh_tile)
     sms = torch.cuda.get_device_properties(h.device).multi_processor_count
     plan = (ctypes.c_int * 8)()
     h.check(h.lib.gccnmf_klnmf_tile_plan(sms, F, T2, K, plan))
     bn_wh, bn_h, bn_w, splits_w, _, rec_wh, rec_h, rec_w = list(plan)
+    if args.wh_tile:
+        bn_wh, rec_wh = args.wh_tile, (F // 128) * ((T2 + args.wh_tile - 1) // args.wh_tile)
     rng = np.random.default_rng(5)
     V = h.to_device((rng.random((F, T2)) ** 3 + 1e-3).astype(np.float32))
     W0 = h.to_device((rng.random((F, K)) + 1e-2).astype(np.float32))
@@ -67,9 +71,9 @@ def main():
     assert used == per_it * 8 * args.iterations, (used, per_it * 8 * args.iterations)
     s = buf.cpu().numpy()[:used].reshape(args.iterations, per_it, 8).astype(np.int64)
 
-    # executed tensor FLOP per launch (products per k-step: 4 in the dual-N loop of G1 / G3, 3 otherwise; tail rows excluded)
+    # executed tensor FLOP per launch (3 hi / lo products per k-step in every contraction; tail rows excluded)
     m_wh = (F // 128) * 128
-    flops = {'G1': 4 * 2.0 * m_wh * T2 * K, 'G2': 3 * 2.0 * K * T2 * F, 'G3': 4 * 2.0 * m_wh * T2 * K, 'G4': 3 * 2.0 * K * F * T2}
+    flops = {'G1': 3 * 2.0 * m_wh * T2 * K, 'G2': 3 * 2.0 * K * T2 * F, 'G3': 3 * 2.0 * m_wh * T2 * K, 'G4': 3 * 2.0 * K * F * T2}
     layout = [('G1', rec_wh), ('G2', rec_h), ('G3', rec_wh), ('G4', rec_w), ('W update', 1)]
     # ns per clock64 cycle, from records whose globaltimer and clock64 windows cover the same stretch
     spans = []
@@ -83,7 +87,7 @@ def main():
         ok = (r[:, 6] > r[:, 1]) & (r[:, 7] > r[:, 0])
         spans.append(np.median((r[ok, 7] - r[ok, 0]) / (r[ok, 6] - r[ok, 1])))
     ns_per_cycle = float(np.median(spans))
-    result = {'card': card(), 'iterations': args.iterations, 'gemm_cluster': args.gemm_cluster, 'gemm_pair': args.gemm_pair,
+    result = {'card': card(), 'iterations': args.iterations, 'gemm_cluster': args.gemm_cluster, 'gemm_pair': args.gemm_pair, 'wh_tile': args.wh_tile,
               'plan': {'bn_wh': bn_wh, 'bn_h': bn_h, 'bn_w': bn_w, 'splits_w': splits_w, 'records': [rec_wh, rec_h, rec_w]},
               'loop_ms_events': e0.elapsed_time(e1), 'ns_per_cycle_est': ns_per_cycle, 'launches': {}}
     starts = {name: rows[name][:, :, 0].min(axis=1) for name, _ in layout}
