@@ -113,6 +113,25 @@ SIGNATURES.update({
     'gccnmf_rt_export': (c_int, [_H, _C, _P, c_size_t, c_int, c_void_p, _S]),
 })
 
+
+class RtmSlotParams(ctypes.Structure):
+    """gccnmf_rtm_slot_params (include/gccnmf_b200.h)."""
+    _fields_ = [('target_index', c_float), ('set_target', c_int), ('epsilon', c_float), ('beta', c_float), ('noise_floor', c_float),
+                ('mode', c_int), ('separation_enabled', c_int), ('localization_enabled', c_int), ('localization_window', c_int),
+                ('active', c_int)]
+
+
+SIGNATURES.update({
+    'gccnmf_rtm_state_bytes': (c_size_t, [_C, c_int]),
+    'gccnmf_rtm_init': (c_int, [_H, _C, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _S]),
+    'gccnmf_rtm_reset_slots': (c_int, [_H, _C, c_int, _P, c_size_t, c_int, c_int, _S]),
+    'gccnmf_rtm_set_params': (c_int, [_H, _C, c_int, _P, c_size_t, c_int, c_int, ctypes.POINTER(RtmSlotParams), _S]),
+    'gccnmf_rtm_process_frames': (c_int, [_H, _C, c_int, _P, c_size_t, _P, _P, _P, _S]),
+    'gccnmf_rtm_process_block': (c_int, [_H, _C, c_int, _P, c_size_t, _P, _P, _P, _S]),
+    'gccnmf_rtm_graph_create': (c_int, [_H, _C, c_int, _P, c_size_t, _P, _P, _P, _P, ctypes.POINTER(c_void_p), _S]),
+    'gccnmf_rtm_export': (c_int, [_H, _C, c_int, _P, c_size_t, c_int, c_int, c_void_p, _S]),
+})
+
 _lib = None
 
 

@@ -16,6 +16,19 @@
 //                     (argmax of the nanmean over the last `localization_window` columns -> target TDOA index of the NEXT block).
 // The rings are circular in place (the reference shifts 8 blocks of memory per call); positions derive from a device-side block
 // counter, so a captured graph replays unchanged block after block.
+//
+// Streams (slots).  One state buffer serves S independent audio streams that share the configuration, W, E, the windows and H0:
+//   [ shared region: twiddles, windows, W, W^T, row / column sums, E^T, H0 ]  [ slot 0 ] [ slot 1 ] ... [ slot S-1 ]
+// Each slot region (fixed stride) holds its RtDev (parameters, block counter, history index, target, `active`), its rings, its
+// GCC-PHAT history and its per-block intermediates.  Every kernel of a block covers all S slots in one launch (a slot dimension in
+// the grid, or several slots per warp where the dictionary is the operand to share), so the kernel count per block does not depend
+// on S.  The single-stream entry points (gccnmf_rt_*) are the S = 1 case of the same carve and kernels.
+// Equivalence: slot s of an S-slot state computes bit for bit what a single-stream state fed the same blocks computes.  Every
+// reduction below has a fixed order that does not depend on the other slots or on the tile shape: rt_atoms is one fmaf chain per
+// output over f = 0 .. F-1 from 0.f (zero padding appends fmaf(0, 0, acc) = acc), the argmax is a maximum under a strict total
+// order (numpy's: NaN first, then value, then the lower index), and the inference / filter kernels sum lane-strided over the
+// contracted index and then through the same xor butterfly for every slot.
+// An inactive slot costs no work: its output slice is written as zeros, its input slice is ignored, its state is left as it was.
 #include <cmath>
 
 #include "common.cuh"
@@ -26,65 +39,84 @@ namespace {
 constexpr int kRtMaxN = 2048;
 constexpr int kRtMaxFrames = 8;          // frames per block the filter kernel keeps in registers
 constexpr int kRtMaxD = 128;
-constexpr int kRtAtomsPerCta = 16;
 constexpr int kRtRingBlocks = 8;         // utils.py:85 numBlocksPerBuffer
+constexpr int kRtMaxStreams = 4096;      // slots per state buffer
+constexpr int kRtAtomsFc = 32;           // f values per shared-memory stage of the atoms contraction
 
-struct RtDev {                           // device-resident parameters + loop-carried state (first bytes of the state buffer)
+struct RtDev {                           // device-resident parameters + loop-carried state (first bytes of a slot region)
   float target, eps, beta, noise_floor;  // gccNMFProcessor.py:196-199 (Theano shared scalars)
   int mode, separation, localization, loc_window;
   int block_counter;                     // blocks completed (incremented by the synthesis kernel)
   int hist_index;                        // write position of the GCC-PHAT history ring (utils.py:45-59)
+  int active;                            // 0: the slot is skipped by every kernel of a block
 };
 
-struct RtLayout {                        // carve of the caller-owned state buffer (pure function of the configuration)
+// Pointer of slot s given the pointer of slot 0 and the slot stride in bytes.
+template <typename T>
+__host__ __device__ __forceinline__ T* rt_slot(T* p0, int s, size_t stride) {
+  return (T*)((const char*)p0 + (size_t)s * stride);
+}
+
+struct RtLayout {                        // carve of the caller-owned state buffer (pure function of the configuration and S)
+  // shared by every slot
+  float *win_a, *win_s, *W, *WT, *recV, *colsumW, *H0, *tw32;
+  double* tw64;
+  float2* ET;
+  // slot 0 (slot s: rt_slot(p, s, stride))
   RtDev* dev;
-  float *in_ring, *out_ring, *win_a, *win_s, *W, *WT, *recV, *colsumW, *G, *gccphat, *Vabs, *H, *H0, *R, *frames, *tw32;
-  double *tw64, *hist, *hmask;
-  float2 *ET, *X, *Y;
+  float *in_ring, *out_ring, *G, *gccphat, *Vabs, *H, *R, *frames;
+  double *hist, *hmask;
+  float2 *X, *Y;
   int32_t* argmax;
-  int F, Fp, L;
-  size_t bytes;
+  int F, Fp, L, S;
+  size_t stride, bytes;
   bool ok;
 };
 
-RtLayout rt_carve(const gccnmf_rt_config& c, void* state, size_t state_bytes) {
+RtLayout rt_carve(const gccnmf_rt_config& c, int S, void* state, size_t state_bytes) {
   RtLayout l{};
   const int N = c.window_size, nT = c.windows_per_block, K = c.num_atoms, D = c.num_tdoas;
   l.F = N / 2 + 1;
   l.Fp = (l.F + 3) & ~3;
   l.L = kRtRingBlocks * c.block_size;
-  WorkspaceCarver w(state ? state : reinterpret_cast<void*>(256), state ? state_bytes : ~size_t(0) >> 1);
-  l.dev = w.take<RtDev>(1);
+  l.S = S;
+  char* base = state ? static_cast<char*>(state) : reinterpret_cast<char*>(256);
+  WorkspaceCarver w(base, ~size_t(0) >> 1);
   l.tw64 = w.take<double>(N);
-  l.hist = w.take<double>((size_t)D * c.history_length);
-  l.hmask = w.take<double>((size_t)K * nT);
   l.tw32 = w.take<float>(N);
-  l.in_ring = w.take<float>((size_t)2 * l.L);
-  l.out_ring = w.take<float>((size_t)2 * l.L);
   l.win_a = w.take<float>(N);
   l.win_s = w.take<float>(N);
   l.W = w.take<float>((size_t)l.F * K);
   l.WT = w.take<float>((size_t)K * l.Fp);
   l.recV = w.take<float>(l.F);
   l.colsumW = w.take<float>(K);
-  l.G = w.take<float>((size_t)nT * D * l.Fp);
-  l.gccphat = w.take<float>((size_t)D * nT);
-  l.Vabs = w.take<float>((size_t)l.F * 2 * nT);
-  l.H = w.take<float>((size_t)K * 2 * nT);
   l.H0 = w.take<float>((size_t)K * 2);
-  l.R = w.take<float>((size_t)l.F * 2 * nT);
-  l.frames = w.take<float>((size_t)2 * nT * N);
   l.ET = w.take<float2>((size_t)D * l.Fp);
-  l.X = w.take<float2>((size_t)2 * l.F * nT);
-  l.Y = w.take<float2>((size_t)2 * l.F * nT);
-  l.argmax = w.take<int32_t>((size_t)K * nT);
-  l.bytes = align_up(w.used, 256);
-  l.ok = state != nullptr && w.ok();
+  const size_t shared = align_up(w.used, 256);
+  WorkspaceCarver v(base + shared, ~size_t(0) >> 1);
+  l.dev = v.take<RtDev>(1);
+  l.hist = v.take<double>((size_t)D * c.history_length);
+  l.hmask = v.take<double>((size_t)K * nT);
+  l.in_ring = v.take<float>((size_t)2 * l.L);
+  l.out_ring = v.take<float>((size_t)2 * l.L);
+  l.G = v.take<float>((size_t)nT * D * l.Fp);
+  l.gccphat = v.take<float>((size_t)D * nT);
+  l.Vabs = v.take<float>((size_t)l.F * 2 * nT);
+  l.H = v.take<float>((size_t)K * 2 * nT);
+  l.R = v.take<float>((size_t)l.F * 2 * nT);
+  l.frames = v.take<float>((size_t)2 * nT * N);
+  l.X = v.take<float2>((size_t)2 * l.F * nT);
+  l.Y = v.take<float2>((size_t)2 * l.F * nT);
+  l.argmax = v.take<int32_t>((size_t)K * nT);
+  l.stride = align_up(v.used, 256);
+  l.bytes = shared + (size_t)S * l.stride;
+  l.ok = state != nullptr && S >= 1 && l.bytes <= state_bytes;
   return l;
 }
 
-int rt_check(gccnmf_handle* h, const gccnmf_rt_config* c) {
+int rt_check(gccnmf_handle* h, const gccnmf_rt_config* c, int S = 1) {
   GCCNMF_REQUIRE(h, c != nullptr, "rt: NULL configuration");
+  GCCNMF_REQUIRE(h, S >= 1 && S <= kRtMaxStreams, "rt: num_streams must be in [1, %d] (got %d)", kRtMaxStreams, S);
   const int N = c->window_size;
   GCCNMF_REQUIRE(h, N >= 64 && N <= kRtMaxN && (N & (N - 1)) == 0, "rt: window_size must be a power of two in [64, %d] (got %d)", kRtMaxN, N);
   GCCNMF_REQUIRE(h, c->hop_size >= 1 && c->block_size >= 1, "rt: hop_size and block_size must be positive");
@@ -127,11 +159,33 @@ __global__ void rt_init_steering_kernel(const float2* __restrict__ E, int F, int
   ET[i] = f < F ? E[(int64_t)f * D + d] : float2{0.f, 0.f};
 }
 
-__global__ void rt_set_params_kernel(RtDev* dev, float target, float eps, float beta, float noise_floor, int mode, int separation, int localization,
-                                     int loc_window, int set_target) {
-  if (set_target) dev->target = target;
-  dev->eps = eps; dev->beta = beta; dev->noise_floor = noise_floor;
-  dev->mode = mode; dev->separation = separation; dev->localization = localization; dev->loc_window = loc_window;
+// Parameters of up to kRtParamsPerLaunch slots, passed by value (the host array is consumed when the launch is enqueued).
+constexpr int kRtParamsPerLaunch = 64;
+struct RtParamsBatch {
+  gccnmf_rtm_slot_params p[kRtParamsPerLaunch];
+};
+
+// set_active = 0 leaves the slot's `active` flag alone (the single-stream entry point has no such parameter).
+__global__ void rt_set_params_kernel(RtDev* dev0, size_t stride, int first, int count, RtParamsBatch b, int set_active) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  RtDev* dev = rt_slot(dev0, first + i, stride);
+  const gccnmf_rtm_slot_params& q = b.p[i];
+  if (q.set_target) dev->target = q.target_index;
+  dev->eps = q.epsilon; dev->beta = q.beta; dev->noise_floor = q.noise_floor;
+  dev->mode = q.mode; dev->separation = q.separation_enabled ? 1 : 0; dev->localization = q.localization_enabled ? 1 : 0;
+  dev->loc_window = q.localization_window;
+  if (set_active) dev->active = q.active ? 1 : 0;
+}
+
+// Defaults of gccNMFProcessor.py:190-199 and `active` for slots [first, first + count) (after their regions were zeroed).
+__global__ void rt_default_params_kernel(RtDev* dev0, size_t stride, int first, int count) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  RtDev* dev = rt_slot(dev0, first + i, stride);
+  dev->target = 10.0f; dev->eps = 2.0f; dev->beta = 1.0f; dev->noise_floor = 0.0f;
+  dev->mode = 1; dev->separation = 1; dev->localization = 0; dev->loc_window = 6;
+  dev->active = 1;
 }
 
 // ---------------------------------------------------------------------------------------------- numerics shared with gcc.cu
@@ -146,7 +200,8 @@ __device__ __forceinline__ float2 rt_coherence(float2 a, float2 b) {
   re = __fmul_rn(re, ib); im = __fmul_rn(im, ib);
   return float2{re, im};
 }
-// numpy.argmax ordering: NaN is a maximum, the first occurrence wins
+// numpy.argmax ordering: NaN is a maximum, the first occurrence wins.  A strict total order on (value, index) pairs, so the
+// argmax is the same whatever order the candidates are compared in.
 __device__ __forceinline__ bool rt_better(float v, int i, float bv, int bi) {
   const bool vn = v != v, bn = bv != bv;
   if (vn || bn) return vn && (!bn || i < bi);
@@ -166,16 +221,26 @@ __device__ __forceinline__ int rt_ring_index(int p, int call, int B, int L) {
   return (int)(a < 0 ? a + L : a);
 }
 
-// ---------------------------------------------------------------------------------------------- A: analysis (one CTA per frame)
+// ---------------------------------------------------------------------------------------------- A: analysis (one CTA per frame and slot)
 __global__ void __launch_bounds__(kFftThreads)
-rt_analysis_kernel(const RtDev* __restrict__ dev, const float* __restrict__ windowed,   // (2, N, nT) or NULL: read the ring + the new block
-                   const float* __restrict__ in_block, const float* __restrict__ in_ring, int B, int L, int hop, int nT,
+rt_analysis_kernel(const RtDev* __restrict__ dev0, size_t stride, const float* __restrict__ windowed,   // (S, 2, N, nT) or NULL: ring + new block
+                   const float* __restrict__ in_blocks, const float* __restrict__ in_ring0, int B, int L, int hop, int nT,
                    const float* __restrict__ win_a, const double2* __restrict__ tw, int N, int log2n, const float2* __restrict__ ET, int D, int Fp,
-                   float2* __restrict__ X, float* __restrict__ G, float* __restrict__ gccphat, float* __restrict__ Vabs,
-                   const float* __restrict__ H0, float* __restrict__ H, int K, int inference) {
+                   float2* __restrict__ X0, float* __restrict__ G0, float* __restrict__ gccphat0, float* __restrict__ Vabs0,
+                   const float* __restrict__ H0, float* __restrict__ Hs0, int K, int inference) {
   __shared__ double2 fft[kRtMaxN];
   __shared__ float2 coh[kRtMaxN / 2 + 1];
-  const int t = blockIdx.x, F = N / 2 + 1;
+  const int t = blockIdx.x, s = blockIdx.y, F = N / 2 + 1;
+  const RtDev* dev = rt_slot(dev0, s, stride);
+  if (!dev->active) return;
+  const float* in_ring = rt_slot(in_ring0, s, stride);
+  const float* in_block = in_blocks ? in_blocks + (int64_t)s * 2 * B : nullptr;
+  if (windowed) windowed += (int64_t)s * 2 * N * nT;
+  float2* X = rt_slot(X0, s, stride);
+  float* G = rt_slot(G0, s, stride);
+  float* gccphat = rt_slot(gccphat0, s, stride);
+  float* Vabs = rt_slot(Vabs0, s, stride);
+  float* H = rt_slot(Hs0, s, stride);
   const int call = dev->block_counter + 1;
   const int w0 = L - N - (nT - 1 - t) * hop;         // utils.py:107 windowIndexes[t]
   for (int i = threadIdx.x; i < N; i += blockDim.x) {
@@ -232,180 +297,343 @@ rt_analysis_kernel(const RtDev* __restrict__ dev, const float* __restrict__ wind
   // gccPHAT[d] = nanmean over f (:214)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int d = warp; d < D; d += kFftThreads / 32) {
-    double s = 0.0;
+    double sum = 0.0;
     int n = 0;
     for (int f = lane; f < F; f += 32) {
       const float v = Gt[(int64_t)d * Fp + f];
-      if (v == v) { s += (double)v; ++n; }
+      if (v == v) { sum += (double)v; ++n; }
     }
-    for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); n += __shfl_xor_sync(0xffffffffu, n, o); }
-    if (lane == 0) gccphat[(int64_t)d * nT + t] = n > 0 ? (float)(s / (double)n) : __int_as_float(0x7fc00000);
+    for (int o = 16; o > 0; o >>= 1) { sum += __shfl_xor_sync(0xffffffffu, sum, o); n += __shfl_xor_sync(0xffffffffu, n, o); }
+    if (lane == 0) gccphat[(int64_t)d * nT + t] = n > 0 ? (float)(sum / (double)n) : __int_as_float(0x7fc00000);
   }
 }
 
 // ---------------------------------------------------------------------------------------------- I: coefficient inference
-// R[f][j] = V[f][j] / sum_k W[f][k] H[k][j]   (gccNMFFunctions.py:76, V / dot(W, H)); one warp per bin, J = 2 nT columns
-template <int J>
+// Slots per warp of the inference and filter kernels: the dictionary row a warp streams is used for all of them.  The register
+// budget is 16 float (inference) or 32 double (filter) accumulators per lane.
+constexpr int rt_inf_slots(int J) { return J >= 16 ? 1 : 16 / J; }
+constexpr int rt_filter_slots(int NT) { return NT >= 8 ? 1 : 8 / NT; }
+
+// R[f][j] = V[f][j] / sum_k W[f][k] H[k][j]   (gccNMFFunctions.py:76, V / dot(W, H)); one warp per bin and SG slots, J = 2 nT
+// columns.  Per slot and column: lane-strided fmaf over k from 0.f, then the xor butterfly.
+template <int J, int SG>
 __global__ void __launch_bounds__(256)
-rt_inf_ratio_kernel(const float* __restrict__ W, const float* __restrict__ H, const float* __restrict__ V, int F, int K, float* __restrict__ R) {
-  const int f = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+rt_inf_ratio_kernel(const RtDev* __restrict__ dev0, size_t stride, int S, const float* __restrict__ W, const float* __restrict__ H0,
+                    const float* __restrict__ V0, int F, int K, float* __restrict__ R0) {
+  const int f = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31, s0 = blockIdx.y * SG;
   if (f >= F) return;
-  float acc[J];
+  bool on[SG];
+  bool any = false;
 #pragma unroll
-  for (int j = 0; j < J; ++j) acc[j] = 0.f;
+  for (int g = 0; g < SG; ++g) {
+    on[g] = s0 + g < S && rt_slot(dev0, s0 + g, stride)->active;
+    any |= on[g];
+  }
+  if (!any) return;
+  float acc[SG][J];
+#pragma unroll
+  for (int g = 0; g < SG; ++g)
+#pragma unroll
+    for (int j = 0; j < J; ++j) acc[g][j] = 0.f;
   for (int k = lane; k < K; k += 32) {
     const float w = W[(int64_t)f * K + k];
 #pragma unroll
-    for (int j = 0; j < J; ++j) acc[j] = fmaf(w, H[(int64_t)k * J + j], acc[j]);
+    for (int g = 0; g < SG; ++g) {
+      if (!on[g]) continue;
+      const float* H = rt_slot(H0, s0 + g, stride);
+#pragma unroll
+      for (int j = 0; j < J; ++j) acc[g][j] = fmaf(w, H[(int64_t)k * J + j], acc[g][j]);
+    }
   }
 #pragma unroll
-  for (int j = 0; j < J; ++j) {
-    float s = acc[j];
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (lane == 0) R[(int64_t)f * J + j] = V[(int64_t)f * J + j] / s;
+  for (int g = 0; g < SG; ++g) {
+    if (!on[g]) continue;
+    const float* V = rt_slot(V0, s0 + g, stride);
+    float* R = rt_slot(R0, s0 + g, stride);
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+      float s = acc[g][j];
+      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      if (lane == 0) R[(int64_t)f * J + j] = V[(int64_t)f * J + j] / s;
+    }
   }
 }
-// H[k][j] *= (sum_f W[f][k] R[f][j]) / (colsum(W)[k] + alpha + eps)   (:76); one warp per atom over the transposed dictionary
-template <int J>
+// H[k][j] *= (sum_f W[f][k] R[f][j]) / (colsum(W)[k] + alpha + eps)   (:76); one warp per atom and SG slots over the transposed
+// dictionary, lane-strided over f, then the xor butterfly.
+template <int J, int SG>
 __global__ void __launch_bounds__(256)
-rt_inf_update_kernel(const float* __restrict__ WT, int Fp, const float* __restrict__ R, int F, int K, const float* __restrict__ colsumW, float alpha,
-                     float eps, float* __restrict__ H) {
-  const int k = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+rt_inf_update_kernel(const RtDev* __restrict__ dev0, size_t stride, int S, const float* __restrict__ WT, int Fp, const float* __restrict__ R0, int F,
+                     int K, const float* __restrict__ colsumW, float alpha, float eps, float* __restrict__ H0) {
+  const int k = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31, s0 = blockIdx.y * SG;
   if (k >= K) return;
-  float acc[J];
+  bool on[SG];
+  bool any = false;
 #pragma unroll
-  for (int j = 0; j < J; ++j) acc[j] = 0.f;
+  for (int g = 0; g < SG; ++g) {
+    on[g] = s0 + g < S && rt_slot(dev0, s0 + g, stride)->active;
+    any |= on[g];
+  }
+  if (!any) return;
+  float acc[SG][J];
+#pragma unroll
+  for (int g = 0; g < SG; ++g)
+#pragma unroll
+    for (int j = 0; j < J; ++j) acc[g][j] = 0.f;
   for (int f = lane; f < F; f += 32) {
     const float w = WT[(int64_t)k * Fp + f];
 #pragma unroll
-    for (int j = 0; j < J; ++j) acc[j] = fmaf(w, R[(int64_t)f * J + j], acc[j]);
+    for (int g = 0; g < SG; ++g) {
+      if (!on[g]) continue;
+      const float* R = rt_slot(R0, s0 + g, stride);
+#pragma unroll
+      for (int j = 0; j < J; ++j) acc[g][j] = fmaf(w, R[(int64_t)f * J + j], acc[g][j]);
+    }
   }
   const float denom = (colsumW[k] + alpha) + eps;
 #pragma unroll
-  for (int j = 0; j < J; ++j) {
-    float s = acc[j];
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (lane == 0) H[(int64_t)k * J + j] = H[(int64_t)k * J + j] * (s / denom);
+  for (int g = 0; g < SG; ++g) {
+    if (!on[g]) continue;
+    float* H = rt_slot(H0, s0 + g, stride);
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+      float s = acc[g][j];
+      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      if (lane == 0) H[(int64_t)k * J + j] = H[(int64_t)k * J + j] * (s / denom);
+    }
   }
 }
 
 // ---------------------------------------------------------------------------------------------- B: per-atom TDOA argmax + atom mask
-// grid (K / 16, nT); thread = (TDOA group dg = tid / 16, atom = tid % 16); TDOAs d = dg + 16 j.
-template <int DJ>        // TDOAs per thread: D <= 16 DJ
+// One register-blocked SIMT tile over rows = (slot, frame, d) and columns = atoms: C[row][k] = sum_f G[row][f] W[f][k].
+// 256 threads = 16 row groups x 16 atom groups; a thread owns TM consecutive rows and TN atoms.  A CTA covers RB = 16 TM rows =
+// RB / Dp whole (slot, frame) pairs (Dp = D rounded up to 32, 64 or 128; rows d >= D are zero and never win) and KB = 16 TN atoms,
+// so the argmax over d of every (pair, atom) it owns is inside the CTA.  Per f stage the W tile is staged in shared memory once
+// and used by every pair of the CTA.  Each output is ONE fmaf chain over f = 0 .. F-1 starting from 0.f, in f order, whatever
+// TM / TN: the float32 values, and so the decisions, do not depend on the tile shape or on the other slots.
+//   TM = Dp / 16 (2, 4, 8), TN = 1: one pair x 16 atoms per CTA (K / 16 x pairs CTAs: latency for few streams)
+//   TM = 8, TN = 8:                 128 rows x 128 atoms per CTA (64 accumulators per thread: throughput for many streams)
+template <int TM, int TN>
 __global__ void __launch_bounds__(256)
-rt_atoms_kernel(const RtDev* __restrict__ dev, const float* __restrict__ G, const float* __restrict__ W, int F, int Fp, int K, int D, int nT,
-                int32_t* __restrict__ argmax, double* __restrict__ hmask) {
-  __shared__ float Gs[16 * DJ][33];
-  __shared__ float Ws[32][kRtAtomsPerCta];
-  __shared__ float vals[16 * DJ][kRtAtomsPerCta + 1];
-  const int t = blockIdx.y, k0 = blockIdx.x * kRtAtomsPerCta;
-  const int atom = threadIdx.x & 15, dg = threadIdx.x >> 4;
-  const float* Gt = G + (int64_t)t * D * Fp;
-  float acc[DJ];
+rt_atoms_kernel(const RtDev* __restrict__ dev0, size_t stride, int pairs, int nT, const float* __restrict__ G0, const float* __restrict__ W, int F,
+                int Fp, int K, int D, int Dp, int32_t* __restrict__ argmax0, double* __restrict__ hmask0) {
+  constexpr int RB = 16 * TM, KB = 16 * TN, GS = RB + 4, FC = kRtAtomsFc;
+  static_assert(RB % 32 == 0 && (TM <= 2 || TM % 4 == 0) && (TN < 4 || TN % 4 == 0), "tile shape");
+  __shared__ __align__(16) float sm[FC * GS + FC * KB];
+  __shared__ int act[RB / 32];
+  float* Gs = sm;                         // [f][row]
+  float* Ws = sm + FC * GS;               // [f][atom]
+  const int ppc = RB / Dp, k0 = blockIdx.x * KB, gp0 = blockIdx.y * ppc;
+  const int ag = threadIdx.x & 15, rg = threadIdx.x >> 4;
+  if (threadIdx.x < ppc) {
+    const int gp = gp0 + threadIdx.x;
+    act[threadIdx.x] = gp < pairs && rt_slot(dev0, gp / nT, stride)->active;
+  }
+  __syncthreads();
+  bool any = false;
+  for (int p = 0; p < ppc; ++p) any |= act[p] != 0;
+  if (!any) return;
+
+  float acc[TM][TN];
 #pragma unroll
-  for (int j = 0; j < DJ; ++j) acc[j] = 0.f;
-  for (int f0 = 0; f0 < F; f0 += 32) {
-    for (int i = threadIdx.x; i < 16 * DJ * 32; i += 256) {
-      const int d = i >> 5, ff = i & 31;
-      Gs[d][ff] = (d < D && f0 + ff < F) ? Gt[(int64_t)d * Fp + f0 + ff] : 0.f;
+  for (int i = 0; i < TM; ++i)
+#pragma unroll
+    for (int j = 0; j < TN; ++j) acc[i][j] = 0.f;
+  auto atom_of = [&](int j) { return TN >= 4 ? (j >> 2) * 64 + ag * 4 + (j & 3) : j * 16 + ag; };
+
+  for (int f0 = 0; f0 < F; f0 += FC) {
+    // G stage: float4 along f (Fp % 4 == 0, G zero on [F, Fp)), transposed into Gs[f][row]
+    for (int i = threadIdx.x; i < RB * (FC / 4); i += 256) {
+      const int row = i / (FC / 4), fq = i - row * (FC / 4), p = row / Dp, d = row - p * Dp, gp = gp0 + p, f = f0 + 4 * fq;
+      float4 v = float4{0.f, 0.f, 0.f, 0.f};
+      if (d < D && act[p] && f < Fp) {
+        const int s = gp / nT, t = gp - s * nT;
+        v = *reinterpret_cast<const float4*>(rt_slot(G0, s, stride) + ((int64_t)t * D + d) * Fp + f);
+      }
+      Gs[(4 * fq + 0) * GS + row] = v.x;
+      Gs[(4 * fq + 1) * GS + row] = v.y;
+      Gs[(4 * fq + 2) * GS + row] = v.z;
+      Gs[(4 * fq + 3) * GS + row] = v.w;
     }
-    for (int i = threadIdx.x; i < 32 * kRtAtomsPerCta; i += 256) {
-      const int ff = i >> 4, a = i & 15;
-      Ws[ff][a] = (f0 + ff < F && k0 + a < K) ? W[(int64_t)(f0 + ff) * K + k0 + a] : 0.f;
+    for (int i = threadIdx.x; i < FC * KB; i += 256) {
+      const int ff = i / KB, a = i - ff * KB;
+      Ws[i] = (f0 + ff < F && k0 + a < K) ? W[(int64_t)(f0 + ff) * K + k0 + a] : 0.f;
     }
     __syncthreads();
-#pragma unroll 8
-    for (int ff = 0; ff < 32; ++ff) {
-      const float w = Ws[ff][atom];
+#pragma unroll 4
+    for (int ff = 0; ff < FC; ++ff) {
+      float a[TM], b[TN];
+      const float* gr = Gs + ff * GS + rg * TM;
+      if constexpr (TM % 4 == 0) {
 #pragma unroll
-      for (int j = 0; j < DJ; ++j) acc[j] = fmaf(Gs[dg + 16 * j][ff], w, acc[j]);     // tensor.dot(realGCC.T, W) in float32 (:259)
+        for (int i = 0; i < TM; i += 4) {
+          const float4 q = *reinterpret_cast<const float4*>(gr + i);
+          a[i] = q.x; a[i + 1] = q.y; a[i + 2] = q.z; a[i + 3] = q.w;
+        }
+      } else {
+#pragma unroll
+        for (int i = 0; i < TM; ++i) a[i] = gr[i];
+      }
+      if constexpr (TN % 4 == 0) {
+#pragma unroll
+        for (int j = 0; j < TN; j += 4) {
+          const float4 q = *reinterpret_cast<const float4*>(Ws + ff * KB + atom_of(j));
+          b[j] = q.x; b[j + 1] = q.y; b[j + 2] = q.z; b[j + 3] = q.w;
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < TN; ++j) b[j] = Ws[ff * KB + atom_of(j)];
+      }
+#pragma unroll
+      for (int i = 0; i < TM; ++i)
+#pragma unroll
+        for (int j = 0; j < TN; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);     // tensor.dot(realGCC.T, W) in float32 (:259)
     }
     __syncthreads();
   }
+  // argmax over d: first over the thread's TM rows, then over the row groups of the pair (partials alias the stage buffers)
+  float* part_v = sm;
+  int* part_i = reinterpret_cast<int*>(sm + 16 * KB);
+  {
+    const int r0 = rg * TM, d0 = r0 - (r0 / Dp) * Dp;
 #pragma unroll
-  for (int j = 0; j < DJ; ++j) vals[dg + 16 * j][atom] = acc[j];
+    for (int j = 0; j < TN; ++j) {
+      float bv = 0.f;
+      int bi = -1;
+#pragma unroll
+      for (int i = 0; i < TM; ++i)
+        if (d0 + i < D && (bi < 0 || rt_better(acc[i][j], d0 + i, bv, bi))) { bv = acc[i][j]; bi = d0 + i; }
+      part_v[rg * KB + atom_of(j)] = bv;
+      part_i[rg * KB + atom_of(j)] = bi;
+    }
+  }
   __syncthreads();
-  if (threadIdx.x < kRtAtomsPerCta && k0 + threadIdx.x < K) {
-    const int a = threadIdx.x;
-    float bv = vals[0][a];
-    int bi = 0;
-    for (int d = 1; d < D; ++d)
-      if (rt_better(vals[d][a], d, bv, bi)) { bv = vals[d][a]; bi = d; }
-    const int64_t o = (int64_t)(k0 + a) * nT + t;
-    argmax[o] = bi;
+  const int groups = Dp / TM;
+  for (int idx = threadIdx.x; idx < ppc * KB; idx += 256) {
+    const int p = idx / KB, a = idx - p * KB, gp = gp0 + p, k = k0 + a;
+    if (!act[p] || k >= K) continue;
+    float bv = 0.f;
+    int bi = -1;
+    for (int r = p * groups; r < (p + 1) * groups; ++r) {
+      const int ci = part_i[r * KB + a];
+      if (ci < 0) continue;
+      const float cv = part_v[r * KB + a];
+      if (bi < 0 || rt_better(cv, ci, bv, bi)) { bv = cv; bi = ci; }
+    }
+    const int s = gp / nT, t = gp - s * nT;
+    const RtDev* dev = rt_slot(dev0, s, stride);
+    const int64_t o = (int64_t)k * nT + t;
+    rt_slot(argmax0, s, stride)[o] = bi;
     // int64 - float32 promotes to float64 in Theano and numpy alike: the mask arithmetic is float64 (:263, :265)
     const double dist = fabs((double)bi - (double)dev->target);
     double m;
     if (dev->mode == 0) m = dist < (double)dev->eps ? 1.0 : 0.0;
     else m = exp(-pow(dist / (double)dev->eps, (double)dev->beta)) / (double)(1.0f + dev->noise_floor) + (double)dev->noise_floor;
-    hmask[o] = m;
+    rt_slot(hmask0, s, stride)[o] = m;
   }
 }
 
-// ---------------------------------------------------------------------------------------------- C: time-frequency mask, one warp per bin
+// ---------------------------------------------------------------------------------------------- C: time-frequency mask, one warp per bin and SG slots
+// Per slot, frame and channel: lane-strided float64 sums over k, then the xor butterfly.
+template <int NT, int SG, bool inference>
 __global__ void __launch_bounds__(256)
-rt_filter_kernel(const RtDev* __restrict__ dev, const float* __restrict__ W, const double* __restrict__ hmask, const float* __restrict__ recV,
-                 const float* __restrict__ H, int inference, const float2* __restrict__ X, int F, int K, int nT, float2* __restrict__ Y) {
-  const int f = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+rt_filter_kernel(const RtDev* __restrict__ dev0, size_t stride, int S, const float* __restrict__ W, const double* __restrict__ hmask0,
+                 const float* __restrict__ recV, const float* __restrict__ H0, const float2* __restrict__ X0, int F, int K, float2* __restrict__ Y0) {
+  const int f = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31, s0 = blockIdx.y * SG;
   if (f >= F) return;
-  if (!dev->separation) {                            // :211 outputSpectrogram = complexMixtureSpectrogram.copy()
-    for (int i = lane; i < 2 * nT; i += 32) {
-      const int c = i / nT, t = i - c * nT;
-      Y[((int64_t)c * F + f) * nT + t] = X[((int64_t)c * F + f) * nT + t];
-    }
-    return;
-  }
-  double num[2][kRtMaxFrames], den[2][kRtMaxFrames];
+  bool on[SG];
+  bool any = false;
 #pragma unroll
-  for (int t = 0; t < kRtMaxFrames; ++t) { num[0][t] = num[1][t] = den[0][t] = den[1][t] = 0.0; }
+  for (int g = 0; g < SG; ++g) {
+    on[g] = false;
+    if (s0 + g >= S) continue;
+    const RtDev* dev = rt_slot(dev0, s0 + g, stride);
+    if (!dev->active) continue;
+    if (!dev->separation) {                          // :211 outputSpectrogram = complexMixtureSpectrogram.copy()
+      const float2* X = rt_slot(X0, s0 + g, stride);
+      float2* Y = rt_slot(Y0, s0 + g, stride);
+      for (int i = lane; i < 2 * NT; i += 32) {
+        const int c = i / NT, t = i - c * NT;
+        Y[((int64_t)c * F + f) * NT + t] = X[((int64_t)c * F + f) * NT + t];
+      }
+      continue;
+    }
+    on[g] = true;
+    any = true;
+  }
+  if (!any) return;
+  double num[SG][2][NT], den[SG][2][NT];
+#pragma unroll
+  for (int g = 0; g < SG; ++g)
+#pragma unroll
+    for (int t = 0; t < NT; ++t) { num[g][0][t] = num[g][1][t] = den[g][0][t] = den[g][1][t] = 0.0; }
   for (int k = lane; k < K; k += 32) {
     const double w = (double)W[(int64_t)f * K + k];
 #pragma unroll
-    for (int t = 0; t < kRtMaxFrames; ++t) {
-      if (t < nT) {
-        const double m = hmask[(int64_t)k * nT + t];
-        if (inference) {                             // sourceEstimate = W . (H * mask), recV = W . H  (ipynb:435-437)
+    for (int g = 0; g < SG; ++g) {
+      if (!on[g]) continue;
+      const double* hmask = rt_slot(hmask0, s0 + g, stride);
+      const float* H = rt_slot(H0, s0 + g, stride);
+#pragma unroll
+      for (int t = 0; t < NT; ++t) {
+        const double m = hmask[(int64_t)k * NT + t];
+        if constexpr (inference) {                   // sourceEstimate = W . (H * mask), recV = W . H  (ipynb:435-437)
 #pragma unroll
           for (int c = 0; c < 2; ++c) {
-            const double hv = (double)H[(int64_t)k * (2 * nT) + 2 * t + c];
-            num[c][t] += w * (hv * m);
-            den[c][t] += w * hv;
+            const double hv = (double)H[(int64_t)k * (2 * NT) + 2 * t + c];
+            num[g][c][t] += w * (hv * m);
+            den[g][c][t] += w * hv;
           }
         } else {
-          num[0][t] += w * m;                        // tensor.dot(W, HMask) (:267)
+          num[g][0][t] += w * m;                     // tensor.dot(W, HMask) (:267)
         }
       }
     }
   }
 #pragma unroll
-  for (int t = 0; t < kRtMaxFrames; ++t) {
-    if (t < nT) {
+  for (int g = 0; g < SG; ++g) {
+    if (!on[g]) continue;
+#pragma unroll
+    for (int t = 0; t < NT; ++t) {
 #pragma unroll
       for (int c = 0; c < 2; ++c) {
-        if (c == 1 && !inference) break;
-        double a = num[c][t], b = den[c][t];
+        if (c == 1 && !inference) continue;
+        double a = num[g][c][t], b = den[g][c][t];
         for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); b += __shfl_xor_sync(0xffffffffu, b, o); }
-        num[c][t] = a; den[c][t] = b;
+        num[g][c][t] = a; den[g][c][t] = b;
       }
     }
-  }
-  if (lane < 2 * nT) {
-    const int c = lane / nT, t = lane - c * nT;
-    double tf = 0.0;
+    if (lane < 2 * NT) {
+      const float2* X = rt_slot(X0, s0 + g, stride);
+      float2* Y = rt_slot(Y0, s0 + g, stride);
+      const int c = lane / NT, t = lane - c * NT;
+      double tf = 0.0;
 #pragma unroll
-    for (int tt = 0; tt < kRtMaxFrames; ++tt)
-      if (tt == t) tf = inference ? num[c & 1][tt] / den[c & 1][tt] : num[0][tt] / (double)recV[f];
-    const float2 x = X[((int64_t)c * F + f) * nT + t];
-    Y[((int64_t)c * F + f) * nT + t] = float2{(float)(tf * (double)x.x), (float)(tf * (double)x.y)};   // inputMask * spectrogram (:209)
+      for (int tt = 0; tt < NT; ++tt)                // register selection (no dynamically indexed local array)
+        if (tt == t) tf = inference ? (c ? num[g][1][tt] / den[g][1][tt] : num[g][0][tt] / den[g][0][tt]) : num[g][0][tt] / (double)recV[f];
+      const float2 x = X[((int64_t)c * F + f) * NT + t];
+      Y[((int64_t)c * F + f) * NT + t] = float2{(float)(tf * (double)x.x), (float)(tf * (double)x.y)};   // inputMask * spectrogram (:209)
+    }
   }
 }
 
-// ---------------------------------------------------------------------------------------------- D: synthesis (one CTA per frame)
+// ---------------------------------------------------------------------------------------------- D: synthesis (one CTA per frame and slot)
 __global__ void __launch_bounds__(kFftThreads)
-rt_synthesis_kernel(RtDev* __restrict__ dev, const float2* __restrict__ Y, const float2* __restrict__ tw, int N, int log2n, int nT,
-                    const float* __restrict__ win_s, float* __restrict__ frames, float* __restrict__ out_windowed, int advance) {
+rt_synthesis_kernel(RtDev* __restrict__ dev0, size_t stride, const float2* __restrict__ Y0, const float2* __restrict__ tw, int N, int log2n, int nT,
+                    const float* __restrict__ win_s, float* __restrict__ frames0, float* __restrict__ out_windowed, int advance) {
   __shared__ float2 fft[kRtMaxN];
-  const int t = blockIdx.x, F = N / 2 + 1;
+  const int t = blockIdx.x, s = blockIdx.y, F = N / 2 + 1;
+  RtDev* dev = rt_slot(dev0, s, stride);
+  if (out_windowed) out_windowed += (int64_t)s * 2 * N * nT;
+  if (!dev->active) {                                            // an inactive slot's output frames are zeros
+    if (out_windowed)
+      for (int i = threadIdx.x; i < N; i += blockDim.x) {
+        out_windowed[((int64_t)0 * N + i) * nT + t] = 0.f;
+        out_windowed[((int64_t)1 * N + i) * nT + t] = 0.f;
+      }
+    return;
+  }
+  const float2* Y = rt_slot(Y0, s, stride);
+  float* frames = rt_slot(frames0, s, stride);
   for (int k = threadIdx.x; k < F; k += blockDim.x) {
     float2 a = Y[((int64_t)0 * F + k) * nT + t], b = Y[((int64_t)1 * F + k) * nT + t];
     if (k == 0 || k == N / 2) { a.y = 0.f; b.y = 0.f; }          // numpy.fft.irfft ignores them
@@ -429,7 +657,7 @@ rt_synthesis_kernel(RtDev* __restrict__ dev, const float2* __restrict__ Y, const
   if (advance && t == 0 && threadIdx.x == 0) atomicAdd(&dev->block_counter, 1);     // the ring kernel that follows uses counter (= this call's number)
 }
 
-// ---------------------------------------------------------------------------------------------- localisation (one CTA, D <= 128 threads used)
+// ---------------------------------------------------------------------------------------------- localisation (one CTA per slot, D <= 128 threads used)
 __device__ void rt_localize(RtDev* dev, const float* __restrict__ gccphat, int D, int nT, double* __restrict__ hist, int hist_len) {
   __shared__ double mean_s[kRtMaxD];
   const int d = threadIdx.x;
@@ -464,23 +692,40 @@ __device__ void rt_localize(RtDev* dev, const float* __restrict__ gccphat, int D
 }
 
 __global__ void __launch_bounds__(128)
-rt_localize_kernel(RtDev* dev, const float* __restrict__ gccphat, int D, int nT, double* __restrict__ hist, int hist_len) {
-  rt_localize(dev, gccphat, D, nT, hist, hist_len);
+rt_localize_kernel(RtDev* dev0, size_t stride, const float* __restrict__ gccphat0, int D, int nT, double* __restrict__ hist0, int hist_len) {
+  const int s = blockIdx.x;
+  RtDev* dev = rt_slot(dev0, s, stride);
+  if (!dev->active) return;
+  rt_localize(dev, rt_slot(gccphat0, s, stride), D, nT, rt_slot(hist0, s, stride), hist_len);
 }
 
 // ---------------------------------------------------------------------------------------------- E: overlap-add ring, block emit, input push
-// CTAs [0, gridDim.x - 1): one thread per logical ring position of the range that changes or is emitted; last CTA: localisation.
+// grid (ring CTAs + 1, S).  CTAs [0, gridDim.x - 1): one thread per logical ring position of the range that changes or is emitted;
+// last CTA: localisation.
 __global__ void __launch_bounds__(128)
-rt_ola_emit_kernel(RtDev* dev, const float* __restrict__ frames, int N, int hop, int nT, int B, int L, int p_first, float* __restrict__ out_ring,
-                   float* __restrict__ out_block, const float* __restrict__ in_block, float* __restrict__ in_ring, const float* __restrict__ gccphat,
-                   int D, double* __restrict__ hist, int hist_len) {
+rt_ola_emit_kernel(RtDev* dev0, size_t stride, const float* __restrict__ frames0, int N, int hop, int nT, int B, int L, int p_first,
+                   float* __restrict__ out_ring0, float* __restrict__ out_blocks, const float* __restrict__ in_blocks, float* __restrict__ in_ring0,
+                   const float* __restrict__ gccphat0, int D, double* __restrict__ hist0, int hist_len) {
+  const int s = blockIdx.y;
+  RtDev* dev = rt_slot(dev0, s, stride);
+  const bool active = dev->active != 0;
   if (blockIdx.x == gridDim.x - 1) {
-    rt_localize(dev, gccphat, D, nT, hist, hist_len);
+    if (active) rt_localize(dev, rt_slot(gccphat0, s, stride), D, nT, rt_slot(hist0, s, stride), hist_len);
     return;
   }
-  const int call = dev->block_counter;               // already advanced by the synthesis kernel
+  float* out_block = out_blocks + (int64_t)s * 2 * B;
   const int p = p_first + blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= L) return;
+  if (!active) {                                     // an inactive slot emits a block of zeros
+    if (p >= L - 3 * B && p < L - 2 * B)
+      for (int c = 0; c < 2; ++c) out_block[c * B + (p - (L - 3 * B))] = 0.f;
+    return;
+  }
+  const float* frames = rt_slot(frames0, s, stride);
+  float* out_ring = rt_slot(out_ring0, s, stride);
+  float* in_ring = rt_slot(in_ring0, s, stride);
+  const float* in_block = in_blocks + (int64_t)s * 2 * B;
+  const int call = dev->block_counter;               // already advanced by the synthesis kernel
   const int q = rt_ring_index(p, call, B, L);
   const int w_first = L - N - (nT - 1) * hop;
 #pragma unroll
@@ -504,65 +749,144 @@ int ilog2_of(int n) {
   return l;
 }
 
-#define RT_CARVE_OR_FAIL(l)                                                                                                        \
-  if (int st__ = rt_check(h, cfg)) return st__;                                                                                    \
-  RtLayout l = rt_carve(*cfg, state, state_bytes);                                                                                 \
+#define RT_CARVE_OR_FAIL(l, S)                                                                                                     \
+  if (int st__ = rt_check(h, cfg, (S))) return st__;                                                                               \
+  RtLayout l = rt_carve(*cfg, (S), state, state_bytes);                                                                            \
   if (!l.ok) return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "rt state buffer missing or too small: need %zu bytes", l.bytes)
 
-// Kernels A .. D (+ inference) of one block; `windowed` != NULL: frames given by the caller (processFrames), else cut from the ring.
-int rt_enqueue_core(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout& l, const float* windowed, const float* in_block, float* out_windowed,
-                    const double* forced_mask, int advance, void* stream) {
-  const int N = cfg->window_size, nT = cfg->windows_per_block, K = cfg->num_atoms, D = cfg->num_tdoas, F = l.F, log2n = ilog2_of(N);
-  const int inf = cfg->inference_iterations;
-  GCCNMF_LAUNCH(h, rt_analysis_kernel, nT, kFftThreads, 0, stream, l.dev, windowed, in_block, l.in_ring, cfg->block_size, l.L, cfg->hop_size, nT, l.win_a,
-                reinterpret_cast<const double2*>(l.tw64), N, log2n, l.ET, D, l.Fp, l.X, l.G, l.gccphat, l.Vabs, l.H0, l.H, K, inf > 0 ? 1 : 0);
-  for (int it = 0; it < inf; ++it) {
-#define RT_INF_CASE(J)                                                                                                             \
-    case J:                                                                                                                        \
-      GCCNMF_LAUNCH(h, rt_inf_ratio_kernel<2 * J>, (F + 7) / 8, 256, 0, stream, l.W, l.H, l.Vabs, F, K, l.R);                        \
-      GCCNMF_LAUNCH(h, rt_inf_update_kernel<2 * J>, (K + 7) / 8, 256, 0, stream, l.WT, l.Fp, l.R, F, K, l.colsumW, cfg->sparsity_alpha, cfg->epsilon, l.H); \
-      break;
-    switch (nT) {
-      RT_INF_CASE(1) RT_INF_CASE(2) RT_INF_CASE(3) RT_INF_CASE(4) RT_INF_CASE(5) RT_INF_CASE(6) RT_INF_CASE(7) RT_INF_CASE(8)
-    }
-#undef RT_INF_CASE
-  }
-  const dim3 grid_b((K + kRtAtomsPerCta - 1) / kRtAtomsPerCta, nT);
-  if (forced_mask) {     // teacher forcing / externally decided masks: the filter uses the caller's (K, nT) float64 atom mask
-    GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.hmask, forced_mask, (size_t)K * nT * sizeof(double), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  } else if (D <= 32) GCCNMF_LAUNCH(h, rt_atoms_kernel<2>, grid_b, 256, 0, stream, l.dev, l.G, l.W, F, l.Fp, K, D, nT, l.argmax, l.hmask);
-  else if (D <= 64) GCCNMF_LAUNCH(h, rt_atoms_kernel<4>, grid_b, 256, 0, stream, l.dev, l.G, l.W, F, l.Fp, K, D, nT, l.argmax, l.hmask);
-  else GCCNMF_LAUNCH(h, rt_atoms_kernel<8>, grid_b, 256, 0, stream, l.dev, l.G, l.W, F, l.Fp, K, D, nT, l.argmax, l.hmask);
-  GCCNMF_LAUNCH(h, rt_filter_kernel, (F + 7) / 8, 256, 0, stream, l.dev, l.W, l.hmask, l.recV, l.H, inf > 0 ? 1 : 0, l.X, F, K, nT, l.Y);
-  GCCNMF_LAUNCH(h, rt_synthesis_kernel, nT, kFftThreads, 0, stream, l.dev, l.Y, reinterpret_cast<const float2*>(l.tw32), N, log2n, nT, l.win_s, l.frames,
-                out_windowed, advance);
+// Several slots per warp (the dictionary row read once for all of them) only while the grid still has kRtWavesForSlotGroups waves
+// of CTAs; with fewer streams one slot per warp keeps the device busy.
+constexpr int kRtWavesForSlotGroups = 4;
+inline bool rt_group_slots(const gccnmf_handle* h, int ctas_x, int S, int SG) {
+  return SG > 1 && S > 1 && (int64_t)ctas_x * ((S + SG - 1) / SG) >= (int64_t)kRtWavesForSlotGroups * h->sm_count;
+}
+
+template <int J, int SG>
+int rt_enqueue_inference_as(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout& l, bool ratio, void* stream) {
+  const int F = l.F, K = cfg->num_atoms, S = l.S, gy = (S + SG - 1) / SG;
+  if (ratio)
+    GCCNMF_LAUNCH(h, (rt_inf_ratio_kernel<J, SG>), dim3((F + 7) / 8, gy), 256, 0, stream, l.dev, l.stride, S, l.W, l.H, l.Vabs, F, K, l.R);
+  else
+    GCCNMF_LAUNCH(h, (rt_inf_update_kernel<J, SG>), dim3((K + 7) / 8, gy), 256, 0, stream, l.dev, l.stride, S, l.WT, l.Fp, l.R, F, K, l.colsumW,
+                  cfg->sparsity_alpha, cfg->epsilon, l.H);
+  return 0;
+}
+template <int J>
+int rt_enqueue_inference(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout& l, void* stream) {
+  constexpr int SG = rt_inf_slots(J);
+  const int F = l.F, K = cfg->num_atoms, S = l.S;
+  const int st = rt_group_slots(h, (F + 7) / 8, S, SG) ? rt_enqueue_inference_as<J, SG>(h, cfg, l, true, stream)
+                                                       : rt_enqueue_inference_as<J, 1>(h, cfg, l, true, stream);
+  if (st) return st;
+  return rt_group_slots(h, (K + 7) / 8, S, SG) ? rt_enqueue_inference_as<J, SG>(h, cfg, l, false, stream)
+                                               : rt_enqueue_inference_as<J, 1>(h, cfg, l, false, stream);
+}
+
+template <int NT, int SG, bool INF>
+int rt_enqueue_filter_as(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout& l, void* stream) {
+  const int F = l.F, K = cfg->num_atoms, S = l.S;
+  GCCNMF_LAUNCH(h, (rt_filter_kernel<NT, SG, INF>), dim3((F + 7) / 8, (S + SG - 1) / SG), 256, 0, stream, l.dev, l.stride, S, l.W, l.hmask, l.recV, l.H,
+                l.X, F, K, l.Y);
+  return 0;
+}
+template <int NT>
+int rt_enqueue_filter(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout& l, void* stream) {
+  constexpr int SG = rt_filter_slots(NT);
+  const bool inf = cfg->inference_iterations > 0;
+  if (!rt_group_slots(h, (l.F + 7) / 8, l.S, SG))
+    return inf ? rt_enqueue_filter_as<NT, 1, true>(h, cfg, l, stream) : rt_enqueue_filter_as<NT, 1, false>(h, cfg, l, stream);
+  return inf ? rt_enqueue_filter_as<NT, SG, true>(h, cfg, l, stream) : rt_enqueue_filter_as<NT, SG, false>(h, cfg, l, stream);
+}
+
+// The atoms tile: 128 x 128 once it fills the device with at least one CTA per SM, else one (slot, frame) pair x 16 atoms.
+template <int DJ>
+int rt_enqueue_atoms(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout& l, void* stream) {
+  const int nT = cfg->windows_per_block, K = cfg->num_atoms, D = cfg->num_tdoas, pairs = l.S * nT, Dp = 16 * DJ;
+  const int big_ctas = ((K + 127) / 128) * ((pairs + 128 / Dp - 1) / (128 / Dp));
+  if (big_ctas >= h->sm_count)
+    GCCNMF_LAUNCH(h, (rt_atoms_kernel<8, 8>), dim3((K + 127) / 128, (pairs + 128 / Dp - 1) / (128 / Dp)), 256, 0, stream, l.dev, l.stride, pairs, nT,
+                  l.G, l.W, l.F, l.Fp, K, D, Dp, l.argmax, l.hmask);
+  else
+    GCCNMF_LAUNCH(h, (rt_atoms_kernel<DJ, 1>), dim3((K + 15) / 16, pairs), 256, 0, stream, l.dev, l.stride, pairs, nT, l.G, l.W, l.F, l.Fp, K, D, Dp,
+                  l.argmax, l.hmask);
   return 0;
 }
 
-}  // namespace
-
-extern "C" {
-
-size_t gccnmf_rt_state_bytes(const gccnmf_rt_config* cfg) {
-  if (!cfg || cfg->window_size < 2 || cfg->block_size < 1 || cfg->windows_per_block < 1 || cfg->num_atoms < 1 || cfg->num_tdoas < 1 ||
-      cfg->history_length < 1)
-    return 0;
-  return rt_carve(*cfg, nullptr, 0).bytes;
+// Kernels A .. D (+ inference) of one block for every slot; `windowed` != NULL: frames given by the caller (processFrames, (S, 2, N, nT)),
+// else cut from the rings and `in_blocks` (S, 2, B).
+int rt_enqueue_core(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout& l, const float* windowed, const float* in_blocks, float* out_windowed,
+                    const double* forced_mask, int advance, void* stream) {
+  const int N = cfg->window_size, nT = cfg->windows_per_block, K = cfg->num_atoms, D = cfg->num_tdoas, log2n = ilog2_of(N), S = l.S;
+  const int inf = cfg->inference_iterations;
+  GCCNMF_LAUNCH(h, rt_analysis_kernel, dim3(nT, S), kFftThreads, 0, stream, l.dev, l.stride, windowed, in_blocks, l.in_ring, cfg->block_size, l.L,
+                cfg->hop_size, nT, l.win_a, reinterpret_cast<const double2*>(l.tw64), N, log2n, l.ET, D, l.Fp, l.X, l.G, l.gccphat, l.Vabs, l.H0, l.H, K,
+                inf > 0 ? 1 : 0);
+  for (int it = 0; it < inf; ++it) {
+    int st = 0;
+    switch (nT) {
+      case 1: st = rt_enqueue_inference<2>(h, cfg, l, stream); break;
+      case 2: st = rt_enqueue_inference<4>(h, cfg, l, stream); break;
+      case 3: st = rt_enqueue_inference<6>(h, cfg, l, stream); break;
+      case 4: st = rt_enqueue_inference<8>(h, cfg, l, stream); break;
+      case 5: st = rt_enqueue_inference<10>(h, cfg, l, stream); break;
+      case 6: st = rt_enqueue_inference<12>(h, cfg, l, stream); break;
+      case 7: st = rt_enqueue_inference<14>(h, cfg, l, stream); break;
+      default: st = rt_enqueue_inference<16>(h, cfg, l, stream); break;
+    }
+    if (st) return st;
+  }
+  int st = 0;
+  if (forced_mask) {     // teacher forcing / externally decided masks: the filter uses the caller's (S, K, nT) float64 atom masks
+    const size_t row = (size_t)K * nT * sizeof(double);
+    GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync(l.hmask, l.stride, forced_mask, row, row, S, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  } else if (D <= 32) st = rt_enqueue_atoms<2>(h, cfg, l, stream);
+  else if (D <= 64) st = rt_enqueue_atoms<4>(h, cfg, l, stream);
+  else st = rt_enqueue_atoms<8>(h, cfg, l, stream);
+  if (st) return st;
+  switch (nT) {
+    case 1: st = rt_enqueue_filter<1>(h, cfg, l, stream); break;
+    case 2: st = rt_enqueue_filter<2>(h, cfg, l, stream); break;
+    case 3: st = rt_enqueue_filter<3>(h, cfg, l, stream); break;
+    case 4: st = rt_enqueue_filter<4>(h, cfg, l, stream); break;
+    case 5: st = rt_enqueue_filter<5>(h, cfg, l, stream); break;
+    case 6: st = rt_enqueue_filter<6>(h, cfg, l, stream); break;
+    case 7: st = rt_enqueue_filter<7>(h, cfg, l, stream); break;
+    default: st = rt_enqueue_filter<8>(h, cfg, l, stream); break;
+  }
+  if (st) return st;
+  GCCNMF_LAUNCH(h, rt_synthesis_kernel, dim3(nT, S), kFftThreads, 0, stream, l.dev, l.stride, l.Y, reinterpret_cast<const float2*>(l.tw32), N, log2n,
+                nT, l.win_s, l.frames, out_windowed, advance);
+  return 0;
 }
 
-// W (F, K) f32, E (F, D) complex64 (expJOmegaTau, gccNMFProcessor.py:248), windows (N) f32, H0 (K, 2) f32 or NULL (all device pointers).
-int gccnmf_rt_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, const float* W, const float* E, const float* analysis_window,
-                   const float* synthesis_window, const float* H0, void* state, size_t state_bytes, void* stream) {
-  GCCNMF_ENTER(h);
-  RT_CARVE_OR_FAIL(l);
+int rt_enqueue_params(gccnmf_handle* h, const RtLayout& l, int first, int count, const gccnmf_rtm_slot_params* params, int set_active, void* stream) {
+  for (int i0 = 0; i0 < count; i0 += kRtParamsPerLaunch) {
+    const int n = count - i0 < kRtParamsPerLaunch ? count - i0 : kRtParamsPerLaunch;
+    RtParamsBatch b{};
+    for (int i = 0; i < n; ++i) b.p[i] = params[i0 + i];
+    GCCNMF_LAUNCH(h, rt_set_params_kernel, 1, kRtParamsPerLaunch, 0, stream, l.dev, l.stride, first + i0, n, b, set_active);
+  }
+  return 0;
+}
+
+// Zeroes the regions of slots [first, first + count) and gives them the defaults of gccNMFProcessor.py:190-199, active.
+int rt_enqueue_reset(gccnmf_handle* h, const RtLayout& l, int first, int count, void* stream) {
+  GCCNMF_CHECK_CUDA(h, cudaMemsetAsync(rt_slot(reinterpret_cast<char*>(l.dev), first, l.stride), 0, (size_t)count * l.stride, (cudaStream_t)stream));
+  GCCNMF_LAUNCH(h, rt_default_params_kernel, (count + 127) / 128, 128, 0, stream, l.dev, l.stride, first, count);
+  return 0;
+}
+
+int rt_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, const float* W, const float* E, const float* analysis_window,
+            const float* synthesis_window, const float* H0, void* state, size_t state_bytes, void* stream) {
+  RT_CARVE_OR_FAIL(l, S);
   GCCNMF_REQUIRE(h, W && E && analysis_window && synthesis_window, "rt_init: NULL pointer");
   GCCNMF_REQUIRE(h, cfg->inference_iterations == 0 || H0 != nullptr, "rt_init: coefficient inference needs the initial H0 (K, 2)");
   cudaStream_t s = (cudaStream_t)stream;
   const int N = cfg->window_size, K = cfg->num_atoms, D = cfg->num_tdoas;
-  GCCNMF_CHECK_CUDA(h, cudaMemsetAsync(state, 0, l.bytes, s));                 // rings, history (initValue = 0), counters
   const double* tw64 = nullptr;
   const float* tw32 = nullptr;
   if (int st = gccnmf_get_twiddles(h, N, &tw64, &tw32)) return st;
+  GCCNMF_CHECK_CUDA(h, cudaMemsetAsync(state, 0, l.bytes, s));                 // rings, history (initValue = 0), counters
   GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.tw64, tw64, (size_t)N * sizeof(double), cudaMemcpyDeviceToDevice, s));
   GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.tw32, tw32, (size_t)N * sizeof(float), cudaMemcpyDeviceToDevice, s));
   GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.win_a, analysis_window, (size_t)N * sizeof(float), cudaMemcpyDeviceToDevice, s));
@@ -572,67 +896,46 @@ int gccnmf_rt_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, const float* W
   const int n = K > l.F ? K : l.F;
   GCCNMF_LAUNCH(h, rt_init_dictionary_kernel, (n + 127) / 128, 128, 0, stream, l.W, l.F, l.Fp, K, l.WT, l.recV, l.colsumW);
   GCCNMF_LAUNCH(h, rt_init_steering_kernel, (D * l.Fp + 255) / 256, 256, 0, stream, reinterpret_cast<const float2*>(E), l.F, l.Fp, D, l.ET);
-  // defaults of gccNMFProcessor.py:190-199
-  GCCNMF_LAUNCH(h, rt_set_params_kernel, 1, 1, 0, stream, l.dev, 10.0f, 2.0f, 1.0f, 0.0f, 1, 1, 0, 6, 1);
+  GCCNMF_LAUNCH(h, rt_default_params_kernel, (S + 127) / 128, 128, 0, stream, l.dev, l.stride, 0, S);
   return GCCNMF_OK;
 }
 
-// setTargetTDOARange (:272-276) + the settable attributes (:136-151).  set_target = 0 leaves the target TDOA index alone (it is
-// loop-carried device state when localisation is on).
-int gccnmf_rt_set_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* state, size_t state_bytes, float target_index, int set_target,
-                         float epsilon, float beta, float noise_floor, int mode, int separation_enabled, int localization_enabled,
-                         int localization_window, void* stream) {
-  GCCNMF_ENTER(h);
-  RT_CARVE_OR_FAIL(l);
-  GCCNMF_REQUIRE(h, mode == 0 || mode == 1, "rt_set_params: mode must be 0 (boxcar) or 1 (window)");
-  GCCNMF_LAUNCH(h, rt_set_params_kernel, 1, 1, 0, stream, l.dev, target_index, epsilon, beta, noise_floor, mode, separation_enabled ? 1 : 0,
-                localization_enabled ? 1 : 0, localization_window, set_target ? 1 : 0);
-  return GCCNMF_OK;
-}
-
-// GCCNMFProcessor.processFrames (:201-231): windowed (2, N, nT) f32 -> out (2, N, nT) f32, both on the device.
-int gccnmf_rt_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* state, size_t state_bytes, const float* windowed, float* out,
-                             const double* forced_atom_mask, void* stream) {
-  GCCNMF_ENTER(h);
-  RT_CARVE_OR_FAIL(l);
-  GCCNMF_REQUIRE(h, windowed && out, "rt_process_frames: NULL pointer");
-  if (int st = rt_enqueue_core(h, cfg, l, windowed, nullptr, out, forced_atom_mask, 0, stream)) return st;
-  GCCNMF_LAUNCH(h, rt_localize_kernel, 1, 128, 0, stream, l.dev, l.gccphat, cfg->num_tdoas, cfg->windows_per_block, l.hist, cfg->history_length);
-  return GCCNMF_OK;
-}
-
-// OverlapAddProcessor.processFrames(GCCNMFProcessor.processFrames) (utils.py:99-116 around gccNMFProcessor.py:201-231):
-// in_block (2, B) f32 -> out_block (2, B) f32 (the block emitted is the one pushed in two calls earlier).
-int gccnmf_rt_process_block(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* state, size_t state_bytes, const float* in_block, float* out_block,
-                            const double* forced_atom_mask, void* stream) {
-  GCCNMF_ENTER(h);
-  RT_CARVE_OR_FAIL(l);
-  GCCNMF_REQUIRE(h, in_block && out_block, "rt_process_block: NULL pointer");
-  if (int st = rt_enqueue_core(h, cfg, l, nullptr, in_block, nullptr, forced_atom_mask, 1, stream)) return st;
+int rt_process_block(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, void* state, size_t state_bytes, const float* in_blocks, float* out_blocks,
+                     const double* forced_atom_mask, void* stream) {
+  RT_CARVE_OR_FAIL(l, S);
+  GCCNMF_REQUIRE(h, in_blocks && out_blocks, "rt_process_block: NULL pointer");
+  if (int st = rt_enqueue_core(h, cfg, l, nullptr, in_blocks, nullptr, forced_atom_mask, 1, stream)) return st;
   const int N = cfg->window_size, nT = cfg->windows_per_block, B = cfg->block_size;
   const int w_first = l.L - N - (nT - 1) * cfg->hop_size;
   const int p_first = w_first < l.L - 3 * B ? w_first : l.L - 3 * B;
   const int ctas = (l.L - p_first + 127) / 128;
-  GCCNMF_LAUNCH(h, rt_ola_emit_kernel, ctas + 1, 128, 0, stream, l.dev, l.frames, N, cfg->hop_size, nT, B, l.L, p_first, l.out_ring, out_block, in_block,
-                l.in_ring, l.gccphat, cfg->num_tdoas, l.hist, cfg->history_length);
+  GCCNMF_LAUNCH(h, rt_ola_emit_kernel, dim3(ctas + 1, S), 128, 0, stream, l.dev, l.stride, l.frames, N, cfg->hop_size, nT, B, l.L, p_first, l.out_ring,
+                out_blocks, in_blocks, l.in_ring, l.gccphat, cfg->num_tdoas, l.hist, cfg->history_length);
   return GCCNMF_OK;
 }
 
-// One block as a CUDA graph: [H2D of in_host ->] the kernels of gccnmf_rt_process_block [-> D2H to out_host].  in_block / out_block
-// are device staging buffers (2, B); in_host / out_host pinned host buffers or NULL.  *graph_exec is a cudaGraphExec_t.
-int gccnmf_rt_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* state, size_t state_bytes, float* in_block, float* out_block,
-                           const float* in_host, float* out_host, void** graph_exec, void* stream) {
-  GCCNMF_ENTER(h);
+int rt_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, void* state, size_t state_bytes, const float* windowed, float* out,
+                      const double* forced_atom_mask, void* stream) {
+  RT_CARVE_OR_FAIL(l, S);
+  GCCNMF_REQUIRE(h, windowed && out, "rt_process_frames: NULL pointer");
+  if (int st = rt_enqueue_core(h, cfg, l, windowed, nullptr, out, forced_atom_mask, 0, stream)) return st;
+  GCCNMF_LAUNCH(h, rt_localize_kernel, S, 128, 0, stream, l.dev, l.stride, l.gccphat, cfg->num_tdoas, cfg->windows_per_block, l.hist, cfg->history_length);
+  return GCCNMF_OK;
+}
+
+int rt_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, void* state, size_t state_bytes, float* in_blocks, float* out_blocks,
+                    const float* in_host, float* out_host, void** graph_exec, void* stream) {
   GCCNMF_REQUIRE(h, graph_exec != nullptr && stream != nullptr, "rt_graph_create: needs a non-default stream and an output slot");
   *graph_exec = nullptr;
-  if (int st = rt_check(h, cfg)) return st;
+  RT_CARVE_OR_FAIL(l, S);
+  GCCNMF_REQUIRE(h, in_blocks && out_blocks, "rt_graph_create: NULL pointer");
   cudaStream_t s = (cudaStream_t)stream;
-  const size_t block_bytes = (size_t)2 * cfg->block_size * sizeof(float);
+  const size_t block_bytes = (size_t)S * 2 * cfg->block_size * sizeof(float);
   GCCNMF_CHECK_CUDA(h, cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
   int st = GCCNMF_OK;
-  if (in_host && cudaMemcpyAsync(in_block, in_host, block_bytes, cudaMemcpyHostToDevice, s) != cudaSuccess) st = GCCNMF_ERR_CUDA;
-  if (st == GCCNMF_OK) st = gccnmf_rt_process_block(h, cfg, state, state_bytes, in_block, out_block, nullptr, stream);
-  if (st == GCCNMF_OK && out_host && cudaMemcpyAsync(out_host, out_block, block_bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess) st = GCCNMF_ERR_CUDA;
+  if (in_host && cudaMemcpyAsync(in_blocks, in_host, block_bytes, cudaMemcpyHostToDevice, s) != cudaSuccess) st = GCCNMF_ERR_CUDA;
+  if (st == GCCNMF_OK) st = rt_process_block(h, cfg, S, state, state_bytes, in_blocks, out_blocks, nullptr, stream);
+  if (st == GCCNMF_OK && out_host && cudaMemcpyAsync(out_host, out_blocks, block_bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess) st = GCCNMF_ERR_CUDA;
   cudaGraph_t graph = nullptr;
   const cudaError_t end = cudaStreamEndCapture(s, &graph);
   if (st != GCCNMF_OK || end != cudaSuccess) {
@@ -646,6 +949,89 @@ int gccnmf_rt_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* 
   if (inst != cudaSuccess) return gccnmf_fail(h, GCCNMF_ERR_CUDA, "rt_graph_create: cudaGraphInstantiate failed: %s", cudaGetErrorString(inst));
   *graph_exec = exec;
   return GCCNMF_OK;
+}
+
+int rt_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, void* state, size_t state_bytes, int slot, int what, void* dst, void* stream) {
+  RT_CARVE_OR_FAIL(l, S);
+  GCCNMF_REQUIRE(h, dst != nullptr, "rt_export: NULL destination");
+  GCCNMF_REQUIRE(h, slot >= 0 && slot < S, "rt_export: slot %d outside [0, %d)", slot, S);
+  const size_t nT = cfg->windows_per_block, K = cfg->num_atoms, D = cfg->num_tdoas, F = l.F, st = l.stride;
+  const void* src = nullptr;
+  size_t bytes = 0;
+  switch (what) {
+    case 0: src = rt_slot(l.gccphat, slot, st); bytes = D * nT * sizeof(float); break;
+    case 1: src = &rt_slot(l.dev, slot, st)->target; bytes = sizeof(float); break;
+    case 2: src = rt_slot(l.hmask, slot, st); bytes = K * nT * sizeof(double); break;
+    case 3: src = rt_slot(l.X, slot, st); bytes = 2 * F * nT * sizeof(float2); break;
+    case 4: src = rt_slot(l.Y, slot, st); bytes = 2 * F * nT * sizeof(float2); break;
+    case 5: src = rt_slot(l.argmax, slot, st); bytes = K * nT * sizeof(int32_t); break;
+    case 6: src = rt_slot(l.H, slot, st); bytes = K * 2 * nT * sizeof(float); break;
+    case 7: src = rt_slot(l.hist, slot, st); bytes = D * (size_t)cfg->history_length * sizeof(double); break;
+    case 8: src = &rt_slot(l.dev, slot, st)->hist_index; bytes = sizeof(int); break;
+    default: return gccnmf_fail(h, GCCNMF_ERR_INVALID_ARGUMENT, "rt_export: unknown item %d", what);
+  }
+  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, (cudaStream_t)stream));
+  return GCCNMF_OK;
+}
+
+int rt_check_range(gccnmf_handle* h, int S, int first, int count) {
+  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < S && count <= S - first, "rtm: slots [%d, %d + %d) outside [0, %d)", first, first, count, S);
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+// ---------------------------------------------------------------------------------------------- single stream (S = 1)
+size_t gccnmf_rt_state_bytes(const gccnmf_rt_config* cfg) {
+  if (!cfg || cfg->window_size < 2 || cfg->block_size < 1 || cfg->windows_per_block < 1 || cfg->num_atoms < 1 || cfg->num_tdoas < 1 ||
+      cfg->history_length < 1)
+    return 0;
+  return rt_carve(*cfg, 1, nullptr, 0).bytes;
+}
+
+// W (F, K) f32, E (F, D) complex64 (expJOmegaTau, gccNMFProcessor.py:248), windows (N) f32, H0 (K, 2) f32 or NULL (all device pointers).
+int gccnmf_rt_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, const float* W, const float* E, const float* analysis_window,
+                   const float* synthesis_window, const float* H0, void* state, size_t state_bytes, void* stream) {
+  GCCNMF_ENTER(h);
+  return rt_init(h, cfg, 1, W, E, analysis_window, synthesis_window, H0, state, state_bytes, stream);
+}
+
+// setTargetTDOARange (:272-276) + the settable attributes (:136-151).  set_target = 0 leaves the target TDOA index alone (it is
+// loop-carried device state when localisation is on).
+int gccnmf_rt_set_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* state, size_t state_bytes, float target_index, int set_target,
+                         float epsilon, float beta, float noise_floor, int mode, int separation_enabled, int localization_enabled,
+                         int localization_window, void* stream) {
+  GCCNMF_ENTER(h);
+  RT_CARVE_OR_FAIL(l, 1);
+  GCCNMF_REQUIRE(h, mode == 0 || mode == 1, "rt_set_params: mode must be 0 (boxcar) or 1 (window)");
+  const gccnmf_rtm_slot_params p{target_index, set_target, epsilon, beta, noise_floor, mode, separation_enabled, localization_enabled,
+                                 localization_window, 1};
+  return rt_enqueue_params(h, l, 0, 1, &p, 0, stream);
+}
+
+// GCCNMFProcessor.processFrames (:201-231): windowed (2, N, nT) f32 -> out (2, N, nT) f32, both on the device.
+int gccnmf_rt_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* state, size_t state_bytes, const float* windowed, float* out,
+                             const double* forced_atom_mask, void* stream) {
+  GCCNMF_ENTER(h);
+  return rt_process_frames(h, cfg, 1, state, state_bytes, windowed, out, forced_atom_mask, stream);
+}
+
+// OverlapAddProcessor.processFrames(GCCNMFProcessor.processFrames) (utils.py:99-116 around gccNMFProcessor.py:201-231):
+// in_block (2, B) f32 -> out_block (2, B) f32 (the block emitted is the one pushed in two calls earlier).
+int gccnmf_rt_process_block(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* state, size_t state_bytes, const float* in_block, float* out_block,
+                            const double* forced_atom_mask, void* stream) {
+  GCCNMF_ENTER(h);
+  return rt_process_block(h, cfg, 1, state, state_bytes, in_block, out_block, forced_atom_mask, stream);
+}
+
+// One block as a CUDA graph: [H2D of in_host ->] the kernels of gccnmf_rt_process_block [-> D2H to out_host].  in_block / out_block
+// are device staging buffers (2, B); in_host / out_host pinned host buffers or NULL.  *graph_exec is a cudaGraphExec_t.
+int gccnmf_rt_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* state, size_t state_bytes, float* in_block, float* out_block,
+                           const float* in_host, float* out_host, void** graph_exec, void* stream) {
+  GCCNMF_ENTER(h);
+  return rt_graph_create(h, cfg, 1, state, state_bytes, in_block, out_block, in_host, out_host, graph_exec, stream);
 }
 
 int gccnmf_rt_graph_launch(gccnmf_handle* h, void* graph_exec, void* stream) {
@@ -668,25 +1054,62 @@ int gccnmf_rt_graph_destroy(gccnmf_handle* h, void* graph_exec) {
 //   7 GCC-PHAT history ring (D, history_length) f64 followed by nothing (its write index is item 8)   8 history write index (1) i32
 int gccnmf_rt_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* state, size_t state_bytes, int what, void* dst, void* stream) {
   GCCNMF_ENTER(h);
-  RT_CARVE_OR_FAIL(l);
-  GCCNMF_REQUIRE(h, dst != nullptr, "rt_export: NULL destination");
-  const size_t nT = cfg->windows_per_block, K = cfg->num_atoms, D = cfg->num_tdoas, F = l.F;
-  const void* src = nullptr;
-  size_t bytes = 0;
-  switch (what) {
-    case 0: src = l.gccphat; bytes = D * nT * sizeof(float); break;
-    case 1: src = &l.dev->target; bytes = sizeof(float); break;
-    case 2: src = l.hmask; bytes = K * nT * sizeof(double); break;
-    case 3: src = l.X; bytes = 2 * F * nT * sizeof(float2); break;
-    case 4: src = l.Y; bytes = 2 * F * nT * sizeof(float2); break;
-    case 5: src = l.argmax; bytes = K * nT * sizeof(int32_t); break;
-    case 6: src = l.H; bytes = K * 2 * nT * sizeof(float); break;
-    case 7: src = l.hist; bytes = D * (size_t)cfg->history_length * sizeof(double); break;
-    case 8: src = &l.dev->hist_index; bytes = sizeof(int); break;
-    default: return gccnmf_fail(h, GCCNMF_ERR_INVALID_ARGUMENT, "rt_export: unknown item %d", what);
-  }
-  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, (cudaStream_t)stream));
-  return GCCNMF_OK;
+  return rt_export(h, cfg, 1, state, state_bytes, 0, what, dst, stream);
+}
+
+// ---------------------------------------------------------------------------------------------- S streams (slots) in one state
+size_t gccnmf_rtm_state_bytes(const gccnmf_rt_config* cfg, int num_streams) {
+  if (rt_check(nullptr, cfg, num_streams) != 0) return 0;
+  return rt_carve(*cfg, num_streams, nullptr, 0).bytes;
+}
+
+int gccnmf_rtm_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, const float* W, const float* E, const float* analysis_window,
+                    const float* synthesis_window, const float* H0, void* state, size_t state_bytes, void* stream) {
+  GCCNMF_ENTER(h);
+  return rt_init(h, cfg, num_streams, W, E, analysis_window, synthesis_window, H0, state, state_bytes, stream);
+}
+
+int gccnmf_rtm_reset_slots(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state, size_t state_bytes, int first_slot, int count,
+                           void* stream) {
+  GCCNMF_ENTER(h);
+  RT_CARVE_OR_FAIL(l, num_streams);
+  if (int st = rt_check_range(h, num_streams, first_slot, count)) return st;
+  return rt_enqueue_reset(h, l, first_slot, count, stream);
+}
+
+int gccnmf_rtm_set_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state, size_t state_bytes, int first_slot, int count,
+                          const gccnmf_rtm_slot_params* params, void* stream) {
+  GCCNMF_ENTER(h);
+  RT_CARVE_OR_FAIL(l, num_streams);
+  if (int st = rt_check_range(h, num_streams, first_slot, count)) return st;
+  GCCNMF_REQUIRE(h, params != nullptr, "rtm_set_params: NULL parameters");
+  for (int i = 0; i < count; ++i)
+    GCCNMF_REQUIRE(h, params[i].mode == 0 || params[i].mode == 1, "rtm_set_params: slot %d: mode must be 0 (boxcar) or 1 (window)", first_slot + i);
+  return rt_enqueue_params(h, l, first_slot, count, params, 1, stream);
+}
+
+int gccnmf_rtm_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state, size_t state_bytes, const float* windowed,
+                              float* out, const double* forced_atom_mask, void* stream) {
+  GCCNMF_ENTER(h);
+  return rt_process_frames(h, cfg, num_streams, state, state_bytes, windowed, out, forced_atom_mask, stream);
+}
+
+int gccnmf_rtm_process_block(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state, size_t state_bytes, const float* in_blocks,
+                             float* out_blocks, const double* forced_atom_mask, void* stream) {
+  GCCNMF_ENTER(h);
+  return rt_process_block(h, cfg, num_streams, state, state_bytes, in_blocks, out_blocks, forced_atom_mask, stream);
+}
+
+int gccnmf_rtm_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state, size_t state_bytes, float* in_blocks,
+                            float* out_blocks, const float* in_host, float* out_host, void** graph_exec, void* stream) {
+  GCCNMF_ENTER(h);
+  return rt_graph_create(h, cfg, num_streams, state, state_bytes, in_blocks, out_blocks, in_host, out_host, graph_exec, stream);
+}
+
+int gccnmf_rtm_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state, size_t state_bytes, int slot, int what, void* dst,
+                      void* stream) {
+  GCCNMF_ENTER(h);
+  return rt_export(h, cfg, num_streams, state, state_bytes, slot, what, dst, stream);
 }
 
 }  // extern "C"

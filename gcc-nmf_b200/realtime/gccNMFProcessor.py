@@ -70,12 +70,7 @@ class GCCNMFProcessor(object):
     def buildFunctions(self, hopSize=None, blockSize=None):
         """Device constants that the reference bakes into its Theano functions (:241-248) and the device-resident state.
         hopSize / blockSize only matter for the ring entry (`processBlock`); `processFrames` gets its frames cut by the caller."""
-        self.W = np.ascontiguousarray(self.dictionariesW[self.dictionaryType][self.dictionarySize], dtype=np.float32)
-        self.numFrequencies, self.numAtom = self.W.shape
-        self.frequenciesInHz = np.linspace(0, self.sampleRate / 2, self.numFrequencies).astype(np.float32)
-        self.maxTDOA = self.microphoneSeparationInMetres / fn.SPEED_OF_SOUND_IN_METRES_PER_SECOND
-        self.hypothesisTDOAs = np.linspace(-self.maxTDOA, self.maxTDOA, self.numTDOAs).astype(np.float32)
-        self.expJOmegaTau = np.exp(np.outer(self.frequenciesInHz, -(2j * np.pi) * self.hypothesisTDOAs)).astype(np.complex64)
+        self.buildConstants()
         historyLength = self.gccPHATHistory.size() if self.gccPHATHistory else 128
         if self.engine is not None:
             self.engine.close()
@@ -91,6 +86,23 @@ class GCCNMFProcessor(object):
         self._target_dirty = True
 
     buildTheanoFunctions = buildFunctions      # the reference's name (:238)
+
+    def buildConstants(self):
+        """The dictionary and the steering vectors expJOmegaTau (:241-248), host-side, without building an engine."""
+        self.W = np.ascontiguousarray(self.dictionariesW[self.dictionaryType][self.dictionarySize], dtype=np.float32)
+        self.numFrequencies, self.numAtom = self.W.shape
+        self.frequenciesInHz = np.linspace(0, self.sampleRate / 2, self.numFrequencies).astype(np.float32)
+        self.maxTDOA = self.microphoneSeparationInMetres / fn.SPEED_OF_SOUND_IN_METRES_PER_SECOND
+        self.hypothesisTDOAs = np.linspace(-self.maxTDOA, self.maxTDOA, self.numTDOAs).astype(np.float32)
+        self.expJOmegaTau = np.exp(np.outer(self.frequenciesInHz, -(2j * np.pi) * self.hypothesisTDOAs)).astype(np.complex64)
+
+    def slotParams(self):
+        """The parameters `processBlock` would send to its engine, as keyword arguments of MultiStreamRealtimeEngine.set_params."""
+        localize = bool(self.tdoaHistory) and bool(self.gccPHATHistory) and bool(self.localizationEnabled)     # :216-222
+        return dict(targetTDOAIndex=float(self.targetTDOAIndex), epsilon=float(self.targetTDOAEpsilon), beta=float(self.targetTDOABeta),
+                    noiseFloor=float(self.targetTDOANoiseFloor), mode=0 if self.targetMode == TARGET_MODE_BOXCAR else 1,
+                    separationEnabled=bool(self.separationEnabled), localizationEnabled=localize,
+                    localizationWindowSize=int(self.localizationWindowSize))
 
     def setTargetTDOARange(self, targetTDOAIndex, targetTDOAEpsilon, targetTDOABeta, targetTDOANoiseFloor):
         """:272-276."""

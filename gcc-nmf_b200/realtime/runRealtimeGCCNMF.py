@@ -120,29 +120,79 @@ class RealtimeGCCNMFNoGUI(object):
         t = np.asarray(self.processingTimes)
         return (float(t.min()), float(t.max()), float(t.mean())) if t.size else (0.0, 0.0, 0.0)
 
+    def _readSamples(self, audioPath):
+        """int16 (or float) stereo wav -> (numChannels, n) float32 (audioProcessor.py:112-116)."""
+        from scipy.io import wavfile
+        sampleRate, data = wavfile.read(audioPath)
+        if sampleRate != self.params.sampleRate:
+            raise ValueError('sample rate of %s is %d, configured %d' % (audioPath, sampleRate, self.params.sampleRate))
+        return pcm2float(data).T if data.dtype.kind in 'iu' else np.asarray(data, np.float32).T
+
+    def _writeOutput(self, out, numSamples, outputPath, alignOutput):
+        from scipy.io import wavfile
+        if alignOutput:
+            out = out[:, self.latencySamples:self.latencySamples + numSamples]
+        if outputPath is not None:
+            wavfile.write(outputPath, self.params.sampleRate, float2pcm(np.ascontiguousarray(out.T)))
+        return out
+
     def run(self, outputPath=None, alignOutput=True):
         """Reads params.audioPath (int16 stereo wav), enhances it block by block and, when `outputPath` is given, writes
         the int16 result.  alignOutput drops the two-block latency so that output sample i corresponds to input sample i."""
-        from scipy.io import wavfile
-        p = self.params
-        sampleRate, data = wavfile.read(p.audioPath)
-        if sampleRate != p.sampleRate:
-            raise ValueError('sample rate of %s is %d, configured %d' % (p.audioPath, sampleRate, p.sampleRate))
-        samples = pcm2float(data).T if data.dtype.kind in 'iu' else np.asarray(data, np.float32).T
+        samples = self._readSamples(self.params.audioPath)
         out = self.processSamples(samples, flush=True)
-        if alignOutput:
-            out = out[:, self.latencySamples:self.latencySamples + samples.shape[1]]
         logging.info('Processing times (min/max/avg): %f, %f, %f' % self.processingTimeStats())
-        if outputPath is not None:
-            wavfile.write(outputPath, sampleRate, float2pcm(np.ascontiguousarray(out.T)))
-        return out
+        return self._writeOutput(out, samples.shape[1], outputPath, alignOutput)
+
+    def runMany(self, audioPaths, outputPaths=None, alignOutput=True):
+        """Several wav files enhanced concurrently, each in its own slot of ONE MultiStreamRealtimeEngine: per block, one graph
+        launch for all files.  Each file gets exactly what `run` gives it alone (same parameters, same kernels, bit for bit);
+        once a file has had its two flush blocks its slot is deactivated.  Returns the output arrays in the order of
+        `audioPaths` and writes them to `outputPaths` when given.  `processingTimes` gets one entry per block of the longest file."""
+        from .multistream import MultiStreamRealtimeEngine
+        g = self.gccNMFProcessor
+        if g is None:
+            raise ValueError('runMany runs the built-in GCCNMFProcessor; this runner was given another processFramesFunction')
+        if outputPaths is not None and len(outputPaths) != len(audioPaths):
+            raise ValueError('%d input paths, %d output paths' % (len(audioPaths), len(outputPaths)))
+        p = self.params
+        B, S = p.blockSize, len(audioPaths)
+        signals = [self._readSamples(path) for path in audioPaths]
+        totals = [(x.shape[1] + B - 1) // B + 2 for x in signals]          # whole blocks + two flush blocks, as processSamples
+        g.buildConstants()
+        engine = MultiStreamRealtimeEngine(g.W, g.expJOmegaTau, g.windowFunction[:, 0], g.synthesisWindowFunction[:, 0], p.hopSize, B,
+                                           p.windowsPerBlock, S, historyLength=g.gccPHATHistory.size() if g.gccPHATHistory else 128,
+                                           numInferenceIterations=g.coefficientInferenceIterations, device=g.device)
+        try:
+            engine.set_params(range(S), **g.slotParams())
+            outs = [np.empty((p.numChannels, t * B), np.float32) for t in totals]
+            blocks = np.zeros((S, p.numChannels, B), np.float32)
+            for b in range(max(totals)):
+                done = [s for s in range(S) if totals[s] == b]
+                if done:
+                    engine.set_active(done, False)
+                for s, x in enumerate(signals):
+                    chunk = x[:, b * B:(b + 1) * B]
+                    blocks[s] = 0
+                    blocks[s, :, :chunk.shape[1]] = chunk
+                startTime = time.time()
+                y = engine.process_blocks(blocks)
+                self.processingTimes.append(time.time() - startTime)
+                for s in range(S):
+                    if b < totals[s]:
+                        outs[s][:, b * B:(b + 1) * B] = y[s]
+        finally:
+            engine.close()
+        logging.info('Processing times (min/max/avg): %f, %f, %f' % self.processingTimeStats())
+        return [self._writeOutput(outs[s], signals[s].shape[1], outputPaths[s] if outputPaths is not None else None, alignOutput)
+                for s in range(S)]
 
 
 def parseArguments(argv=None):
     """config.py:122-127 plus the output path and the dictionary directory (the reference takes DATA_DIR from defs.py)."""
     parser = argparse.ArgumentParser(description='Headless real-time GCC-NMF speech enhancement (H100)')
-    parser.add_argument('-i', '--input', help='input wav file path', required=True)
-    parser.add_argument('-o', '--output', help='output wav file path', required=True)
+    parser.add_argument('-i', '--input', nargs='+', help='input wav file path(s); several are enhanced concurrently in one engine', required=True)
+    parser.add_argument('-o', '--output', nargs='+', help='output wav file path(s), one per input', required=True)
     parser.add_argument('-d', '--data-dir', help='directory with chimeTrainSet.npy and / or pretrainedW/', required=True)
     parser.add_argument('--dictionary-size', type=int, default=DEFAULT_PARAMS['dictionarySize'])
     return parser.parse_args(argv)
@@ -151,5 +201,11 @@ def parseArguments(argv=None):
 if __name__ == '__main__':
     logging.getLogger().setLevel(logging.INFO)
     args = parseArguments()
-    RealtimeGCCNMFNoGUI(args.input, dataDir=args.data_dir, dictionarySize=args.dictionary_size,
-                        dictionarySizes=[args.dictionary_size]).run(args.output)
+    if len(args.input) != len(args.output):
+        raise SystemExit('%d input paths, %d output paths' % (len(args.input), len(args.output)))
+    runner = RealtimeGCCNMFNoGUI(args.input[0], dataDir=args.data_dir, dictionarySize=args.dictionary_size,
+                                 dictionarySizes=[args.dictionary_size])
+    if len(args.input) == 1:
+        runner.run(args.output[0])
+    else:
+        runner.runMany(args.input, args.output)

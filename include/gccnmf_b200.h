@@ -367,6 +367,48 @@ GCCNMF_API int gccnmf_rt_graph_destroy(gccnmf_handle* h, void* graph_exec);
 GCCNMF_API int gccnmf_rt_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* state, size_t state_bytes, int what,
                      void* dst, void* stream);
 
+/* ---- the real-time block path for S independent streams (slots) in one state buffer ----------------------
+ * The slots share the configuration, W, E, the windows and H0; each owns its rings, block counter, GCC-PHAT history, target
+ * TDOA index and parameters, plus an `active` flag.  One block of every slot is the same five kernels (+ two per inference
+ * iteration) as one stream, in one launch each, and one CUDA graph launch when captured.  Slot s computes bit for bit what a
+ * single-stream state (gccnmf_rt_*, the S = 1 case of the same kernels) fed the same blocks and parameters computes.  An
+ * inactive slot is skipped: its output slice is zeros, its input slice is ignored, its state stays as it was.  Buffers of all
+ * slots are slot-major: in / out blocks (S, 2, B), windowed frames (S, 2, N, nT), forced atom masks (S, K, nT) f64.
+ * Out-of-range num_streams (1 .. 4096), slot ranges and too small state buffers fail before anything is enqueued. */
+typedef struct gccnmf_rtm_slot_params {
+  float target_index; int set_target;      /* set_target = 0 keeps the device-resident target TDOA index             */
+  float epsilon, beta, noise_floor;
+  int mode;                                /* 0 boxcar, 1 window (:262-265)                                           */
+  int separation_enabled, localization_enabled, localization_window;
+  int active;                              /* 0: the slot is skipped by every block until re-activated                 */
+} gccnmf_rtm_slot_params;
+/* Host only; 0 for num_streams < 1 or an invalid configuration.  Grows linearly in num_streams. */
+GCCNMF_API size_t gccnmf_rtm_state_bytes(const gccnmf_rt_config* cfg, int num_streams);
+/* As gccnmf_rt_init, for every slot: all slots active, with the defaults of gccNMFProcessor.py:190-199. */
+GCCNMF_API int gccnmf_rtm_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, const float* W, const float* E,
+                    const float* analysis_window, const float* synthesis_window, const float* H0, void* state,
+                    size_t state_bytes, void* stream);
+/* Slots [first_slot, first_slot + count) go back to what gccnmf_rtm_init leaves (zeroed rings, history and counters, default
+ * parameters, active); the other slots are untouched.  Stream-ordered: may sit between two launches of an instantiated graph. */
+GCCNMF_API int gccnmf_rtm_reset_slots(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state,
+                           size_t state_bytes, int first_slot, int count, void* stream);
+/* params: host array of `count` entries, consumed before the call returns. */
+GCCNMF_API int gccnmf_rtm_set_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state,
+                          size_t state_bytes, int first_slot, int count, const gccnmf_rtm_slot_params* params, void* stream);
+GCCNMF_API int gccnmf_rtm_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state,
+                              size_t state_bytes, const float* windowed, float* out, const double* forced_atom_mask,
+                              void* stream);
+GCCNMF_API int gccnmf_rtm_process_block(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state,
+                             size_t state_bytes, const float* in_blocks, float* out_blocks, const double* forced_atom_mask,
+                             void* stream);
+/* Launch / destroy with gccnmf_rt_graph_launch / gccnmf_rt_graph_destroy. */
+GCCNMF_API int gccnmf_rtm_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state,
+                            size_t state_bytes, float* in_blocks, float* out_blocks, const float* in_host, float* out_host,
+                            void** graph_exec, void* stream);
+/* Item `what` of slot `slot`, as gccnmf_rt_export. */
+GCCNMF_API int gccnmf_rtm_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state, size_t state_bytes,
+                      int slot, int what, void* dst, void* stream);
+
 /*
  * The building block the KL-NMF loop runs on (klnmf_tma.cu): the same 3-product contraction, TMA-fed, over operands
  * that are pre-split into bf16 hi/lo planes and kept in ONE orientation each; an operand contracted over its
