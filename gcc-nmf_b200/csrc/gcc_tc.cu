@@ -441,16 +441,24 @@ __global__ void abs_colsum_kernel(const float* __restrict__ W, int F, int K, flo
 }
 
 // Candidate refinement (the default): the GEMM epilogue leaves, per flagged (atom, frame), the set of TDOAs whose value lies within
-// the margin of the best -- 2 or 3 of D as a rule -- and only those are recomputed in float64.  One warp per pair; lanes stride
-// the bins over TRANSPOSED copies of the coherence (T, F), W (K, F) and E (D, F), so every load of a warp is one contiguous row
-// segment (the first version gathered: 700 MB of 32-byte sectors at the headline shape); each lane accumulates its bins in order
-// (one fma per bin, as the float64 kernel), then a shuffle tree adds the 32 partial sums.
+// the margin of the best -- 2 or 3 of D as a rule -- and only those are recomputed in float64.  One warp per pair.  The lanes load
+// 32 consecutive bins of TRANSPOSED copies of the coherence (T, F), W (K, F) and E (D, F), so every load of a warp is one contiguous
+// row segment (the first version gathered: 700 MB of 32-byte sectors at the headline shape), form Re(C E) of their bin for each
+// candidate and stage it in shared memory; lane j then adds the 32 bins into candidate j's sum, one fma per bin in bin order.  So
+// every candidate is ONE fma chain over f = 0 .. F - 1, the float64 kernel's summation order (tdoa_gccnmf_kernel, gcc.cu): values
+// that differ only at float64 rounding level -- the two central TDOAs of mono input -- are ordered exactly as it orders them.
+// (Lane-strided partial sums added by a shuffle tree, the previous form, round differently and flipped such decisions.)  The next
+// 32 bins are loaded while the chains run.
 constexpr int kRefineGroup = 8;        // candidates per pass over the bins
 __global__ void __launch_bounds__(256)
 refine_candidates_kernel(const int2* __restrict__ list, const uint4* __restrict__ candidates, const int* __restrict__ count, int capacity,
                          const float2* __restrict__ cohT, const float* __restrict__ WT, const double2* __restrict__ ET, int F, int64_t Fp, int D,
                          int T, int32_t* __restrict__ argmax) {
-  const int lane = threadIdx.x & 31;
+  __shared__ double re_s[8][kRefineGroup][33];     // per warp: Re(C E) of 32 bins per candidate (row padded: conflict-free reads)
+  __shared__ double w_s[8][32];                    // per warp: W of the 32 bins
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  double (*re)[33] = re_s[wib];
+  double* wv = w_s[wib];
   const int warps = gridDim.x * (blockDim.x >> 5);
   const int n = min(*count, capacity);
   for (int p = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); p < n; p += warps) {
@@ -471,24 +479,43 @@ refine_candidates_kernel(const int2* __restrict__ list, const uint4* __restrict_
         ds[nd++] = word * 32 + b;
       }
       if (nd == 0) break;
-      double acc[kRefineGroup];
-#pragma unroll
-      for (int j = 0; j < kRefineGroup; ++j) acc[j] = 0.0;
-      for (int f = lane; f < F; f += 32) {
+      double g[kRefineGroup], w = 0.0;                    // this lane's bin of the chunk: Re(C E) per candidate, W
+      auto load = [&](int f0) {
+        const int f = f0 + lane;
+        if (f >= F) return;
         const float2 c = crow[f];
-        const double w = (double)wrow[f];
+        w = (double)wrow[f];
 #pragma unroll
         for (int j = 0; j < kRefineGroup; ++j)
           if (j < nd) {
             const double2 e = ET[(int64_t)ds[j] * Fp + f];
-            acc[j] = fma((double)c.x * e.x - (double)c.y * e.y, w, acc[j]);
+            g[j] = (double)c.x * e.x - (double)c.y * e.y;
           }
+      };
+      load(0);
+      double acc = 0.0;                                   // lane j < nd: candidate ds[j]
+      for (int f0 = 0; f0 < F; f0 += 32) {
+#pragma unroll
+        for (int j = 0; j < kRefineGroup; ++j)
+          if (j < nd) re[j][lane] = g[j];
+        wv[lane] = w;
+        __syncwarp();
+        if (f0 + 32 < F) load(f0 + 32);
+        if (lane < nd) {
+          const double* r = re[lane];
+          if (F - f0 >= 32) {
+#pragma unroll 8
+            for (int s = 0; s < 32; ++s) acc = fma(r[s], wv[s], acc);
+          } else {
+            for (int s = 0; s < F - f0; ++s) acc = fma(r[s], wv[s], acc);
+          }
+        }
+        __syncwarp();
       }
 #pragma unroll
-      for (int j = 0; j < kRefineGroup; ++j) {
+      for (int j = 0; j < kRefineGroup; ++j) {            // ascending TDOAs: numpy's first-maximum rule
         if (j < nd) {
-          double v = acc[j];
-          for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+          const double v = __shfl_sync(0xffffffffu, acc, j);
           if (bi < 0 || argmax_better64(v, ds[j], bv, bi)) { bv = v; bi = ds[j]; }
         }
       }
@@ -726,7 +753,8 @@ int gccnmf_tdoa_argmax(gccnmf_handle* h, const float* coherence, int F, int T, c
     GCCNMF_LAUNCH(h, refine_argmax_kernel, h->sm_count * 4, 256, 0, stream, w.list, w.count, w.capacity,
                   reinterpret_cast<const float2*>(coherence), F, T, reinterpret_cast<const double2*>(E), D, W, K, argmax);
   }
-  // more near-ties than the list holds (never seen: the list holds 1/8 of all decisions): the caller must fall back
+  // more near-ties than the list holds (at least 1/8 of all decisions): the caller must fall back to the float64 kernel.  Mono input
+  // (identical channels) gets there: the two central TDOAs of the symmetric grid tie in nearly every decision.
   if (overflow_flag) GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(overflow_flag, w.count, sizeof(int), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return GCCNMF_OK;
 }

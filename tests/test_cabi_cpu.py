@@ -42,6 +42,28 @@ def test_host_helpers(lib):
     assert lib.gccnmf_status_string(-5).decode().startswith('no CUDA device')
 
 
+def test_tdoa_argmax_host_helpers(lib):
+    """gccnmf_tdoa_argmax_workspace_bytes: 256 (the float64 kernel runs, no workspace) for every shape the tensor-core argmax does
+    not cover -- D not a power of two in [8, 128], K % 8 != 0, K < 64, F < 32, T D < 256 -- and a real workspace at the edges it
+    does; gccnmf_tdoa_argmax_refine_capacity: min(K T, max(65536, K T / 8)) decisions."""
+    ws = lib.gccnmf_tdoa_argmax_workspace_bytes
+    F, T, D, K = 513, 100, 64, 128
+    assert ws(F, T, D, K) > 2 * T * D * 520 * 2                         # the G planes alone: 2 x T D x Fp bf16
+    for edge in [(32, T, D, K), (F, 4, 64, K), (F, 32, 8, K), (F, T, 128, K), (F, T, D, 64), (F, T, D, 72)]:
+        assert ws(*edge) > 256, edge
+    for uncovered in [(F, T, 48, K), (F, T, 4, K), (F, T, 256, K), (F, T, 96, K),    # D
+                      (F, T, D, 132), (F, T, D, 1020),                                # K % 8 != 0
+                      (F, T, D, 56), (F, T, D, 8),                                    # K < 64
+                      (31, T, D, K), (1, T, D, K),                                    # F < 32
+                      (F, 3, 64, K), (F, 31, 8, K), (F, 1, 128, K)]:                  # T D < 256
+        assert ws(*uncovered) == 256, uncovered
+    assert ws(0, T, D, K) == 0 and ws(F, T, D, 0) == 0
+    cap = lib.gccnmf_tdoa_argmax_refine_capacity
+    for K, T in [(1, 1), (64, 100), (128, 500), (128, 512), (128, 1024), (1024, 1872), (4096, 37494)]:
+        assert cap(K, T) == min(K * T, max(65536, K * T // 8)), (K, T)
+    assert cap(0, 10) == 0 and cap(10, 0) == 0
+
+
 def test_no_cpu_fallback():
     import torch
     if torch.cuda.is_available():
