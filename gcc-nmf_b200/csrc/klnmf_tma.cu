@@ -704,22 +704,25 @@ double kstep_cycles(int bn, bool dual) { return (dual && 2 * bn <= 256) ? mma_cy
 double epilogue_cycles(int bn, double per_column) { return per_column * bn; }
 constexpr double kWaveCycles = 8000.0;
 
-int m_tiles_of(int M, bool simt_tail) {
+// m tiles of a launch of `bn`-column tiles, by the launch's own rule (launch_plane_gemm): SIMT tail rows only when the m tiles of
+// an n tile can share its columns, at most 128 each (F = 129 .. 136 with 256-column tiles runs two m tiles, not one).
+int m_tiles_of(int M, bool simt_tail, int bn) {
   const int tail = M % tgemm::kBM;
-  return (simt_tail && tail != 0 && tail <= kTailRowsMax && M > tgemm::kBM) ? M / tgemm::kBM : (M + tgemm::kBM - 1) / tgemm::kBM;
+  return (simt_tail && tail != 0 && tail <= kTailRowsMax && M > tgemm::kBM && (M / tgemm::kBM) * 128 >= bn) ? M / tgemm::kBM
+                                                                                                           : (M + tgemm::kBM - 1) / tgemm::kBM;
 }
 
 struct TilePlan { int bn, splits; };
 
 // Picks the tile width (and k-split count when `allow_split`) with the smallest estimated time.
-TilePlan plan_tiles(int sm_count, int m_tiles, int N, int Kc, bool allow_split, const int* widths, int n_widths, double epi_per_column,
+TilePlan plan_tiles(int sm_count, int M, bool simt_tail, int N, int Kc, bool allow_split, const int* widths, int n_widths, double epi_per_column,
                     bool dual = false) {
   TilePlan best{128, 1};
   double best_cost = 1e300;
   const int total_kb = (Kc + kKB - 1) / kKB;
   for (int i = 0; i < n_widths; ++i) {
     const int bn = widths[i];
-    const int tiles = m_tiles * ((N + bn - 1) / bn);
+    const int tiles = m_tiles_of(M, simt_tail, bn) * ((N + bn - 1) / bn);
     int splits = 1;
     if (allow_split) splits = std::max(1, std::min(std::min(kMaxSplits, sm_count / std::max(1, tiles)), total_kb / 4));
     const int kb = (total_kb + splits - 1) / splits;
@@ -742,9 +745,9 @@ struct Plan {
 
 Plan make_plan(const gccnmf_handle* h, int F, int T2, int K) {
   Plan p;
-  p.bn_wh = h->wh_tile ? h->wh_tile : plan_tiles(h->sm_count, m_tiles_of(F, true), T2, K, false, kWidthsWH, 4, kEpiRatioCycles, true).bn;
-  p.bn_h = plan_tiles(h->sm_count, m_tiles_of(K, false), T2, F, false, kWidthsAll, 5, kEpiUpdateHCycles).bn;
-  p.w = plan_tiles(h->sm_count, m_tiles_of(K, false), F, T2, true, kWidthsAll, 5, kEpiStoreCycles);
+  p.bn_wh = h->wh_tile ? h->wh_tile : plan_tiles(h->sm_count, F, true, T2, K, false, kWidthsWH, 4, kEpiRatioCycles, true).bn;
+  p.bn_h = plan_tiles(h->sm_count, K, false, T2, F, false, kWidthsAll, 5, kEpiUpdateHCycles).bn;
+  p.w = plan_tiles(h->sm_count, K, false, F, T2, true, kWidthsAll, 5, kEpiStoreCycles);
   p.rowsum_slots = (T2 + p.bn_h - 1) / p.bn_h;
   return p;
 }
@@ -804,7 +807,7 @@ bool wh_split2(gccnmf_handle* h, int F, int T2, int K) {
   if (!h->wh_split2 || K < 128) return false;
   int resident = 0;
   if (plane_gemm_z_clusters<false, false, EpiRatioPlanes>(h, kWhSplitTile, 2, &resident)) return false;
-  const int tiles = m_tiles_of(F, true) * ((T2 + kWhSplitTile - 1) / kWhSplitTile);
+  const int tiles = m_tiles_of(F, true, kWhSplitTile) * ((T2 + kWhSplitTile - 1) / kWhSplitTile);
   return resident >= tiles && 2 * tiles <= h->sm_count;
 }
 int launch_wh(gccnmf_handle* h, const Plan& p, const Operand& Wk, const Operand& HTk, int F, int T2, int K, const EpiRatioPlanes& e, void* stream) {
@@ -820,7 +823,7 @@ bool w_cluster_reduce(gccnmf_handle* h, const Plan& p, int F, int K) {
   if (!h->w_cluster_reduce || p.w.splits < 2 || p.w.splits > 8) return false;
   int resident = 0;
   if (plane_gemm_z_clusters<true, true, EpiStoreT>(h, p.w.bn, p.w.splits, &resident)) return false;
-  const int tiles = m_tiles_of(K, false) * ((F + p.w.bn - 1) / p.w.bn);
+  const int tiles = m_tiles_of(K, false, p.w.bn) * ((F + p.w.bn - 1) / p.w.bn);
   return resident >= tiles;
 }
 
@@ -1151,9 +1154,9 @@ int gccnmf_klnmf_tile_plan(int sm_count, int F, int T2, int K, int* out) {
   h.sm_count = sm_count;
   const Plan p = make_plan(&h, F, T2, K);
   out[0] = p.bn_wh; out[1] = p.bn_h; out[2] = p.w.bn; out[3] = p.w.splits; out[4] = p.rowsum_slots;
-  out[5] = m_tiles_of(F, true) * ((T2 + p.bn_wh - 1) / p.bn_wh);
-  out[6] = m_tiles_of(K, false) * ((T2 + p.bn_h - 1) / p.bn_h);
-  out[7] = m_tiles_of(K, false) * ((F + p.w.bn - 1) / p.w.bn) * p.w.splits;
+  out[5] = m_tiles_of(F, true, p.bn_wh) * ((T2 + p.bn_wh - 1) / p.bn_wh);
+  out[6] = m_tiles_of(K, false, p.bn_h) * ((T2 + p.bn_h - 1) / p.bn_h);
+  out[7] = m_tiles_of(K, false, p.w.bn) * ((F + p.w.bn - 1) / p.w.bn) * p.w.splits;
   return GCCNMF_OK;
 }
 

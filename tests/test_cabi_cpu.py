@@ -107,6 +107,12 @@ def test_klnmf_tile_plan_fills_the_chip(lib):
     # fewer SMs -> the planner may not use more CTAs than a wave when a single-wave choice exists
     assert lib.gccnmf_klnmf_tile_plan(132, 513, 3744, 1024, out) == 0
     assert out[7] <= 132
+    # F = 129 .. 136 (a 256-point FFT): the m tile of a 256-column W.H tile cannot share its columns among the SIMT tail rows (at
+    # most 128 each), so the launch runs two m tiles; the planner must cost and count the same CTAs
+    for F in (129, 136):
+        for T2 in range(16000, 36000, 250):
+            assert lib.gccnmf_klnmf_tile_plan(132, F, T2, 32, out) == 0
+            assert out[5] == (2 if out[0] > 128 else 1) * -(-T2 // out[0]), (F, T2, list(out))
 
 
 def test_pull_exchange_buffer_layout(lib):
