@@ -1006,6 +1006,8 @@ int gccnmf_rt_set_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* st
   GCCNMF_ENTER(h);
   RT_CARVE_OR_FAIL(l, 1);
   GCCNMF_REQUIRE(h, mode == 0 || mode == 1, "rt_set_params: mode must be 0 (boxcar) or 1 (window)");
+  // gccPHATHistory[:, -w:] (:221) takes the last w columns only for w >= 1; w = 0 would take the whole history
+  GCCNMF_REQUIRE(h, localization_window >= 1, "rt_set_params: localization_window must be >= 1 (got %d)", localization_window);
   const gccnmf_rtm_slot_params p{target_index, set_target, epsilon, beta, noise_floor, mode, separation_enabled, localization_enabled,
                                  localization_window, 1};
   return rt_enqueue_params(h, l, 0, 1, &p, 0, stream);
@@ -1083,8 +1085,11 @@ int gccnmf_rtm_set_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num
   RT_CARVE_OR_FAIL(l, num_streams);
   if (int st = rt_check_range(h, num_streams, first_slot, count)) return st;
   GCCNMF_REQUIRE(h, params != nullptr, "rtm_set_params: NULL parameters");
-  for (int i = 0; i < count; ++i)
+  for (int i = 0; i < count; ++i) {
     GCCNMF_REQUIRE(h, params[i].mode == 0 || params[i].mode == 1, "rtm_set_params: slot %d: mode must be 0 (boxcar) or 1 (window)", first_slot + i);
+    GCCNMF_REQUIRE(h, params[i].localization_window >= 1, "rtm_set_params: slot %d: localization_window must be >= 1 (got %d)", first_slot + i,
+                   params[i].localization_window);
+  }
   return rt_enqueue_params(h, l, first_slot, count, params, 1, stream);
 }
 

@@ -342,7 +342,7 @@ GCCNMF_API int gccnmf_rt_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, con
                    const float* analysis_window, const float* synthesis_window, const float* H0, void* state,
                    size_t state_bytes, void* stream);
 /* setTargetTDOARange (:272-276) and the attributes GCCNMFProcess sets (:136-151).  mode 0 boxcar / 1 window (:262-265).
- * set_target = 0 keeps the device-resident target TDOA index (it is loop-carried when localisation is enabled). */
+ * localization_window >= 1 columns (GCCNMF_ERR_INVALID_ARGUMENT otherwise).  set_target = 0 keeps the device-resident target TDOA index (it is loop-carried when localisation is enabled). */
 GCCNMF_API int gccnmf_rt_set_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* state, size_t state_bytes,
                          float target_index, int set_target, float epsilon, float beta, float noise_floor, int mode,
                          int separation_enabled, int localization_enabled, int localization_window, void* stream);
