@@ -130,6 +130,15 @@ SIGNATURES.update({
     'gccnmf_rtm_process_block': (c_int, [_H, _C, c_int, _P, c_size_t, _P, _P, _P, _S]),
     'gccnmf_rtm_graph_create': (c_int, [_H, _C, c_int, _P, c_size_t, _P, _P, _P, _P, ctypes.POINTER(c_void_p), _S]),
     'gccnmf_rtm_export': (c_int, [_H, _C, c_int, _P, c_size_t, c_int, c_int, c_void_p, _S]),
+    'gccnmf_rtsep_state_bytes': (c_size_t, [_C, c_int, c_int]),
+    'gccnmf_rtsep_init': (c_int, [_H, _C, c_int, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _S]),
+    'gccnmf_rtsep_reset_slots': (c_int, [_H, _C, c_int, c_int, _P, c_size_t, c_int, c_int, _S]),
+    'gccnmf_rtsep_set_params': (c_int, [_H, _C, c_int, c_int, _P, c_size_t, c_int, c_int, ctypes.POINTER(RtmSlotParams), _S]),
+    'gccnmf_rtsep_set_targets': (c_int, [_H, _C, c_int, c_int, _P, c_size_t, c_int, c_int, ctypes.POINTER(c_int32), _S]),
+    'gccnmf_rtsep_process_frames': (c_int, [_H, _C, c_int, c_int, _P, c_size_t, _P, _P, _S]),
+    'gccnmf_rtsep_process_block': (c_int, [_H, _C, c_int, c_int, _P, c_size_t, _P, _P, _S]),
+    'gccnmf_rtsep_graph_create': (c_int, [_H, _C, c_int, c_int, _P, c_size_t, _P, _P, _P, _P, ctypes.POINTER(c_void_p), _S]),
+    'gccnmf_rtsep_export': (c_int, [_H, _C, c_int, c_int, _P, c_size_t, c_int, c_int, c_void_p, _S]),
 })
 
 _lib = None

@@ -120,5 +120,34 @@ struct WorkspaceCarver {
   bool ok() const { return base != nullptr && used <= size; }
 };
 
+// scipy.signal.argrelmax(x) (order 1, mode 'clip': strict local maxima, never the end points), then the S largest peaks
+// (gccNMFFunctions.py:100: peakIndexes[argsort(x[peakIndexes])[-numSources:]]) in ascending index order (:113), by every thread of
+// one CTA.  x: D values in shared memory, written before the call; peak / chosen: D bytes of shared scratch.  Thread 0 writes the
+// min(S, peaks) chosen indexes to out and gets the number of peaks back (the other threads' return value is unspecified).
+__device__ inline int select_peaks(const double* x, int D, int S, unsigned char* peak, unsigned char* chosen, int* num_peaks, int32_t* out) {
+  if (threadIdx.x == 0) *num_peaks = 0;
+  __syncthreads();
+  for (int d = threadIdx.x; d < D; d += blockDim.x) {
+    const bool p = d > 0 && d < D - 1 && x[d] > x[d - 1] && x[d] > x[d + 1];
+    peak[d] = p ? 1 : 0;
+    chosen[d] = 0;
+    if (p) atomicAdd(num_peaks, 1);
+  }
+  __syncthreads();
+  for (int d = threadIdx.x; d < D; d += blockDim.x) {
+    if (!peak[d]) continue;
+    int larger = 0;      // peaks that argsort places after this one: larger value, or the same value at a higher index
+    for (int e = 0; e < D; ++e)
+      if (peak[e] && (x[e] > x[d] || (x[e] == x[d] && e > d))) ++larger;
+    chosen[d] = larger < S ? 1 : 0;
+  }
+  __syncthreads();
+  if (threadIdx.x != 0) return 0;
+  int n = 0;
+  for (int d = 0; d < D && n < S; ++d)
+    if (chosen[d]) out[n++] = d;
+  return *num_peaks;
+}
+
 void gccnmf_tmap_cache_free(gccnmf_handle* h);
 int gccnmf_get_twiddles(gccnmf_handle* h, int n, const double** tw64, const float** tw32);

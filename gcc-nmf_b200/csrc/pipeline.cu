@@ -16,36 +16,16 @@ namespace {
 
 constexpr int kPickMaxD = 1024;
 
-// scipy.signal.argrelmax(x) (order 1, mode 'clip': strict local maxima, never the end points), then the numSources largest
-// peaks (gccNMFFunctions.py:100: peakIndexes[argsort(x[peakIndexes])[-numSources:]]), returned in ascending index order (:113).
+// The numSources largest strict local maxima of the mean angular spectrum (select_peaks), ascending; missing ones are 0.
 __global__ void pick_targets_kernel(const double* __restrict__ mean_angular, int D, int S, int32_t* __restrict__ targets, int32_t* __restrict__ status) {
   __shared__ double x[kPickMaxD];
   __shared__ unsigned char peak[kPickMaxD], chosen[kPickMaxD];
   __shared__ int num_peaks;
   for (int d = threadIdx.x; d < D; d += blockDim.x) x[d] = mean_angular[d];
-  if (threadIdx.x == 0) num_peaks = 0;
-  __syncthreads();
-  for (int d = threadIdx.x; d < D; d += blockDim.x) {
-    const bool p = d > 0 && d < D - 1 && x[d] > x[d - 1] && x[d] > x[d + 1];
-    peak[d] = p ? 1 : 0;
-    chosen[d] = 0;
-    if (p) atomicAdd(&num_peaks, 1);
-  }
-  __syncthreads();
-  for (int d = threadIdx.x; d < D; d += blockDim.x) {
-    if (!peak[d]) continue;
-    int larger = 0;      // peaks that argsort places after this one: larger value, or the same value at a higher index
-    for (int e = 0; e < D; ++e)
-      if (peak[e] && (x[e] > x[d] || (x[e] == x[d] && e > d))) ++larger;
-    chosen[d] = larger < S ? 1 : 0;
-  }
-  __syncthreads();
+  const int peaks = select_peaks(x, D, S, peak, chosen, &num_peaks, targets);
   if (threadIdx.x == 0) {
-    int n = 0;
-    for (int d = 0; d < D && n < S; ++d)
-      if (chosen[d]) targets[n++] = d;
-    for (int i = n; i < S; ++i) targets[i] = 0;
-    if (num_peaks < S) atomicOr(status, 1);          // the reference aborts here (:102-104)
+    for (int i = peaks < S ? peaks : S; i < S; ++i) targets[i] = 0;
+    if (peaks < S) atomicOr(status, 1);              // the reference aborts here (:102-104)
   }
 }
 

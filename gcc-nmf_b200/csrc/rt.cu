@@ -29,6 +29,13 @@
 // order (numpy's: NaN first, then value, then the lower index), and the inference / filter kernels sum lane-strided over the
 // contracted index and then through the same xor butterfly for every slot.
 // An inactive slot costs no work: its output slice is written as zeros, its input slice is ignored, its state is left as it was.
+//
+// Sources (gccnmf_rtsep_*, P >= 2 target TDOAs per slot, the reference's TARGET_MODE_MULTIPLE).  rt_atoms also keeps the P target
+// rows gccNMF[tau_s][k] of its accumulators and gives every atom to the source whose value wins under rt_better: P one-hot masks.
+// Each slot then carries P copies of the mask, Y, synthesis frames and output ring, one source region of fixed stride after
+// another; filter, synthesis and emit run once per source (a source dimension in the grid), each source through the same code
+// and order a single-target slot runs.  Analysis, inference, the input ring and the localisation run once per slot; with
+// localisation on, the P largest peaks of the windowed GCC-PHAT mean become the targets of the next block.
 #include <cmath>
 
 #include "common.cuh"
@@ -42,6 +49,7 @@ constexpr int kRtMaxD = 128;
 constexpr int kRtRingBlocks = 8;         // utils.py:85 numBlocksPerBuffer
 constexpr int kRtMaxStreams = 4096;      // slots per state buffer
 constexpr int kRtAtomsFc = 32;           // f values per shared-memory stage of the atoms contraction
+constexpr int kRtMaxSources = GCCNMF_RTSEP_MAX_SOURCES;
 
 struct RtDev {                           // device-resident parameters + loop-carried state (first bytes of a slot region)
   float target, eps, beta, noise_floor;  // gccNMFProcessor.py:196-199 (Theano shared scalars)
@@ -68,18 +76,28 @@ struct RtLayout {                        // carve of the caller-owned state buff
   double *hist, *hmask;
   float2 *X, *Y;
   int32_t* argmax;
-  int F, Fp, L, S;
+  // what filter, synthesis and emit read and write per source: source q of slot s at rt_slot(rt_slot(p, s, stride), q, src_stride).
+  // P = 0: the slot's own hmask, Y, frames and out_ring with src_stride 0.  P > 0: P source regions appended to the slot (the
+  // slot's own four are then unused), plus the targets, the status word and the target rows gccNMF[tau_q] (P, K, nT).
+  double* smask;
+  float2* sY;
+  float *sframes, *sout, *tval;
+  int32_t *targets, *status;
+  size_t src_stride;
+  int F, Fp, L, S, P, D;
   size_t stride, bytes;
   bool ok;
 };
 
-RtLayout rt_carve(const gccnmf_rt_config& c, int S, void* state, size_t state_bytes) {
+RtLayout rt_carve(const gccnmf_rt_config& c, int S, int P, void* state, size_t state_bytes) {
   RtLayout l{};
   const int N = c.window_size, nT = c.windows_per_block, K = c.num_atoms, D = c.num_tdoas;
   l.F = N / 2 + 1;
   l.Fp = (l.F + 3) & ~3;
   l.L = kRtRingBlocks * c.block_size;
   l.S = S;
+  l.P = P;
+  l.D = D;
   char* base = state ? static_cast<char*>(state) : reinterpret_cast<char*>(256);
   WorkspaceCarver w(base, ~size_t(0) >> 1);
   l.tw64 = w.take<double>(N);
@@ -108,15 +126,33 @@ RtLayout rt_carve(const gccnmf_rt_config& c, int S, void* state, size_t state_by
   l.X = v.take<float2>((size_t)2 * l.F * nT);
   l.Y = v.take<float2>((size_t)2 * l.F * nT);
   l.argmax = v.take<int32_t>((size_t)K * nT);
+  l.smask = l.hmask;
+  l.sY = l.Y;
+  l.sframes = l.frames;
+  l.sout = l.out_ring;
+  if (P > 0) {
+    l.targets = v.take<int32_t>(kRtMaxSources);
+    l.status = v.take<int32_t>(1);
+    l.tval = v.take<float>((size_t)P * K * nT);
+    char* src0 = v.take<char>(0);
+    WorkspaceCarver u(src0, ~size_t(0) >> 1);
+    l.smask = u.take<double>((size_t)K * nT);
+    l.sY = u.take<float2>((size_t)2 * l.F * nT);
+    l.sframes = u.take<float>((size_t)2 * nT * N);
+    l.sout = u.take<float>((size_t)2 * l.L);
+    l.src_stride = align_up(u.used, 256);
+    v.take<char>((size_t)P * l.src_stride);
+  }
   l.stride = align_up(v.used, 256);
   l.bytes = shared + (size_t)S * l.stride;
   l.ok = state != nullptr && S >= 1 && l.bytes <= state_bytes;
   return l;
 }
 
-int rt_check(gccnmf_handle* h, const gccnmf_rt_config* c, int S = 1) {
+int rt_check(gccnmf_handle* h, const gccnmf_rt_config* c, int S = 1, int P = 0) {
   GCCNMF_REQUIRE(h, c != nullptr, "rt: NULL configuration");
   GCCNMF_REQUIRE(h, S >= 1 && S <= kRtMaxStreams, "rt: num_streams must be in [1, %d] (got %d)", kRtMaxStreams, S);
+  GCCNMF_REQUIRE(h, P == 0 || (P >= 2 && P <= kRtMaxSources), "rt: num_sources must be in [2, %d] (got %d)", kRtMaxSources, P);
   const int N = c->window_size;
   GCCNMF_REQUIRE(h, N >= 64 && N <= kRtMaxN && (N & (N - 1)) == 0, "rt: window_size must be a power of two in [64, %d] (got %d)", kRtMaxN, N);
   GCCNMF_REQUIRE(h, c->hop_size >= 1 && c->block_size >= 1, "rt: hop_size and block_size must be positive");
@@ -178,14 +214,28 @@ __global__ void rt_set_params_kernel(RtDev* dev0, size_t stride, int first, int 
   if (set_active) dev->active = q.active ? 1 : 0;
 }
 
-// Defaults of gccNMFProcessor.py:190-199 and `active` for slots [first, first + count) (after their regions were zeroed).
-__global__ void rt_default_params_kernel(RtDev* dev0, size_t stride, int first, int count) {
+// Defaults of gccNMFProcessor.py:190-199 and `active` for slots [first, first + count) (after their regions were zeroed); with P
+// sources, targets spread evenly over the D TDOAs: floor((2 q + 1) D / (2 P)).
+__global__ void rt_default_params_kernel(RtDev* dev0, size_t stride, int first, int count, int32_t* targets0, int P, int D) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= count) return;
   RtDev* dev = rt_slot(dev0, first + i, stride);
   dev->target = 10.0f; dev->eps = 2.0f; dev->beta = 1.0f; dev->noise_floor = 0.0f;
   dev->mode = 1; dev->separation = 1; dev->localization = 0; dev->loc_window = 6;
   dev->active = 1;
+  for (int q = 0; q < P; ++q) rt_slot(targets0, first + i, stride)[q] = (2 * q + 1) * D / (2 * P);
+}
+
+// Target TDOA indexes of up to kRtParamsPerLaunch slots, P per slot, by value; -1 keeps a source's target.
+struct RtTargetsBatch {
+  int32_t t[kRtParamsPerLaunch * kRtMaxSources];
+};
+__global__ void rt_set_targets_kernel(int32_t* targets0, size_t stride, int first, int count, int P, RtTargetsBatch b) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  int32_t* t = rt_slot(targets0, first + i, stride);
+  for (int q = 0; q < P; ++q)
+    if (b.t[i * P + q] >= 0) t[q] = b.t[i * P + q];
 }
 
 // ---------------------------------------------------------------------------------------------- numerics shared with gcc.cu
@@ -412,14 +462,20 @@ rt_inf_update_kernel(const RtDev* __restrict__ dev0, size_t stride, int S, const
 // TM / TN: the float32 values, and so the decisions, do not depend on the tile shape or on the other slots.
 //   TM = Dp / 16 (2, 4, 8), TN = 1: one pair x 16 atoms per CTA (K / 16 x pairs CTAs: latency for few streams)
 //   TM = 8, TN = 8:                 128 rows x 128 atoms per CTA (64 accumulators per thread: throughput for many streams)
+// P > 0 sources: the P target rows of every (pair, atom) go through shared memory to one pass that writes the P one-hot masks
+// (source q of slot s at rt_slot(rt_slot(hmask0, s, stride), q, src_stride)) and the values (tval, (P, K, nT) per slot); the
+// single-target mask is not written.
 template <int TM, int TN>
 __global__ void __launch_bounds__(256)
 rt_atoms_kernel(const RtDev* __restrict__ dev0, size_t stride, int pairs, int nT, const float* __restrict__ G0, const float* __restrict__ W, int F,
-                int Fp, int K, int D, int Dp, int32_t* __restrict__ argmax0, double* __restrict__ hmask0) {
+                int Fp, int K, int D, int Dp, int32_t* __restrict__ argmax0, double* __restrict__ hmask0, const int32_t* __restrict__ targets0, int P,
+                size_t src_stride, float* __restrict__ tval0) {
   constexpr int RB = 16 * TM, KB = 16 * TN, GS = RB + 4, FC = kRtAtomsFc;
   static_assert(RB % 32 == 0 && (TM <= 2 || TM % 4 == 0) && (TN < 4 || TN % 4 == 0), "tile shape");
+  static_assert(32 * KB + (RB / 32) * kRtMaxSources * KB <= FC * GS + FC * KB, "target rows must fit beside the argmax partials");
   __shared__ __align__(16) float sm[FC * GS + FC * KB];
   __shared__ int act[RB / 32];
+  __shared__ int tgt[RB / 32][kRtMaxSources];
   float* Gs = sm;                         // [f][row]
   float* Ws = sm + FC * GS;               // [f][atom]
   const int ppc = RB / Dp, k0 = blockIdx.x * KB, gp0 = blockIdx.y * ppc;
@@ -427,6 +483,7 @@ rt_atoms_kernel(const RtDev* __restrict__ dev0, size_t stride, int pairs, int nT
   if (threadIdx.x < ppc) {
     const int gp = gp0 + threadIdx.x;
     act[threadIdx.x] = gp < pairs && rt_slot(dev0, gp / nT, stride)->active;
+    for (int q = 0; q < P; ++q) tgt[threadIdx.x][q] = act[threadIdx.x] ? rt_slot(targets0, gp / nT, stride)[q] : -1;
   }
   __syncthreads();
   bool any = false;
@@ -506,6 +563,19 @@ rt_atoms_kernel(const RtDev* __restrict__ dev0, size_t stride, int pairs, int nT
       part_i[rg * KB + atom_of(j)] = bi;
     }
   }
+  float* tv = sm + 32 * KB;               // target rows [pair][source][atom], after the argmax partials
+  if (P > 0) {
+    const int r0 = rg * TM, p = r0 / Dp, d0 = r0 - p * Dp;
+    for (int q = 0; q < P; ++q) {
+      const int i = tgt[p][q] - d0;       // a duplicate target is a second copy of the same row
+      if (i < 0 || i >= TM) continue;
+#pragma unroll
+      for (int ii = 0; ii < TM; ++ii)     // register selection (no dynamically indexed local array)
+        if (ii == i)
+#pragma unroll
+          for (int j = 0; j < TN; ++j) tv[(p * kRtMaxSources + q) * KB + atom_of(j)] = acc[ii][j];
+    }
+  }
   __syncthreads();
   const int groups = Dp / TM;
   for (int idx = threadIdx.x; idx < ppc * KB; idx += 256) {
@@ -523,6 +593,20 @@ rt_atoms_kernel(const RtDev* __restrict__ dev0, size_t stride, int pairs, int nT
     const RtDev* dev = rt_slot(dev0, s, stride);
     const int64_t o = (int64_t)k * nT + t;
     rt_slot(argmax0, s, stride)[o] = bi;
+    if (P > 0) {                          // gccNMFFunctions.py:137-143 per block: the winning source takes the atom
+      const float* v = tv + p * kRtMaxSources * KB + a;
+      float wv = v[0];
+      int wi = 0;
+      for (int q = 1; q < P; ++q)
+        if (rt_better(v[q * KB], q, wv, wi)) { wv = v[q * KB]; wi = q; }
+      double* m0 = rt_slot(hmask0, s, stride);
+      float* tval = rt_slot(tval0, s, stride);
+      for (int q = 0; q < P; ++q) {
+        rt_slot(m0, q, src_stride)[o] = q == wi ? 1.0 : 0.0;
+        tval[((int64_t)q * K + k) * nT + t] = v[q * KB];
+      }
+      continue;
+    }
     // int64 - float32 promotes to float64 in Theano and numpy alike: the mask arithmetic is float64 (:263, :265)
     const double dist = fabs((double)bi - (double)dev->target);
     double m;
@@ -533,13 +617,17 @@ rt_atoms_kernel(const RtDev* __restrict__ dev0, size_t stride, int pairs, int nT
 }
 
 // ---------------------------------------------------------------------------------------------- C: time-frequency mask, one warp per bin and SG slots
-// Per slot, frame and channel: lane-strided float64 sums over k, then the xor butterfly.
+// Per slot, frame and channel: lane-strided float64 sums over k, then the xor butterfly.  blockIdx.z: the source (mask and Y at
+// src_stride per source).
 template <int NT, int SG, bool inference>
 __global__ void __launch_bounds__(256)
 rt_filter_kernel(const RtDev* __restrict__ dev0, size_t stride, int S, const float* __restrict__ W, const double* __restrict__ hmask0,
-                 const float* __restrict__ recV, const float* __restrict__ H0, const float2* __restrict__ X0, int F, int K, float2* __restrict__ Y0) {
+                 const float* __restrict__ recV, const float* __restrict__ H0, const float2* __restrict__ X0, int F, int K, float2* __restrict__ Y0,
+                 size_t src_stride) {
   const int f = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31, s0 = blockIdx.y * SG;
   if (f >= F) return;
+  hmask0 = rt_slot(hmask0, blockIdx.z, src_stride);
+  Y0 = rt_slot(Y0, blockIdx.z, src_stride);
   bool on[SG];
   bool any = false;
 #pragma unroll
@@ -616,14 +704,17 @@ rt_filter_kernel(const RtDev* __restrict__ dev0, size_t stride, int S, const flo
   }
 }
 
-// ---------------------------------------------------------------------------------------------- D: synthesis (one CTA per frame and slot)
+// ---------------------------------------------------------------------------------------------- D: synthesis (one CTA per frame, slot and source)
 __global__ void __launch_bounds__(kFftThreads)
 rt_synthesis_kernel(RtDev* __restrict__ dev0, size_t stride, const float2* __restrict__ Y0, const float2* __restrict__ tw, int N, int log2n, int nT,
-                    const float* __restrict__ win_s, float* __restrict__ frames0, float* __restrict__ out_windowed, int advance) {
+                    const float* __restrict__ win_s, float* __restrict__ frames0, float* __restrict__ out_windowed, int advance, size_t src_stride) {
   __shared__ float2 fft[kRtMaxN];
   const int t = blockIdx.x, s = blockIdx.y, F = N / 2 + 1;
   RtDev* dev = rt_slot(dev0, s, stride);
-  if (out_windowed) out_windowed += (int64_t)s * 2 * N * nT;
+  Y0 = rt_slot(Y0, blockIdx.z, src_stride);
+  frames0 = rt_slot(frames0, blockIdx.z, src_stride);
+  if (out_windowed) out_windowed += ((int64_t)s * gridDim.z + blockIdx.z) * 2 * N * nT;      // (S, P, 2, N, nT)
+  advance = advance && blockIdx.z == 0;
   if (!dev->active) {                                            // an inactive slot's output frames are zeros
     if (out_windowed)
       for (int i = threadIdx.x; i < N; i += blockDim.x) {
@@ -658,8 +749,13 @@ rt_synthesis_kernel(RtDev* __restrict__ dev0, size_t stride, const float2* __res
 }
 
 // ---------------------------------------------------------------------------------------------- localisation (one CTA per slot, D <= 128 threads used)
-__device__ void rt_localize(RtDev* dev, const float* __restrict__ gccphat, int D, int nT, double* __restrict__ hist, int hist_len) {
+// P > 0: the P largest peaks of the mean (select_peaks) replace `targets`; with fewer peaks the targets stay and status bit 0 is set.
+__device__ void rt_localize(RtDev* dev, const float* __restrict__ gccphat, int D, int nT, double* __restrict__ hist, int hist_len,
+                            int32_t* __restrict__ targets, int32_t* __restrict__ status, int P) {
   __shared__ double mean_s[kRtMaxD];
+  __shared__ unsigned char peak_s[kRtMaxD], chosen_s[kRtMaxD];
+  __shared__ int num_peaks_s;
+  __shared__ int32_t pick_s[kRtMaxSources];
   const int d = threadIdx.x;
   int idx = dev->hist_index;
   // gccPHATHistory.set(nanmean(realGCC, axis=0).T)   (:214 -> utils.py:45-59)
@@ -679,6 +775,19 @@ __device__ void rt_localize(RtDev* dev, const float* __restrict__ gccphat, int D
     mean_s[d] = n > 0 ? s / (double)n : __longlong_as_double(0x7ff8000000000000LL);
   }
   __syncthreads();
+  if (P > 0) {
+    if (dev->localization) {            // estimateTargetTDOAIndexesFromAngularSpectrum, numSources branch (gccNMFFunctions.py:94-116)
+      const int peaks = select_peaks(mean_s, D, P, peak_s, chosen_s, &num_peaks_s, pick_s);
+      if (d == 0) {
+        if (peaks >= P)
+          for (int q = 0; q < P; ++q) targets[q] = pick_s[q];
+        else
+          *status |= GCCNMF_RTSEP_STATUS_FEW_PEAKS;
+      }
+    }
+    if (d == 0) dev->hist_index = idx;
+    return;
+  }
   if (d == 0) {
     if (dev->localization) {
       double bv = mean_s[0];
@@ -692,28 +801,34 @@ __device__ void rt_localize(RtDev* dev, const float* __restrict__ gccphat, int D
 }
 
 __global__ void __launch_bounds__(128)
-rt_localize_kernel(RtDev* dev0, size_t stride, const float* __restrict__ gccphat0, int D, int nT, double* __restrict__ hist0, int hist_len) {
+rt_localize_kernel(RtDev* dev0, size_t stride, const float* __restrict__ gccphat0, int D, int nT, double* __restrict__ hist0, int hist_len,
+                   int32_t* __restrict__ targets0, int32_t* __restrict__ status0, int P) {
   const int s = blockIdx.x;
   RtDev* dev = rt_slot(dev0, s, stride);
   if (!dev->active) return;
-  rt_localize(dev, rt_slot(gccphat0, s, stride), D, nT, rt_slot(hist0, s, stride), hist_len);
+  rt_localize(dev, rt_slot(gccphat0, s, stride), D, nT, rt_slot(hist0, s, stride), hist_len, rt_slot(targets0, s, stride), rt_slot(status0, s, stride), P);
 }
 
 // ---------------------------------------------------------------------------------------------- E: overlap-add ring, block emit, input push
-// grid (ring CTAs + 1, S).  CTAs [0, gridDim.x - 1): one thread per logical ring position of the range that changes or is emitted;
-// last CTA: localisation.
+// grid (ring CTAs + 1, S, sources).  CTAs [0, gridDim.x - 1): one thread per logical ring position of the range that changes or is
+// emitted, into the source's own output ring; last CTA of source 0: localisation.  Source 0 pushes the input block.
 __global__ void __launch_bounds__(128)
 rt_ola_emit_kernel(RtDev* dev0, size_t stride, const float* __restrict__ frames0, int N, int hop, int nT, int B, int L, int p_first,
                    float* __restrict__ out_ring0, float* __restrict__ out_blocks, const float* __restrict__ in_blocks, float* __restrict__ in_ring0,
-                   const float* __restrict__ gccphat0, int D, double* __restrict__ hist0, int hist_len) {
-  const int s = blockIdx.y;
+                   const float* __restrict__ gccphat0, int D, double* __restrict__ hist0, int hist_len, int32_t* __restrict__ targets0,
+                   int32_t* __restrict__ status0, int P, size_t src_stride) {
+  const int s = blockIdx.y, z = blockIdx.z;
   RtDev* dev = rt_slot(dev0, s, stride);
   const bool active = dev->active != 0;
   if (blockIdx.x == gridDim.x - 1) {
-    if (active) rt_localize(dev, rt_slot(gccphat0, s, stride), D, nT, rt_slot(hist0, s, stride), hist_len);
+    if (active && z == 0)
+      rt_localize(dev, rt_slot(gccphat0, s, stride), D, nT, rt_slot(hist0, s, stride), hist_len, rt_slot(targets0, s, stride),
+                  rt_slot(status0, s, stride), P);
     return;
   }
-  float* out_block = out_blocks + (int64_t)s * 2 * B;
+  frames0 = rt_slot(frames0, z, src_stride);
+  out_ring0 = rt_slot(out_ring0, z, src_stride);
+  float* out_block = out_blocks + ((int64_t)s * gridDim.z + z) * 2 * B;       // (S, P, 2, B)
   const int p = p_first + blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= L) return;
   if (!active) {                                     // an inactive slot emits a block of zeros
@@ -739,7 +854,7 @@ rt_ola_emit_kernel(RtDev* dev0, size_t stride, const float* __restrict__ frames0
     }
     out_ring[c * L + q] = acc;
     if (p >= L - 3 * B && p < L - 2 * B) out_block[c * B + (p - (L - 3 * B))] = acc;   // outputFrames = outputBuffer[:, -3B:-2B] (:115)
-    if (p >= L - B) in_ring[c * L + q] = in_block[c * B + (p - (L - B))];              // inputBuffer[:, -B:] = inputFrames (:102)
+    if (p >= L - B && z == 0) in_ring[c * L + q] = in_block[c * B + (p - (L - B))];    // inputBuffer[:, -B:] = inputFrames (:102)
   }
 }
 
@@ -749,10 +864,13 @@ int ilog2_of(int n) {
   return l;
 }
 
-#define RT_CARVE_OR_FAIL(l, S)                                                                                                     \
-  if (int st__ = rt_check(h, cfg, (S))) return st__;                                                                               \
-  RtLayout l = rt_carve(*cfg, (S), state, state_bytes);                                                                            \
+#define RT_CARVE_OR_FAIL_P(l, S, P)                                                                                                \
+  if (int st__ = rt_check(h, cfg, (S), (P))) return st__;                                                                          \
+  RtLayout l = rt_carve(*cfg, (S), (P), state, state_bytes);                                                                       \
   if (!l.ok) return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "rt state buffer missing or too small: need %zu bytes", l.bytes)
+#define RT_CARVE_OR_FAIL(l, S) RT_CARVE_OR_FAIL_P(l, S, 0)
+
+inline int rt_sources_grid(const RtLayout& l) { return l.P > 0 ? l.P : 1; }
 
 // Several slots per warp (the dictionary row read once for all of them) only while the grid still has kRtWavesForSlotGroups waves
 // of CTAs; with fewer streams one slot per warp keeps the device busy.
@@ -785,8 +903,8 @@ int rt_enqueue_inference(gccnmf_handle* h, const gccnmf_rt_config* cfg, const Rt
 template <int NT, int SG, bool INF>
 int rt_enqueue_filter_as(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout& l, void* stream) {
   const int F = l.F, K = cfg->num_atoms, S = l.S;
-  GCCNMF_LAUNCH(h, (rt_filter_kernel<NT, SG, INF>), dim3((F + 7) / 8, (S + SG - 1) / SG), 256, 0, stream, l.dev, l.stride, S, l.W, l.hmask, l.recV, l.H,
-                l.X, F, K, l.Y);
+  GCCNMF_LAUNCH(h, (rt_filter_kernel<NT, SG, INF>), dim3((F + 7) / 8, (S + SG - 1) / SG, rt_sources_grid(l)), 256, 0, stream, l.dev, l.stride, S, l.W,
+                l.smask, l.recV, l.H, l.X, F, K, l.sY, l.src_stride);
   return 0;
 }
 template <int NT>
@@ -805,10 +923,10 @@ int rt_enqueue_atoms(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayo
   const int big_ctas = ((K + 127) / 128) * ((pairs + 128 / Dp - 1) / (128 / Dp));
   if (big_ctas >= h->sm_count)
     GCCNMF_LAUNCH(h, (rt_atoms_kernel<8, 8>), dim3((K + 127) / 128, (pairs + 128 / Dp - 1) / (128 / Dp)), 256, 0, stream, l.dev, l.stride, pairs, nT,
-                  l.G, l.W, l.F, l.Fp, K, D, Dp, l.argmax, l.hmask);
+                  l.G, l.W, l.F, l.Fp, K, D, Dp, l.argmax, l.smask, l.targets, l.P, l.src_stride, l.tval);
   else
     GCCNMF_LAUNCH(h, (rt_atoms_kernel<DJ, 1>), dim3((K + 15) / 16, pairs), 256, 0, stream, l.dev, l.stride, pairs, nT, l.G, l.W, l.F, l.Fp, K, D, Dp,
-                  l.argmax, l.hmask);
+                  l.argmax, l.smask, l.targets, l.P, l.src_stride, l.tval);
   return 0;
 }
 
@@ -854,8 +972,8 @@ int rt_enqueue_core(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayou
     default: st = rt_enqueue_filter<8>(h, cfg, l, stream); break;
   }
   if (st) return st;
-  GCCNMF_LAUNCH(h, rt_synthesis_kernel, dim3(nT, S), kFftThreads, 0, stream, l.dev, l.stride, l.Y, reinterpret_cast<const float2*>(l.tw32), N, log2n,
-                nT, l.win_s, l.frames, out_windowed, advance);
+  GCCNMF_LAUNCH(h, rt_synthesis_kernel, dim3(nT, S, rt_sources_grid(l)), kFftThreads, 0, stream, l.dev, l.stride, l.sY,
+                reinterpret_cast<const float2*>(l.tw32), N, log2n, nT, l.win_s, l.sframes, out_windowed, advance, l.src_stride);
   return 0;
 }
 
@@ -872,13 +990,13 @@ int rt_enqueue_params(gccnmf_handle* h, const RtLayout& l, int first, int count,
 // Zeroes the regions of slots [first, first + count) and gives them the defaults of gccNMFProcessor.py:190-199, active.
 int rt_enqueue_reset(gccnmf_handle* h, const RtLayout& l, int first, int count, void* stream) {
   GCCNMF_CHECK_CUDA(h, cudaMemsetAsync(rt_slot(reinterpret_cast<char*>(l.dev), first, l.stride), 0, (size_t)count * l.stride, (cudaStream_t)stream));
-  GCCNMF_LAUNCH(h, rt_default_params_kernel, (count + 127) / 128, 128, 0, stream, l.dev, l.stride, first, count);
+  GCCNMF_LAUNCH(h, rt_default_params_kernel, (count + 127) / 128, 128, 0, stream, l.dev, l.stride, first, count, l.targets, l.P, l.D);
   return 0;
 }
 
-int rt_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, const float* W, const float* E, const float* analysis_window,
+int rt_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, const float* W, const float* E, const float* analysis_window,
             const float* synthesis_window, const float* H0, void* state, size_t state_bytes, void* stream) {
-  RT_CARVE_OR_FAIL(l, S);
+  RT_CARVE_OR_FAIL_P(l, S, P);
   GCCNMF_REQUIRE(h, W && E && analysis_window && synthesis_window, "rt_init: NULL pointer");
   GCCNMF_REQUIRE(h, cfg->inference_iterations == 0 || H0 != nullptr, "rt_init: coefficient inference needs the initial H0 (K, 2)");
   cudaStream_t s = (cudaStream_t)stream;
@@ -896,46 +1014,48 @@ int rt_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, const float* W
   const int n = K > l.F ? K : l.F;
   GCCNMF_LAUNCH(h, rt_init_dictionary_kernel, (n + 127) / 128, 128, 0, stream, l.W, l.F, l.Fp, K, l.WT, l.recV, l.colsumW);
   GCCNMF_LAUNCH(h, rt_init_steering_kernel, (D * l.Fp + 255) / 256, 256, 0, stream, reinterpret_cast<const float2*>(E), l.F, l.Fp, D, l.ET);
-  GCCNMF_LAUNCH(h, rt_default_params_kernel, (S + 127) / 128, 128, 0, stream, l.dev, l.stride, 0, S);
+  GCCNMF_LAUNCH(h, rt_default_params_kernel, (S + 127) / 128, 128, 0, stream, l.dev, l.stride, 0, S, l.targets, l.P, l.D);
   return GCCNMF_OK;
 }
 
-int rt_process_block(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, void* state, size_t state_bytes, const float* in_blocks, float* out_blocks,
-                     const double* forced_atom_mask, void* stream) {
-  RT_CARVE_OR_FAIL(l, S);
+int rt_process_block(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, void* state, size_t state_bytes, const float* in_blocks,
+                     float* out_blocks, const double* forced_atom_mask, void* stream) {
+  RT_CARVE_OR_FAIL_P(l, S, P);
   GCCNMF_REQUIRE(h, in_blocks && out_blocks, "rt_process_block: NULL pointer");
   if (int st = rt_enqueue_core(h, cfg, l, nullptr, in_blocks, nullptr, forced_atom_mask, 1, stream)) return st;
   const int N = cfg->window_size, nT = cfg->windows_per_block, B = cfg->block_size;
   const int w_first = l.L - N - (nT - 1) * cfg->hop_size;
   const int p_first = w_first < l.L - 3 * B ? w_first : l.L - 3 * B;
   const int ctas = (l.L - p_first + 127) / 128;
-  GCCNMF_LAUNCH(h, rt_ola_emit_kernel, dim3(ctas + 1, S), 128, 0, stream, l.dev, l.stride, l.frames, N, cfg->hop_size, nT, B, l.L, p_first, l.out_ring,
-                out_blocks, in_blocks, l.in_ring, l.gccphat, cfg->num_tdoas, l.hist, cfg->history_length);
+  GCCNMF_LAUNCH(h, rt_ola_emit_kernel, dim3(ctas + 1, S, rt_sources_grid(l)), 128, 0, stream, l.dev, l.stride, l.sframes, N, cfg->hop_size, nT, B, l.L,
+                p_first, l.sout, out_blocks, in_blocks, l.in_ring, l.gccphat, cfg->num_tdoas, l.hist, cfg->history_length, l.targets, l.status, l.P,
+                l.src_stride);
   return GCCNMF_OK;
 }
 
-int rt_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, void* state, size_t state_bytes, const float* windowed, float* out,
+int rt_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, void* state, size_t state_bytes, const float* windowed, float* out,
                       const double* forced_atom_mask, void* stream) {
-  RT_CARVE_OR_FAIL(l, S);
+  RT_CARVE_OR_FAIL_P(l, S, P);
   GCCNMF_REQUIRE(h, windowed && out, "rt_process_frames: NULL pointer");
   if (int st = rt_enqueue_core(h, cfg, l, windowed, nullptr, out, forced_atom_mask, 0, stream)) return st;
-  GCCNMF_LAUNCH(h, rt_localize_kernel, S, 128, 0, stream, l.dev, l.stride, l.gccphat, cfg->num_tdoas, cfg->windows_per_block, l.hist, cfg->history_length);
+  GCCNMF_LAUNCH(h, rt_localize_kernel, S, 128, 0, stream, l.dev, l.stride, l.gccphat, cfg->num_tdoas, cfg->windows_per_block, l.hist, cfg->history_length,
+                l.targets, l.status, l.P);
   return GCCNMF_OK;
 }
 
-int rt_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, void* state, size_t state_bytes, float* in_blocks, float* out_blocks,
+int rt_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, void* state, size_t state_bytes, float* in_blocks, float* out_blocks,
                     const float* in_host, float* out_host, void** graph_exec, void* stream) {
   GCCNMF_REQUIRE(h, graph_exec != nullptr && stream != nullptr, "rt_graph_create: needs a non-default stream and an output slot");
   *graph_exec = nullptr;
-  RT_CARVE_OR_FAIL(l, S);
+  RT_CARVE_OR_FAIL_P(l, S, P);
   GCCNMF_REQUIRE(h, in_blocks && out_blocks, "rt_graph_create: NULL pointer");
   cudaStream_t s = (cudaStream_t)stream;
-  const size_t block_bytes = (size_t)S * 2 * cfg->block_size * sizeof(float);
+  const size_t block_bytes = (size_t)S * 2 * cfg->block_size * sizeof(float), out_bytes = block_bytes * rt_sources_grid(l);
   GCCNMF_CHECK_CUDA(h, cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
   int st = GCCNMF_OK;
   if (in_host && cudaMemcpyAsync(in_blocks, in_host, block_bytes, cudaMemcpyHostToDevice, s) != cudaSuccess) st = GCCNMF_ERR_CUDA;
-  if (st == GCCNMF_OK) st = rt_process_block(h, cfg, S, state, state_bytes, in_blocks, out_blocks, nullptr, stream);
-  if (st == GCCNMF_OK && out_host && cudaMemcpyAsync(out_host, out_blocks, block_bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess) st = GCCNMF_ERR_CUDA;
+  if (st == GCCNMF_OK) st = rt_process_block(h, cfg, S, P, state, state_bytes, in_blocks, out_blocks, nullptr, stream);
+  if (st == GCCNMF_OK && out_host && cudaMemcpyAsync(out_host, out_blocks, out_bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess) st = GCCNMF_ERR_CUDA;
   cudaGraph_t graph = nullptr;
   const cudaError_t end = cudaStreamEndCapture(s, &graph);
   if (st != GCCNMF_OK || end != cudaSuccess) {
@@ -951,26 +1071,35 @@ int rt_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, void* 
   return GCCNMF_OK;
 }
 
-int rt_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, void* state, size_t state_bytes, int slot, int what, void* dst, void* stream) {
-  RT_CARVE_OR_FAIL(l, S);
+// Items 2 and 4 are source 0's with P > 0; items 9 .. 13 exist only with P > 0.
+int rt_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, void* state, size_t state_bytes, int slot, int what, void* dst, void* stream) {
+  RT_CARVE_OR_FAIL_P(l, S, P);
   GCCNMF_REQUIRE(h, dst != nullptr, "rt_export: NULL destination");
   GCCNMF_REQUIRE(h, slot >= 0 && slot < S, "rt_export: slot %d outside [0, %d)", slot, S);
   const size_t nT = cfg->windows_per_block, K = cfg->num_atoms, D = cfg->num_tdoas, F = l.F, st = l.stride;
   const void* src = nullptr;
-  size_t bytes = 0;
-  switch (what) {
+  size_t bytes = 0, rows = 1;            // rows > 1: one row of `bytes` per source, src_stride apart in the state
+  switch (P > 0 ? what : what < 9 ? what : -1) {
     case 0: src = rt_slot(l.gccphat, slot, st); bytes = D * nT * sizeof(float); break;
     case 1: src = &rt_slot(l.dev, slot, st)->target; bytes = sizeof(float); break;
-    case 2: src = rt_slot(l.hmask, slot, st); bytes = K * nT * sizeof(double); break;
+    case 2: src = rt_slot(l.smask, slot, st); bytes = K * nT * sizeof(double); break;
     case 3: src = rt_slot(l.X, slot, st); bytes = 2 * F * nT * sizeof(float2); break;
-    case 4: src = rt_slot(l.Y, slot, st); bytes = 2 * F * nT * sizeof(float2); break;
+    case 4: src = rt_slot(l.sY, slot, st); bytes = 2 * F * nT * sizeof(float2); break;
     case 5: src = rt_slot(l.argmax, slot, st); bytes = K * nT * sizeof(int32_t); break;
     case 6: src = rt_slot(l.H, slot, st); bytes = K * 2 * nT * sizeof(float); break;
     case 7: src = rt_slot(l.hist, slot, st); bytes = D * (size_t)cfg->history_length * sizeof(double); break;
     case 8: src = &rt_slot(l.dev, slot, st)->hist_index; bytes = sizeof(int); break;
+    case 9: src = rt_slot(l.targets, slot, st); bytes = (size_t)P * sizeof(int32_t); break;
+    case 10: src = rt_slot(l.smask, slot, st); bytes = K * nT * sizeof(double); rows = P; break;
+    case 11: src = rt_slot(l.tval, slot, st); bytes = (size_t)P * K * nT * sizeof(float); break;
+    case 12: src = rt_slot(l.sY, slot, st); bytes = 2 * F * nT * sizeof(float2); rows = P; break;
+    case 13: src = rt_slot(l.status, slot, st); bytes = sizeof(int32_t); break;
     default: return gccnmf_fail(h, GCCNMF_ERR_INVALID_ARGUMENT, "rt_export: unknown item %d", what);
   }
-  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, (cudaStream_t)stream));
+  if (rows > 1)
+    GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync(dst, bytes, src, l.src_stride, bytes, rows, cudaMemcpyDefault, (cudaStream_t)stream));
+  else
+    GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, (cudaStream_t)stream));
   return GCCNMF_OK;
 }
 
@@ -988,14 +1117,14 @@ size_t gccnmf_rt_state_bytes(const gccnmf_rt_config* cfg) {
   if (!cfg || cfg->window_size < 2 || cfg->block_size < 1 || cfg->windows_per_block < 1 || cfg->num_atoms < 1 || cfg->num_tdoas < 1 ||
       cfg->history_length < 1)
     return 0;
-  return rt_carve(*cfg, 1, nullptr, 0).bytes;
+  return rt_carve(*cfg, 1, 0, nullptr, 0).bytes;
 }
 
 // W (F, K) f32, E (F, D) complex64 (expJOmegaTau, gccNMFProcessor.py:248), windows (N) f32, H0 (K, 2) f32 or NULL (all device pointers).
 int gccnmf_rt_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, const float* W, const float* E, const float* analysis_window,
                    const float* synthesis_window, const float* H0, void* state, size_t state_bytes, void* stream) {
   GCCNMF_ENTER(h);
-  return rt_init(h, cfg, 1, W, E, analysis_window, synthesis_window, H0, state, state_bytes, stream);
+  return rt_init(h, cfg, 1, 0, W, E, analysis_window, synthesis_window, H0, state, state_bytes, stream);
 }
 
 // setTargetTDOARange (:272-276) + the settable attributes (:136-151).  set_target = 0 leaves the target TDOA index alone (it is
@@ -1017,7 +1146,7 @@ int gccnmf_rt_set_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* st
 int gccnmf_rt_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* state, size_t state_bytes, const float* windowed, float* out,
                              const double* forced_atom_mask, void* stream) {
   GCCNMF_ENTER(h);
-  return rt_process_frames(h, cfg, 1, state, state_bytes, windowed, out, forced_atom_mask, stream);
+  return rt_process_frames(h, cfg, 1, 0, state, state_bytes, windowed, out, forced_atom_mask, stream);
 }
 
 // OverlapAddProcessor.processFrames(GCCNMFProcessor.processFrames) (utils.py:99-116 around gccNMFProcessor.py:201-231):
@@ -1025,7 +1154,7 @@ int gccnmf_rt_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, void
 int gccnmf_rt_process_block(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* state, size_t state_bytes, const float* in_block, float* out_block,
                             const double* forced_atom_mask, void* stream) {
   GCCNMF_ENTER(h);
-  return rt_process_block(h, cfg, 1, state, state_bytes, in_block, out_block, forced_atom_mask, stream);
+  return rt_process_block(h, cfg, 1, 0, state, state_bytes, in_block, out_block, forced_atom_mask, stream);
 }
 
 // One block as a CUDA graph: [H2D of in_host ->] the kernels of gccnmf_rt_process_block [-> D2H to out_host].  in_block / out_block
@@ -1033,7 +1162,7 @@ int gccnmf_rt_process_block(gccnmf_handle* h, const gccnmf_rt_config* cfg, void*
 int gccnmf_rt_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* state, size_t state_bytes, float* in_block, float* out_block,
                            const float* in_host, float* out_host, void** graph_exec, void* stream) {
   GCCNMF_ENTER(h);
-  return rt_graph_create(h, cfg, 1, state, state_bytes, in_block, out_block, in_host, out_host, graph_exec, stream);
+  return rt_graph_create(h, cfg, 1, 0, state, state_bytes, in_block, out_block, in_host, out_host, graph_exec, stream);
 }
 
 int gccnmf_rt_graph_launch(gccnmf_handle* h, void* graph_exec, void* stream) {
@@ -1056,19 +1185,19 @@ int gccnmf_rt_graph_destroy(gccnmf_handle* h, void* graph_exec) {
 //   7 GCC-PHAT history ring (D, history_length) f64 followed by nothing (its write index is item 8)   8 history write index (1) i32
 int gccnmf_rt_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, void* state, size_t state_bytes, int what, void* dst, void* stream) {
   GCCNMF_ENTER(h);
-  return rt_export(h, cfg, 1, state, state_bytes, 0, what, dst, stream);
+  return rt_export(h, cfg, 1, 0, state, state_bytes, 0, what, dst, stream);
 }
 
 // ---------------------------------------------------------------------------------------------- S streams (slots) in one state
 size_t gccnmf_rtm_state_bytes(const gccnmf_rt_config* cfg, int num_streams) {
   if (rt_check(nullptr, cfg, num_streams) != 0) return 0;
-  return rt_carve(*cfg, num_streams, nullptr, 0).bytes;
+  return rt_carve(*cfg, num_streams, 0, nullptr, 0).bytes;
 }
 
 int gccnmf_rtm_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, const float* W, const float* E, const float* analysis_window,
                     const float* synthesis_window, const float* H0, void* state, size_t state_bytes, void* stream) {
   GCCNMF_ENTER(h);
-  return rt_init(h, cfg, num_streams, W, E, analysis_window, synthesis_window, H0, state, state_bytes, stream);
+  return rt_init(h, cfg, num_streams, 0, W, E, analysis_window, synthesis_window, H0, state, state_bytes, stream);
 }
 
 int gccnmf_rtm_reset_slots(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state, size_t state_bytes, int first_slot, int count,
@@ -1096,25 +1225,124 @@ int gccnmf_rtm_set_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num
 int gccnmf_rtm_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state, size_t state_bytes, const float* windowed,
                               float* out, const double* forced_atom_mask, void* stream) {
   GCCNMF_ENTER(h);
-  return rt_process_frames(h, cfg, num_streams, state, state_bytes, windowed, out, forced_atom_mask, stream);
+  return rt_process_frames(h, cfg, num_streams, 0, state, state_bytes, windowed, out, forced_atom_mask, stream);
 }
 
 int gccnmf_rtm_process_block(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state, size_t state_bytes, const float* in_blocks,
                              float* out_blocks, const double* forced_atom_mask, void* stream) {
   GCCNMF_ENTER(h);
-  return rt_process_block(h, cfg, num_streams, state, state_bytes, in_blocks, out_blocks, forced_atom_mask, stream);
+  return rt_process_block(h, cfg, num_streams, 0, state, state_bytes, in_blocks, out_blocks, forced_atom_mask, stream);
 }
 
 int gccnmf_rtm_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state, size_t state_bytes, float* in_blocks,
                             float* out_blocks, const float* in_host, float* out_host, void** graph_exec, void* stream) {
   GCCNMF_ENTER(h);
-  return rt_graph_create(h, cfg, num_streams, state, state_bytes, in_blocks, out_blocks, in_host, out_host, graph_exec, stream);
+  return rt_graph_create(h, cfg, num_streams, 0, state, state_bytes, in_blocks, out_blocks, in_host, out_host, graph_exec, stream);
 }
 
 int gccnmf_rtm_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state, size_t state_bytes, int slot, int what, void* dst,
                       void* stream) {
   GCCNMF_ENTER(h);
-  return rt_export(h, cfg, num_streams, state, state_bytes, slot, what, dst, stream);
+  return rt_export(h, cfg, num_streams, 0, state, state_bytes, slot, what, dst, stream);
+}
+
+// ---------------------------------------------------------------------------------------------- S streams x P sources
+size_t gccnmf_rtsep_state_bytes(const gccnmf_rt_config* cfg, int num_streams, int num_sources) {
+  if (num_sources == 0 || rt_check(nullptr, cfg, num_streams, num_sources) != 0) return 0;
+  return rt_carve(*cfg, num_streams, num_sources, nullptr, 0).bytes;
+}
+
+int gccnmf_rtsep_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, const float* W, const float* E,
+                      const float* analysis_window, const float* synthesis_window, const float* H0, void* state, size_t state_bytes, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, num_sources != 0, "rtsep: num_sources must be in [2, %d] (got 0)", kRtMaxSources);
+  return rt_init(h, cfg, num_streams, num_sources, W, E, analysis_window, synthesis_window, H0, state, state_bytes, stream);
+}
+
+int gccnmf_rtsep_reset_slots(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state, size_t state_bytes,
+                             int first_slot, int count, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, num_sources != 0, "rtsep: num_sources must be in [2, %d] (got 0)", kRtMaxSources);
+  RT_CARVE_OR_FAIL_P(l, num_streams, num_sources);
+  if (int st = rt_check_range(h, num_streams, first_slot, count)) return st;
+  return rt_enqueue_reset(h, l, first_slot, count, stream);
+}
+
+// mode, target_index and set_target are ignored: the sources' masks are one-hot by construction and their targets come from
+// gccnmf_rtsep_set_targets or the localisation.
+int gccnmf_rtsep_set_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state, size_t state_bytes,
+                            int first_slot, int count, const gccnmf_rtm_slot_params* params, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, num_sources != 0, "rtsep: num_sources must be in [2, %d] (got 0)", kRtMaxSources);
+  RT_CARVE_OR_FAIL_P(l, num_streams, num_sources);
+  if (int st = rt_check_range(h, num_streams, first_slot, count)) return st;
+  GCCNMF_REQUIRE(h, params != nullptr, "rtsep_set_params: NULL parameters");
+  for (int i = 0; i < count; ++i) {
+    GCCNMF_REQUIRE(h, params[i].localization_window >= 1, "rtsep_set_params: slot %d: localization_window must be >= 1 (got %d)", first_slot + i,
+                   params[i].localization_window);
+    // a strict local maximum needs both neighbours (argrelmax never returns the end points)
+    GCCNMF_REQUIRE(h, !params[i].localization_enabled || cfg->num_tdoas >= 3, "rtsep_set_params: slot %d: localisation needs num_tdoas >= 3 (got %d)",
+                   first_slot + i, cfg->num_tdoas);
+  }
+  for (int i0 = 0; i0 < count; i0 += kRtParamsPerLaunch) {
+    const int n = count - i0 < kRtParamsPerLaunch ? count - i0 : kRtParamsPerLaunch;
+    gccnmf_rtm_slot_params p[kRtParamsPerLaunch];
+    for (int i = 0; i < n; ++i) {
+      p[i] = params[i0 + i];
+      p[i].set_target = 0;
+      p[i].mode = 1;
+    }
+    if (int st = rt_enqueue_params(h, l, first_slot + i0, n, p, 1, stream)) return st;
+  }
+  return GCCNMF_OK;
+}
+
+int gccnmf_rtsep_set_targets(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state, size_t state_bytes,
+                             int first_slot, int count, const int32_t* targets_host, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, num_sources != 0, "rtsep: num_sources must be in [2, %d] (got 0)", kRtMaxSources);
+  RT_CARVE_OR_FAIL_P(l, num_streams, num_sources);
+  if (int st = rt_check_range(h, num_streams, first_slot, count)) return st;
+  GCCNMF_REQUIRE(h, targets_host != nullptr, "rtsep_set_targets: NULL targets");
+  const int P = num_sources;
+  for (int i = 0; i < count * P; ++i)
+    GCCNMF_REQUIRE(h, targets_host[i] >= -1 && targets_host[i] < cfg->num_tdoas, "rtsep_set_targets: slot %d source %d: target %d outside [0, %d) (or -1)",
+                   first_slot + i / P, i % P, targets_host[i], cfg->num_tdoas);
+  for (int i0 = 0; i0 < count; i0 += kRtParamsPerLaunch) {
+    const int n = count - i0 < kRtParamsPerLaunch ? count - i0 : kRtParamsPerLaunch;
+    RtTargetsBatch b{};
+    memcpy(b.t, targets_host + (size_t)i0 * P, (size_t)n * P * sizeof(int32_t));
+    GCCNMF_LAUNCH(h, rt_set_targets_kernel, 1, kRtParamsPerLaunch, 0, stream, l.targets, l.stride, first_slot + i0, n, P, b);
+  }
+  return GCCNMF_OK;
+}
+
+int gccnmf_rtsep_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state, size_t state_bytes,
+                                const float* windowed, float* out, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, num_sources != 0, "rtsep: num_sources must be in [2, %d] (got 0)", kRtMaxSources);
+  return rt_process_frames(h, cfg, num_streams, num_sources, state, state_bytes, windowed, out, nullptr, stream);
+}
+
+int gccnmf_rtsep_process_block(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state, size_t state_bytes,
+                               const float* in_blocks, float* out_blocks, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, num_sources != 0, "rtsep: num_sources must be in [2, %d] (got 0)", kRtMaxSources);
+  return rt_process_block(h, cfg, num_streams, num_sources, state, state_bytes, in_blocks, out_blocks, nullptr, stream);
+}
+
+int gccnmf_rtsep_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state, size_t state_bytes,
+                              float* in_blocks, float* out_blocks, const float* in_host, float* out_host, void** graph_exec, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, num_sources != 0, "rtsep: num_sources must be in [2, %d] (got 0)", kRtMaxSources);
+  return rt_graph_create(h, cfg, num_streams, num_sources, state, state_bytes, in_blocks, out_blocks, in_host, out_host, graph_exec, stream);
+}
+
+int gccnmf_rtsep_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state, size_t state_bytes, int slot,
+                        int what, void* dst, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, num_sources != 0, "rtsep: num_sources must be in [2, %d] (got 0)", kRtMaxSources);
+  return rt_export(h, cfg, num_streams, num_sources, state, state_bytes, slot, what, dst, stream);
 }
 
 }  // extern "C"

@@ -13,6 +13,13 @@ the windowed frames, one D2H of the result and one synchronisation.
 `coefficientInferenceIterations` (an extension, default 0) switches on the per-frame H-only KL updates of
 notebooks/onlineSpeechEnhancement.ipynb:433-438 in the same kernel sequence.  History buffers (the reference's
 SharedMemoryCircularBuffer objects) are optional duck-typed objects with `.set(values)` / `.getUnraveledArray()`.
+
+`targetMode = TARGET_MODE_MULTIPLE` with `numSources` = P >= 2 (set before `reset`) separates the input into P sources, one per
+target TDOA index: the multi-target rule of gccNMFFunctions.py:118-143 per block (csrc/rt.cu, `MultiStreamRealtimeEngine` with
+numSources).  `processFrames` / `processBlock` then return (P, 2, N, nT) / (P, 2, B); `setTargetTDOAIndexes(indexes)` (the
+method the reference calls at gccNMFProcessor.py:111 but never defines) sets the targets, and with localisation on the device
+replaces them block by block with the P largest peaks of the windowed GCC-PHAT mean.  `targetTDOAIndexes` mirrors the device's
+targets after every call.
 """
 import logging
 
@@ -20,6 +27,7 @@ import numpy as np
 
 from .. import gccNMFFunctions as fn
 from . import engine as rt
+from . import multistream as rtm
 
 TARGET_MODE_BOXCAR = 0               # gccNMFProcessor.py:35-37
 TARGET_MODE_MULTIPLE = 1             # declared by the reference, not implemented there (its graph has no such branch, :262-265)
@@ -55,6 +63,9 @@ class GCCNMFProcessor(object):
         self.targetTDOAEpsilon = np.float32(2.0)
         self.targetTDOABeta = np.float32(1.0)
         self.targetTDOANoiseFloor = np.float32(0.0)
+        self.numSources = None               # TARGET_MODE_MULTIPLE: sources per input (:131 lists it among the reset parameters)
+        self.targetTDOAIndexes = None        # TARGET_MODE_MULTIPLE: the device's targets after the last call
+        self._targets_pending = None
         self.coefficientInferenceIterations = coefficientInferenceIterations
         self.device = device
         self.engine = None
@@ -75,12 +86,23 @@ class GCCNMFProcessor(object):
         if self.engine is not None:
             self.engine.close()
         self._geometry = (int(hopSize or self.windowSize), int(blockSize or self.windowSize * self.numTimePerChunk))
-        self.engine = rt.RealtimeEngine(self.W, self.expJOmegaTau, self.windowFunction[:, 0], self.synthesisWindowFunction[:, 0],
-                                        hopSize=self._geometry[0], blockSize=self._geometry[1], windowsPerBlock=self.numTimePerChunk,
-                                        historyLength=historyLength, numInferenceIterations=self.coefficientInferenceIterations,
-                                        device=self.device)
-        if self.targetMode not in (TARGET_MODE_BOXCAR, TARGET_MODE_WINDOW_FUNCTION):
-            raise ValueError('targetMode %r: the reference builds a mask for TARGET_MODE_BOXCAR and TARGET_MODE_WINDOW_FUNCTION only' % (self.targetMode,))
+        if self.targetMode not in (TARGET_MODE_BOXCAR, TARGET_MODE_MULTIPLE, TARGET_MODE_WINDOW_FUNCTION):
+            raise ValueError('targetMode %r: expected TARGET_MODE_BOXCAR, TARGET_MODE_MULTIPLE or TARGET_MODE_WINDOW_FUNCTION' % (self.targetMode,))
+        if self.targetMode == TARGET_MODE_MULTIPLE:
+            if self.numSources is None or not 2 <= int(self.numSources) <= rtm.MAX_SOURCES:
+                raise ValueError('TARGET_MODE_MULTIPLE needs numSources in [2, %d] (got %r)' % (rtm.MAX_SOURCES, self.numSources))
+            self.engine = rtm.MultiStreamRealtimeEngine(self.W, self.expJOmegaTau, self.windowFunction[:, 0], self.synthesisWindowFunction[:, 0],
+                                                        self._geometry[0], self._geometry[1], self.numTimePerChunk, 1,
+                                                        historyLength=historyLength, numInferenceIterations=self.coefficientInferenceIterations,
+                                                        device=self.device, numSources=int(self.numSources))
+            if self.targetTDOAIndexes is not None and self._targets_pending is None:
+                self._targets_pending = self.targetTDOAIndexes
+            self.targetTDOAIndexes = self.engine.export(0, rtm.EXPORT_TARGETS)
+        else:
+            self.engine = rt.RealtimeEngine(self.W, self.expJOmegaTau, self.windowFunction[:, 0], self.synthesisWindowFunction[:, 0],
+                                            hopSize=self._geometry[0], blockSize=self._geometry[1], windowsPerBlock=self.numTimePerChunk,
+                                            historyLength=historyLength, numInferenceIterations=self.coefficientInferenceIterations,
+                                            device=self.device)
         self._builtTargetMode = self.targetMode        # the reference bakes the mode into the graph at build time (:262-265)
         self._sent = None
         self._target_dirty = True
@@ -112,11 +134,27 @@ class GCCNMFProcessor(object):
         self.targetTDOANoiseFloor = np.float32(targetTDOANoiseFloor)
         self._target_dirty = True
 
+    def setTargetTDOAIndexes(self, targetTDOAIndexes):
+        """TARGET_MODE_MULTIPLE: the numSources target TDOA indexes (integers in [0, numTDOAs)) of the next call; -1 keeps one.
+        With localisation on, the device replaces them after every block."""
+        idx = np.asarray(targetTDOAIndexes)
+        if self.numSources is None or idx.shape != (int(self.numSources),):
+            raise ValueError('expected %r target TDOA indexes, got %r' % (self.numSources, idx.shape))
+        self._targets_pending = [int(i) for i in idx]
+
     def _sync_params(self):
         """Pushes the Python-side attributes to the device when they changed (stream-ordered, no synchronisation)."""
         localize = bool(self.tdoaHistory) and bool(self.gccPHATHistory) and bool(self.localizationEnabled)     # :216-222
         now = (float(self.targetTDOAEpsilon), float(self.targetTDOABeta), float(self.targetTDOANoiseFloor), int(self._builtTargetMode),
                bool(self.separationEnabled), localize, int(self.localizationWindowSize))
+        if self._builtTargetMode == TARGET_MODE_MULTIPLE:
+            if now != self._sent:
+                self.engine.set_params(0, None, now[0], now[1], now[2], 1, now[4], now[5], now[6])
+                self._sent = now
+            if self._targets_pending is not None:
+                self.engine.set_targets(0, [self._targets_pending])
+                self._targets_pending = None
+            return
         if self._target_dirty or now != self._sent:
             self.engine.set_params(float(self.targetTDOAIndex) if self._target_dirty else None, now[0], now[1], now[2],
                                    0 if now[3] == TARGET_MODE_BOXCAR else 1, now[4], now[5], now[6])
@@ -126,6 +164,13 @@ class GCCNMFProcessor(object):
     def _mirror_histories(self):
         """Optional host-side mirrors for a GUI; the numbers are the device state of the call that just finished."""
         e = self.engine
+        if self._builtTargetMode == TARGET_MODE_MULTIPLE:       # per-source masks and spectra: MultiStreamRealtimeEngine.export
+            self.targetTDOAIndexes = e.export(0, rtm.EXPORT_TARGETS)
+            if self.inputSpectrogramHistory:
+                self.inputSpectrogramHistory.set(-np.mean(np.abs(e.export(0, rt.EXPORT_INPUT_SPEC)), axis=0) ** (1 / 3.0))
+            if self.gccPHATHistory:
+                self.gccPHATHistory.set(e.export(0, rt.EXPORT_GCCPHAT))
+            return
         if self.separationEnabled and self.coefficientMaskHistories:
             self.coefficientMaskHistories[self.dictionarySize].set(1 - e.export(rt.EXPORT_ATOM_MASK))
         if self.inputSpectrogramHistory:
@@ -141,22 +186,32 @@ class GCCNMFProcessor(object):
 
     # ------------------------------------------------------------------ :201-231
     def processFrames(self, windowedSamples, forcedAtomMask=None):
-        """windowedSamples (2, N, nT) float32 -> (2, N, nT) float32.  forcedAtomMask (K, nT): use this atom mask instead of the
-        one derived from the TDOA argmax (teacher-forced parity tests)."""
+        """windowedSamples (2, N, nT) float32 -> (2, N, nT) float32, or (numSources, 2, N, nT) in TARGET_MODE_MULTIPLE.
+        forcedAtomMask (K, nT): use this atom mask instead of the one derived from the TDOA argmax (teacher-forced parity tests;
+        not in TARGET_MODE_MULTIPLE)."""
         if self.engine is None:
             self.buildFunctions()
         self._sync_params()
-        out = self.engine.process_frames(np.asarray(windowedSamples, dtype=np.float32), forcedAtomMask).copy()
+        x = np.asarray(windowedSamples, dtype=np.float32)
+        if self._builtTargetMode == TARGET_MODE_MULTIPLE:
+            out = self.engine.process_frames(x[None], forcedAtomMask)[0].copy()
+        else:
+            out = self.engine.process_frames(x, forcedAtomMask).copy()
         self._mirror_histories()
         return out
 
     def processBlock(self, inputFrames, hopSize, blockSize, useGraph=True, forcedAtomMask=None):
         """One audio block through the device-resident overlap-add rings AND processFrames as a single CUDA graph launch:
         OverlapAddProcessor.processFrames(self.processFrames) of gccNMF/realtime/utils.py:99-116 / gccNMFProcessor.py:97.
-        inputFrames (2, blockSize) float32 -> the next output block (2, blockSize) float32 (two blocks of latency, utils.py:115)."""
+        inputFrames (2, blockSize) float32 -> the next output block (2, blockSize) float32 (two blocks of latency, utils.py:115),
+        or (numSources, 2, blockSize) in TARGET_MODE_MULTIPLE."""
         if self.engine is None or self._geometry != (int(hopSize), int(blockSize)):
             self.buildFunctions(hopSize, blockSize)
         self._sync_params()
-        out = self.engine.process_block(np.asarray(inputFrames, dtype=np.float32), use_graph=useGraph, forcedAtomMask=forcedAtomMask)
+        x = np.asarray(inputFrames, dtype=np.float32)
+        if self._builtTargetMode == TARGET_MODE_MULTIPLE:
+            out = self.engine.process_blocks(x[None], use_graph=useGraph, forcedAtomMask=forcedAtomMask)[0].copy()
+        else:
+            out = self.engine.process_block(x, use_graph=useGraph, forcedAtomMask=forcedAtomMask)
         self._mirror_histories()
         return out

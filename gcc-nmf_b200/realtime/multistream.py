@@ -8,6 +8,12 @@ synchronisation.  Slot s is bit-identical to a `RealtimeEngine` fed the same blo
 
 Join / leave without rebuilding the graph: `set_active(slots, False)` makes the kernels skip a slot (its output block is zeros, its
 input block is ignored, its state stays as it was); `reset_slots(slots)` puts slots back to the state of a fresh engine.
+
+Sources (`numSources` = P >= 2, `gccnmf_rtsep_*`): every slot is separated into P sources, one per target TDOA index (the
+reference's TARGET_MODE_MULTIPLE, gccNMFFunctions.py:118-143 per block), and every call returns P output blocks per slot.  The
+targets come from `set_targets` or, with localisation on, from the P largest peaks of the windowed GCC-PHAT mean (the targets of
+the next block).  Source q of a slot computes bit for bit what a single-target slot computes when it is fed the exported mask of
+source q as its atom mask; the P masks partition the atoms, so the P outputs sum to the separation-off output.
 """
 import ctypes
 
@@ -17,6 +23,15 @@ from .._lib import RtConfig, RtmSlotParams, default_handle
 from .engine import (EXPORT_ARGMAX, EXPORT_ATOM_MASK, EXPORT_GCCPHAT, EXPORT_H, EXPORT_HISTORY, EXPORT_HISTORY_INDEX,  # noqa: F401
                      EXPORT_INPUT_SPEC, EXPORT_OUTPUT_SPEC, EXPORT_TARGET)
 
+# export items of an engine with sources (gccnmf_rtsep_export); EXPORT_ATOM_MASK and EXPORT_OUTPUT_SPEC are then source 0's
+EXPORT_TARGETS = 9                   # (P,) int32 target TDOA indexes of the next block
+EXPORT_SOURCE_MASKS = 10             # (P, K, nT) float64 one-hot atom masks
+EXPORT_TARGET_VALUES = 11            # (P, K, nT) float32 gccNMF[target] per atom and frame
+EXPORT_SOURCE_SPECS = 12             # (P, 2, F, nT) complex64 output spectrograms
+EXPORT_STATUS = 13                   # (1,) int32, bit 0 (STATUS_FEW_PEAKS): the localisation found fewer than P peaks (sticky)
+STATUS_FEW_PEAKS = 1
+MAX_SOURCES = 8
+
 # gccNMFProcessor.py:190-199 -- what gccnmf_rtm_init and gccnmf_rtm_reset_slots leave in a slot
 DEFAULT_SLOT_PARAMS = dict(targetTDOAIndex=10.0, epsilon=2.0, beta=1.0, noiseFloor=0.0, mode=1, separationEnabled=True,
                            localizationEnabled=False, localizationWindowSize=6, active=True)
@@ -24,7 +39,10 @@ DEFAULT_SLOT_PARAMS = dict(targetTDOAIndex=10.0, epsilon=2.0, beta=1.0, noiseFlo
 
 class MultiStreamRealtimeEngine(object):
     def __init__(self, W, expJOmegaTau, analysisWindow, synthesisWindow, hopSize, blockSize, windowsPerBlock, numStreams, historyLength=128,
-                 numInferenceIterations=0, sparsityAlpha=0.0, epsilon=1e-16, seedValue=0, device=0):
+                 numInferenceIterations=0, sparsityAlpha=0.0, epsilon=1e-16, seedValue=0, device=0, numSources=0):
+        self.P = int(numSources)
+        if self.P != 0 and not 2 <= self.P <= MAX_SOURCES:
+            raise ValueError('numSources must be 0 (one output per slot) or in [2, %d] (got %d)' % (MAX_SOURCES, self.P))
         self.h = default_handle(device)
         torch = self.torch = self.h.torch
         W = np.ascontiguousarray(W, dtype=np.float32)
@@ -38,7 +56,8 @@ class MultiStreamRealtimeEngine(object):
         self.hop, self.B, self.nT = int(hopSize), int(blockSize), int(windowsPerBlock)
         self.cfg = RtConfig(N, self.hop, self.B, self.nT, K, self.D, int(historyLength), int(numInferenceIterations),
                             float(sparsityAlpha), float(epsilon))
-        self.state_bytes = int(self.h.lib.gccnmf_rtm_state_bytes(ctypes.byref(self.cfg), self.S))
+        self.state_bytes = int(self.h.lib.gccnmf_rtsep_state_bytes(ctypes.byref(self.cfg), self.S, self.P) if self.P else
+                               self.h.lib.gccnmf_rtm_state_bytes(ctypes.byref(self.cfg), self.S))
         if self.state_bytes == 0:
             raise ValueError('invalid real-time configuration or number of streams (%d)' % self.S)
         self.stream = torch.cuda.Stream(device=self.h.device)
@@ -51,14 +70,15 @@ class MultiStreamRealtimeEngine(object):
         self._const = [dev(W), dev(E.view(np.float32).reshape(F, 2 * self.D)), dev(np.asarray(analysisWindow, np.float32)),
                        dev(np.asarray(synthesisWindow, np.float32)), dev(H0) if H0 is not None else None]
         S = self.S
+        per_slot = (self.P,) if self.P else ()          # outputs: (S, [P,] 2, ...)
         self.in_host = torch.zeros((S, 2, self.B), dtype=torch.float32).pin_memory()
-        self.out_host = torch.zeros((S, 2, self.B), dtype=torch.float32).pin_memory()
+        self.out_host = torch.zeros((S,) + per_slot + (2, self.B), dtype=torch.float32).pin_memory()
         self.in_dev = torch.zeros((S, 2, self.B), dtype=torch.float32, device=self.h.device)
-        self.out_dev = torch.zeros((S, 2, self.B), dtype=torch.float32, device=self.h.device)
+        self.out_dev = torch.zeros((S,) + per_slot + (2, self.B), dtype=torch.float32, device=self.h.device)
         self.frames_in_host = torch.zeros((S, 2, N, self.nT), dtype=torch.float32).pin_memory()
-        self.frames_out_host = torch.zeros((S, 2, N, self.nT), dtype=torch.float32).pin_memory()
+        self.frames_out_host = torch.zeros((S,) + per_slot + (2, N, self.nT), dtype=torch.float32).pin_memory()
         self.frames_in_dev = torch.zeros((S, 2, N, self.nT), dtype=torch.float32, device=self.h.device)
-        self.frames_out_dev = torch.zeros((S, 2, N, self.nT), dtype=torch.float32, device=self.h.device)
+        self.frames_out_dev = torch.zeros((S,) + per_slot + (2, N, self.nT), dtype=torch.float32, device=self.h.device)
         self._graph = None
         self._exports = {}
         self._params = [dict(DEFAULT_SLOT_PARAMS) for _ in range(S)]      # host mirror of what each slot holds
@@ -67,6 +87,14 @@ class MultiStreamRealtimeEngine(object):
     # ------------------------------------------------------------------ state
     def _check(self, status):
         self.h.check(status)
+
+    def _abi(self, name, *args):
+        """gccnmf_rtm_<name>(h, cfg, S, state, state_bytes, *args), or gccnmf_rtsep_<name>(h, cfg, S, P, ...) with sources."""
+        if self.P:
+            fn, head = getattr(self.h.lib, 'gccnmf_rtsep_' + name), (self.S, self.P)
+        else:
+            fn, head = getattr(self.h.lib, 'gccnmf_rtm_' + name), (self.S,)
+        self._check(fn(self.h.h, ctypes.byref(self.cfg), *head, self.state.data_ptr(), self.state_bytes, *args))
 
     def _slots(self, slots):
         if isinstance(slots, slice):
@@ -97,9 +125,12 @@ class MultiStreamRealtimeEngine(object):
         torch.cuda.current_stream(self.h.device).synchronize()
         c = self._const
         with torch.cuda.stream(self.stream):
-            self._check(self.h.lib.gccnmf_rtm_init(self.h.h, ctypes.byref(self.cfg), self.S, c[0].data_ptr(), c[1].data_ptr(), c[2].data_ptr(),
-                                                   c[3].data_ptr(), c[4].data_ptr() if c[4] is not None else None,
-                                                   self.state.data_ptr(), self.state_bytes, self.stream.cuda_stream))
+            args = (c[0].data_ptr(), c[1].data_ptr(), c[2].data_ptr(), c[3].data_ptr(), c[4].data_ptr() if c[4] is not None else None,
+                    self.state.data_ptr(), self.state_bytes, self.stream.cuda_stream)
+            if self.P:
+                self._check(self.h.lib.gccnmf_rtsep_init(self.h.h, ctypes.byref(self.cfg), self.S, self.P, *args))
+            else:
+                self._check(self.h.lib.gccnmf_rtm_init(self.h.h, ctypes.byref(self.cfg), self.S, *args))
         self.stream.synchronize()
         self._params = [dict(DEFAULT_SLOT_PARAMS) for _ in range(self.S)]
 
@@ -107,8 +138,7 @@ class MultiStreamRealtimeEngine(object):
         """The given slots back to a fresh state; the others are untouched.  Stream-ordered: the graph is kept."""
         slots = self._slots(slots)
         for first, count in self._runs(slots):
-            self._check(self.h.lib.gccnmf_rtm_reset_slots(self.h.h, ctypes.byref(self.cfg), self.S, self.state.data_ptr(), self.state_bytes,
-                                                          first, count, self.stream.cuda_stream))
+            self._abi('reset_slots', first, count, self.stream.cuda_stream)
         for s in slots:
             self._params[s] = dict(DEFAULT_SLOT_PARAMS)
 
@@ -121,8 +151,7 @@ class MultiStreamRealtimeEngine(object):
                 arr[i] = RtmSlotParams(float(t if t is not None else 0.0), 1 if (set_target and t is not None) else 0, float(p['epsilon']),
                                        float(p['beta']), float(p['noiseFloor']), int(p['mode']), 1 if p['separationEnabled'] else 0,
                                        1 if p['localizationEnabled'] else 0, int(p['localizationWindowSize']), 1 if p['active'] else 0)
-            self._check(self.h.lib.gccnmf_rtm_set_params(self.h.h, ctypes.byref(self.cfg), self.S, self.state.data_ptr(), self.state_bytes,
-                                                         first, count, arr, self.stream.cuda_stream))
+            self._abi('set_params', first, count, arr, self.stream.cuda_stream)
 
     def set_params(self, slots, targetTDOAIndex=None, epsilon=2.0, beta=1.0, noiseFloor=0.0, mode=1, separationEnabled=True,
                    localizationEnabled=False, localizationWindowSize=6):
@@ -152,26 +181,46 @@ class MultiStreamRealtimeEngine(object):
     def is_active(self, slot):
         return bool(self._params[self._slots(slot)[0]]['active'])
 
+    def set_targets(self, slots, indexes):
+        """Target TDOA indexes of the given slots' P sources from the next block on (GCCNMFProcessor.setTargetTDOAIndexes):
+        indexes (len(slots), P) or one row of P for every slot, integers in [0, D); -1 keeps that source's target.  With
+        localisation on, the next block's localisation replaces them again."""
+        if not self.P:
+            raise ValueError('set_targets needs an engine with numSources >= 2')
+        slots = self._slots(slots)
+        if len(set(slots)) != len(slots):
+            raise ValueError('duplicate slots')
+        idx = np.asarray(indexes)
+        if idx.size and not np.array_equal(idx, np.round(idx)):
+            raise ValueError('target TDOA indexes must be integers')
+        idx = np.broadcast_to(idx.astype(np.int64), (len(slots), self.P))
+        rows = dict(zip(slots, idx))
+        for first, count in self._runs(slots):
+            arr = np.ascontiguousarray([rows[s] for s in range(first, first + count)], dtype=np.int32)
+            self._abi('set_targets', first, count, arr.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), self.stream.cuda_stream)
+
     # ------------------------------------------------------------------ per-block work
     def build_graph(self):
         if self._graph is None:
             g = ctypes.c_void_p()
-            self._check(self.h.lib.gccnmf_rtm_graph_create(self.h.h, ctypes.byref(self.cfg), self.S, self.state.data_ptr(), self.state_bytes,
-                                                           self.in_dev.data_ptr(), self.out_dev.data_ptr(), self.in_host.data_ptr(),
-                                                           self.out_host.data_ptr(), ctypes.byref(g), self.stream.cuda_stream))
+            self._abi('graph_create', self.in_dev.data_ptr(), self.out_dev.data_ptr(), self.in_host.data_ptr(), self.out_host.data_ptr(),
+                      ctypes.byref(g), self.stream.cuda_stream)
             self._graph = g
         return self._graph
 
     def _forced(self, forcedAtomMask):
         if forcedAtomMask is None:
             return None
+        if self.P:
+            raise ValueError('forcedAtomMask: the sources of an engine with numSources >= 2 take their masks from their targets')
         m = self.torch.as_tensor(np.ascontiguousarray(forcedAtomMask, dtype=np.float64).reshape(self.S, self.K, self.nT))
         self._forced_dev = m.to(self.h.device)          # kept alive until the stream has consumed it
         return self._forced_dev.data_ptr()
 
     def process_blocks(self, blocks, use_graph=True, forcedAtomMask=None):
-        """blocks (S, 2, B) float32 (host) -> (S, 2, B) float32 view of the pinned output buffer (overwritten by the next call).
-        forcedAtomMask (S, K, nT) float64 replaces the per-atom TDOA decisions of every slot (kernel by kernel, no graph)."""
+        """blocks (S, 2, B) float32 (host) -> (S, 2, B) float32 view of the pinned output buffer (overwritten by the next call);
+        (S, P, 2, B) with sources.  forcedAtomMask (S, K, nT) float64 replaces the per-atom TDOA decisions of every slot (kernel by
+        kernel, no graph; not with sources)."""
         self.in_host.numpy()[:] = blocks
         if use_graph and forcedAtomMask is None:
             self._check(self.h.lib.gccnmf_rt_graph_launch(self.h.h, self.build_graph(), self.stream.cuda_stream))
@@ -180,29 +229,30 @@ class MultiStreamRealtimeEngine(object):
             self.torch.cuda.current_stream(self.h.device).synchronize()
             with self.torch.cuda.stream(self.stream):
                 self.in_dev.copy_(self.in_host, non_blocking=True)
-                self._check(self.h.lib.gccnmf_rtm_process_block(self.h.h, ctypes.byref(self.cfg), self.S, self.state.data_ptr(), self.state_bytes,
-                                                                self.in_dev.data_ptr(), self.out_dev.data_ptr(), forced, self.stream.cuda_stream))
+                self._abi('process_block', self.in_dev.data_ptr(), self.out_dev.data_ptr(), *(() if self.P else (forced,)),
+                          self.stream.cuda_stream)
                 self.out_host.copy_(self.out_dev, non_blocking=True)
         self.stream.synchronize()
         return self.out_host.numpy()
 
     def process_frames(self, windowedSamples, forcedAtomMask=None):
-        """windowedSamples (S, 2, N, nT) float32 (host) -> (S, 2, N, nT) float32: GCCNMFProcessor.processFrames per slot."""
+        """windowedSamples (S, 2, N, nT) float32 (host) -> (S, 2, N, nT) float32 ((S, P, 2, N, nT) with sources):
+        GCCNMFProcessor.processFrames per slot."""
         self.frames_in_host.numpy()[:] = windowedSamples
         forced = self._forced(forcedAtomMask)
         if forced is not None:
             self.torch.cuda.current_stream(self.h.device).synchronize()
         with self.torch.cuda.stream(self.stream):
             self.frames_in_dev.copy_(self.frames_in_host, non_blocking=True)
-            self._check(self.h.lib.gccnmf_rtm_process_frames(self.h.h, ctypes.byref(self.cfg), self.S, self.state.data_ptr(), self.state_bytes,
-                                                             self.frames_in_dev.data_ptr(), self.frames_out_dev.data_ptr(), forced,
-                                                             self.stream.cuda_stream))
+            self._abi('process_frames', self.frames_in_dev.data_ptr(), self.frames_out_dev.data_ptr(), *(() if self.P else (forced,)),
+                      self.stream.cuda_stream)
             self.frames_out_host.copy_(self.frames_out_dev, non_blocking=True)
         self.stream.synchronize()
         return self.frames_out_host.numpy()
 
     def export(self, slot, what):
-        """Host copy of one item of slot `slot`'s state after the last block (items as RealtimeEngine.export)."""
+        """Host copy of one item of slot `slot`'s state after the last block (items as RealtimeEngine.export; with sources also
+        EXPORT_TARGETS .. EXPORT_STATUS)."""
         torch = self.torch
         slot = self._slots(slot)[0]
         shapes = {EXPORT_GCCPHAT: ((self.D, self.nT), torch.float32), EXPORT_TARGET: ((1,), torch.float32),
@@ -210,12 +260,18 @@ class MultiStreamRealtimeEngine(object):
                   EXPORT_OUTPUT_SPEC: ((2, self.F, self.nT), torch.complex64), EXPORT_ARGMAX: ((self.K, self.nT), torch.int32),
                   EXPORT_H: ((self.K, 2 * self.nT), torch.float32), EXPORT_HISTORY: ((self.D, self.cfg.history_length), torch.float64),
                   EXPORT_HISTORY_INDEX: ((1,), torch.int32)}
+        if self.P:
+            P, K, nT = self.P, self.K, self.nT
+            shapes.update({EXPORT_TARGETS: ((P,), torch.int32), EXPORT_SOURCE_MASKS: ((P, K, nT), torch.float64),
+                           EXPORT_TARGET_VALUES: ((P, K, nT), torch.float32), EXPORT_SOURCE_SPECS: ((P, 2, self.F, nT), torch.complex64),
+                           EXPORT_STATUS: ((1,), torch.int32)})
+        if what not in shapes:
+            raise ValueError('unknown export item %r' % (what,))
         buf = self._exports.get(what)
         if buf is None:
             shape, dtype = shapes[what]
             buf = self._exports[what] = torch.zeros(shape, dtype=dtype).pin_memory()
-        self._check(self.h.lib.gccnmf_rtm_export(self.h.h, ctypes.byref(self.cfg), self.S, self.state.data_ptr(), self.state_bytes, slot, int(what),
-                                                 buf.data_ptr(), self.stream.cuda_stream))
+        self._abi('export', slot, int(what), buf.data_ptr(), self.stream.cuda_stream)
         self.stream.synchronize()
         return buf.numpy().copy()
 

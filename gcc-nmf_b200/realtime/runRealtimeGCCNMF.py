@@ -12,6 +12,10 @@ a pair of Events, i.e. strictly synchronously -- here the same two steps are cal
 
 PyAudio, Qt and the parameter queues are out of scope (SURVEY.md section 2, rows 8, 10, 13); the per-block processing
 times the reference logs every 2 s (audioProcessor.py:98-102) are returned as min / max / mean.
+
+`numSources` = P >= 2 separates the file into P sources instead (GCCNMFProcessor in TARGET_MODE_MULTIPLE, targets from the
+localisation): every block goes through the device-resident rings (`GCCNMFProcessor.processBlock`), the arrays gain a leading
+source axis and `run` writes one wav file per source.
 """
 import argparse
 import logging
@@ -30,7 +34,8 @@ DEFAULT_PARAMS = dict(
     localizationEnabled=True, localizationWindowSize=6,
     numChannels=2, sampleRate=16000, deviceIndex=None,
     windowSize=1024, hopSize=512, blockSize=512,
-    dictionarySize=64, dictionarySizes=[64, 128, 256, 512, 1024], dictionaryType='Pretrained', numHUpdates=0)
+    dictionarySize=64, dictionarySizes=[64, 128, 256, 512, 1024], dictionaryType='Pretrained', numHUpdates=0,
+    numSources=0)                            # 0: enhancement (one output); P >= 2: P separated sources
 HEADLESS_TARGET_TDOA_INDEX = 9.60          # runRealtimeGCCNMF.py:144
 
 
@@ -79,9 +84,15 @@ class RealtimeGCCNMFNoGUI(object):
             g.setTargetTDOARange(HEADLESS_TARGET_TDOA_INDEX, p.targetTDOAEpsilon, p.targetTDOABeta, p.targetTDOANoiseFloor)
             g.numTDOAs = p.numTDOAs
             g.separationEnabled = True
+            if p.numSources:
+                from .gccNMFProcessor import TARGET_MODE_MULTIPLE
+                g.targetMode = TARGET_MODE_MULTIPLE
+                g.numSources = p.numSources
             g.reset()
             self.gccNMFProcessor = g
             processFramesFunction = g.processFrames
+        elif p.numSources:
+            raise ValueError('numSources runs the built-in GCCNMFProcessor; this runner was given a processFramesFunction')
         self.processFramesFunction = processFramesFunction
         self.processingTimes = []
 
@@ -91,16 +102,22 @@ class RealtimeGCCNMFNoGUI(object):
         return 2 * self.params.blockSize
 
     def processBlock(self, block):
-        """block (numChannels, blockSize) float32 -> the next output block (a view that is overwritten by the next call)."""
+        """block (numChannels, blockSize) float32 -> the next output block (a view that is overwritten by the next call), or
+        (numSources, numChannels, blockSize) with sources."""
+        p = self.params
         startTime = time.time()
-        self.inputFrames[:] = block
-        self.oladProcessor.processFrames(self.processFramesFunction)
+        if p.numSources:
+            out = self.gccNMFProcessor.processBlock(block, p.hopSize, p.blockSize)
+        else:
+            self.inputFrames[:] = block
+            self.oladProcessor.processFrames(self.processFramesFunction)
+            out = self.outputFrames
         self.processingTimes.append(time.time() - startTime)
-        return self.outputFrames
+        return out
 
     def processSamples(self, samples, flush=True):
-        """samples (numChannels, n) float32 -> (numChannels, n_out) float32: whole blocks of the file, then (flush) two
-        silent blocks so that the tail leaves the overlap-add ring; n_out = (blocks [+ 2]) * blockSize."""
+        """samples (numChannels, n) float32 -> (numChannels, n_out) float32 ((numSources, numChannels, n_out) with sources): whole
+        blocks of the file, then (flush) two silent blocks so that the tail leaves the overlap-add ring; n_out = (blocks [+ 2]) * blockSize."""
         p = self.params
         samples = np.asarray(samples, dtype=np.float32)
         if samples.ndim != 2 or samples.shape[0] != p.numChannels:
@@ -110,9 +127,9 @@ class RealtimeGCCNMFNoGUI(object):
         total = numBlocks + (2 if flush else 0)
         padded = np.zeros((p.numChannels, total * B), np.float32)
         padded[:, :samples.shape[1]] = samples
-        out = np.empty_like(padded)
+        out = np.empty(((p.numSources,) if p.numSources else ()) + padded.shape, np.float32)
         for b in range(total):
-            out[:, b * B:(b + 1) * B] = self.processBlock(padded[:, b * B:(b + 1) * B])
+            out[..., b * B:(b + 1) * B] = self.processBlock(padded[:, b * B:(b + 1) * B])
         return out
 
     def processingTimeStats(self):
@@ -131,18 +148,25 @@ class RealtimeGCCNMFNoGUI(object):
     def _writeOutput(self, out, numSamples, outputPath, alignOutput):
         from scipy.io import wavfile
         if alignOutput:
-            out = out[:, self.latencySamples:self.latencySamples + numSamples]
+            out = out[..., self.latencySamples:self.latencySamples + numSamples]
         if outputPath is not None:
             wavfile.write(outputPath, self.params.sampleRate, float2pcm(np.ascontiguousarray(out.T)))
         return out
 
     def run(self, outputPath=None, alignOutput=True):
         """Reads params.audioPath (int16 stereo wav), enhances it block by block and, when `outputPath` is given, writes
-        the int16 result.  alignOutput drops the two-block latency so that output sample i corresponds to input sample i."""
-        samples = self._readSamples(self.params.audioPath)
+        the int16 result.  alignOutput drops the two-block latency so that output sample i corresponds to input sample i.
+        With sources, `outputPath` is a list of numSources paths (one wav per source) and the result is (numSources, 2, n)."""
+        p = self.params
+        samples = self._readSamples(p.audioPath)
         out = self.processSamples(samples, flush=True)
         logging.info('Processing times (min/max/avg): %f, %f, %f' % self.processingTimeStats())
-        return self._writeOutput(out, samples.shape[1], outputPath, alignOutput)
+        if not p.numSources:
+            return self._writeOutput(out, samples.shape[1], outputPath, alignOutput)
+        if outputPath is not None and len(outputPath) != p.numSources:
+            raise ValueError('%d sources, %d output paths' % (p.numSources, len(outputPath)))
+        return np.stack([self._writeOutput(out[s], samples.shape[1], outputPath[s] if outputPath is not None else None, alignOutput)
+                         for s in range(p.numSources)])
 
     def runMany(self, audioPaths, outputPaths=None, alignOutput=True):
         """Several wav files enhanced concurrently, each in its own slot of ONE MultiStreamRealtimeEngine: per block, one graph
@@ -153,6 +177,8 @@ class RealtimeGCCNMFNoGUI(object):
         g = self.gccNMFProcessor
         if g is None:
             raise ValueError('runMany runs the built-in GCCNMFProcessor; this runner was given another processFramesFunction')
+        if self.params.numSources:
+            raise ValueError('runMany enhances one source per file; numSources is not supported there')
         if outputPaths is not None and len(outputPaths) != len(audioPaths):
             raise ValueError('%d input paths, %d output paths' % (len(audioPaths), len(outputPaths)))
         p = self.params
@@ -192,20 +218,27 @@ def parseArguments(argv=None):
     """config.py:122-127 plus the output path and the dictionary directory (the reference takes DATA_DIR from defs.py)."""
     parser = argparse.ArgumentParser(description='Headless real-time GCC-NMF speech enhancement (H100)')
     parser.add_argument('-i', '--input', nargs='+', help='input wav file path(s); several are enhanced concurrently in one engine', required=True)
-    parser.add_argument('-o', '--output', nargs='+', help='output wav file path(s), one per input', required=True)
+    parser.add_argument('-o', '--output', nargs='+', help='output wav file path(s): one per input, or one per source with --num-sources',
+                        required=True)
     parser.add_argument('-d', '--data-dir', help='directory with chimeTrainSet.npy and / or pretrainedW/', required=True)
     parser.add_argument('--dictionary-size', type=int, default=DEFAULT_PARAMS['dictionarySize'])
+    parser.add_argument('--num-sources', type=int, default=0, help='separate one input into this many sources (2 .. 8) instead of enhancing it')
     return parser.parse_args(argv)
 
 
 if __name__ == '__main__':
     logging.getLogger().setLevel(logging.INFO)
     args = parseArguments()
-    if len(args.input) != len(args.output):
+    if args.num_sources:
+        if len(args.input) != 1 or len(args.output) != args.num_sources:
+            raise SystemExit('--num-sources %d: one input path and %d output paths' % (args.num_sources, args.num_sources))
+    elif len(args.input) != len(args.output):
         raise SystemExit('%d input paths, %d output paths' % (len(args.input), len(args.output)))
     runner = RealtimeGCCNMFNoGUI(args.input[0], dataDir=args.data_dir, dictionarySize=args.dictionary_size,
-                                 dictionarySizes=[args.dictionary_size])
-    if len(args.input) == 1:
+                                 dictionarySizes=[args.dictionary_size], numSources=args.num_sources)
+    if args.num_sources:
+        runner.run(args.output)
+    elif len(args.input) == 1:
         runner.run(args.output[0])
     else:
         runner.runMany(args.input, args.output)

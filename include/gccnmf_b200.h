@@ -409,6 +409,48 @@ GCCNMF_API int gccnmf_rtm_graph_create(gccnmf_handle* h, const gccnmf_rt_config*
 GCCNMF_API int gccnmf_rtm_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state, size_t state_bytes,
                       int slot, int what, void* dst, void* stream);
 
+/* ---- S streams, each separated into P sources: one output block per target TDOA (TARGET_MODE_MULTIPLE) ---------------
+ * The multi-target rule of gccNMFFunctions.py:118-143 applied per block.  A slot has P target TDOA indexes tau_0 .. tau_{P-1}
+ * in [0, D), 2 <= P <= 8.  For every atom k and frame t the winner is argmax_q gccNMF[tau_q][t][k] (the float32 values of the
+ * per-atom contraction) under numpy.argmax's order: a NaN first, then the larger value, then the lower source index (so an
+ * all-NaN column, which numpy.nanargmax rejects, and every tie go to the lowest source).  mask_q = (winner == q) (f64 0 / 1);
+ * source q is then exactly the single-target filter and synthesis fed mask_q, overlap-added into its own output ring.  The P
+ * masks partition the atoms, so the P outputs sum to the separation-off output up to float64 rounding of the mask sums.
+ * Separation off: every source outputs the mixture.  Inactive slot: every source outputs zeros.
+ * Targets: gccnmf_rtsep_set_targets, or with localisation on the P largest strict local maxima of the windowed GCC-PHAT mean in
+ * ascending order (estimateTargetTDOAIndexesFromAngularSpectrum, gccNMFFunctions.py:94-116) become the targets of the NEXT
+ * block; with fewer than P peaks the targets stay and status bit GCCNMF_RTSEP_STATUS_FEW_PEAKS is set (sticky until reset).
+ * Defaults after init / reset_slots: tau_q = floor((2 q + 1) D / (2 P)).
+ * Buffers: in blocks (S, 2, B), out blocks (S, P, 2, B), windowed frames in (S, 2, N, nT), out (S, P, 2, N, nT).
+ * Export items 0 .. 8 as gccnmf_rt_export (2 and 4: source 0's), plus 9 targets (P) i32, 10 source masks (P, K, nT) f64,
+ * 11 target values gccNMF[tau_q] (P, K, nT) f32, 12 output spectrograms (P, 2, F, nT) c64, 13 status word i32.
+ * num_sources outside [2, 8], targets outside [0, D) and localisation with D < 3 fail before anything is enqueued. */
+#define GCCNMF_RTSEP_MAX_SOURCES 8
+#define GCCNMF_RTSEP_STATUS_FEW_PEAKS 1
+/* Host only; 0 for an invalid configuration, num_streams or num_sources.  Grows linearly in num_streams. */
+GCCNMF_API size_t gccnmf_rtsep_state_bytes(const gccnmf_rt_config* cfg, int num_streams, int num_sources);
+GCCNMF_API int gccnmf_rtsep_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, const float* W,
+                      const float* E, const float* analysis_window, const float* synthesis_window, const float* H0, void* state,
+                      size_t state_bytes, void* stream);
+GCCNMF_API int gccnmf_rtsep_reset_slots(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state,
+                             size_t state_bytes, int first_slot, int count, void* stream);
+/* As gccnmf_rtm_set_params; mode, target_index and set_target are ignored. */
+GCCNMF_API int gccnmf_rtsep_set_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state,
+                            size_t state_bytes, int first_slot, int count, const gccnmf_rtm_slot_params* params, void* stream);
+/* targets_host: count x P host array, consumed before the call returns; -1 keeps that source's target. */
+GCCNMF_API int gccnmf_rtsep_set_targets(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state,
+                             size_t state_bytes, int first_slot, int count, const int32_t* targets_host, void* stream);
+GCCNMF_API int gccnmf_rtsep_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state,
+                                size_t state_bytes, const float* windowed, float* out, void* stream);
+GCCNMF_API int gccnmf_rtsep_process_block(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state,
+                               size_t state_bytes, const float* in_blocks, float* out_blocks, void* stream);
+/* Launch / destroy with gccnmf_rt_graph_launch / gccnmf_rt_graph_destroy. */
+GCCNMF_API int gccnmf_rtsep_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state,
+                              size_t state_bytes, float* in_blocks, float* out_blocks, const float* in_host, float* out_host,
+                              void** graph_exec, void* stream);
+GCCNMF_API int gccnmf_rtsep_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state,
+                        size_t state_bytes, int slot, int what, void* dst, void* stream);
+
 /*
  * The building block the KL-NMF loop runs on (klnmf_tma.cu): the same 3-product contraction, TMA-fed, over operands
  * that are pre-split into bf16 hi/lo planes and kept in ONE orientation each; an operand contracted over its
