@@ -141,6 +141,23 @@ SIGNATURES.update({
     'gccnmf_rtsep_export': (c_int, [_H, _C, c_int, c_int, _P, c_size_t, c_int, c_int, c_void_p, _S]),
 })
 
+_PP = ctypes.POINTER(c_void_p)   # host array of device pointers
+_BANK = [_H, _C, c_int, c_int, c_int, c_int, _P, c_size_t]     # h, cfg, S, P, Qd, Qe, state, state_bytes
+SIGNATURES.update({
+    'gccnmf_rtbank_state_bytes': (c_size_t, [_C, c_int, c_int, c_int, c_int]),
+    'gccnmf_rtbank_init': (c_int, _BANK + [_PP, ctypes.POINTER(c_int), _PP, _PP, _P, _P, _S]),
+    'gccnmf_rtbank_load_dictionary': (c_int, _BANK + [c_int, _P, c_int, _P, _S]),
+    'gccnmf_rtbank_load_steering': (c_int, _BANK + [c_int, _P, _S]),
+    'gccnmf_rtbank_assign': (c_int, _BANK + [c_int, c_int, ctypes.POINTER(c_int32), ctypes.POINTER(c_int32), _S]),
+    'gccnmf_rtbank_reset_slots': (c_int, _BANK + [c_int, c_int, _S]),
+    'gccnmf_rtbank_set_params': (c_int, _BANK + [c_int, c_int, ctypes.POINTER(RtmSlotParams), _S]),
+    'gccnmf_rtbank_set_targets': (c_int, _BANK + [c_int, c_int, ctypes.POINTER(c_int32), _S]),
+    'gccnmf_rtbank_process_frames': (c_int, _BANK + [_P, _P, _P, _S]),
+    'gccnmf_rtbank_process_block': (c_int, _BANK + [_P, _P, _P, _S]),
+    'gccnmf_rtbank_graph_create': (c_int, _BANK + [_P, _P, _P, _P, ctypes.POINTER(c_void_p), _S]),
+    'gccnmf_rtbank_export': (c_int, _BANK + [c_int, c_int, c_void_p, _S]),
+})
+
 _lib = None
 
 

@@ -36,6 +36,16 @@
 // another; filter, synthesis and emit run once per source (a source dimension in the grid), each source through the same code
 // and order a single-target slot runs.  Analysis, inference, the input ring and the localisation run once per slot; with
 // localisation on, the P largest peaks of the windowed GCC-PHAT mean become the targets of the next block.
+//
+// Bank (gccnmf_rtbank_*, the reference's per-processor dictionary size / type and microphone spacing, gccNMFProcessor.py:131-157).
+// The shared region holds Qd dictionary entries (W, W^T, recV, colsumW, H0, each sized at K_max = cfg.num_atoms, entry i with its
+// own K_i <= K_max) and Qe steering entries (E^T) at fixed strides, the K_i table and the slots sorted by dictionary (stable).
+// Every slot region ends with the slot's (dictionary, steering) pair.  Each kernel reads the entries of its slot through one
+// by-value RtBank argument; the empty bank (gccnmf_rt_*, rtm, rtsep) puts every slot on the layout's one dictionary and table.
+// Slot s on (i, j) computes bit for bit what a single-stream state built with (W_i, E_j) computes: every per-output order
+// depends only on the contracted index.  The inference and filter kernels run one slot per warp with a bank; rt_atoms takes its
+// (slot, frame) pairs in dictionary order, so a CTA spans more than one entry only where the sorted order changes entry, and
+// then runs its f loop once per entry.
 #include <cmath>
 
 #include "common.cuh"
@@ -50,6 +60,7 @@ constexpr int kRtRingBlocks = 8;         // utils.py:85 numBlocksPerBuffer
 constexpr int kRtMaxStreams = 4096;      // slots per state buffer
 constexpr int kRtAtomsFc = 32;           // f values per shared-memory stage of the atoms contraction
 constexpr int kRtMaxSources = GCCNMF_RTSEP_MAX_SOURCES;
+constexpr int kRtMaxBank = GCCNMF_RTBANK_MAX_ENTRIES;   // dictionary entries and steering entries, each
 
 struct RtDev {                           // device-resident parameters + loop-carried state (first bytes of a slot region)
   float target, eps, beta, noise_floor;  // gccNMFProcessor.py:196-199 (Theano shared scalars)
@@ -64,6 +75,19 @@ template <typename T>
 __host__ __device__ __forceinline__ T* rt_slot(T* p0, int s, size_t stride) {
   return (T*)((const char*)p0 + (size_t)s * stride);
 }
+
+// Where the kernels find a slot's dictionary and steering entries.  All zero (the empty bank): every slot on entry 0 of K atoms.
+struct RtBank {
+  int32_t* assign;                       // slot 0's (dictionary, steering, K_i of the last block computed), slot-strided
+  const int32_t* K;                      // K_i of every dictionary entry
+  const int32_t* order;                  // the S slots sorted by dictionary index (stable)
+  size_t dict_stride, steer_stride;      // bytes from one entry to the next (W, W^T, recV, colsumW, H0 / E^T)
+};
+__device__ __forceinline__ int2 rt_entry(const RtBank& b, int s, size_t stride) {
+  return b.assign ? *reinterpret_cast<const int2*>(rt_slot(b.assign, s, stride)) : int2{0, 0};
+}
+__device__ __forceinline__ int rt_sorted_slot(const RtBank& b, int i) { return b.order ? b.order[i] : i; }
+__device__ __forceinline__ int rt_atoms_of(const RtBank& b, int dict, int K) { return b.K ? b.K[dict] : K; }
 
 struct RtLayout {                        // carve of the caller-owned state buffer (pure function of the configuration and S)
   // shared by every slot
@@ -84,12 +108,17 @@ struct RtLayout {                        // carve of the caller-owned state buff
   float *sframes, *sout, *tval;
   int32_t *targets, *status;
   size_t src_stride;
+  // Qd, Qe > 0: W .. H0 and ET above are entry 0 of the bank (entry i at rt_slot(p, i, bank.dict_stride) / bank.steer_stride),
+  // bank_K (Qd), order (S) in the shared region, assign (2 per slot) at the end of every slot region.
+  RtBank bank;
+  int32_t *bank_K, *order, *assign;
+  int Qd, Qe;
   int F, Fp, L, S, P, D;
   size_t stride, bytes;
   bool ok;
 };
 
-RtLayout rt_carve(const gccnmf_rt_config& c, int S, int P, void* state, size_t state_bytes) {
+RtLayout rt_carve(const gccnmf_rt_config& c, int S, int P, void* state, size_t state_bytes, int Qd = 0, int Qe = 0) {
   RtLayout l{};
   const int N = c.window_size, nT = c.windows_per_block, K = c.num_atoms, D = c.num_tdoas;
   l.F = N / 2 + 1;
@@ -98,18 +127,33 @@ RtLayout rt_carve(const gccnmf_rt_config& c, int S, int P, void* state, size_t s
   l.S = S;
   l.P = P;
   l.D = D;
+  l.Qd = Qd;
+  l.Qe = Qe;
   char* base = state ? static_cast<char*>(state) : reinterpret_cast<char*>(256);
   WorkspaceCarver w(base, ~size_t(0) >> 1);
   l.tw64 = w.take<double>(N);
   l.tw32 = w.take<float>(N);
   l.win_a = w.take<float>(N);
   l.win_s = w.take<float>(N);
-  l.W = w.take<float>((size_t)l.F * K);
-  l.WT = w.take<float>((size_t)K * l.Fp);
-  l.recV = w.take<float>(l.F);
-  l.colsumW = w.take<float>(K);
-  l.H0 = w.take<float>((size_t)K * 2);
+  {                                      // the one dictionary, or entry 0 of Qd (each carved alike from a 256-aligned base)
+    WorkspaceCarver u(w.take<char>(0), ~size_t(0) >> 1);
+    l.W = u.take<float>((size_t)l.F * K);
+    l.WT = u.take<float>((size_t)K * l.Fp);
+    l.recV = u.take<float>(l.F);
+    l.colsumW = u.take<float>(K);
+    l.H0 = u.take<float>((size_t)K * 2);
+    l.bank.dict_stride = Qd > 0 ? align_up(u.used, 256) : 0;
+    w.take<char>(Qd > 0 ? Qd * l.bank.dict_stride : u.used);
+  }
   l.ET = w.take<float2>((size_t)D * l.Fp);
+  if (Qe > 0) {
+    l.bank.steer_stride = align_up((size_t)D * l.Fp * sizeof(float2), 256);
+    w.take<char>((size_t)(Qe - 1) * l.bank.steer_stride);
+  }
+  if (Qd > 0) {
+    l.bank_K = w.take<int32_t>(kRtMaxBank);
+    l.order = w.take<int32_t>(S);
+  }
   const size_t shared = align_up(w.used, 256);
   WorkspaceCarver v(base + shared, ~size_t(0) >> 1);
   l.dev = v.take<RtDev>(1);
@@ -143,6 +187,12 @@ RtLayout rt_carve(const gccnmf_rt_config& c, int S, int P, void* state, size_t s
     l.src_stride = align_up(u.used, 256);
     v.take<char>((size_t)P * l.src_stride);
   }
+  if (Qd > 0) {
+    l.assign = v.take<int32_t>(3);       // zeroed by init and reset_slots: entries (0, 0), no block computed yet
+    l.bank.assign = l.assign;
+    l.bank.K = l.bank_K;
+    l.bank.order = l.order;
+  }
   l.stride = align_up(v.used, 256);
   l.bytes = shared + (size_t)S * l.stride;
   l.ok = state != nullptr && S >= 1 && l.bytes <= state_bytes;
@@ -167,11 +217,20 @@ int rt_check(gccnmf_handle* h, const gccnmf_rt_config* c, int S = 1, int P = 0) 
   return 0;
 }
 
+// A bank needs entries of both kinds (the empty bank is the rtm / rtsep layout).
+int rt_check_bank(gccnmf_handle* h, int Qd, int Qe) {
+  GCCNMF_REQUIRE(h, Qd >= 1 && Qd <= kRtMaxBank && Qe >= 1 && Qe <= kRtMaxBank,
+                 "rtbank: num_dictionaries and num_steerings must be in [1, %d] (got %d, %d)", kRtMaxBank, Qd, Qe);
+  return 0;
+}
+
 // ---------------------------------------------------------------------------------------------- init-time kernels
+// K_out (bank entries): the entry's atom count, written for the kernels of the next blocks.
 __global__ void rt_init_dictionary_kernel(const float* __restrict__ W, int F, int Fp, int K, float* __restrict__ WT, float* __restrict__ recV,
-                                          float* __restrict__ colsumW) {
+                                          float* __restrict__ colsumW, int32_t* __restrict__ K_out) {
   // one thread per atom: column sum in row order (numpy.sum(W, axis=0)) + transposed copy; one thread per bin: row sum
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (K_out && i == 0) *K_out = K;
   if (i < K) {
     float s = 0.f;
     for (int f = 0; f < Fp; ++f) {
@@ -238,6 +297,46 @@ __global__ void rt_set_targets_kernel(int32_t* targets0, size_t stride, int firs
     if (b.t[i * P + q] >= 0) t[q] = b.t[i * P + q];
 }
 
+// (dictionary, steering) entries of up to kRtParamsPerLaunch slots, by value; -1 keeps the slot's entry.
+struct RtAssignBatch {
+  int32_t d[kRtParamsPerLaunch], e[kRtParamsPerLaunch];
+};
+__global__ void rt_assign_kernel(int32_t* assign0, size_t stride, int first, int count, RtAssignBatch b) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  int32_t* a = rt_slot(assign0, first + i, stride);
+  if (b.d[i] >= 0) a[0] = b.d[i];
+  if (b.e[i] >= 0) a[1] = b.e[i];
+}
+
+// Stable counting sort of the S slots by dictionary index, by one warp over chunks of 32 slots: order lists the slots of entry 0
+// in slot order, then those of entry 1, ...  Inactive slots are listed too (the kernels skip them).
+__global__ void __launch_bounds__(32) rt_sort_slots_kernel(const int32_t* __restrict__ assign0, size_t stride, int S, int Qd, int32_t* __restrict__ order) {
+  __shared__ int base[kRtMaxBank];
+  const int lane = threadIdx.x;
+  for (int i = lane; i < Qd; i += 32) base[i] = 0;
+  __syncwarp();
+  for (int pass = 0; pass < 2; ++pass) {               // 0: count per entry, 1: place
+    for (int s0 = 0; s0 < S; s0 += 32) {
+      const int s = s0 + lane;
+      const int d = s < S ? rt_slot(assign0, s, stride)[0] : -1;
+      const unsigned peers = __match_any_sync(0xffffffffu, d);
+      const bool leader = lane == __ffs(peers) - 1;
+      if (pass == 1 && d >= 0) order[base[d] + __popc(peers & ((1u << lane) - 1u))] = s;
+      __syncwarp();
+      if (leader && d >= 0) base[d] += __popc(peers);
+      __syncwarp();
+    }
+    if (pass == 0 && lane == 0)                        // counts -> first positions
+      for (int i = 0, sum = 0; i < Qd; ++i) {
+        const int n = base[i];
+        base[i] = sum;
+        sum += n;
+      }
+    __syncwarp();
+  }
+}
+
 // ---------------------------------------------------------------------------------------------- numerics shared with gcc.cu
 // numpy / Theano complex64 arithmetic of  X0 * conj(X1) / |X0| / |X1|  (gccNMFProcessor.py:253; runGCCNMF.py:44)
 __device__ __forceinline__ float2 rt_coherence(float2 a, float2 b) {
@@ -277,12 +376,17 @@ rt_analysis_kernel(const RtDev* __restrict__ dev0, size_t stride, const float* _
                    const float* __restrict__ in_blocks, const float* __restrict__ in_ring0, int B, int L, int hop, int nT,
                    const float* __restrict__ win_a, const double2* __restrict__ tw, int N, int log2n, const float2* __restrict__ ET, int D, int Fp,
                    float2* __restrict__ X0, float* __restrict__ G0, float* __restrict__ gccphat0, float* __restrict__ Vabs0,
-                   const float* __restrict__ H0, float* __restrict__ Hs0, int K, int inference) {
+                   const float* __restrict__ H0, float* __restrict__ Hs0, int K, int inference, RtBank bank) {
   __shared__ double2 fft[kRtMaxN];
   __shared__ float2 coh[kRtMaxN / 2 + 1];
   const int t = blockIdx.x, s = blockIdx.y, F = N / 2 + 1;
   const RtDev* dev = rt_slot(dev0, s, stride);
   if (!dev->active) return;
+  const int2 entry = rt_entry(bank, s, stride);      // the slot's steering table and inference seed
+  ET = rt_slot(ET, entry.y, bank.steer_stride);
+  H0 = rt_slot(H0, entry.x, bank.dict_stride);
+  K = rt_atoms_of(bank, entry.x, K);
+  if (bank.assign && t == 0 && threadIdx.x == 0) rt_slot(bank.assign, s, stride)[2] = K;    // the shape of this block's K-shaped items
   const float* in_ring = rt_slot(in_ring0, s, stride);
   const float* in_block = in_blocks ? in_blocks + (int64_t)s * 2 * B : nullptr;
   if (windowed) windowed += (int64_t)s * 2 * N * nT;
@@ -365,13 +469,19 @@ constexpr int rt_inf_slots(int J) { return J >= 16 ? 1 : 16 / J; }
 constexpr int rt_filter_slots(int NT) { return NT >= 8 ? 1 : 8 / NT; }
 
 // R[f][j] = V[f][j] / sum_k W[f][k] H[k][j]   (gccNMFFunctions.py:76, V / dot(W, H)); one warp per bin and SG slots, J = 2 nT
-// columns.  Per slot and column: lane-strided fmaf over k from 0.f, then the xor butterfly.
+// columns.  Per slot and column: lane-strided fmaf over k from 0.f, then the xor butterfly.  With a bank, one slot per warp (SG = 1)
+// and the W, W^T and colsumW of the slot's dictionary entry: the order over k does not depend on the entry.
 template <int J, int SG>
 __global__ void __launch_bounds__(256)
 rt_inf_ratio_kernel(const RtDev* __restrict__ dev0, size_t stride, int S, const float* __restrict__ W, const float* __restrict__ H0,
-                    const float* __restrict__ V0, int F, int K, float* __restrict__ R0) {
+                    const float* __restrict__ V0, int F, int K, float* __restrict__ R0, RtBank bank) {
   const int f = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31, s0 = blockIdx.y * SG;
   if (f >= F) return;
+  if constexpr (SG == 1) {                           // the slot's dictionary entry (grouped warps run without a bank only)
+    const int dict = rt_entry(bank, s0, stride).x;
+    W = rt_slot(W, dict, bank.dict_stride);
+    K = rt_atoms_of(bank, dict, K);
+  }
   bool on[SG];
   bool any = false;
 #pragma unroll
@@ -413,9 +523,15 @@ rt_inf_ratio_kernel(const RtDev* __restrict__ dev0, size_t stride, int S, const 
 template <int J, int SG>
 __global__ void __launch_bounds__(256)
 rt_inf_update_kernel(const RtDev* __restrict__ dev0, size_t stride, int S, const float* __restrict__ WT, int Fp, const float* __restrict__ R0, int F,
-                     int K, const float* __restrict__ colsumW, float alpha, float eps, float* __restrict__ H0) {
+                     int K, const float* __restrict__ colsumW, float alpha, float eps, float* __restrict__ H0, RtBank bank) {
   const int k = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31, s0 = blockIdx.y * SG;
-  if (k >= K) return;
+  if (k >= K) return;                                // the grid is rounded up to whole CTAs of 8 warps
+  if constexpr (SG == 1) {                           // the slot's dictionary entry (grouped warps run without a bank only)
+    const int dict = rt_entry(bank, s0, stride).x;
+    if (k >= rt_atoms_of(bank, dict, K)) return;    // the grid covers K_max atoms
+    WT = rt_slot(WT, dict, bank.dict_stride);
+    colsumW = rt_slot(colsumW, dict, bank.dict_stride);
+  }
   bool on[SG];
   bool any = false;
 #pragma unroll
@@ -469,21 +585,27 @@ template <int TM, int TN>
 __global__ void __launch_bounds__(256)
 rt_atoms_kernel(const RtDev* __restrict__ dev0, size_t stride, int pairs, int nT, const float* __restrict__ G0, const float* __restrict__ W, int F,
                 int Fp, int K, int D, int Dp, int32_t* __restrict__ argmax0, double* __restrict__ hmask0, const int32_t* __restrict__ targets0, int P,
-                size_t src_stride, float* __restrict__ tval0) {
+                size_t src_stride, float* __restrict__ tval0, RtBank bank) {
   constexpr int RB = 16 * TM, KB = 16 * TN, GS = RB + 4, FC = kRtAtomsFc;
   static_assert(RB % 32 == 0 && (TM <= 2 || TM % 4 == 0) && (TN < 4 || TN % 4 == 0), "tile shape");
   static_assert(32 * KB + (RB / 32) * kRtMaxSources * KB <= FC * GS + FC * KB, "target rows must fit beside the argmax partials");
   __shared__ __align__(16) float sm[FC * GS + FC * KB];
-  __shared__ int act[RB / 32];
+  __shared__ int act[RB / 32], slot_of[RB / 32], dict_of[RB / 32], atoms_of[RB / 32];
   __shared__ int tgt[RB / 32][kRtMaxSources];
   float* Gs = sm;                         // [f][row]
   float* Ws = sm + FC * GS;               // [f][atom]
-  const int ppc = RB / Dp, k0 = blockIdx.x * KB, gp0 = blockIdx.y * ppc;
+  // pairs per CTA: the narrow tile is launched with Dp = 16 TM, one pair, which lets the compiler drop the per-entry pass loop
+  const int ppc = TN == 1 ? 1 : RB / Dp, k0 = blockIdx.x * KB, gp0 = blockIdx.y * ppc;
   const int ag = threadIdx.x & 15, rg = threadIdx.x >> 4;
-  if (threadIdx.x < ppc) {
+  if (threadIdx.x < ppc) {                // pair gp: frame gp % nT of the slot at sorted position gp / nT
     const int gp = gp0 + threadIdx.x;
-    act[threadIdx.x] = gp < pairs && rt_slot(dev0, gp / nT, stride)->active;
-    for (int q = 0; q < P; ++q) tgt[threadIdx.x][q] = act[threadIdx.x] ? rt_slot(targets0, gp / nT, stride)[q] : -1;
+    const int s = gp < pairs ? rt_sorted_slot(bank, gp / nT) : 0;
+    const int e = rt_entry(bank, s, stride).x;
+    slot_of[threadIdx.x] = s;
+    dict_of[threadIdx.x] = e;
+    atoms_of[threadIdx.x] = rt_atoms_of(bank, e, K);
+    act[threadIdx.x] = gp < pairs && rt_slot(dev0, s, stride)->active && k0 < atoms_of[threadIdx.x];
+    for (int q = 0; q < P; ++q) tgt[threadIdx.x][q] = act[threadIdx.x] ? rt_slot(targets0, s, stride)[q] : -1;
   }
   __syncthreads();
   bool any = false;
@@ -496,56 +618,69 @@ rt_atoms_kernel(const RtDev* __restrict__ dev0, size_t stride, int pairs, int nT
 #pragma unroll
     for (int j = 0; j < TN; ++j) acc[i][j] = 0.f;
   auto atom_of = [&](int j) { return TN >= 4 ? (j >> 2) * 64 + ag * 4 + (j & 3) : j * 16 + ag; };
+  const int mine = (rg * TM) / Dp;        // the pair of this thread's rows (a warp's rows lie in one pair)
 
-  for (int f0 = 0; f0 < F; f0 += FC) {
-    // G stage: float4 along f (Fp % 4 == 0, G zero on [F, Fp)), transposed into Gs[f][row]
-    for (int i = threadIdx.x; i < RB * (FC / 4); i += 256) {
-      const int row = i / (FC / 4), fq = i - row * (FC / 4), p = row / Dp, d = row - p * Dp, gp = gp0 + p, f = f0 + 4 * fq;
-      float4 v = float4{0.f, 0.f, 0.f, 0.f};
-      if (d < D && act[p] && f < Fp) {
-        const int s = gp / nT, t = gp - s * nT;
-        v = *reinterpret_cast<const float4*>(rt_slot(G0, s, stride) + ((int64_t)t * D + d) * Fp + f);
+  // One f loop per distinct dictionary entry of the CTA's active pairs (one pass unless the pairs straddle entries); a thread
+  // accumulates only in its own pair's pass, so every output is still one fmaf chain over f.
+  for (int pass = 0; pass < ppc; ++pass) {
+    bool first = act[pass] != 0;
+    for (int p = 0; p < pass; ++p) first &= !(act[p] && dict_of[p] == dict_of[pass]);
+    if (!first) continue;
+    const int e = dict_of[pass], Ke = atoms_of[pass];
+    const float* We = rt_slot(W, e, bank.dict_stride);
+    const bool accumulate = TN == 1 || (act[mine] && dict_of[mine] == e);     // the narrow tile's one pair is active here
+    for (int f0 = 0; f0 < F; f0 += FC) {
+      // G stage: float4 along f (Fp % 4 == 0, G zero on [F, Fp)), transposed into Gs[f][row]
+      for (int i = threadIdx.x; i < RB * (FC / 4); i += 256) {
+        const int row = i / (FC / 4), fq = i - row * (FC / 4), p = row / Dp, d = row - p * Dp, gp = gp0 + p, f = f0 + 4 * fq;
+        float4 v = float4{0.f, 0.f, 0.f, 0.f};
+        if (d < D && act[p] && (TN == 1 || dict_of[p] == e) && f < Fp) {
+          const int t = gp % nT;
+          v = *reinterpret_cast<const float4*>(rt_slot(G0, slot_of[p], stride) + ((int64_t)t * D + d) * Fp + f);
+        }
+        Gs[(4 * fq + 0) * GS + row] = v.x;
+        Gs[(4 * fq + 1) * GS + row] = v.y;
+        Gs[(4 * fq + 2) * GS + row] = v.z;
+        Gs[(4 * fq + 3) * GS + row] = v.w;
       }
-      Gs[(4 * fq + 0) * GS + row] = v.x;
-      Gs[(4 * fq + 1) * GS + row] = v.y;
-      Gs[(4 * fq + 2) * GS + row] = v.z;
-      Gs[(4 * fq + 3) * GS + row] = v.w;
-    }
-    for (int i = threadIdx.x; i < FC * KB; i += 256) {
-      const int ff = i / KB, a = i - ff * KB;
-      Ws[i] = (f0 + ff < F && k0 + a < K) ? W[(int64_t)(f0 + ff) * K + k0 + a] : 0.f;
-    }
-    __syncthreads();
+      for (int i = threadIdx.x; i < FC * KB; i += 256) {
+        const int ff = i / KB, a = i - ff * KB;
+        Ws[i] = (f0 + ff < F && k0 + a < Ke) ? We[(int64_t)(f0 + ff) * Ke + k0 + a] : 0.f;
+      }
+      __syncthreads();
+      if (accumulate) {
 #pragma unroll 4
-    for (int ff = 0; ff < FC; ++ff) {
-      float a[TM], b[TN];
-      const float* gr = Gs + ff * GS + rg * TM;
-      if constexpr (TM % 4 == 0) {
+        for (int ff = 0; ff < FC; ++ff) {
+          float a[TM], b[TN];
+          const float* gr = Gs + ff * GS + rg * TM;
+          if constexpr (TM % 4 == 0) {
 #pragma unroll
-        for (int i = 0; i < TM; i += 4) {
-          const float4 q = *reinterpret_cast<const float4*>(gr + i);
-          a[i] = q.x; a[i + 1] = q.y; a[i + 2] = q.z; a[i + 3] = q.w;
+            for (int i = 0; i < TM; i += 4) {
+              const float4 q = *reinterpret_cast<const float4*>(gr + i);
+              a[i] = q.x; a[i + 1] = q.y; a[i + 2] = q.z; a[i + 3] = q.w;
+            }
+          } else {
+#pragma unroll
+            for (int i = 0; i < TM; ++i) a[i] = gr[i];
+          }
+          if constexpr (TN % 4 == 0) {
+#pragma unroll
+            for (int j = 0; j < TN; j += 4) {
+              const float4 q = *reinterpret_cast<const float4*>(Ws + ff * KB + atom_of(j));
+              b[j] = q.x; b[j + 1] = q.y; b[j + 2] = q.z; b[j + 3] = q.w;
+            }
+          } else {
+#pragma unroll
+            for (int j = 0; j < TN; ++j) b[j] = Ws[ff * KB + atom_of(j)];
+          }
+#pragma unroll
+          for (int i = 0; i < TM; ++i)
+#pragma unroll
+            for (int j = 0; j < TN; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);     // tensor.dot(realGCC.T, W) in float32 (:259)
         }
-      } else {
-#pragma unroll
-        for (int i = 0; i < TM; ++i) a[i] = gr[i];
       }
-      if constexpr (TN % 4 == 0) {
-#pragma unroll
-        for (int j = 0; j < TN; j += 4) {
-          const float4 q = *reinterpret_cast<const float4*>(Ws + ff * KB + atom_of(j));
-          b[j] = q.x; b[j + 1] = q.y; b[j + 2] = q.z; b[j + 3] = q.w;
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < TN; ++j) b[j] = Ws[ff * KB + atom_of(j)];
-      }
-#pragma unroll
-      for (int i = 0; i < TM; ++i)
-#pragma unroll
-        for (int j = 0; j < TN; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);     // tensor.dot(realGCC.T, W) in float32 (:259)
+      __syncthreads();
     }
-    __syncthreads();
   }
   // argmax over d: first over the thread's TM rows, then over the row groups of the pair (partials alias the stage buffers)
   float* part_v = sm;
@@ -579,8 +714,8 @@ rt_atoms_kernel(const RtDev* __restrict__ dev0, size_t stride, int pairs, int nT
   __syncthreads();
   const int groups = Dp / TM;
   for (int idx = threadIdx.x; idx < ppc * KB; idx += 256) {
-    const int p = idx / KB, a = idx - p * KB, gp = gp0 + p, k = k0 + a;
-    if (!act[p] || k >= K) continue;
+    const int p = idx / KB, a = idx - p * KB, gp = gp0 + p, k = k0 + a, Kp = atoms_of[p];
+    if (!act[p] || k >= Kp) continue;
     float bv = 0.f;
     int bi = -1;
     for (int r = p * groups; r < (p + 1) * groups; ++r) {
@@ -589,7 +724,7 @@ rt_atoms_kernel(const RtDev* __restrict__ dev0, size_t stride, int pairs, int nT
       const float cv = part_v[r * KB + a];
       if (bi < 0 || rt_better(cv, ci, bv, bi)) { bv = cv; bi = ci; }
     }
-    const int s = gp / nT, t = gp - s * nT;
+    const int s = slot_of[p], t = gp % nT;
     const RtDev* dev = rt_slot(dev0, s, stride);
     const int64_t o = (int64_t)k * nT + t;
     rt_slot(argmax0, s, stride)[o] = bi;
@@ -603,7 +738,7 @@ rt_atoms_kernel(const RtDev* __restrict__ dev0, size_t stride, int pairs, int nT
       float* tval = rt_slot(tval0, s, stride);
       for (int q = 0; q < P; ++q) {
         rt_slot(m0, q, src_stride)[o] = q == wi ? 1.0 : 0.0;
-        tval[((int64_t)q * K + k) * nT + t] = v[q * KB];
+        tval[((int64_t)q * Kp + k) * nT + t] = v[q * KB];          // (P, K_i, nT)
       }
       continue;
     }
@@ -618,14 +753,20 @@ rt_atoms_kernel(const RtDev* __restrict__ dev0, size_t stride, int pairs, int nT
 
 // ---------------------------------------------------------------------------------------------- C: time-frequency mask, one warp per bin and SG slots
 // Per slot, frame and channel: lane-strided float64 sums over k, then the xor butterfly.  blockIdx.z: the source (mask and Y at
-// src_stride per source).
+// src_stride per source).  With a bank, one slot per warp and the W, recV and K_i of the slot's dictionary entry.
 template <int NT, int SG, bool inference>
 __global__ void __launch_bounds__(256)
 rt_filter_kernel(const RtDev* __restrict__ dev0, size_t stride, int S, const float* __restrict__ W, const double* __restrict__ hmask0,
                  const float* __restrict__ recV, const float* __restrict__ H0, const float2* __restrict__ X0, int F, int K, float2* __restrict__ Y0,
-                 size_t src_stride) {
+                 size_t src_stride, RtBank bank) {
   const int f = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31, s0 = blockIdx.y * SG;
   if (f >= F) return;
+  if constexpr (SG == 1) {                           // the slot's dictionary entry (grouped warps run without a bank only)
+    const int dict = rt_entry(bank, s0, stride).x;
+    W = rt_slot(W, dict, bank.dict_stride);
+    recV = rt_slot(recV, dict, bank.dict_stride);
+    K = rt_atoms_of(bank, dict, K);
+  }
   hmask0 = rt_slot(hmask0, blockIdx.z, src_stride);
   Y0 = rt_slot(Y0, blockIdx.z, src_stride);
   bool on[SG];
@@ -864,39 +1005,40 @@ int ilog2_of(int n) {
   return l;
 }
 
-#define RT_CARVE_OR_FAIL_P(l, S, P)                                                                                                \
+#define RT_CARVE_OR_FAIL_B(l, S, P, Qd, Qe)                                                                                        \
   if (int st__ = rt_check(h, cfg, (S), (P))) return st__;                                                                          \
-  RtLayout l = rt_carve(*cfg, (S), (P), state, state_bytes);                                                                       \
+  RtLayout l = rt_carve(*cfg, (S), (P), state, state_bytes, (Qd), (Qe));                                                           \
   if (!l.ok) return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "rt state buffer missing or too small: need %zu bytes", l.bytes)
+#define RT_CARVE_OR_FAIL_P(l, S, P) RT_CARVE_OR_FAIL_B(l, S, P, 0, 0)
 #define RT_CARVE_OR_FAIL(l, S) RT_CARVE_OR_FAIL_P(l, S, 0)
 
 inline int rt_sources_grid(const RtLayout& l) { return l.P > 0 ? l.P : 1; }
 
 // Several slots per warp (the dictionary row read once for all of them) only while the grid still has kRtWavesForSlotGroups waves
-// of CTAs; with fewer streams one slot per warp keeps the device busy.
+// of CTAs; with fewer streams one slot per warp keeps the device busy.  A bank runs one slot per warp (each on its own entry).
 constexpr int kRtWavesForSlotGroups = 4;
-inline bool rt_group_slots(const gccnmf_handle* h, int ctas_x, int S, int SG) {
-  return SG > 1 && S > 1 && (int64_t)ctas_x * ((S + SG - 1) / SG) >= (int64_t)kRtWavesForSlotGroups * h->sm_count;
+inline bool rt_group_slots(const gccnmf_handle* h, const RtLayout& l, int ctas_x, int SG) {
+  return SG > 1 && l.S > 1 && l.Qd == 0 && (int64_t)ctas_x * ((l.S + SG - 1) / SG) >= (int64_t)kRtWavesForSlotGroups * h->sm_count;
 }
 
 template <int J, int SG>
 int rt_enqueue_inference_as(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout& l, bool ratio, void* stream) {
   const int F = l.F, K = cfg->num_atoms, S = l.S, gy = (S + SG - 1) / SG;
   if (ratio)
-    GCCNMF_LAUNCH(h, (rt_inf_ratio_kernel<J, SG>), dim3((F + 7) / 8, gy), 256, 0, stream, l.dev, l.stride, S, l.W, l.H, l.Vabs, F, K, l.R);
+    GCCNMF_LAUNCH(h, (rt_inf_ratio_kernel<J, SG>), dim3((F + 7) / 8, gy), 256, 0, stream, l.dev, l.stride, S, l.W, l.H, l.Vabs, F, K, l.R, l.bank);
   else
     GCCNMF_LAUNCH(h, (rt_inf_update_kernel<J, SG>), dim3((K + 7) / 8, gy), 256, 0, stream, l.dev, l.stride, S, l.WT, l.Fp, l.R, F, K, l.colsumW,
-                  cfg->sparsity_alpha, cfg->epsilon, l.H);
+                  cfg->sparsity_alpha, cfg->epsilon, l.H, l.bank);
   return 0;
 }
 template <int J>
 int rt_enqueue_inference(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout& l, void* stream) {
   constexpr int SG = rt_inf_slots(J);
-  const int F = l.F, K = cfg->num_atoms, S = l.S;
-  const int st = rt_group_slots(h, (F + 7) / 8, S, SG) ? rt_enqueue_inference_as<J, SG>(h, cfg, l, true, stream)
+  const int F = l.F, K = cfg->num_atoms;
+  const int st = rt_group_slots(h, l, (F + 7) / 8, SG) ? rt_enqueue_inference_as<J, SG>(h, cfg, l, true, stream)
                                                        : rt_enqueue_inference_as<J, 1>(h, cfg, l, true, stream);
   if (st) return st;
-  return rt_group_slots(h, (K + 7) / 8, S, SG) ? rt_enqueue_inference_as<J, SG>(h, cfg, l, false, stream)
+  return rt_group_slots(h, l, (K + 7) / 8, SG) ? rt_enqueue_inference_as<J, SG>(h, cfg, l, false, stream)
                                                : rt_enqueue_inference_as<J, 1>(h, cfg, l, false, stream);
 }
 
@@ -904,14 +1046,14 @@ template <int NT, int SG, bool INF>
 int rt_enqueue_filter_as(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout& l, void* stream) {
   const int F = l.F, K = cfg->num_atoms, S = l.S;
   GCCNMF_LAUNCH(h, (rt_filter_kernel<NT, SG, INF>), dim3((F + 7) / 8, (S + SG - 1) / SG, rt_sources_grid(l)), 256, 0, stream, l.dev, l.stride, S, l.W,
-                l.smask, l.recV, l.H, l.X, F, K, l.sY, l.src_stride);
+                l.smask, l.recV, l.H, l.X, F, K, l.sY, l.src_stride, l.bank);
   return 0;
 }
 template <int NT>
 int rt_enqueue_filter(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout& l, void* stream) {
   constexpr int SG = rt_filter_slots(NT);
   const bool inf = cfg->inference_iterations > 0;
-  if (!rt_group_slots(h, (l.F + 7) / 8, l.S, SG))
+  if (!rt_group_slots(h, l, (l.F + 7) / 8, SG))
     return inf ? rt_enqueue_filter_as<NT, 1, true>(h, cfg, l, stream) : rt_enqueue_filter_as<NT, 1, false>(h, cfg, l, stream);
   return inf ? rt_enqueue_filter_as<NT, SG, true>(h, cfg, l, stream) : rt_enqueue_filter_as<NT, SG, false>(h, cfg, l, stream);
 }
@@ -923,10 +1065,10 @@ int rt_enqueue_atoms(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayo
   const int big_ctas = ((K + 127) / 128) * ((pairs + 128 / Dp - 1) / (128 / Dp));
   if (big_ctas >= h->sm_count)
     GCCNMF_LAUNCH(h, (rt_atoms_kernel<8, 8>), dim3((K + 127) / 128, (pairs + 128 / Dp - 1) / (128 / Dp)), 256, 0, stream, l.dev, l.stride, pairs, nT,
-                  l.G, l.W, l.F, l.Fp, K, D, Dp, l.argmax, l.smask, l.targets, l.P, l.src_stride, l.tval);
+                  l.G, l.W, l.F, l.Fp, K, D, Dp, l.argmax, l.smask, l.targets, l.P, l.src_stride, l.tval, l.bank);
   else
     GCCNMF_LAUNCH(h, (rt_atoms_kernel<DJ, 1>), dim3((K + 15) / 16, pairs), 256, 0, stream, l.dev, l.stride, pairs, nT, l.G, l.W, l.F, l.Fp, K, D, Dp,
-                  l.argmax, l.smask, l.targets, l.P, l.src_stride, l.tval);
+                  l.argmax, l.smask, l.targets, l.P, l.src_stride, l.tval, l.bank);
   return 0;
 }
 
@@ -938,7 +1080,7 @@ int rt_enqueue_core(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayou
   const int inf = cfg->inference_iterations;
   GCCNMF_LAUNCH(h, rt_analysis_kernel, dim3(nT, S), kFftThreads, 0, stream, l.dev, l.stride, windowed, in_blocks, l.in_ring, cfg->block_size, l.L,
                 cfg->hop_size, nT, l.win_a, reinterpret_cast<const double2*>(l.tw64), N, log2n, l.ET, D, l.Fp, l.X, l.G, l.gccphat, l.Vabs, l.H0, l.H, K,
-                inf > 0 ? 1 : 0);
+                inf > 0 ? 1 : 0, l.bank);
   for (int it = 0; it < inf; ++it) {
     int st = 0;
     switch (nT) {
@@ -987,40 +1129,85 @@ int rt_enqueue_params(gccnmf_handle* h, const RtLayout& l, int first, int count,
   return 0;
 }
 
-// Zeroes the regions of slots [first, first + count) and gives them the defaults of gccNMFProcessor.py:190-199, active.
-int rt_enqueue_reset(gccnmf_handle* h, const RtLayout& l, int first, int count, void* stream) {
-  GCCNMF_CHECK_CUDA(h, cudaMemsetAsync(rt_slot(reinterpret_cast<char*>(l.dev), first, l.stride), 0, (size_t)count * l.stride, (cudaStream_t)stream));
-  GCCNMF_LAUNCH(h, rt_default_params_kernel, (count + 127) / 128, 128, 0, stream, l.dev, l.stride, first, count, l.targets, l.P, l.D);
+// A bank's slots in dictionary order, after every change of an assignment (stream-ordered, like the changes themselves).
+int rt_enqueue_sort(gccnmf_handle* h, const RtLayout& l, void* stream) {
+  if (l.Qd > 0) GCCNMF_LAUNCH(h, rt_sort_slots_kernel, 1, 32, 0, stream, l.assign, l.stride, l.S, l.Qd, l.order);
   return 0;
 }
 
-int rt_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, const float* W, const float* E, const float* analysis_window,
-            const float* synthesis_window, const float* H0, void* state, size_t state_bytes, void* stream) {
-  RT_CARVE_OR_FAIL_P(l, S, P);
-  GCCNMF_REQUIRE(h, W && E && analysis_window && synthesis_window, "rt_init: NULL pointer");
-  GCCNMF_REQUIRE(h, cfg->inference_iterations == 0 || H0 != nullptr, "rt_init: coefficient inference needs the initial H0 (K, 2)");
+// Zeroes the regions of slots [first, first + count) and gives them the defaults of gccNMFProcessor.py:190-199, active (and bank
+// entries (0, 0)).
+int rt_enqueue_reset(gccnmf_handle* h, const RtLayout& l, int first, int count, void* stream) {
+  GCCNMF_CHECK_CUDA(h, cudaMemsetAsync(rt_slot(reinterpret_cast<char*>(l.dev), first, l.stride), 0, (size_t)count * l.stride, (cudaStream_t)stream));
+  GCCNMF_LAUNCH(h, rt_default_params_kernel, (count + 127) / 128, 128, 0, stream, l.dev, l.stride, first, count, l.targets, l.P, l.D);
+  return rt_enqueue_sort(h, l, stream);
+}
+
+// Dictionary entry i (the layout's one dictionary without a bank): W (F, Ki) and H0 (Ki, 2) or NULL, device pointers.
+int rt_enqueue_dictionary(gccnmf_handle* h, const RtLayout& l, int i, const float* W, int Ki, const float* H0, void* stream) {
   cudaStream_t s = (cudaStream_t)stream;
-  const int N = cfg->window_size, K = cfg->num_atoms, D = cfg->num_tdoas;
+  const size_t st = l.bank.dict_stride;
+  float* We = rt_slot(l.W, i, st);
+  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(We, W, (size_t)l.F * Ki * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  if (H0) GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(rt_slot(l.H0, i, st), H0, (size_t)Ki * 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  const int n = Ki > l.F ? Ki : l.F;
+  GCCNMF_LAUNCH(h, rt_init_dictionary_kernel, (n + 127) / 128, 128, 0, stream, We, l.F, l.Fp, Ki, rt_slot(l.WT, i, st), rt_slot(l.recV, i, st),
+                rt_slot(l.colsumW, i, st), l.bank_K ? l.bank_K + i : nullptr);
+  return 0;
+}
+
+// Steering entry j (the layout's one table without a bank): E (F, D) complex64, a device pointer.
+int rt_enqueue_steering(gccnmf_handle* h, const RtLayout& l, int j, const float* E, void* stream) {
+  GCCNMF_LAUNCH(h, rt_init_steering_kernel, (l.D * l.Fp + 255) / 256, 256, 0, stream, reinterpret_cast<const float2*>(E), l.F, l.Fp, l.D,
+                rt_slot(l.ET, j, l.bank.steer_stride));
+  return 0;
+}
+
+// Qd dictionaries W[i] (F, K[i]) with H0[i] (K[i], 2) (H0 or H0[i] NULL without inference) and Qe steering tables E[j]; the
+// single-stream, rtm and rtsep entries pass one of each with Qd = Qe = 0 (no bank).
+int rt_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, int Qd, int Qe, const float* const* W, const int* K,
+            const float* const* H0, const float* const* E, const float* analysis_window, const float* synthesis_window, void* state,
+            size_t state_bytes, void* stream) {
+  RT_CARVE_OR_FAIL_B(l, S, P, Qd, Qe);
+  const int nd = Qd > 0 ? Qd : 1, ne = Qe > 0 ? Qe : 1;
+  GCCNMF_REQUIRE(h, W && K && E && analysis_window && synthesis_window, "rt_init: NULL pointer");
+  for (int i = 0; i < nd; ++i) {
+    GCCNMF_REQUIRE(h, W[i] != nullptr, "rt_init: NULL pointer");
+    GCCNMF_REQUIRE(h, K[i] >= 1 && K[i] <= cfg->num_atoms, "rt_init: dictionary %d: %d atoms outside [1, num_atoms = %d]", i, K[i], cfg->num_atoms);
+    GCCNMF_REQUIRE(h, cfg->inference_iterations == 0 || (H0 && H0[i]), "rt_init: coefficient inference needs the initial H0 (K, 2)");
+  }
+  for (int j = 0; j < ne; ++j) GCCNMF_REQUIRE(h, E[j] != nullptr, "rt_init: NULL pointer");
+  cudaStream_t s = (cudaStream_t)stream;
+  const int N = cfg->window_size;
   const double* tw64 = nullptr;
   const float* tw32 = nullptr;
   if (int st = gccnmf_get_twiddles(h, N, &tw64, &tw32)) return st;
-  GCCNMF_CHECK_CUDA(h, cudaMemsetAsync(state, 0, l.bytes, s));                 // rings, history (initValue = 0), counters
+  GCCNMF_CHECK_CUDA(h, cudaMemsetAsync(state, 0, l.bytes, s));                 // rings, history (initValue = 0), counters, entries (0, 0)
   GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.tw64, tw64, (size_t)N * sizeof(double), cudaMemcpyDeviceToDevice, s));
   GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.tw32, tw32, (size_t)N * sizeof(float), cudaMemcpyDeviceToDevice, s));
   GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.win_a, analysis_window, (size_t)N * sizeof(float), cudaMemcpyDeviceToDevice, s));
   GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.win_s, synthesis_window, (size_t)N * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.W, W, (size_t)l.F * K * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  if (H0) GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.H0, H0, (size_t)K * 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  const int n = K > l.F ? K : l.F;
-  GCCNMF_LAUNCH(h, rt_init_dictionary_kernel, (n + 127) / 128, 128, 0, stream, l.W, l.F, l.Fp, K, l.WT, l.recV, l.colsumW);
-  GCCNMF_LAUNCH(h, rt_init_steering_kernel, (D * l.Fp + 255) / 256, 256, 0, stream, reinterpret_cast<const float2*>(E), l.F, l.Fp, D, l.ET);
+  for (int i = 0; i < nd; ++i)
+    if (int st = rt_enqueue_dictionary(h, l, i, W[i], K[i], H0 ? H0[i] : nullptr, stream)) return st;
+  for (int j = 0; j < ne; ++j)
+    if (int st = rt_enqueue_steering(h, l, j, E[j], stream)) return st;
   GCCNMF_LAUNCH(h, rt_default_params_kernel, (S + 127) / 128, 128, 0, stream, l.dev, l.stride, 0, S, l.targets, l.P, l.D);
-  return GCCNMF_OK;
+  return rt_enqueue_sort(h, l, stream);
+}
+
+// The single-stream, rtm and rtsep form: one dictionary of cfg.num_atoms atoms, one steering table.
+int rt_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, const float* W, const float* E, const float* analysis_window,
+            const float* synthesis_window, const float* H0, void* state, size_t state_bytes, void* stream) {
+  const float* Ws[1] = {W};
+  const float* Es[1] = {E};
+  const float* H0s[1] = {H0};
+  const int Ks[1] = {cfg ? cfg->num_atoms : 0};
+  return rt_init(h, cfg, S, P, 0, 0, Ws, Ks, H0 ? H0s : nullptr, Es, analysis_window, synthesis_window, state, state_bytes, stream);
 }
 
 int rt_process_block(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, void* state, size_t state_bytes, const float* in_blocks,
-                     float* out_blocks, const double* forced_atom_mask, void* stream) {
-  RT_CARVE_OR_FAIL_P(l, S, P);
+                     float* out_blocks, const double* forced_atom_mask, void* stream, int Qd = 0, int Qe = 0) {
+  RT_CARVE_OR_FAIL_B(l, S, P, Qd, Qe);
   GCCNMF_REQUIRE(h, in_blocks && out_blocks, "rt_process_block: NULL pointer");
   if (int st = rt_enqueue_core(h, cfg, l, nullptr, in_blocks, nullptr, forced_atom_mask, 1, stream)) return st;
   const int N = cfg->window_size, nT = cfg->windows_per_block, B = cfg->block_size;
@@ -1034,8 +1221,8 @@ int rt_process_block(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P
 }
 
 int rt_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, void* state, size_t state_bytes, const float* windowed, float* out,
-                      const double* forced_atom_mask, void* stream) {
-  RT_CARVE_OR_FAIL_P(l, S, P);
+                      const double* forced_atom_mask, void* stream, int Qd = 0, int Qe = 0) {
+  RT_CARVE_OR_FAIL_B(l, S, P, Qd, Qe);
   GCCNMF_REQUIRE(h, windowed && out, "rt_process_frames: NULL pointer");
   if (int st = rt_enqueue_core(h, cfg, l, windowed, nullptr, out, forced_atom_mask, 0, stream)) return st;
   GCCNMF_LAUNCH(h, rt_localize_kernel, S, 128, 0, stream, l.dev, l.stride, l.gccphat, cfg->num_tdoas, cfg->windows_per_block, l.hist, cfg->history_length,
@@ -1044,17 +1231,17 @@ int rt_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int 
 }
 
 int rt_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, void* state, size_t state_bytes, float* in_blocks, float* out_blocks,
-                    const float* in_host, float* out_host, void** graph_exec, void* stream) {
+                    const float* in_host, float* out_host, void** graph_exec, void* stream, int Qd = 0, int Qe = 0) {
   GCCNMF_REQUIRE(h, graph_exec != nullptr && stream != nullptr, "rt_graph_create: needs a non-default stream and an output slot");
   *graph_exec = nullptr;
-  RT_CARVE_OR_FAIL_P(l, S, P);
+  RT_CARVE_OR_FAIL_B(l, S, P, Qd, Qe);
   GCCNMF_REQUIRE(h, in_blocks && out_blocks, "rt_graph_create: NULL pointer");
   cudaStream_t s = (cudaStream_t)stream;
   const size_t block_bytes = (size_t)S * 2 * cfg->block_size * sizeof(float), out_bytes = block_bytes * rt_sources_grid(l);
   GCCNMF_CHECK_CUDA(h, cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
   int st = GCCNMF_OK;
   if (in_host && cudaMemcpyAsync(in_blocks, in_host, block_bytes, cudaMemcpyHostToDevice, s) != cudaSuccess) st = GCCNMF_ERR_CUDA;
-  if (st == GCCNMF_OK) st = rt_process_block(h, cfg, S, P, state, state_bytes, in_blocks, out_blocks, nullptr, stream);
+  if (st == GCCNMF_OK) st = rt_process_block(h, cfg, S, P, state, state_bytes, in_blocks, out_blocks, nullptr, stream, Qd, Qe);
   if (st == GCCNMF_OK && out_host && cudaMemcpyAsync(out_host, out_blocks, out_bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess) st = GCCNMF_ERR_CUDA;
   cudaGraph_t graph = nullptr;
   const cudaError_t end = cudaStreamEndCapture(s, &graph);
@@ -1071,15 +1258,31 @@ int rt_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P,
   return GCCNMF_OK;
 }
 
-// Items 2 and 4 are source 0's with P > 0; items 9 .. 13 exist only with P > 0.
-int rt_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, void* state, size_t state_bytes, int slot, int what, void* dst, void* stream) {
-  RT_CARVE_OR_FAIL_P(l, S, P);
+// Items 2 and 4 are source 0's with P > 0; items 9 .. 13 exist only with P > 0, item 14 only with a bank.  With a bank the
+// K-shaped items (2, 5, 6, 10, 11) have the K_i of the block they were computed in (of the slot's current dictionary before its
+// first block), read from the device after the work queued before.
+int rt_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, void* state, size_t state_bytes, int slot, int what, void* dst, void* stream,
+              int Qd = 0, int Qe = 0) {
+  RT_CARVE_OR_FAIL_B(l, S, P, Qd, Qe);
   GCCNMF_REQUIRE(h, dst != nullptr, "rt_export: NULL destination");
   GCCNMF_REQUIRE(h, slot >= 0 && slot < S, "rt_export: slot %d outside [0, %d)", slot, S);
-  const size_t nT = cfg->windows_per_block, K = cfg->num_atoms, D = cfg->num_tdoas, F = l.F, st = l.stride;
+  const size_t nT = cfg->windows_per_block, D = cfg->num_tdoas, F = l.F, st = l.stride;
+  size_t K = cfg->num_atoms;
+  const bool known = what >= 0 && (what < 9 || (P > 0 && what < 14) || (Qd > 0 && what == 14));
+  if (known && Qd > 0 && (what == 2 || what == 5 || what == 6 || what == 10 || what == 11)) {
+    int32_t entry[3] = {0, 0, 0}, Ki = 0;                // dictionary, steering, K_i of the last block computed (0: none yet)
+    GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(entry, rt_slot(l.assign, slot, st), sizeof(entry), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+    GCCNMF_CHECK_CUDA(h, cudaStreamSynchronize((cudaStream_t)stream));
+    Ki = entry[2];
+    if (Ki == 0) {
+      GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(&Ki, l.bank_K + entry[0], sizeof(Ki), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+      GCCNMF_CHECK_CUDA(h, cudaStreamSynchronize((cudaStream_t)stream));
+    }
+    K = (size_t)Ki;
+  }
   const void* src = nullptr;
   size_t bytes = 0, rows = 1;            // rows > 1: one row of `bytes` per source, src_stride apart in the state
-  switch (P > 0 ? what : what < 9 ? what : -1) {
+  switch (known ? what : -1) {
     case 0: src = rt_slot(l.gccphat, slot, st); bytes = D * nT * sizeof(float); break;
     case 1: src = &rt_slot(l.dev, slot, st)->target; bytes = sizeof(float); break;
     case 2: src = rt_slot(l.smask, slot, st); bytes = K * nT * sizeof(double); break;
@@ -1094,6 +1297,7 @@ int rt_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, void*
     case 11: src = rt_slot(l.tval, slot, st); bytes = (size_t)P * K * nT * sizeof(float); break;
     case 12: src = rt_slot(l.sY, slot, st); bytes = 2 * F * nT * sizeof(float2); rows = P; break;
     case 13: src = rt_slot(l.status, slot, st); bytes = sizeof(int32_t); break;
+    case 14: src = rt_slot(l.assign, slot, st); bytes = 2 * sizeof(int32_t); break;
     default: return gccnmf_fail(h, GCCNMF_ERR_INVALID_ARGUMENT, "rt_export: unknown item %d", what);
   }
   if (rows > 1)
@@ -1106,6 +1310,52 @@ int rt_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, void*
 int rt_check_range(gccnmf_handle* h, int S, int first, int count) {
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < S && count <= S - first, "rtm: slots [%d, %d + %d) outside [0, %d)", first, first, count, S);
   return 0;
+}
+
+// Per-slot parameters of slots [first_slot, first_slot + count): as given without sources; with P sources mode, target_index and
+// set_target are ignored (the masks are one-hot, the targets come from set_targets or the localisation).
+int rt_slot_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout& l, int first_slot, int count, const gccnmf_rtm_slot_params* params,
+                   void* stream) {
+  if (int st = rt_check_range(h, l.S, first_slot, count)) return st;
+  const char* name = l.P > 0 ? "rtsep_set_params" : "rtm_set_params";
+  GCCNMF_REQUIRE(h, params != nullptr, "%s: NULL parameters", name);
+  for (int i = 0; i < count; ++i) {
+    GCCNMF_REQUIRE(h, l.P > 0 || params[i].mode == 0 || params[i].mode == 1, "%s: slot %d: mode must be 0 (boxcar) or 1 (window)", name, first_slot + i);
+    GCCNMF_REQUIRE(h, params[i].localization_window >= 1, "%s: slot %d: localization_window must be >= 1 (got %d)", name, first_slot + i,
+                   params[i].localization_window);
+    // a strict local maximum needs both neighbours (argrelmax never returns the end points)
+    GCCNMF_REQUIRE(h, l.P == 0 || !params[i].localization_enabled || cfg->num_tdoas >= 3, "%s: slot %d: localisation needs num_tdoas >= 3 (got %d)",
+                   name, first_slot + i, cfg->num_tdoas);
+  }
+  if (l.P == 0) return rt_enqueue_params(h, l, first_slot, count, params, 1, stream);
+  for (int i0 = 0; i0 < count; i0 += kRtParamsPerLaunch) {
+    const int n = count - i0 < kRtParamsPerLaunch ? count - i0 : kRtParamsPerLaunch;
+    gccnmf_rtm_slot_params p[kRtParamsPerLaunch];
+    for (int i = 0; i < n; ++i) {
+      p[i] = params[i0 + i];
+      p[i].set_target = 0;
+      p[i].mode = 1;
+    }
+    if (int st = rt_enqueue_params(h, l, first_slot + i0, n, p, 1, stream)) return st;
+  }
+  return GCCNMF_OK;
+}
+
+int rt_set_targets(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout& l, int first_slot, int count, const int32_t* targets_host,
+                   void* stream) {
+  if (int st = rt_check_range(h, l.S, first_slot, count)) return st;
+  GCCNMF_REQUIRE(h, targets_host != nullptr, "rtsep_set_targets: NULL targets");
+  const int P = l.P;
+  for (int i = 0; i < count * P; ++i)
+    GCCNMF_REQUIRE(h, targets_host[i] >= -1 && targets_host[i] < cfg->num_tdoas, "rtsep_set_targets: slot %d source %d: target %d outside [0, %d) (or -1)",
+                   first_slot + i / P, i % P, targets_host[i], cfg->num_tdoas);
+  for (int i0 = 0; i0 < count; i0 += kRtParamsPerLaunch) {
+    const int n = count - i0 < kRtParamsPerLaunch ? count - i0 : kRtParamsPerLaunch;
+    RtTargetsBatch b{};
+    memcpy(b.t, targets_host + (size_t)i0 * P, (size_t)n * P * sizeof(int32_t));
+    GCCNMF_LAUNCH(h, rt_set_targets_kernel, 1, kRtParamsPerLaunch, 0, stream, l.targets, l.stride, first_slot + i0, n, P, b);
+  }
+  return GCCNMF_OK;
 }
 
 }  // namespace
@@ -1212,14 +1462,7 @@ int gccnmf_rtm_set_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num
                           const gccnmf_rtm_slot_params* params, void* stream) {
   GCCNMF_ENTER(h);
   RT_CARVE_OR_FAIL(l, num_streams);
-  if (int st = rt_check_range(h, num_streams, first_slot, count)) return st;
-  GCCNMF_REQUIRE(h, params != nullptr, "rtm_set_params: NULL parameters");
-  for (int i = 0; i < count; ++i) {
-    GCCNMF_REQUIRE(h, params[i].mode == 0 || params[i].mode == 1, "rtm_set_params: slot %d: mode must be 0 (boxcar) or 1 (window)", first_slot + i);
-    GCCNMF_REQUIRE(h, params[i].localization_window >= 1, "rtm_set_params: slot %d: localization_window must be >= 1 (got %d)", first_slot + i,
-                   params[i].localization_window);
-  }
-  return rt_enqueue_params(h, l, first_slot, count, params, 1, stream);
+  return rt_slot_params(h, cfg, l, first_slot, count, params, stream);
 }
 
 int gccnmf_rtm_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, void* state, size_t state_bytes, const float* windowed,
@@ -1275,26 +1518,7 @@ int gccnmf_rtsep_set_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, int n
   GCCNMF_ENTER(h);
   GCCNMF_REQUIRE(h, num_sources != 0, "rtsep: num_sources must be in [2, %d] (got 0)", kRtMaxSources);
   RT_CARVE_OR_FAIL_P(l, num_streams, num_sources);
-  if (int st = rt_check_range(h, num_streams, first_slot, count)) return st;
-  GCCNMF_REQUIRE(h, params != nullptr, "rtsep_set_params: NULL parameters");
-  for (int i = 0; i < count; ++i) {
-    GCCNMF_REQUIRE(h, params[i].localization_window >= 1, "rtsep_set_params: slot %d: localization_window must be >= 1 (got %d)", first_slot + i,
-                   params[i].localization_window);
-    // a strict local maximum needs both neighbours (argrelmax never returns the end points)
-    GCCNMF_REQUIRE(h, !params[i].localization_enabled || cfg->num_tdoas >= 3, "rtsep_set_params: slot %d: localisation needs num_tdoas >= 3 (got %d)",
-                   first_slot + i, cfg->num_tdoas);
-  }
-  for (int i0 = 0; i0 < count; i0 += kRtParamsPerLaunch) {
-    const int n = count - i0 < kRtParamsPerLaunch ? count - i0 : kRtParamsPerLaunch;
-    gccnmf_rtm_slot_params p[kRtParamsPerLaunch];
-    for (int i = 0; i < n; ++i) {
-      p[i] = params[i0 + i];
-      p[i].set_target = 0;
-      p[i].mode = 1;
-    }
-    if (int st = rt_enqueue_params(h, l, first_slot + i0, n, p, 1, stream)) return st;
-  }
-  return GCCNMF_OK;
+  return rt_slot_params(h, cfg, l, first_slot, count, params, stream);
 }
 
 int gccnmf_rtsep_set_targets(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state, size_t state_bytes,
@@ -1302,19 +1526,7 @@ int gccnmf_rtsep_set_targets(gccnmf_handle* h, const gccnmf_rt_config* cfg, int 
   GCCNMF_ENTER(h);
   GCCNMF_REQUIRE(h, num_sources != 0, "rtsep: num_sources must be in [2, %d] (got 0)", kRtMaxSources);
   RT_CARVE_OR_FAIL_P(l, num_streams, num_sources);
-  if (int st = rt_check_range(h, num_streams, first_slot, count)) return st;
-  GCCNMF_REQUIRE(h, targets_host != nullptr, "rtsep_set_targets: NULL targets");
-  const int P = num_sources;
-  for (int i = 0; i < count * P; ++i)
-    GCCNMF_REQUIRE(h, targets_host[i] >= -1 && targets_host[i] < cfg->num_tdoas, "rtsep_set_targets: slot %d source %d: target %d outside [0, %d) (or -1)",
-                   first_slot + i / P, i % P, targets_host[i], cfg->num_tdoas);
-  for (int i0 = 0; i0 < count; i0 += kRtParamsPerLaunch) {
-    const int n = count - i0 < kRtParamsPerLaunch ? count - i0 : kRtParamsPerLaunch;
-    RtTargetsBatch b{};
-    memcpy(b.t, targets_host + (size_t)i0 * P, (size_t)n * P * sizeof(int32_t));
-    GCCNMF_LAUNCH(h, rt_set_targets_kernel, 1, kRtParamsPerLaunch, 0, stream, l.targets, l.stride, first_slot + i0, n, P, b);
-  }
-  return GCCNMF_OK;
+  return rt_set_targets(h, cfg, l, first_slot, count, targets_host, stream);
 }
 
 int gccnmf_rtsep_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state, size_t state_bytes,
@@ -1343,6 +1555,131 @@ int gccnmf_rtsep_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_s
   GCCNMF_ENTER(h);
   GCCNMF_REQUIRE(h, num_sources != 0, "rtsep: num_sources must be in [2, %d] (got 0)", kRtMaxSources);
   return rt_export(h, cfg, num_streams, num_sources, state, state_bytes, slot, what, dst, stream);
+}
+
+
+// ---------------------------------------------------------------------------------------------- S streams x P sources over a bank
+// of Qd dictionaries and Qe steering tables
+#define RT_BANK_OR_FAIL(l)                                                                                                         \
+  if (int st__ = rt_check_bank(h, num_dictionaries, num_steerings)) return st__;                                                  \
+  RT_CARVE_OR_FAIL_B(l, num_streams, num_sources, num_dictionaries, num_steerings)
+
+size_t gccnmf_rtbank_state_bytes(const gccnmf_rt_config* cfg, int num_streams, int num_sources, int num_dictionaries, int num_steerings) {
+  const bool empty = num_dictionaries == 0 && num_steerings == 0;
+  if (!empty && rt_check_bank(nullptr, num_dictionaries, num_steerings) != 0) return 0;
+  if (rt_check(nullptr, cfg, num_streams, num_sources) != 0) return 0;
+  return rt_carve(*cfg, num_streams, num_sources, nullptr, 0, num_dictionaries, num_steerings).bytes;
+}
+
+int gccnmf_rtbank_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, int num_dictionaries, int num_steerings,
+                       void* state, size_t state_bytes, const float* const* W, const int* num_atoms, const float* const* H0, const float* const* E,
+                       const float* analysis_window, const float* synthesis_window, void* stream) {
+  GCCNMF_ENTER(h);
+  if (int st = rt_check_bank(h, num_dictionaries, num_steerings)) return st;
+  return rt_init(h, cfg, num_streams, num_sources, num_dictionaries, num_steerings, W, num_atoms, H0, E, analysis_window, synthesis_window, state,
+                 state_bytes, stream);
+}
+
+int gccnmf_rtbank_load_dictionary(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, int num_dictionaries,
+                                  int num_steerings, void* state, size_t state_bytes, int index, const float* W, int num_atoms, const float* H0,
+                                  void* stream) {
+  GCCNMF_ENTER(h);
+  RT_BANK_OR_FAIL(l);
+  GCCNMF_REQUIRE(h, index >= 0 && index < num_dictionaries, "rtbank_load_dictionary: entry %d outside [0, %d)", index, num_dictionaries);
+  GCCNMF_REQUIRE(h, num_atoms >= 1 && num_atoms <= cfg->num_atoms, "rtbank_load_dictionary: %d atoms outside [1, num_atoms = %d]", num_atoms,
+                 cfg->num_atoms);
+  GCCNMF_REQUIRE(h, W != nullptr, "rtbank_load_dictionary: NULL dictionary");
+  GCCNMF_REQUIRE(h, cfg->inference_iterations == 0 || H0 != nullptr, "rtbank_load_dictionary: coefficient inference needs the initial H0 (K, 2)");
+  return rt_enqueue_dictionary(h, l, index, W, num_atoms, H0, stream);
+}
+
+int gccnmf_rtbank_load_steering(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, int num_dictionaries, int num_steerings,
+                                void* state, size_t state_bytes, int index, const float* E, void* stream) {
+  GCCNMF_ENTER(h);
+  RT_BANK_OR_FAIL(l);
+  GCCNMF_REQUIRE(h, index >= 0 && index < num_steerings, "rtbank_load_steering: entry %d outside [0, %d)", index, num_steerings);
+  GCCNMF_REQUIRE(h, E != nullptr, "rtbank_load_steering: NULL steering table");
+  return rt_enqueue_steering(h, l, index, E, stream);
+}
+
+int gccnmf_rtbank_assign(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, int num_dictionaries, int num_steerings,
+                         void* state, size_t state_bytes, int first_slot, int count, const int32_t* dictionary, const int32_t* steering, void* stream) {
+  GCCNMF_ENTER(h);
+  RT_BANK_OR_FAIL(l);
+  if (int st = rt_check_range(h, num_streams, first_slot, count)) return st;
+  for (int i = 0; i < count; ++i) {
+    GCCNMF_REQUIRE(h, !dictionary || (dictionary[i] >= -1 && dictionary[i] < num_dictionaries),
+                   "rtbank_assign: slot %d: dictionary %d outside [0, %d) (or -1)", first_slot + i, dictionary[i], num_dictionaries);
+    GCCNMF_REQUIRE(h, !steering || (steering[i] >= -1 && steering[i] < num_steerings), "rtbank_assign: slot %d: steering %d outside [0, %d) (or -1)",
+                   first_slot + i, steering[i], num_steerings);
+  }
+  for (int i0 = 0; i0 < count; i0 += kRtParamsPerLaunch) {
+    const int n = count - i0 < kRtParamsPerLaunch ? count - i0 : kRtParamsPerLaunch;
+    RtAssignBatch b{};
+    for (int i = 0; i < n; ++i) {
+      b.d[i] = dictionary ? dictionary[i0 + i] : -1;
+      b.e[i] = steering ? steering[i0 + i] : -1;
+    }
+    GCCNMF_LAUNCH(h, rt_assign_kernel, 1, kRtParamsPerLaunch, 0, stream, l.assign, l.stride, first_slot + i0, n, b);
+  }
+  return rt_enqueue_sort(h, l, stream);
+}
+
+int gccnmf_rtbank_reset_slots(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, int num_dictionaries, int num_steerings,
+                              void* state, size_t state_bytes, int first_slot, int count, void* stream) {
+  GCCNMF_ENTER(h);
+  RT_BANK_OR_FAIL(l);
+  if (int st = rt_check_range(h, num_streams, first_slot, count)) return st;
+  return rt_enqueue_reset(h, l, first_slot, count, stream);
+}
+
+int gccnmf_rtbank_set_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, int num_dictionaries, int num_steerings,
+                             void* state, size_t state_bytes, int first_slot, int count, const gccnmf_rtm_slot_params* params, void* stream) {
+  GCCNMF_ENTER(h);
+  RT_BANK_OR_FAIL(l);
+  return rt_slot_params(h, cfg, l, first_slot, count, params, stream);
+}
+
+int gccnmf_rtbank_set_targets(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, int num_dictionaries, int num_steerings,
+                              void* state, size_t state_bytes, int first_slot, int count, const int32_t* targets_host, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, num_sources != 0, "rtbank_set_targets: needs num_sources in [2, %d] (got 0)", kRtMaxSources);
+  RT_BANK_OR_FAIL(l);
+  return rt_set_targets(h, cfg, l, first_slot, count, targets_host, stream);
+}
+
+int gccnmf_rtbank_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, int num_dictionaries,
+                                 int num_steerings, void* state, size_t state_bytes, const float* windowed, float* out, const double* forced_atom_mask,
+                                 void* stream) {
+  GCCNMF_ENTER(h);
+  if (int st = rt_check_bank(h, num_dictionaries, num_steerings)) return st;
+  GCCNMF_REQUIRE(h, num_sources == 0 || !forced_atom_mask, "rtbank_process_frames: forced atom masks need num_sources = 0");
+  return rt_process_frames(h, cfg, num_streams, num_sources, state, state_bytes, windowed, out, forced_atom_mask, stream, num_dictionaries, num_steerings);
+}
+
+int gccnmf_rtbank_process_block(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, int num_dictionaries, int num_steerings,
+                                void* state, size_t state_bytes, const float* in_blocks, float* out_blocks, const double* forced_atom_mask, void* stream) {
+  GCCNMF_ENTER(h);
+  if (int st = rt_check_bank(h, num_dictionaries, num_steerings)) return st;
+  GCCNMF_REQUIRE(h, num_sources == 0 || !forced_atom_mask, "rtbank_process_block: forced atom masks need num_sources = 0");
+  return rt_process_block(h, cfg, num_streams, num_sources, state, state_bytes, in_blocks, out_blocks, forced_atom_mask, stream, num_dictionaries,
+                          num_steerings);
+}
+
+int gccnmf_rtbank_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, int num_dictionaries, int num_steerings,
+                               void* state, size_t state_bytes, float* in_blocks, float* out_blocks, const float* in_host, float* out_host,
+                               void** graph_exec, void* stream) {
+  GCCNMF_ENTER(h);
+  if (int st = rt_check_bank(h, num_dictionaries, num_steerings)) return st;
+  return rt_graph_create(h, cfg, num_streams, num_sources, state, state_bytes, in_blocks, out_blocks, in_host, out_host, graph_exec, stream,
+                         num_dictionaries, num_steerings);
+}
+
+int gccnmf_rtbank_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, int num_dictionaries, int num_steerings,
+                         void* state, size_t state_bytes, int slot, int what, void* dst, void* stream) {
+  GCCNMF_ENTER(h);
+  if (int st = rt_check_bank(h, num_dictionaries, num_steerings)) return st;
+  return rt_export(h, cfg, num_streams, num_sources, state, state_bytes, slot, what, dst, stream, num_dictionaries, num_steerings);
 }
 
 }  // extern "C"

@@ -34,6 +34,13 @@ TARGET_MODE_MULTIPLE = 1             # declared by the reference, not implemente
 TARGET_MODE_WINDOW_FUNCTION = 2
 
 
+def steeringVectors(frequenciesInHz, microphoneSeparationInMetres, numTDOAs):
+    """(maxTDOA, hypothesisTDOAs (D,) float32, expJOmegaTau (F, D) complex64) of a microphone spacing (:241-248)."""
+    maxTDOA = microphoneSeparationInMetres / fn.SPEED_OF_SOUND_IN_METRES_PER_SECOND
+    hypothesisTDOAs = np.linspace(-maxTDOA, maxTDOA, numTDOAs).astype(np.float32)
+    return maxTDOA, hypothesisTDOAs, np.exp(np.outer(frequenciesInHz, -(2j * np.pi) * hypothesisTDOAs)).astype(np.complex64)
+
+
 class GCCNMFProcessor(object):
     def __init__(self, sampleRate, windowSize, numTimePerChunk, dictionariesW, dictionaryType, dictionarySize, numHUpdates,
                  microphoneSeparationInMetres, localizationEnabled, localizationWindowSize, gccPHATHistory=None, tdoaHistory=None,
@@ -114,9 +121,8 @@ class GCCNMFProcessor(object):
         self.W = np.ascontiguousarray(self.dictionariesW[self.dictionaryType][self.dictionarySize], dtype=np.float32)
         self.numFrequencies, self.numAtom = self.W.shape
         self.frequenciesInHz = np.linspace(0, self.sampleRate / 2, self.numFrequencies).astype(np.float32)
-        self.maxTDOA = self.microphoneSeparationInMetres / fn.SPEED_OF_SOUND_IN_METRES_PER_SECOND
-        self.hypothesisTDOAs = np.linspace(-self.maxTDOA, self.maxTDOA, self.numTDOAs).astype(np.float32)
-        self.expJOmegaTau = np.exp(np.outer(self.frequenciesInHz, -(2j * np.pi) * self.hypothesisTDOAs)).astype(np.complex64)
+        self.maxTDOA, self.hypothesisTDOAs, self.expJOmegaTau = steeringVectors(self.frequenciesInHz, self.microphoneSeparationInMetres,
+                                                                                self.numTDOAs)
 
     def slotParams(self):
         """The parameters `processBlock` would send to its engine, as keyword arguments of MultiStreamRealtimeEngine.set_params."""

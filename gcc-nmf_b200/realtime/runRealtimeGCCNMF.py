@@ -168,11 +168,15 @@ class RealtimeGCCNMFNoGUI(object):
         return np.stack([self._writeOutput(out[s], samples.shape[1], outputPath[s] if outputPath is not None else None, alignOutput)
                          for s in range(p.numSources)])
 
-    def runMany(self, audioPaths, outputPaths=None, alignOutput=True):
+    def runMany(self, audioPaths, outputPaths=None, alignOutput=True, dictionarySizes=None, microphoneSeparations=None):
         """Several wav files enhanced concurrently, each in its own slot of ONE MultiStreamRealtimeEngine: per block, one graph
         launch for all files.  Each file gets exactly what `run` gives it alone (same parameters, same kernels, bit for bit);
         once a file has had its two flush blocks its slot is deactivated.  Returns the output arrays in the order of
-        `audioPaths` and writes them to `outputPaths` when given.  `processingTimes` gets one entry per block of the longest file."""
+        `audioPaths` and writes them to `outputPaths` when given.  `processingTimes` gets one entry per block of the longest file.
+        dictionarySizes / microphoneSeparations: one per file (None: the runner's own), built into one bank of the distinct
+        dictionaries of params.dictionariesW[dictionaryType] and the steering tables of the distinct spacings; each file then gets
+        what `run` gives it with that dictionary size and spacing."""
+        from .gccNMFProcessor import steeringVectors
         from .multistream import MultiStreamRealtimeEngine
         g = self.gccNMFProcessor
         if g is None:
@@ -186,10 +190,22 @@ class RealtimeGCCNMFNoGUI(object):
         signals = [self._readSamples(path) for path in audioPaths]
         totals = [(x.shape[1] + B - 1) // B + 2 for x in signals]          # whole blocks + two flush blocks, as processSamples
         g.buildConstants()
-        engine = MultiStreamRealtimeEngine(g.W, g.expJOmegaTau, g.windowFunction[:, 0], g.synthesisWindowFunction[:, 0], p.hopSize, B,
+        W, E, entries = g.W, g.expJOmegaTau, None
+        if dictionarySizes is not None or microphoneSeparations is not None:
+            sizes = [g.dictionarySize] * S if dictionarySizes is None else [int(k) for k in dictionarySizes]
+            seps = [g.microphoneSeparationInMetres] * S if microphoneSeparations is None else [float(m) for m in microphoneSeparations]
+            if len(sizes) != S or len(seps) != S:
+                raise ValueError('one dictionary size and one microphone separation per file (%d files)' % S)
+            distinctSizes, distinctSeps = sorted(set(sizes)), sorted(set(seps))
+            W = [np.ascontiguousarray(p.dictionariesW[g.dictionaryType][k], dtype=np.float32) for k in distinctSizes]
+            E = [steeringVectors(g.frequenciesInHz, m, g.numTDOAs)[2] for m in distinctSeps]
+            entries = ([distinctSizes.index(k) for k in sizes], [distinctSeps.index(m) for m in seps])
+        engine = MultiStreamRealtimeEngine(W, E, g.windowFunction[:, 0], g.synthesisWindowFunction[:, 0], p.hopSize, B,
                                            p.windowsPerBlock, S, historyLength=g.gccPHATHistory.size() if g.gccPHATHistory else 128,
                                            numInferenceIterations=g.coefficientInferenceIterations, device=g.device)
         try:
+            if entries is not None:
+                engine.assign(range(S), *entries)
             engine.set_params(range(S), **g.slotParams())
             outs = [np.empty((p.numChannels, t * B), np.float32) for t in totals]
             blocks = np.zeros((S, p.numChannels, B), np.float32)

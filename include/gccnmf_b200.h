@@ -451,6 +451,69 @@ GCCNMF_API int gccnmf_rtsep_graph_create(gccnmf_handle* h, const gccnmf_rt_confi
 GCCNMF_API int gccnmf_rtsep_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, void* state,
                         size_t state_bytes, int slot, int what, void* dst, void* stream);
 
+/* ---- S streams (x P sources) over a bank of dictionaries and steering tables ----------------------------------------------
+ * The reference rebuilds a processor when its dictionary size / type or microphone spacing changes (gccNMFProcessor.py:131-157,
+ * buildTheanoFunctions :238-270): a new W and expJOmegaTau, the same rings and GCC-PHAT history.  Here the state holds
+ * num_dictionaries = Qd dictionary entries, entry i with its own K_i in [1, cfg.num_atoms = K_max] atoms, and num_steerings = Qe
+ * steering entries (F, D), 1 <= Qd, Qe <= 64; every slot is on one entry of each.  N, hop, B, nT, D, the history length and the
+ * inference settings stay engine-wide.  num_sources: 0 (one output per slot, as gccnmf_rtm_*) or 2 .. 8 (as gccnmf_rtsep_*).
+ * Slot s on (i, j) computes bit for bit what a one-stream state built with (W_i, E_j) computes from the same blocks and
+ * parameters: every output block and every export item.
+ * - init: host arrays of Qd device pointers W_i (F, K_i) f32, Qd host ints K_i, Qd device pointers H0_i (K_i, 2) f32 (the array
+ *   or its entries NULL when inference_iterations == 0) and Qe device pointers E_j (F, D) complex64.  Every slot on (0, 0).
+ * - load_dictionary / load_steering rewrite one entry; assign moves slots [first_slot, first_slot + count) to the entries of
+ *   the host arrays `dictionary` / `steering` (count each, -1 or a NULL array keeps the slot's entry).  All three are
+ *   stream-ordered and may sit between two launches of an instantiated graph; they act from the next block on and keep the
+ *   slot's rings, history, targets, block counter and parameters.  reset_slots also puts the slots back on (0, 0).
+ * - Forced atom masks (num_sources = 0): (S, K_max, nT) f64; rows k >= K_i of a slot are ignored.
+ * - export: items as gccnmf_rtm_export / gccnmf_rtsep_export, the K-shaped ones (2, 5, 6, 10, 11) at the K_i of the block
+ *   they were computed in (of the slot's current dictionary before its first block; these wait for the stream to read K_i),
+ *   plus 14: the slot's (dictionary, steering) entries (2) i32.
+ * num_dictionaries = num_steerings = 0 in gccnmf_rtbank_state_bytes gives the gccnmf_rtm / gccnmf_rtsep size.  K_i outside
+ * [1, K_max], entries outside the bank and more than 64 entries fail with GCCNMF_ERR_INVALID_ARGUMENT. */
+#define GCCNMF_RTBANK_MAX_ENTRIES 64
+#define GCCNMF_RTBANK_EXPORT_ASSIGNMENT 14
+GCCNMF_API size_t gccnmf_rtbank_state_bytes(const gccnmf_rt_config* cfg, int num_streams, int num_sources, int num_dictionaries,
+                                 int num_steerings);
+GCCNMF_API int gccnmf_rtbank_init(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, int num_dictionaries,
+                       int num_steerings, void* state, size_t state_bytes, const float* const* W, const int* num_atoms,
+                       const float* const* H0, const float* const* E, const float* analysis_window, const float* synthesis_window,
+                       void* stream);
+GCCNMF_API int gccnmf_rtbank_load_dictionary(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources,
+                                  int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int index, const float* W,
+                                  int num_atoms, const float* H0, void* stream);
+GCCNMF_API int gccnmf_rtbank_load_steering(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources,
+                                int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int index, const float* E,
+                                void* stream);
+GCCNMF_API int gccnmf_rtbank_assign(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources, int num_dictionaries,
+                         int num_steerings, void* state, size_t state_bytes, int first_slot, int count, const int32_t* dictionary,
+                         const int32_t* steering, void* stream);
+GCCNMF_API int gccnmf_rtbank_reset_slots(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources,
+                              int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int first_slot, int count,
+                              void* stream);
+/* As gccnmf_rtm_set_params (num_sources = 0) or gccnmf_rtsep_set_params. */
+GCCNMF_API int gccnmf_rtbank_set_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources,
+                             int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int first_slot, int count,
+                             const gccnmf_rtm_slot_params* params, void* stream);
+/* As gccnmf_rtsep_set_targets; needs num_sources >= 2. */
+GCCNMF_API int gccnmf_rtbank_set_targets(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources,
+                              int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int first_slot, int count,
+                              const int32_t* targets_host, void* stream);
+/* forced_atom_mask: NULL, or (S, K_max, nT) f64 with num_sources = 0. */
+GCCNMF_API int gccnmf_rtbank_process_frames(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources,
+                                 int num_dictionaries, int num_steerings, void* state, size_t state_bytes, const float* windowed,
+                                 float* out, const double* forced_atom_mask, void* stream);
+GCCNMF_API int gccnmf_rtbank_process_block(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources,
+                                int num_dictionaries, int num_steerings, void* state, size_t state_bytes, const float* in_blocks,
+                                float* out_blocks, const double* forced_atom_mask, void* stream);
+/* Launch / destroy with gccnmf_rt_graph_launch / gccnmf_rt_graph_destroy. */
+GCCNMF_API int gccnmf_rtbank_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources,
+                               int num_dictionaries, int num_steerings, void* state, size_t state_bytes, float* in_blocks,
+                               float* out_blocks, const float* in_host, float* out_host, void** graph_exec, void* stream);
+GCCNMF_API int gccnmf_rtbank_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources,
+                         int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int slot, int what, void* dst,
+                         void* stream);
+
 /*
  * The building block the KL-NMF loop runs on (klnmf_tma.cu): the same 3-product contraction, TMA-fed, over operands
  * that are pre-split into bf16 hi/lo planes and kept in ONE orientation each; an operand contracted over its
