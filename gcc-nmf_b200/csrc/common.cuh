@@ -124,6 +124,9 @@ struct WorkspaceCarver {
 // (gccNMFFunctions.py:100: peakIndexes[argsort(x[peakIndexes])[-numSources:]]) in ascending index order (:113), by every thread of
 // one CTA.  x: D values in shared memory, written before the call; peak / chosen: D bytes of shared scratch.  Thread 0 writes the
 // min(S, peaks) chosen indexes to out and gets the number of peaks back (the other threads' return value is unspecified).
+// Equal peak values are ranked in stable order (argsort(kind='stable'): of two equal peaks the higher index ranks higher, so it
+// is kept first).  The reference's default np.argsort is not stable, so when peak values tie exactly the host drop-in may keep a
+// different one of them; with distinct peak values the two choose the same targets.
 __device__ inline int select_peaks(const double* x, int D, int S, unsigned char* peak, unsigned char* chosen, int* num_peaks, int32_t* out) {
   if (threadIdx.x == 0) *num_peaks = 0;
   __syncthreads();

@@ -16,9 +16,13 @@ constexpr int kAngT = 16;     // frames per CTA
 constexpr int kAngWarps = 4;  // warps per CTA: each takes a quarter of the staged bins (partial sums added in warp order at the end)
 constexpr int kAngMaxD = 128;
 
-// numpy's complex64 arithmetic for  X0 * conj(X1) / |X0| / |X1|  (runGCCNMF.py:44): float32 products,
-// magnitude correctly rounded (hypotf), division by a real done as multiplication by the float32
-// reciprocal (numpy's complex division with a zero imaginary divisor).
+// X0 * conj(X1) / |X0| / |X1|  (runGCCNMF.py:44) by a fixed float32 formula: re = rn(rn(ax bx) + rn(ay by)),
+// im = rn(rn(ay bx) - rn(ax by)) with every product rounded on its own (no FMA contraction), magnitudes
+// float32(sqrt(double re^2 + double im^2)) (correctly rounded), then two multiplications by float32
+// reciprocals (numpy divides a complex by a real magnitude that way).  This is not numpy's bits: numpy's
+// complex64 product contracts one product of each part into an FMA and its abs() is not correctly
+// rounded, both depending on the host's SIMD path; on an AVX-512 host about a third of the values are
+// bit-equal and the largest difference is 8 * 2^-24 (oracle/offline_exact.py pins this formula bit for bit).
 __device__ __forceinline__ float2 phat_coherence(float2 a, float2 b) {
   float re = __fadd_rn(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
   float im = __fsub_rn(__fmul_rn(a.y, b.x), __fmul_rn(a.x, b.y));
@@ -250,14 +254,21 @@ tdoa_gccnmf_kernel(int K, int N, int F, LoadWAtoms aload, LoadRealGCC bload, int
 __global__ void coeff_mask_kernel(const float* __restrict__ G, int S, int64_t KT, float* __restrict__ masks, int32_t* all_nan_flag) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= KT) return;
-  int best = -1;
-  float bv = 0.f;
-  for (int s = 0; s < S; ++s) {  // numpy.nanargmax: ignore NaN, first maximum wins
+  // numpy.nanargmax: NaN is replaced by -inf, then the first maximum wins (so a NaN before -inf is chosen over it); a column
+  // that is all NaN raises in numpy: here it sets the flag and gets no source
+  int best = 0;
+  float bv = -INFINITY;
+  bool any = false;
+  for (int s = 0; s < S; ++s) {
     const float v = G[(int64_t)s * KT + i];
     if (isnan(v)) continue;
-    if (best < 0 || v > bv) { best = s; bv = v; }
+    any = true;
+    if (v > bv) { best = s; bv = v; }
   }
-  if (best < 0 && all_nan_flag) *all_nan_flag = 1;
+  if (!any) {
+    best = -1;
+    if (all_nan_flag) *all_nan_flag = 1;
+  }
   for (int s = 0; s < S; ++s) masks[(int64_t)s * KT + i] = (s == best) ? 1.f : 0.f;
 }
 

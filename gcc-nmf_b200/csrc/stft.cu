@@ -127,7 +127,8 @@ istft_frames_kernel(const float2* __restrict__ spec, int batch, const float2* __
 }
 
 // y[b][j] = gain * OLA[b][offset + j];  OLA[m] = sum over frames i (ascending) of window[m - i hop] * frame_i[m - i hop]
-// with the reference's rounding: y = float32(float64(y) + window * float64(frame))  (librosaSTFT.py:279-281).
+// rounded to float32 after every add like the reference (librosaSTFT.py:279-281), but the float64 product and sum are
+// contracted into one DFMA: y = float32(fma(window, float64(frame), float64(y))), where the reference rounds the product first.
 __global__ void ola_gather_kernel(const float* __restrict__ frames, const double* __restrict__ window, int n, int hop,
                                   int T, int64_t offset, int64_t length, float gain, float* __restrict__ y) {
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
