@@ -158,6 +158,29 @@ SIGNATURES.update({
     'gccnmf_rtbank_export': (c_int, _BANK + [c_int, c_int, c_void_p, _S]),
 })
 
+class LLConfig(ctypes.Structure):
+    """gccnmf_ll_config (include/gccnmf_b200.h)."""
+    _fields_ = [('window_size', c_int), ('hop_size', c_int), ('hops_per_call', c_int), ('num_atoms', c_int), ('num_tdoas', c_int),
+                ('num_streams', c_int), ('inference_iterations', c_int), ('sparsity_alpha', c_float), ('epsilon', c_float)]
+
+
+class LLStreamParams(ctypes.Structure):
+    """gccnmf_ll_stream_params (include/gccnmf_b200.h)."""
+    _fields_ = [('epsilon', c_float), ('active', c_int), ('target_override', c_int)]
+
+
+_LC = ctypes.POINTER(LLConfig)
+SIGNATURES.update({
+    'gccnmf_ll_state_bytes': (c_size_t, [_LC]),
+    'gccnmf_ll_init': (c_int, [_H, _LC, _P, _P, _P, _P, c_float, _P, _P, c_size_t, _S]),
+    'gccnmf_ll_reset_streams': (c_int, [_H, _LC, _P, c_size_t, c_int, c_int, _S]),
+    'gccnmf_ll_set_params': (c_int, [_H, _LC, _P, c_size_t, c_int, c_int, ctypes.POINTER(LLStreamParams), _S]),
+    'gccnmf_ll_process': (c_int, [_H, _LC, _P, c_size_t, c_int, _P, _P, _S]),
+    'gccnmf_ll_graph_create': (c_int, [_H, _LC, _P, c_size_t, c_int, _P, _P, _P, _P, ctypes.POINTER(c_void_p), _S]),
+    'gccnmf_ll_export': (c_int, [_H, _LC, _P, c_size_t, c_int, c_int, c_void_p, _S]),
+})
+
+
 _lib = None
 
 

@@ -191,7 +191,12 @@ __device__ __forceinline__ bool argmax_better(double v, int i, double bv, int bi
 template <bool ARGMAX>
 __global__ void __launch_bounds__(kGccThreads)
 tdoa_gccnmf_kernel(int K, int N, int F, LoadWAtoms aload, LoadRealGCC bload, int T, int D, float* __restrict__ values,
-                   int32_t* __restrict__ argmax) {
+                   int32_t* __restrict__ argmax, const int32_t* __restrict__ gate, int gate_capacity, int32_t* __restrict__ ran) {
+  // gated form (the graph-safe fallback of the tensor-core argmax): nothing to do unless its refinement list overflowed
+  if (gate) {
+    if (*gate <= gate_capacity) return;
+    if (ran && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) *ran = 1;
+  }
   double acc[GTM][GTN];
   const int m0 = blockIdx.y * GM, n0 = blockIdx.x * GN;
   gemm_simt_mainloop<double, GM, GN, GK, GTM, GTN>(acc, m0, n0, F, aload, bload);
@@ -515,10 +520,10 @@ int gccnmf_tdoa_gccnmf(gccnmf_handle* h, const float* coherence, int F, int T, c
   dim3 grid((N + GN - 1) / GN, (K + GM - 1) / GM);
   if (argmax) {
     auto k = tdoa_gccnmf_kernel<true>;
-    GCCNMF_LAUNCH(h, k, grid, kGccThreads, 0, stream, K, N, F, a, b, T, D, values, argmax);
+    GCCNMF_LAUNCH(h, k, grid, kGccThreads, 0, stream, K, N, F, a, b, T, D, values, argmax, nullptr, 0, nullptr);
   } else {
     auto k = tdoa_gccnmf_kernel<false>;
-    GCCNMF_LAUNCH(h, k, grid, kGccThreads, 0, stream, K, N, F, a, b, T, D, values, argmax);
+    GCCNMF_LAUNCH(h, k, grid, kGccThreads, 0, stream, K, N, F, a, b, T, D, values, argmax, nullptr, 0, nullptr);
   }
   return GCCNMF_OK;
 }
@@ -599,3 +604,21 @@ int gccnmf_wiener_apply_h(gccnmf_handle* h, const float* mask, const float* W, c
 }
 
 }  // extern "C"
+
+// The argmax of gccnmf_tdoa_gccnmf as a launch that reads the refinement count of gccnmf_tdoa_argmax on the device and returns at
+// once unless it exceeds `capacity`; then it overwrites every decision with the float64 one and sets *ran = 1.  No host
+// synchronisation, so it can follow the tensor-core argmax inside a captured graph.
+int gccnmf_tdoa_gccnmf_gated(gccnmf_handle* h, const float* coherence, int F, int T, const double* E, int D, const float* W, int K,
+                             int32_t* argmax, const int32_t* gate, int capacity, int32_t* ran, void* stream) {
+  GCCNMF_REQUIRE(h, F > 0 && T > 0 && D > 0 && K > 0 && coherence && E && W && argmax && gate, "tdoa_gccnmf_gated: bad arguments");
+  GCCNMF_REQUIRE(h, (int64_t)T * D < (int64_t)1 << 31, "tdoa_gccnmf_gated: T * D overflows int32");
+  if (!(is_pow2(D) && D >= 4 && D <= GN))
+    return gccnmf_fail(h, GCCNMF_ERR_UNSUPPORTED, "tdoa_gccnmf_gated: numTDOAs must be a power of two in [4, %d] (got %d)", GN, D);
+  const int N = T * D;
+  LoadWAtoms a{W, K, F};
+  LoadRealGCC b{reinterpret_cast<const float2*>(coherence), reinterpret_cast<const double2*>(E), F, T, D, N};
+  dim3 grid((N + GN - 1) / GN, (K + GM - 1) / GM);
+  auto k = tdoa_gccnmf_kernel<true>;
+  GCCNMF_LAUNCH(h, k, grid, kGccThreads, 0, stream, K, N, F, a, b, T, D, nullptr, argmax, gate, capacity, ran);
+  return GCCNMF_OK;
+}

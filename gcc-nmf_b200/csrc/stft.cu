@@ -27,7 +27,7 @@ template <int FB>
 __global__ void __launch_bounds__(kFftThreads)
 stft_kernel(const float* __restrict__ samples, int64_t sample_stride, int channels, const double* __restrict__ window,
             const double2* __restrict__ tw, int n, int log2n, int hop, int T, int conjugate,
-            float2* __restrict__ X, float* __restrict__ V) {
+            float2* __restrict__ X, float* __restrict__ V, int frames_per_seg, int64_t seg_stride) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   double2* fft = reinterpret_cast<double2*>(smem_raw);
   float2* stage = reinterpret_cast<float2*>(smem_raw + (size_t)n * sizeof(double2));
@@ -36,7 +36,9 @@ stft_kernel(const float* __restrict__ samples, int64_t sample_stride, int channe
   const int frames = min(FB, T - t0);
 
   for (int fb = 0; fb < frames; ++fb) {
-    const int64_t start = (int64_t)(t0 + fb) * hop;
+    // frame t is frame t % frames_per_seg of segment t / frames_per_seg (one signal: frames_per_seg = T, seg_stride = 0)
+    const int t = t0 + fb;
+    const int64_t start = (int64_t)(t / frames_per_seg) * seg_stride + (int64_t)(t % frames_per_seg) * hop;
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
       const double w = window[i];
       const double l = w * (double)samples[start + i];
@@ -188,6 +190,64 @@ int gccnmf_get_twiddles(gccnmf_handle* h, int n, const double** tw64, const floa
   return 0;
 }
 
+// Frames of `segments` signals in one launch: frame (g, i) starts at g * seg_stride + i * hop of each channel row, for
+// i < frames_per_seg, and is column g * frames_per_seg + i of X.  Every frame is transformed on its own, so its bits do not depend
+// on how many frames share the launch.
+int gccnmf_stft_segments(gccnmf_handle* h, const float* samples, int64_t sample_stride, int channels, int segments, int frames_per_seg,
+                         int64_t seg_stride, const double* window, int n_fft, int hop, int conjugate, float* X, float* V, void* stream) {
+  const int log2n = ilog2_exact(n_fft);
+  if (log2n < 5 || log2n > 12) return gccnmf_fail(h, GCCNMF_ERR_UNSUPPORTED, "stft: n_fft must be a power of two in [32, 4096] (got %d)", n_fft);
+  GCCNMF_REQUIRE(h, channels == 1 || channels == 2, "stft: channels must be 1 or 2 (got %d)", channels);
+  GCCNMF_REQUIRE(h, hop >= 1, "Invalid hop_length: %d", hop);
+  GCCNMF_REQUIRE(h, segments >= 1 && frames_per_seg >= 1 && (int64_t)segments * frames_per_seg < ((int64_t)1 << 31), "stft: bad frame count");
+  const int T = segments * frames_per_seg;
+  GCCNMF_REQUIRE(h, samples && window && X, "stft: NULL pointer");
+  const double* tw = nullptr;
+  if (int st = gccnmf_get_twiddles(h, n_fft, &tw, nullptr)) return st;
+  const int F = n_fft / 2 + 1;
+  auto smem_for = [&](int fb) { return (size_t)n_fft * sizeof(double2) + (size_t)channels * F * fb * sizeof(float2); };
+#define GCCNMF_STFT_CASE(FB)                                                                                  \
+  {                                                                                                           \
+    auto k = stft_kernel<FB>;                                                                                 \
+    const size_t smem = smem_for(FB);                                                                         \
+    if (int st = set_smem(h, k, smem)) return st;                                                             \
+    GCCNMF_LAUNCH(h, k, (T + FB - 1) / FB, kFftThreads, smem, stream, samples, sample_stride, channels,       \
+                  window, reinterpret_cast<const double2*>(tw), n_fft, log2n, hop, T, conjugate,             \
+                  reinterpret_cast<float2*>(X), V, frames_per_seg, seg_stride);                               \
+  }
+  if (T >= 8 && smem_for(8) <= 160 * 1024) GCCNMF_STFT_CASE(8)
+  else if (T >= 4 && smem_for(4) <= 160 * 1024) GCCNMF_STFT_CASE(4)
+  else GCCNMF_STFT_CASE(1)
+#undef GCCNMF_STFT_CASE
+  return GCCNMF_OK;
+}
+
+// The per-frame inverse transforms of gccnmf_istft_ola without the overlap-add: spec (batch, F, T) c64 -> frames (batch', T, n) f32
+// (batch' = batch rounded up to even), the arithmetic of every frame exactly as there.
+int gccnmf_istft_frames(gccnmf_handle* h, const float* spec, int batch, int n_fft, int T, int conjugate, float* frames, void* stream) {
+  const int log2n = ilog2_exact(n_fft);
+  if (log2n < 5 || log2n > 12) return gccnmf_fail(h, GCCNMF_ERR_UNSUPPORTED, "istft: n_fft must be a power of two in [32, 4096] (got %d)", n_fft);
+  GCCNMF_REQUIRE(h, batch >= 1 && T >= 1 && spec && frames, "istft: bad arguments");
+  const float* tw = nullptr;
+  if (int st = gccnmf_get_twiddles(h, n_fft, nullptr, &tw)) return st;
+  const int F = n_fft / 2 + 1;
+  auto smem_for = [&](int fb) { return (size_t)n_fft * sizeof(float2) + (size_t)2 * F * fb * sizeof(float2); };
+#define GCCNMF_ISTFT_CASE(FB)                                                                                 \
+  {                                                                                                           \
+    auto k = istft_frames_kernel<FB>;                                                                         \
+    const size_t smem = smem_for(FB);                                                                         \
+    if (int st = set_smem(h, k, smem)) return st;                                                             \
+    GCCNMF_LAUNCH(h, k, dim3((T + FB - 1) / FB, (batch + 1) / 2), kFftThreads, smem, stream,                  \
+                  reinterpret_cast<const float2*>(spec), batch, reinterpret_cast<const float2*>(tw), n_fft,   \
+                  log2n, T, conjugate, frames);                                                               \
+  }
+  if (T >= 8 && smem_for(8) <= 160 * 1024) GCCNMF_ISTFT_CASE(8)
+  else if (T >= 4 && smem_for(4) <= 160 * 1024) GCCNMF_ISTFT_CASE(4)
+  else GCCNMF_ISTFT_CASE(1)
+#undef GCCNMF_ISTFT_CASE
+  return GCCNMF_OK;
+}
+
 extern "C" {
 
 int gccnmf_stft_num_frames(int64_t num_samples, int n_fft, int hop) {
@@ -205,25 +265,7 @@ int gccnmf_stft(gccnmf_handle* h, const float* samples, int64_t sample_stride, i
   GCCNMF_REQUIRE(h, hop >= 1, "Invalid hop_length: %d", hop);
   const int T = gccnmf_stft_num_frames(num_samples, n_fft, hop);
   GCCNMF_REQUIRE(h, T >= 1, "Buffer is too short (n=%lld) for frame_length=%d", (long long)num_samples, n_fft);
-  GCCNMF_REQUIRE(h, samples && window && X, "stft: NULL pointer");
-  const double* tw = nullptr;
-  if (int st = gccnmf_get_twiddles(h, n_fft, &tw, nullptr)) return st;
-  const int F = n_fft / 2 + 1;
-  auto smem_for = [&](int fb) { return (size_t)n_fft * sizeof(double2) + (size_t)channels * F * fb * sizeof(float2); };
-#define GCCNMF_STFT_CASE(FB)                                                                                  \
-  {                                                                                                           \
-    auto k = stft_kernel<FB>;                                                                                 \
-    const size_t smem = smem_for(FB);                                                                         \
-    if (int st = set_smem(h, k, smem)) return st;                                                             \
-    GCCNMF_LAUNCH(h, k, (T + FB - 1) / FB, kFftThreads, smem, stream, samples, sample_stride, channels,       \
-                  window, reinterpret_cast<const double2*>(tw), n_fft, log2n, hop, T, conjugate,             \
-                  reinterpret_cast<float2*>(X), V);                                                           \
-  }
-  if (T >= 8 && smem_for(8) <= 160 * 1024) GCCNMF_STFT_CASE(8)
-  else if (T >= 4 && smem_for(4) <= 160 * 1024) GCCNMF_STFT_CASE(4)
-  else GCCNMF_STFT_CASE(1)
-#undef GCCNMF_STFT_CASE
-  return GCCNMF_OK;
+  return gccnmf_stft_segments(h, samples, sample_stride, channels, 1, T, 0, window, n_fft, hop, conjugate, X, V, stream);
 }
 
 int64_t gccnmf_istft_length(int n_fft, int hop, int T, int center) {
@@ -247,24 +289,8 @@ int gccnmf_istft_ola(gccnmf_handle* h, const float* spec, int batch, int n_fft, 
   GCCNMF_REQUIRE(h, y != nullptr, "istft: NULL output pointer");
   if (!workspace || workspace_bytes < gccnmf_istft_workspace_bytes(batch, n_fft, T))
     return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "istft workspace too small: need %zu bytes", gccnmf_istft_workspace_bytes(batch, n_fft, T));
-  const float* tw = nullptr;
-  if (int st = gccnmf_get_twiddles(h, n_fft, nullptr, &tw)) return st;
-  const int F = n_fft / 2 + 1;
   float* frames = static_cast<float*>(workspace);
-  auto smem_for = [&](int fb) { return (size_t)n_fft * sizeof(float2) + (size_t)2 * F * fb * sizeof(float2); };
-#define GCCNMF_ISTFT_CASE(FB)                                                                                 \
-  {                                                                                                           \
-    auto k = istft_frames_kernel<FB>;                                                                         \
-    const size_t smem = smem_for(FB);                                                                         \
-    if (int st = set_smem(h, k, smem)) return st;                                                             \
-    GCCNMF_LAUNCH(h, k, dim3((T + FB - 1) / FB, (batch + 1) / 2), kFftThreads, smem, stream,                  \
-                  reinterpret_cast<const float2*>(spec), batch, reinterpret_cast<const float2*>(tw), n_fft,   \
-                  log2n, T, conjugate, frames);                                                               \
-  }
-  if (T >= 8 && smem_for(8) <= 160 * 1024) GCCNMF_ISTFT_CASE(8)
-  else if (T >= 4 && smem_for(4) <= 160 * 1024) GCCNMF_ISTFT_CASE(4)
-  else GCCNMF_ISTFT_CASE(1)
-#undef GCCNMF_ISTFT_CASE
+  if (int st = gccnmf_istft_frames(h, spec, batch, n_fft, T, conjugate, frames, stream)) return st;
   const int64_t length = gccnmf_istft_length(n_fft, hop, T, center);
   if (length > 0) {
     const int64_t offset = center ? n_fft / 2 : 0;

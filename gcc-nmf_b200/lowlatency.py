@@ -1,0 +1,256 @@
+"""Streaming form of the online / low-latency notebook loop (csrc/lowlatency.cu, `gccnmf_ll_*` in include/gccnmf_b200.h).
+
+One `LowLatencyEngine` holds S independent streams on the device.  Each `process` call takes `hops * hop` new samples per stream
+and returns as many finished output samples per stream; output sample p of a stream is sample p - `latency` of what
+`online.performOnlineSpeechEnhancement` computes on the whole recording (samples before the stream's first frame are zero).  A
+call is one stream-ordered unit on the device, optionally one CUDA graph launch.
+
+The synthesis is a weight vector w applied to every frame in the overlap-add and a gain g applied to every output sample
+(`synthesisWeights`):
+  'online'      gainPerFrame=True of the batch function: w = gainFactor, g = 1
+  'lowlatency'  gainPerFrame=False (the low-latency notebook, which never applies its synthesis window): w = 1, g = gainFactor
+  'windowed'    applySynthesisWindow=True: w = the synthesis window, g = gainFactor
+with gainFactor = 2 hop / N.  The latency is Q hop - hop - z samples, Q = ceil(N / hop) and z the first nonzero index of w; when hop
+divides N that is N - hop for the first two, and 2m - hop - 1 for the asymmetric synthesis window of
+lowLatencySpeechEnhancement.ipynb:382-392 (its first weight is zero).
+"""
+import ctypes
+
+import numpy as np
+
+from ._lib import LLConfig, LLStreamParams, default_handle
+
+SYNTHESIS_MODES = ('online', 'lowlatency', 'windowed')
+
+EXPORT_X, EXPORT_COHERENCE, EXPORT_ANGULAR, EXPORT_ACC_MAX, EXPORT_TARGETS, EXPORT_ARGMAX, EXPORT_MASKS, EXPORT_WIENER, EXPORT_Y, \
+    EXPORT_REFINED, EXPORT_STATUS, EXPORT_H, EXPORT_VALID, EXPORT_CARRY = range(14)
+
+
+def synthesisWeights(mode, synthesisWindow, hopSize):
+    """(w (N) float64, g float32) of a synthesis mode (see the module docstring)."""
+    N = len(synthesisWindow)
+    gainFactor = hopSize / float(N) * 2
+    if mode == 'online':
+        return np.full(N, gainFactor), np.float32(1.0)
+    if mode == 'lowlatency':
+        return np.ones(N), np.float32(gainFactor)
+    if mode == 'windowed':
+        return np.ascontiguousarray(synthesisWindow, dtype=np.float64), np.float32(gainFactor)
+    raise ValueError('synthesis must be one of %s (got %r)' % (SYNTHESIS_MODES, mode))
+
+
+def latencyOf(weights, hopSize):
+    """Samples between the newest input and the output emitted with it: Q hop - hop - z, Q = ceil(N / hop), z the first nonzero
+    index of the weights (a frame ends in the hop that completes it, and its first z weights are zero)."""
+    nz = np.flatnonzero(np.asarray(weights) != 0)
+    if len(nz) == 0:
+        raise ValueError('the synthesis weights are all zero')
+    hop = int(hopSize)
+    return -(-len(weights) // hop) * hop - hop - int(nz[0])
+
+
+def batchArguments(mode):
+    """The performOnlineSpeechEnhancement keywords that compute what a synthesis mode streams."""
+    return {'online': dict(gainPerFrame=True), 'lowlatency': dict(gainPerFrame=False),
+            'windowed': dict(gainPerFrame=False, applySynthesisWindow=True)}[mode]
+
+
+class LowLatencyEngine(object):
+    def __init__(self, W, expJOmegaTau, analysisWindow, synthesisWindow, hopSize, numStreams=1, hopsPerCall=1, synthesis='lowlatency',
+                 targetTDOAEpsilon=1.0, numInferenceIterations=0, sparsityAlpha=0.0, epsilon=1e-16, seedValue=0, device=0):
+        self.h = default_handle(device)
+        torch = self.torch = self.h.torch
+        W = np.ascontiguousarray(W, dtype=np.float32)
+        E = np.ascontiguousarray(expJOmegaTau, dtype=np.complex128)
+        F, K = W.shape
+        N = len(analysisWindow)
+        if N != 2 * (F - 1) or E.shape[0] != F or len(synthesisWindow) != N:
+            raise ValueError('W (F, K), expJOmegaTau (F, D) and the windows (N = 2 (F - 1)) do not agree')
+        self.F, self.K, self.N, self.D = F, K, N, E.shape[1]
+        self.hop, self.S, self.C = int(hopSize), int(numStreams), int(hopsPerCall)
+        self.synthesis = synthesis
+        self.weights, self.gain = synthesisWeights(synthesis, synthesisWindow, self.hop)
+        self.latency = latencyOf(self.weights, self.hop)
+        if self.latency < 0:
+            raise ValueError('the synthesis weights start less than a hop before the end of the frame')
+        self.cfg = LLConfig(N, self.hop, self.C, K, self.D, self.S, int(numInferenceIterations), float(sparsityAlpha), float(epsilon))
+        self.state_bytes = int(self.h.lib.gccnmf_ll_state_bytes(ctypes.byref(self.cfg)))
+        if self.state_bytes == 0:
+            raise ValueError('invalid low-latency configuration (N a power of two in [32, 4096], 1 <= hop <= N, 1 <= hopsPerCall <= 64, '
+                             'D a power of two in [4, 128], 1 <= numStreams <= 4096)')
+        self.inference = numInferenceIterations > 0
+        self.stream = torch.cuda.Stream(device=self.h.device)      # a capturable stream of its own
+        self.state = torch.empty(self.state_bytes, dtype=torch.uint8, device=self.h.device)
+        H0 = None
+        if self.inference:
+            np.random.seed(seedValue)                                 # gccNMFFunctions.py:70,73, as online.py draws it
+            H0 = (np.random.random((K, 2)).astype(np.float32) + epsilon).astype(np.float32)
+        dev = lambda a: torch.as_tensor(np.ascontiguousarray(a)).to(self.h.device)      # noqa: E731
+        self._const = [dev(W), dev(E.view(np.float64).reshape(F, 2 * self.D)), dev(np.asarray(analysisWindow, np.float64)),
+                       dev(self.weights), dev(H0) if H0 is not None else None]
+        self._eps = np.full(self.S, float(targetTDOAEpsilon), np.float32)
+        self._active = np.ones(self.S, np.int32)
+        self._override = np.full(self.S, -1, np.int32)
+        self._io = {}
+        self._graphs = {}
+        self._exports = {}
+        self.last_hops = None
+        self.h.torch.cuda.current_stream(self.h.device).synchronize()
+        c = self._const
+        with torch.cuda.stream(self.stream):
+            self._check(self.h.lib.gccnmf_ll_init(self.h.h, ctypes.byref(self.cfg), c[0].data_ptr(), c[1].data_ptr(), c[2].data_ptr(),
+                                                  c[3].data_ptr(), float(self.gain), c[4].data_ptr() if c[4] is not None else None,
+                                                  self.state.data_ptr(), self.state_bytes, self.stream.cuda_stream))
+        self._send_params(0, self.S)
+        self.stream.synchronize()
+
+    def _check(self, status):
+        self.h.check(status)
+
+    def _streams(self, streams):
+        if streams is None:
+            return np.arange(self.S)
+        idx = np.atleast_1d(np.asarray(streams, dtype=np.int64))
+        if idx.size == 0 or idx.min() < 0 or idx.max() >= self.S:
+            raise ValueError('streams outside [0, %d)' % self.S)
+        return idx
+
+    def _send_params(self, first, count):
+        arr = (LLStreamParams * count)()
+        for i in range(count):
+            s = first + i
+            arr[i] = LLStreamParams(float(self._eps[s]), int(self._active[s]), int(self._override[s]))
+        self._check(self.h.lib.gccnmf_ll_set_params(self.h.h, ctypes.byref(self.cfg), self.state.data_ptr(), self.state_bytes, first, count,
+                                                    arr, self.stream.cuda_stream))
+
+    def _send_streams(self, idx):
+        lo, hi = int(idx.min()), int(idx.max())
+        self._send_params(lo, hi - lo + 1)
+        self.stream.synchronize()
+
+    # ------------------------------------------------------------------ settings (stream-ordered: they act from the next call)
+    def set_params(self, streams=None, targetTDOAEpsilon=None, targetOverride=None):
+        """Per-stream epsilon of the boxcar atom mask, and a target TDOA index that replaces the localised one (-1: none)."""
+        idx = self._streams(streams)
+        if targetTDOAEpsilon is not None:
+            self._eps[idx] = targetTDOAEpsilon
+        if targetOverride is not None:
+            o = np.broadcast_to(np.asarray(targetOverride, dtype=np.int64), idx.shape)
+            if o.min() < -1 or o.max() >= self.D:
+                raise ValueError('targetOverride outside [0, %d) (or -1)' % self.D)
+            self._override[idx] = o
+        self._send_streams(idx)
+
+    def set_active(self, streams, active):
+        """An inactive stream outputs zeros and its state does not change."""
+        idx = self._streams(streams)
+        self._active[idx] = 1 if active else 0
+        self._send_streams(idx)
+
+    def reset(self, streams=None):
+        """The streams start over (rings zeroed, running maximum -inf, no frames yet); their parameters stay."""
+        idx = np.unique(self._streams(streams))
+        breaks = np.flatnonzero(np.diff(idx) != 1) + 1          # one call per contiguous run of streams
+        for run in np.split(idx, breaks):
+            self._check(self.h.lib.gccnmf_ll_reset_streams(self.h.h, ctypes.byref(self.cfg), self.state.data_ptr(), self.state_bytes,
+                                                           int(run[0]), len(run), self.stream.cuda_stream))
+        self.stream.synchronize()
+
+    # ------------------------------------------------------------------ per-call work
+    def _buffers(self, hops):
+        b = self._io.get(hops)
+        if b is None:
+            torch = self.torch
+            shape = (self.S, 2, hops * self.hop)
+            b = self._io[hops] = (torch.zeros(shape, dtype=torch.float32).pin_memory(), torch.zeros(shape, dtype=torch.float32).pin_memory(),
+                                  torch.zeros(shape, dtype=torch.float32, device=self.h.device),
+                                  torch.zeros(shape, dtype=torch.float32, device=self.h.device))
+        return b
+
+    def build_graph(self, hops=None):
+        """The graph of a call of `hops` hops (default: hopsPerCall): H2D of the pinned input, the kernels, D2H of the output."""
+        hops = self.C if hops is None else int(hops)
+        g = self._graphs.get(hops)
+        if g is None:
+            in_host, out_host, in_dev, out_dev = self._buffers(hops)
+            g = ctypes.c_void_p()
+            self._check(self.h.lib.gccnmf_ll_graph_create(self.h.h, ctypes.byref(self.cfg), self.state.data_ptr(), self.state_bytes, hops,
+                                                          in_dev.data_ptr(), out_dev.data_ptr(), in_host.data_ptr(), out_host.data_ptr(),
+                                                          ctypes.byref(g), self.stream.cuda_stream))
+            self._graphs[hops] = g
+        return g
+
+    def process(self, x, use_graph=True):
+        """x (S, 2, hops * hop) float32 -> (S, 2, hops * hop) float32 (a copy)."""
+        x = np.asarray(x, dtype=np.float32)
+        if x.ndim != 3 or x.shape[0] != self.S or x.shape[1] != 2 or x.shape[2] % self.hop != 0:
+            raise ValueError('x must be (%d, 2, hops * %d)' % (self.S, self.hop))
+        hops = x.shape[2] // self.hop
+        if not 1 <= hops <= self.C:
+            raise ValueError('a call takes 1 .. %d hops (got %d)' % (self.C, hops))
+        in_host, out_host, in_dev, out_dev = self._buffers(hops)
+        in_host.numpy()[:] = x
+        if use_graph:
+            self._check(self.h.lib.gccnmf_rt_graph_launch(self.h.h, self.build_graph(hops), self.stream.cuda_stream))
+        else:
+            with self.torch.cuda.stream(self.stream):
+                in_dev.copy_(in_host, non_blocking=True)
+                self._check(self.h.lib.gccnmf_ll_process(self.h.h, ctypes.byref(self.cfg), self.state.data_ptr(), self.state_bytes, hops,
+                                                         in_dev.data_ptr(), out_dev.data_ptr(), self.stream.cuda_stream))
+                out_host.copy_(out_dev, non_blocking=True)
+        self.stream.synchronize()
+        self.last_hops = hops
+        return out_host.numpy().copy()
+
+    def export(self, what):
+        """Host copy of one item of the last call (see gccnmf_ll_export); T = S hops columns, column s hops + i = frame i of stream s."""
+        if self.last_hops is None:
+            raise RuntimeError('no call yet')
+        torch = self.torch
+        T, F, K, D = self.S * self.last_hops, self.F, self.K, self.D
+        shapes = {EXPORT_X: ((2, F, T), torch.complex64), EXPORT_COHERENCE: ((F, T), torch.complex64), EXPORT_ANGULAR: ((D, T), torch.float64),
+                  EXPORT_ACC_MAX: ((D, T), torch.float64), EXPORT_TARGETS: ((T,), torch.int32), EXPORT_ARGMAX: ((K, T), torch.int32),
+                  EXPORT_MASKS: ((K, T), torch.float32), EXPORT_WIENER: (((2, F, T) if self.inference else (F, T)), torch.float32),
+                  EXPORT_Y: ((2, F, T), torch.complex64), EXPORT_REFINED: ((1,), torch.int32), EXPORT_STATUS: ((1,), torch.int32),
+                  EXPORT_H: ((K, 2 * T), torch.float32), EXPORT_VALID: ((T,), torch.int32), EXPORT_CARRY: ((self.S, D), torch.float64)}
+        shape, dtype = shapes[what]
+        key = (what, shape)
+        buf = self._exports.get(key)
+        if buf is None:
+            buf = self._exports[key] = torch.zeros(shape, dtype=dtype).pin_memory()
+        self._check(self.h.lib.gccnmf_ll_export(self.h.h, ctypes.byref(self.cfg), self.state.data_ptr(), self.state_bytes, self.last_hops,
+                                                int(what), buf.data_ptr(), self.stream.cuda_stream))
+        self.stream.synchronize()
+        return buf.numpy().copy()
+
+    def close(self):
+        if self.h.h:
+            for g in self._graphs.values():
+                self.h.lib.gccnmf_rt_graph_destroy(self.h.h, g)
+        self._graphs = {}
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def streamSignals(signals, W, expJOmegaTau, analysisWindow, synthesisWindow, hopSize, hopsPerCall=1, synthesis='lowlatency',
+                  targetTDOAEpsilon=1.0, numInferenceIterations=0, use_graph=True, device=0, **kwargs):
+    """Streams a list of stereo signals (2, n_i) through one engine, one stream each, hopsPerCall hops per call, and returns the
+    outputs aligned with the input: out_i[:, p] = output sample p + latency (the batch function's targetEstimateSamplesOLA), each
+    (2, n_i).  Shorter signals are followed by silence; the engine is flushed with `latency` samples of silence at the end."""
+    sig = [np.asarray(s, dtype=np.float32) for s in signals]
+    eng = LowLatencyEngine(W, expJOmegaTau, analysisWindow, synthesisWindow, hopSize, numStreams=len(sig), hopsPerCall=hopsPerCall,
+                           synthesis=synthesis, targetTDOAEpsilon=targetTDOAEpsilon, numInferenceIterations=numInferenceIterations,
+                           device=device, **kwargs)
+    step = eng.hop * eng.C
+    total = max(s.shape[1] for s in sig) + eng.latency
+    total = -(-total // step) * step
+    x = np.zeros((len(sig), 2, total), np.float32)
+    for i, s in enumerate(sig):
+        x[i, :, :s.shape[1]] = s
+    y = np.concatenate([eng.process(x[:, :, p:p + step], use_graph=use_graph) for p in range(0, total, step)], axis=2)
+    eng.close()
+    return [y[i, :, eng.latency:eng.latency + s.shape[1]] for i, s in enumerate(sig)]

@@ -42,7 +42,7 @@ def getAsymmetricSynthesisWindow(k, m, d):
 def performOnlineSpeechEnhancement(stereoSamples, sampleRate, W, analysisWindow, synthesisWindow, hopSize, numTDOAs,
                                    microphoneSeparationInMetres, targetTDOAEpsilon, numInferenceIterations=0,
                                    gainPerFrame=False, device=0, sparsityAlpha=0, epsilon=1e-16, seedValue=0,
-                                   _forcedTargetTDOAs=None, _forcedAtomMasks=None):
+                                   _forcedTargetTDOAs=None, _forcedAtomMasks=None, applySynthesisWindow=False):
     """Returns the notebook's tuple (lowLatencySpeechEnhancement.ipynb:583-584):
     inputSpectrogram, outputSpectrogram, targetEstimateSamplesOLA, gccPHATAccumulatedMax, targetTDOAs,
     angularSpectrogram, atomMasks, wienerFilters.
@@ -55,6 +55,10 @@ def performOnlineSpeechEnhancement(stereoSamples, sampleRate, W, analysisWindow,
     reference: gccNMFFunctions.inferCoefficientsKLNMF restates it from gccNMFFunctions.py:73,76), then
     wiener = (W . (H * mask)) / (W . H).  Every frame starts from the same seeded H0 (the call re-seeds), and H-only updates
     are independent per column, so all frames run as ONE (F, 2T) problem on the KL-NMF kernels.
+
+    applySynthesisWindow=True weights every frame by synthesisWindow in the overlap-add (the gain stays at the end) instead of the
+    notebooks' unweighted frames: with the asymmetric synthesis window a frame then touches only its last 2m samples, which is the
+    low latency the windows were designed for (lowlatency.py streams it with 2m - hop - 1 samples of latency).
 
     _forcedTargetTDOAs / _forcedAtomMasks (tests): teacher-force the integer decisions of the loop.
     """
@@ -99,8 +103,11 @@ def performOnlineSpeechEnhancement(stereoSamples, sampleRate, W, analysisWindow,
         Y, wiener = h.wiener_apply(atomMasks, Wd, X, want_filter=True)                            # :429-431, :440
         wf = wiener.cpu().numpy().astype(np.float64)
         wf = np.stack([wf, wf])
-    ones = np.full(N, gainFactor if gainPerFrame else 1.0)
-    y = h.istft_ola(Y, h.to_device(ones), N, hopSize, gain=np.float32(1.0 if gainPerFrame else gainFactor),
+    if applySynthesisWindow:
+        weights = np.ascontiguousarray(synthesisWindow, dtype=np.float64)
+    else:
+        weights = np.full(N, gainFactor if gainPerFrame else 1.0)
+    y = h.istft_ola(Y, h.to_device(weights), N, hopSize, gain=np.float32(1.0 if gainPerFrame and not applySynthesisWindow else gainFactor),
                     center=False, conjugate=False)                                                # :443-447 / :575-580
     out = np.zeros_like(stereoSamples)
     out[:, :y.shape[1]] = y.cpu().numpy()

@@ -514,6 +514,68 @@ GCCNMF_API int gccnmf_rtbank_export(gccnmf_handle* h, const gccnmf_rt_config* cf
                          int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int slot, int what, void* dst,
                          void* stream);
 
+/* ---- a11 streamed: the online / low-latency notebook loop for S streams ---------------------------------------------
+ * onlineSpeechEnhancement.ipynb:406-447 / lowLatencySpeechEnhancement.ipynb:511-584 as performOnlineSpeechEnhancement computes
+ * them in batch, one hop at a time.  Each call pushes hops * hop new samples per stream (1 <= hops <= hops_per_call) and emits
+ * as many finished output samples per stream: output sample p is overlap-add sample p - L, L = Q hop - hop - z with
+ * Q = ceil(N / hop) and z the first nonzero index of the synthesis weights w (N - hop - z when hop divides N; samples before the
+ * first frame are zero).  Per frame: float64 rfft of
+ * frame x analysis window rounded to complex64, PHAT coherence, angular spectrum, running maximum carried across calls, target =
+ * argmax, all-TDOA GCC-NMF argmax per atom (tensor cores + float64 refinement, and a gated float64 launch when the refinement
+ * list overflows), boxcar atom mask with the stream's epsilon, Wiener filter (W . mask) / rowsum(W) or, with inference, the
+ * H-inferred filter, inverse FFT, then acc = float32(fma(w[r], frame[r], acc)) into an N-sample output ring in frame order and
+ * gain x acc out.  One call is stream-ordered with no host synchronisation and can be captured as one CUDA graph.
+ * Constraints: N a power of two in [32, 4096], 1 <= hop <= N, 1 <= C <= 64, D a power of two in [4, 128], 1 <= S <= 4096,
+ * z <= (Q - 1) hop, and with inference (K + N / 2 + 1) x 4 <= 227 KiB. */
+typedef struct gccnmf_ll_config {
+  int window_size;           /* N                                                                       */
+  int hop_size;              /* hop                                                                     */
+  int hops_per_call;         /* C: the most hops one call may push                                      */
+  int num_atoms;             /* K                                                                       */
+  int num_tdoas;             /* D                                                                       */
+  int num_streams;           /* S                                                                       */
+  int inference_iterations;  /* 0: (W . mask) / rowsum(W); > 0: H-only KL updates of every frame from H0 */
+  float sparsity_alpha;      /* of the inference updates (gccNMFFunctions.py:76)                        */
+  float epsilon;
+} gccnmf_ll_config;
+/* Per-stream settings (host struct): epsilon of the boxcar atom mask (|argmax - target| < epsilon); active = 0 makes the
+ * stream output zeros and leaves its state untouched; target_override >= 0 replaces the localised target TDOA index. */
+typedef struct gccnmf_ll_stream_params {
+  float epsilon;
+  int active;
+  int target_override;
+} gccnmf_ll_stream_params;
+/* 0 for an invalid configuration. */
+GCCNMF_API size_t gccnmf_ll_state_bytes(const gccnmf_ll_config* cfg);
+/* W (F, K) f32; E (F, D) complex128 expJOmegaTau; analysis_window (N) f64; synthesis_weights (N) f64 = w; gain g (applied to
+ * every emitted sample); H0 (K, 2) f32 (NULL when inference_iterations == 0).  All five are DEVICE pointers.  init reads w back
+ * on `stream` and waits for it (the latency depends on it), so it synchronises `stream` once; it fails before enqueueing
+ * anything else when w starts too late.  Every stream starts empty and active, with epsilon 1 and no target override. */
+GCCNMF_API int gccnmf_ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, const float* W, const double* E,
+                   const double* analysis_window, const double* synthesis_weights, float gain, const float* H0, void* state,
+                   size_t state_bytes, void* stream);
+/* Streams [first, first + count) go back to an empty stream (rings zeroed, running maximum -inf, frame count 0); their
+ * parameters stay. */
+GCCNMF_API int gccnmf_ll_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int first,
+                            int count, void* stream);
+GCCNMF_API int gccnmf_ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int first,
+                         int count, const gccnmf_ll_stream_params* params_host, void* stream);
+/* in (S, 2, hops * hop) f32 -> out (S, 2, hops * hop) f32, device buffers. */
+GCCNMF_API int gccnmf_ll_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops,
+                      const float* in, float* out, void* stream);
+/* gccnmf_ll_process(hops) as an instantiated CUDA graph ([H2D of in_host ->] kernels [-> D2H to out_host]); launch and destroy with
+ * gccnmf_rt_graph_launch / gccnmf_rt_graph_destroy. */
+GCCNMF_API int gccnmf_ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops,
+                           float* in, float* out, const float* in_host, float* out_host, void** graph_exec, void* stream);
+/* Items of the last call, which pushed `hops` hops (T = S hops columns, column s hops + i = frame i of stream s's call):
+ *   0 X (2, F, T) c64   1 coherence (F, T) c64   2 angular (D, T) f64   3 accumulated max (D, T) f64   4 targets (T) i32
+ *   5 TDOA argmax per atom (K, T) i32   6 atom masks (K, T) f32   7 Wiener filters (F, T) f32, or (2, F, T) with inference
+ *   8 Y (2, F, T) c64   9 refined count (1) i32   10 status (1) i32: 1 when the float64 fallback ran   11 H (K, 2T) f32
+ *   (inference only)   12 frame valid (T) i32: 0 for a frame that starts before the stream's first sample   13 carried
+ *   accumulated max (S, D) f64 */
+GCCNMF_API int gccnmf_ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, int what,
+                     void* dst, void* stream);
+
 /*
  * The building block the KL-NMF loop runs on (klnmf_tma.cu): the same 3-product contraction, TMA-fed, over operands
  * that are pre-split into bf16 hi/lo planes and kept in ONE orientation each; an operand contracted over its
