@@ -85,6 +85,42 @@ def _worker(rank, world, port, out):
         dist.destroy_process_group()
 
 
+class RecordingOps(object):
+    """Stand-in for Handle.klnmf_begin / klnmf_step_pull / klnmf_end that records every call klnmf_sharded_pull makes."""
+
+    def __init__(self):
+        self.calls = []
+
+    def klnmf_begin(self, V, W, H):
+        self.calls.append(('begin', V, W, H))
+
+    def klnmf_step_pull(self, V, W, H, iteration, epoch, rank, world, bases, layout_T2, two_shot, direct, sparsity_alpha=0.0, epsilon=1e-16):
+        self.calls.append(('step', V, W, H, iteration, epoch, rank, world, bases, layout_T2, two_shot, direct, sparsity_alpha, epsilon))
+
+    def klnmf_end(self, W, H, iterations_done):
+        self.calls.append(('end', W, H, iterations_done))
+
+
+@pytest.mark.parametrize('two_shot,direct', [(0, False), (0, True), (1, True), (2, False)])
+def test_klnmf_sharded_pull_bookkeeping(two_shot, direct):
+    """Two runs on one exchange: begin first, end(numIterations) last, and every step gets the iteration, the epoch the run
+    started at (0, then the first run's count: the buffer's counters keep counting), and the exchange's rank, world, bases,
+    layout_T2, form and direct flag unchanged; the exchange's epoch ends at the total."""
+    import types
+    from gcc_nmf_b200 import distributed as d
+    bases = object()
+    px = types.SimpleNamespace(epoch=0, rank=2, world=3, bases=bases, layout_T2=1000, two_shot=two_shot, direct=direct)
+    V, W, H = object(), object(), object()
+    for iters, epoch in ((3, 0), (2, 3)):
+        ops = RecordingOps()
+        assert d.klnmf_sharded_pull(ops, px, V, W, H, iters, 0.3, 0.25) == (W, H)
+        assert ops.calls[0] == ('begin', V, W, H)
+        assert ops.calls[-1] == ('end', W, H, iters)
+        assert ops.calls[1:-1] == [('step', V, W, H, it, epoch, 2, 3, bases, 1000, two_shot, direct, 0.3, 0.25) for it in range(iters)]
+        assert all(c[8] is bases for c in ops.calls[1:-1])
+    assert px.epoch == 5
+
+
 def test_shard_bookkeeping():
     from gcc_nmf_b200 import distributed as d
     for total, world in [(1872, 8), (37, 2), (10, 3), (7, 7)]:

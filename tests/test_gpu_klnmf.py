@@ -53,7 +53,7 @@ def h():
 
 
 DEFAULT_OPTIONS = {'force_simt_nmf': 0, 'nmf_pdl': 1, 'wh_tile': 0, 'gemm_cluster': -1, 'gemm_pair': -1, 'gemm_preload': 1,
-                   'gemm_streaming': 0, 'l2_persist': 0, 'w_cluster_reduce': 1, 'wh_split2': 0}
+                   'gemm_streaming': 0, 'l2_persist': 0, 'w_cluster_reduce': 1, 'wh_split2': 0, 'pull_force_pack': 0}
 
 
 class options(object):
