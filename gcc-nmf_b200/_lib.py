@@ -178,6 +178,14 @@ SIGNATURES.update({
     'gccnmf_ll_process': (c_int, [_H, _LC, _P, c_size_t, c_int, _P, _P, _S]),
     'gccnmf_ll_graph_create': (c_int, [_H, _LC, _P, c_size_t, c_int, _P, _P, _P, _P, ctypes.POINTER(c_void_p), _S]),
     'gccnmf_ll_export': (c_int, [_H, _LC, _P, c_size_t, c_int, c_int, c_void_p, _S]),
+    'gccnmf_llsep_state_bytes': (c_size_t, [_LC, c_int]),
+    'gccnmf_llsep_init': (c_int, [_H, _LC, c_int, _P, _P, _P, _P, c_float, _P, _P, c_size_t, _S]),
+    'gccnmf_llsep_reset_streams': (c_int, [_H, _LC, c_int, _P, c_size_t, c_int, c_int, _S]),
+    'gccnmf_llsep_set_params': (c_int, [_H, _LC, c_int, _P, c_size_t, c_int, c_int, ctypes.POINTER(LLStreamParams), _S]),
+    'gccnmf_llsep_set_targets': (c_int, [_H, _LC, c_int, _P, c_size_t, c_int, c_int, ctypes.POINTER(c_int32), _S]),
+    'gccnmf_llsep_process': (c_int, [_H, _LC, c_int, _P, c_size_t, c_int, _P, _P, _S]),
+    'gccnmf_llsep_graph_create': (c_int, [_H, _LC, c_int, _P, c_size_t, c_int, _P, _P, _P, _P, ctypes.POINTER(c_void_p), _S]),
+    'gccnmf_llsep_export': (c_int, [_H, _LC, c_int, _P, c_size_t, c_int, c_int, c_void_p, _S]),
 })
 
 

@@ -1,6 +1,7 @@
 // GCC-PHAT localisation and GCC-NMF masking kernels.
 //   phat_angspec       runGCCNMF.py:44 + gccNMFFunctions.py:85-92      (a3, a4)
 //   tdoa_gccnmf        gccNMFFunctions.py:118-135; offlineSpeechEnhancement.ipynb:444-450; online :422  (a6, a10, a11)
+//   target_gccnmf      gccNMFFunctions.py:118-135 at P targets that change per frame (the low-latency path's sources)
 //   coeff_mask         gccNMFFunctions.py:137-143                        (a7)
 //   argmax_mask        offlineSpeechEnhancement.ipynb:466-472            (a10 mask)
 //   masked_recon_phase gccNMFFunctions.py:145-151                        (a8)
@@ -169,15 +170,27 @@ struct LoadWAtoms {  // A(m = atom, k = f) = W[f][atom]
   const float* W; int K, F;
   __device__ double operator()(int m, int f) const { return (m < K && f < F) ? (double)__ldg(W + (int64_t)f * K + m) : 0.0; }
 };
+// Re(c * e) of a coherence value and a steering value, the B operand of every GCC-NMF contraction.  One function for all the
+// loaders below, so that the compiler cannot contract the expression differently in one of them: a target value then has the
+// bits of the all-TDOA value at the same (TDOA, atom, frame).
+__device__ __forceinline__ double re_coh_steer(float2 c, double2 e) { return (double)c.x * e.x - (double)c.y * e.y; }
+
 struct LoadRealGCC {  // B(n = t * D + d, k = f) = Re(coherence[f][t] * E[f][d])
   static constexpr bool kContigK = false;
   const float2* coh; const double2* E; int F, T, D, N;
   __device__ double operator()(int n, int f) const {
     if (n >= N || f >= F) return 0.0;
     const int t = n / D, d = n - t * D;
-    const float2 c = __ldg(coh + (int64_t)f * T + t);
-    const double2 e = __ldg(E + (int64_t)f * D + d);
-    return (double)c.x * e.x - (double)c.y * e.y;
+    return re_coh_steer(__ldg(coh + (int64_t)f * T + t), __ldg(E + (int64_t)f * D + d));
+  }
+};
+struct LoadTargetGCC {  // B(n = t * P + q, k = f) = Re(coherence[f][t] * E[f][targets[t * P + q]]): P targets per frame
+  static constexpr bool kContigK = false;
+  const float2* coh; const double2* E; const int32_t* targets; int F, T, D, P, N;
+  __device__ double operator()(int n, int f) const {
+    if (n >= N || f >= F) return 0.0;
+    const int t = n / P;
+    return re_coh_steer(__ldg(coh + (int64_t)f * T + t), __ldg(E + (int64_t)f * D + __ldg(targets + n)));
   }
 };
 
@@ -251,6 +264,30 @@ tdoa_gccnmf_kernel(int K, int N, int F, LoadWAtoms aload, LoadRealGCC bload, int
         const int n_first = n0 + half * (GN / 2) + tx * (GTN / 2);
         if ((tx % lanes) == 0 && m < K && n_first < N) argmax[(int64_t)m * T + n_first / D] = bi[half];
       }
+    }
+  }
+}
+
+// getTargetTDOAGCCNMFs with P targets per frame: values (P, K, T) f32, values[q][k][t] = float32(sum_f W[f][k] Re(coh[f][t] E[f][tau])),
+// tau = targets[t P + q].  The same main loop as tdoa_gccnmf_kernel (an fma chain over f from 0 per output), so every value has the
+// bits of the all-TDOA value at (tau, k, t).  BN = 32 is the narrow column tile for small T P; it changes no sum.
+template <int BN, int TN>
+__global__ void __launch_bounds__((GM / GTM) * (BN / TN))
+target_gccnmf_kernel(int K, int N, int F, LoadWAtoms aload, LoadTargetGCC bload, int T, int P, float* __restrict__ values) {
+  double acc[GTM][TN];
+  const int m0 = blockIdx.y * GM, n0 = blockIdx.x * BN;
+  gemm_simt_mainloop<double, GM, BN, GK, GTM, TN>(acc, m0, n0, F, aload, bload);
+  constexpr int TX = BN / TN;
+#pragma unroll
+  for (int i = 0; i < GTM; ++i) {
+    const int m = gemm_row<GM, GTM, TX>(m0, i);
+    if (m >= K) continue;
+#pragma unroll
+    for (int j = 0; j < TN; ++j) {
+      const int n = gemm_col<BN, TN, TX>(n0, j);
+      if (n >= N) continue;
+      const int t = n / P, q = n - t * P;
+      values[((int64_t)q * K + m) * T + t] = (float)acc[i][j];
     }
   }
 }
@@ -620,5 +657,27 @@ int gccnmf_tdoa_gccnmf_gated(gccnmf_handle* h, const float* coherence, int F, in
   dim3 grid((N + GN - 1) / GN, (K + GM - 1) / GM);
   auto k = tdoa_gccnmf_kernel<true>;
   GCCNMF_LAUNCH(h, k, grid, kGccThreads, 0, stream, K, N, F, a, b, T, D, nullptr, argmax, gate, capacity, ran);
+  return GCCNMF_OK;
+}
+
+// values (P, K, T) f32 = the float64 GCC-NMF contraction at P target TDOAs per frame, targets (T, P) i32 on the device (each in
+// [0, D)).  Bit for bit the values gccnmf_tdoa_gccnmf writes at those (TDOA, atom, frame).  Column tiles of 128, or 32 when the
+// wide tiles would leave SMs idle.
+int gccnmf_target_gccnmf(gccnmf_handle* h, const float* coherence, int F, int T, const double* E, int D, const float* W, int K,
+                         const int32_t* targets, int P, float* values, void* stream) {
+  GCCNMF_REQUIRE(h, F > 0 && T > 0 && D > 0 && K > 0 && P > 0 && coherence && E && W && targets && values, "target_gccnmf: bad arguments");
+  GCCNMF_REQUIRE(h, (int64_t)T * P < (int64_t)1 << 31 && (int64_t)P * K * T < (int64_t)1 << 31, "target_gccnmf: T x P or P x K x T overflows int32");
+  const int N = T * P;
+  LoadWAtoms a{W, K, F};
+  LoadTargetGCC b{reinterpret_cast<const float2*>(coherence), reinterpret_cast<const double2*>(E), targets, F, T, D, P, N};
+  const int mt = (K + GM - 1) / GM;
+  if ((int64_t)((N + GN - 1) / GN) * mt >= h->sm_count) {
+    auto k = target_gccnmf_kernel<GN, GTN>;
+    GCCNMF_LAUNCH(h, k, dim3((N + GN - 1) / GN, mt), (GM / GTM) * (GN / GTN), 0, stream, K, N, F, a, b, T, P, values);
+  } else {
+    constexpr int kBN = 32, kTN = 4;
+    auto k = target_gccnmf_kernel<kBN, kTN>;
+    GCCNMF_LAUNCH(h, k, dim3((N + kBN - 1) / kBN, mt), (GM / GTM) * (kBN / kTN), 0, stream, K, N, F, a, b, T, P, values);
+  }
   return GCCNMF_OK;
 }

@@ -17,6 +17,17 @@
 //                  emitted positions, move the input ring on
 // Every column is computed on its own in each stage, so the result of a stream does not depend on the other streams or on how its
 // samples are split into calls.
+//
+// With P sources per stream (gccnmf_llsep_*) the stages after phat_angspec are instead:
+//   ll_src_targets     running maximum as above, then per frame the P largest peaks of it (select_peaks) as the stream's targets,
+//                      held when there are fewer (status bit 0); overrides replace them    -> column targets (T, P)
+//   target_gccnmf      the float64 GCC-NMF values at each column's P targets (gcc.cu)      -> values (P, K, T)
+//   coeff_mask         one-hot masks per source (gcc.cu); an all-NaN (k, t) goes to no source and sets bit 1 of the call's status
+//   ll_infer           (inference only) once per column, H shared by the sources
+//   wiener             per source, with its mask
+//   istft frames       one launch over the (P, 2) spectra
+//   ll_src_ola_emit    per (stream, source): ll_ola_emit_kernel's overlap-add and emit into the source's own ring
+//   ll_src_advance     per stream, after every source has emitted: the input ring and the hop count move on
 #include <cmath>
 
 #include "common.cuh"
@@ -26,6 +37,8 @@ int gccnmf_stft_segments(gccnmf_handle* h, const float* samples, int64_t sample_
 int gccnmf_istft_frames(gccnmf_handle* h, const float* spec, int batch, int n_fft, int T, int conjugate, float* frames, void* stream);
 int gccnmf_tdoa_gccnmf_gated(gccnmf_handle* h, const float* coherence, int F, int T, const double* E, int D, const float* W, int K,
                              int32_t* argmax, const int32_t* gate, int capacity, int32_t* ran, void* stream);
+int gccnmf_target_gccnmf(gccnmf_handle* h, const float* coherence, int F, int T, const double* E, int D, const float* W, int K,
+                         const int32_t* targets, int P, float* values, void* stream);
 
 namespace {
 
@@ -44,17 +57,24 @@ struct LLHeader {
 
 struct LLLayout {
   int S, N, hop, C, K, D, F, Q, R;   // Q = ceil(N / hop): hops a frame spans; R = (Q - 1) hop: input ring length
+  int P;                             // sources per stream (0: one enhanced target)
   size_t bytes;
   LLHeader* head;
   LLStream* streams;
   double *win_a, *w_syn, *E, *carry, *acc, *ang;
   float *W, *WT, *colsumW, *H0, *in_ring, *out_ring, *stage, *X, *V, *coh, *mask, *wiener, *Y, *H, *frames, *ws_wiener;
-  int32_t *targets, *valid, *argmax, *counters;   // counters: [0] refined count, [1] status
+  // counters: [0] refined count, [1] status; with sources [2] coeff_mask's all-NaN flag, [3] the call's status word
+  int32_t *targets, *valid, *argmax, *counters;
   void* ws_argmax;
   size_t n_argmax;
+  // sources only: per stream the carried targets and overrides (kLLMaxSources each) and a status word; per call the values and
+  // masks (P, K, T) and the column targets (T, P).  out_ring, wiener, Y and frames then hold P times as much.
+  int32_t *src_targets, *src_override, *src_status, *col_targets;
+  float *values, *src_mask;
 };
 
 bool is_pow2(int x) { return x > 0 && (x & (x - 1)) == 0; }
+constexpr int kLLMaxSources = 8;
 constexpr int kLLInferMaxSmem = 227 * 1024;   // the H100's opt-in dynamic shared memory per block
 
 int ll_check(gccnmf_handle* h, const gccnmf_ll_config* cfg) {
@@ -76,13 +96,26 @@ int ll_check(gccnmf_handle* h, const gccnmf_ll_config* cfg) {
   return 0;
 }
 
-LLLayout ll_carve(const gccnmf_ll_config& c, void* base) {
+// P = 0: the single-target entries; 2 <= P <= 8: gccnmf_llsep_*
+int ll_check(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P) {
+  if (int st = ll_check(h, cfg)) return st;
+  if (P == 0) return 0;
+  GCCNMF_REQUIRE(h, P >= 2 && P <= kLLMaxSources, "llsep: num_sources must be in [2, %d] (got %d)", kLLMaxSources, P);
+  const int64_t T = (int64_t)cfg->num_streams * cfg->hops_per_call;
+  GCCNMF_REQUIRE(h, T * P < ((int64_t)1 << 31) && (int64_t)P * cfg->num_atoms * T < ((int64_t)1 << 31),
+                 "llsep: T x P or P x K x T overflows int32 (T = S x C)");
+  return 0;
+}
+
+LLLayout ll_carve(const gccnmf_ll_config& c, int P, void* base) {
   WorkspaceCarver w(base ? base : reinterpret_cast<void*>(256), base ? ~size_t(0) >> 1 : ~size_t(0) >> 1);
   LLLayout l{};
   l.S = c.num_streams; l.N = c.window_size; l.hop = c.hop_size; l.C = c.hops_per_call; l.K = c.num_atoms; l.D = c.num_tdoas;
   l.F = l.N / 2 + 1; l.Q = (l.N + l.hop - 1) / l.hop; l.R = (l.Q - 1) * l.hop;
   const size_t S = l.S, N = l.N, F = l.F, K = l.K, D = l.D, T = S * l.C;
   const bool inf = c.inference_iterations > 0;
+  l.P = P;
+  const size_t Pm = P > 0 ? P : 1;   // copies of the per-target buffers
   l.head = w.take<LLHeader>(1);
   l.streams = w.take<LLStream>(S);
   l.counters = w.take<int32_t>(4);
@@ -94,7 +127,7 @@ LLLayout ll_carve(const gccnmf_ll_config& c, void* base) {
   l.colsumW = w.take<float>(inf ? K : 0);
   l.H0 = w.take<float>(inf ? K * 2 : 0);
   l.in_ring = w.take<float>(S * 2 * l.R);
-  l.out_ring = w.take<float>(S * 2 * N);
+  l.out_ring = w.take<float>(S * Pm * 2 * N);
   l.carry = w.take<double>(S * D);
   l.stage = w.take<float>(2 * S * (l.R + (size_t)l.C * l.hop));
   l.X = w.take<float>(2 * 2 * F * T);
@@ -106,21 +139,29 @@ LLLayout ll_carve(const gccnmf_ll_config& c, void* base) {
   l.valid = w.take<int32_t>(T);
   l.argmax = w.take<int32_t>(K * T);
   l.mask = w.take<float>(K * T);
-  l.wiener = w.take<float>((inf ? 2 : 1) * F * T);
-  l.Y = w.take<float>(2 * 2 * F * T);
+  l.wiener = w.take<float>(Pm * (inf ? 2 : 1) * F * T);
+  l.Y = w.take<float>(Pm * 2 * 2 * F * T);
   l.H = w.take<float>(inf ? K * 2 * T : 0);
-  l.frames = w.take<float>(2 * T * N);
+  l.frames = w.take<float>(Pm * 2 * T * N);
   l.ws_wiener = w.take<float>(gccnmf_wiener_apply_workspace_bytes((int)F) / sizeof(float));
   l.n_argmax = gccnmf_tdoa_argmax_workspace_bytes((int)F, (int)T, (int)D, (int)K);
   l.ws_argmax = w.take<unsigned char>(l.n_argmax);
+  // sources: appended to the single-target layout (nothing is taken with P = 0, so that layout is unchanged)
+  const size_t Ps = P;
+  l.src_targets = w.take<int32_t>(P ? S * kLLMaxSources : 0);
+  l.src_override = w.take<int32_t>(P ? S * kLLMaxSources : 0);
+  l.src_status = w.take<int32_t>(P ? S : 0);
+  l.col_targets = w.take<int32_t>(T * Ps);
+  l.values = w.take<float>(Ps * K * T);
+  l.src_mask = w.take<float>(Ps * K * T);
   l.bytes = align_up(w.used, 256);
   return l;
 }
 
-#define LL_CARVE_OR_FAIL(l)                                                                                          \
-  if (int st__ = ll_check(h, cfg)) return st__;                                                                      \
+#define LL_CARVE_OR_FAIL(l, P)                                                                                       \
+  if (int st__ = ll_check(h, cfg, P)) return st__;                                                                   \
   GCCNMF_REQUIRE(h, state != nullptr, "ll: NULL state");                                                             \
-  const LLLayout l = ll_carve(*cfg, state);                                                                          \
+  const LLLayout l = ll_carve(*cfg, P, state);                                                                       \
   if (state_bytes < l.bytes) return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "ll: state too small: need %zu bytes", l.bytes);
 
 // ---------------------------------------------------------------------------------------------- kernels
@@ -197,10 +238,10 @@ __device__ __forceinline__ bool ll_argmax_better(double v, int i, double bv, int
   return v > bv || (v == bv && i < bi);
 }
 
-// One CTA per stream, thread d = TDOA: the running maximum of cummax_time_kernel from the carried one over the call's valid frames,
-// then target[t] = argmax over d (argmax_tdoa_kernel), or the stream's override.
-__global__ void ll_targets_kernel(const LLStream* __restrict__ streams, const double* __restrict__ ang, const int32_t* __restrict__ valid, int D,
-                                  int hops, int T, double* __restrict__ carry, double* __restrict__ acc, int32_t* __restrict__ targets) {
+// The running maximum of cummax_time_kernel from the carried one over stream s's valid frames of the call (thread d = TDOA), written
+// to acc for every frame of the call; the carry is stored when the stream is active.
+__device__ __forceinline__ void ll_running_max(const LLStream* __restrict__ streams, const double* __restrict__ ang, const int32_t* __restrict__ valid,
+                                               int D, int hops, int T, double* __restrict__ carry, double* __restrict__ acc) {
   const int s = blockIdx.x, d = threadIdx.x;
   const int t0 = s * hops;
   if (d < D) {
@@ -214,6 +255,15 @@ __global__ void ll_targets_kernel(const LLStream* __restrict__ streams, const do
     }
     if (streams[s].active) carry[(int64_t)s * D + d] = m;
   }
+}
+
+// One CTA per stream, thread d = TDOA: the running maximum, then target[t] = argmax over d (argmax_tdoa_kernel), or the stream's
+// override.
+__global__ void ll_targets_kernel(const LLStream* __restrict__ streams, const double* __restrict__ ang, const int32_t* __restrict__ valid, int D,
+                                  int hops, int T, double* __restrict__ carry, double* __restrict__ acc, int32_t* __restrict__ targets) {
+  const int s = blockIdx.x, d = threadIdx.x;
+  const int t0 = s * hops;
+  ll_running_max(streams, ang, valid, D, hops, T, carry, acc);
   __syncthreads();
   if (d < hops) {
     const int t = t0 + d;
@@ -226,6 +276,44 @@ __global__ void ll_targets_kernel(const LLStream* __restrict__ streams, const do
     const int o = streams[s].target_override;
     targets[t] = o >= 0 ? o : bi;
   }
+}
+
+// Sources: one CTA per stream (128 threads, thread d = TDOA).  The running maximum as above, then frame by frame in order: the P
+// largest strict local maxima of the frame's running maximum (select_peaks, ascending) become the stream's targets; with fewer
+// peaks the targets stay and status bit 0 is set.  Column targets (T, P) = the targets, or the source's override where it is >= 0.
+// Invalid frames (before the first sample, inactive stream) change nothing.
+__global__ void __launch_bounds__(128)
+ll_src_targets_kernel(const LLStream* __restrict__ streams, const double* __restrict__ ang, const int32_t* __restrict__ valid, int D, int hops,
+                      int T, int P, double* __restrict__ carry, double* __restrict__ acc, int32_t* __restrict__ src_targets,
+                      const int32_t* __restrict__ src_override, int32_t* __restrict__ src_status, int32_t* __restrict__ col_targets) {
+  __shared__ double x_s[128];
+  __shared__ unsigned char peak_s[128], chosen_s[128];
+  __shared__ int num_peaks_s;
+  __shared__ int32_t pick_s[kLLMaxSources], cur_s[kLLMaxSources];
+  const int s = blockIdx.x, d = threadIdx.x;
+  const int t0 = s * hops;
+  ll_running_max(streams, ang, valid, D, hops, T, carry, acc);
+  if (d < P) cur_s[d] = src_targets[(int64_t)s * kLLMaxSources + d];
+  __syncthreads();
+  for (int i = 0; i < hops; ++i) {
+    const int t = t0 + i;
+    if (valid[t]) {                      // the same for every thread of the CTA
+      if (d < D) x_s[d] = acc[(int64_t)d * T + t];
+      const int peaks = select_peaks(x_s, D, P, peak_s, chosen_s, &num_peaks_s, pick_s);
+      if (d == 0) {
+        if (peaks >= P)
+          for (int q = 0; q < P; ++q) cur_s[q] = pick_s[q];
+        else
+          src_status[s] |= GCCNMF_LLSEP_STATUS_FEW_PEAKS;
+      }
+      __syncthreads();
+    }
+    if (d < P) {
+      const int o = src_override[(int64_t)s * kLLMaxSources + d];
+      col_targets[(int64_t)t * P + d] = o >= 0 ? o : cur_s[d];
+    }
+  }
+  if (d < P) src_targets[(int64_t)s * kLLMaxSources + d] = cur_s[d];
 }
 
 // mask[k][t] = |argmax[k][t] - target[t]| < epsilon of t's stream   (atom_mask_kernel mode 0)
@@ -273,24 +361,15 @@ ll_infer_kernel(const float* __restrict__ W, const float* __restrict__ WT, const
   for (int k = threadIdx.x; k < K; k += blockDim.x) Hout[(int64_t)k * (2 * T) + col] = Hs[k];
 }
 
-// One CTA per stream.  For each frame of the call in order: ring[p] = float32(fma(w[r], frame[r], ring[p])) for r >= z,
-// p = (j hop + r) mod N (ola_gather_kernel's chain: the weights below z are zero and would leave every sum as it is), then
-// emit the hop samples [j hop + z, j hop + z + hop) times the gain and zero them.  Then the input ring moves on.
-__global__ void __launch_bounds__(256)
-ll_ola_emit_kernel(LLStream* __restrict__ streams, const LLHeader* __restrict__ head, const double* __restrict__ w, const float* __restrict__ frames,
-                   int N, int hop, int hops, int T, int frames_before_first, float* __restrict__ out_ring, float* __restrict__ out,
-                   const float* __restrict__ stage, float* __restrict__ in_ring, int R) {
-  const int s = blockIdx.x;
+// For each frame of the call in order: ring[p] = float32(fma(w[r], frame[r], ring[p])) for r >= z, p = (j hop + r) mod N
+// (ola_gather_kernel's chain: the weights below z are zero and would leave every sum as it is), then emit the hop samples
+// [j hop + z, j hop + z + hop) times the gain and zero them.  frames (2, T, N) of one target, ring (2, N), o (2, hops hop).
+__device__ __forceinline__ void ll_ola_emit(const LLHeader* __restrict__ head, const double* __restrict__ w, const float* __restrict__ frames,
+                                            int N, int hop, int hops, int T, int frames_before_first, long long h0, int s, float* __restrict__ ring,
+                                            float* __restrict__ o) {
   const int n = hops * hop;
-  float* o = out + (int64_t)s * 2 * n;
-  if (!streams[s].active) {
-    for (int i = threadIdx.x; i < 2 * n; i += blockDim.x) o[i] = 0.f;
-    return;
-  }
   const int z = head->z;
   const float gain = head->gain;
-  const long long h0 = streams[s].hops;
-  float* ring = out_ring + (int64_t)s * 2 * N;
   for (int i = 0; i < hops; ++i) {
     const long long j = h0 + i + 1 - frames_before_first;
     const int base = (int)(((j % N) * hop % N + N) % N);          // (j hop) mod N
@@ -313,14 +392,113 @@ ll_ola_emit_kernel(LLStream* __restrict__ streams, const LLHeader* __restrict__ 
     }
     __syncthreads();
   }
-  // the last R samples of the staging rows are the next call's input ring
-  const int S = gridDim.x;
+}
+
+// The last R samples of stream s's staging rows are the next call's input ring; the stream has pushed `hops` more hops.
+__device__ __forceinline__ void ll_advance(LLStream* __restrict__ streams, int s, int S, const float* __restrict__ stage, float* __restrict__ in_ring,
+                                           int R, int n, int hops, long long h0) {
   const int64_t Lseg = (int64_t)R + n;
   for (int e = threadIdx.x; e < 2 * R; e += blockDim.x) {
     const int ch = e >= R, q = e - ch * R;
     in_ring[((int64_t)s * 2 + ch) * R + q] = stage[((int64_t)ch * S + s) * Lseg + n + q];
   }
   if (threadIdx.x == 0) streams[s].hops = h0 + hops;
+}
+
+// One CTA per stream: overlap-add and emit, then the input ring moves on.
+__global__ void __launch_bounds__(256)
+ll_ola_emit_kernel(LLStream* __restrict__ streams, const LLHeader* __restrict__ head, const double* __restrict__ w, const float* __restrict__ frames,
+                   int N, int hop, int hops, int T, int frames_before_first, float* __restrict__ out_ring, float* __restrict__ out,
+                   const float* __restrict__ stage, float* __restrict__ in_ring, int R) {
+  const int s = blockIdx.x;
+  const int n = hops * hop;
+  float* o = out + (int64_t)s * 2 * n;
+  if (!streams[s].active) {
+    for (int i = threadIdx.x; i < 2 * n; i += blockDim.x) o[i] = 0.f;
+    return;
+  }
+  const long long h0 = streams[s].hops;
+  ll_ola_emit(head, w, frames, N, hop, hops, T, frames_before_first, h0, s, out_ring + (int64_t)s * 2 * N, o);
+  ll_advance(streams, s, gridDim.x, stage, in_ring, R, n, hops, h0);
+}
+
+// Sources: CTA (s, q) overlap-adds source q's frames (P, 2, T, N) into its own ring and emits into out (S, P, 2, hops hop).  It
+// only reads the stream's hop count: ll_src_advance_kernel moves the stream on once every source has emitted.
+__global__ void __launch_bounds__(256)
+ll_src_ola_emit_kernel(const LLStream* __restrict__ streams, const LLHeader* __restrict__ head, const double* __restrict__ w,
+                       const float* __restrict__ frames, int N, int hop, int hops, int T, int frames_before_first, float* __restrict__ out_ring,
+                       float* __restrict__ out) {
+  const int s = blockIdx.x, q = blockIdx.y, P = gridDim.y;
+  const int n = hops * hop;
+  const int64_t sq = (int64_t)s * P + q;
+  float* o = out + sq * 2 * n;
+  if (!streams[s].active) {
+    for (int i = threadIdx.x; i < 2 * n; i += blockDim.x) o[i] = 0.f;
+    return;
+  }
+  ll_ola_emit(head, w, frames + (int64_t)q * 2 * T * N, N, hop, hops, T, frames_before_first, streams[s].hops, s, out_ring + sq * 2 * N, o);
+}
+
+// Sources: one CTA per stream after every source has emitted; CTA 0 also turns coeff_mask's all-NaN flag into the call's status.
+__global__ void __launch_bounds__(256)
+ll_src_advance_kernel(LLStream* __restrict__ streams, int hops, int hop, const float* __restrict__ stage, float* __restrict__ in_ring, int R,
+                      int32_t* __restrict__ counters) {
+  const int s = blockIdx.x;
+  if (s == 0 && threadIdx.x == 0) counters[3] = counters[2] ? GCCNMF_LLSEP_STATUS_ALL_NAN : 0;
+  if (!streams[s].active) return;
+  ll_advance(streams, s, gridDim.x, stage, in_ring, R, hops * hop, hops, streams[s].hops);
+}
+
+// Sources: stream s's P output rings zeroed, targets back to the defaults floor((2 q + 1) D / (2 P)), status cleared; with
+// set_defaults (init) no overrides.
+__global__ void ll_src_reset_kernel(int first, int count, int P, int D, int N, float* __restrict__ out_ring, int32_t* __restrict__ src_targets,
+                                    int32_t* __restrict__ src_override, int32_t* __restrict__ src_status, int set_defaults) {
+  const int s = first + blockIdx.x;
+  if (blockIdx.x >= count) return;
+  for (int i = threadIdx.x; i < P * 2 * N; i += blockDim.x) out_ring[(int64_t)s * P * 2 * N + i] = 0.f;
+  if (threadIdx.x < kLLMaxSources) {
+    const int q = threadIdx.x;
+    src_targets[(int64_t)s * kLLMaxSources + q] = q < P ? (2 * q + 1) * D / (2 * P) : 0;
+    if (set_defaults) src_override[(int64_t)s * kLLMaxSources + q] = -1;
+  }
+  if (threadIdx.x == 0) src_status[s] = 0;
+}
+
+struct LLTargetsBatch { int32_t t[kLLParamsPerLaunch * kLLMaxSources]; };
+
+__global__ void ll_src_override_kernel(int32_t* __restrict__ src_override, int first, int count, int P, LLTargetsBatch b) {
+  const int i = threadIdx.x;
+  if (i >= count) return;
+  for (int q = 0; q < P; ++q) src_override[(int64_t)(first + i) * kLLMaxSources + q] = b.t[i * P + q];
+}
+
+// Sources, after the shared front (push, STFT, PHAT / angular): targets, the target contraction, coeff_mask, per source the
+// filter (with inference on the shared H), then one inverse FFT of all (P, 2) spectra, emit per (stream, source), advance.
+int ll_enqueue_sources(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l, int hops, float* out, void* stream) {
+  const int S = l.S, N = l.N, hop = l.hop, F = l.F, K = l.K, D = l.D, P = l.P, T = S * hops;
+  const bool inf = cfg->inference_iterations > 0;
+  GCCNMF_LAUNCH(h, ll_src_targets_kernel, S, 128, 0, stream, l.streams, l.ang, l.valid, D, hops, T, P, l.carry, l.acc, l.src_targets,
+                l.src_override, l.src_status, l.col_targets);
+  if (int e = gccnmf_target_gccnmf(h, l.coh, F, T, l.E, D, l.W, K, l.col_targets, P, l.values, stream)) return e;
+  if (int e = gccnmf_coeff_mask(h, l.values, P, K, T, l.src_mask, l.counters + 2, stream)) return e;
+  const size_t KT = (size_t)K * T, FT = (size_t)F * T;
+  if (inf) {
+    const size_t smem = (size_t)(K + F) * sizeof(float);
+    if (smem > 48 * 1024) GCCNMF_CHECK_CUDA(h, cudaFuncSetAttribute(ll_infer_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    GCCNMF_LAUNCH(h, ll_infer_kernel, dim3(T, 2), 256, smem, stream, l.W, l.WT, l.colsumW, l.H0, l.V, F, K, T, cfg->inference_iterations,
+                  cfg->sparsity_alpha, cfg->epsilon, l.H);
+    for (int q = 0; q < P; ++q)
+      if (int e = gccnmf_wiener_apply_h(h, l.src_mask + q * KT, l.W, l.H, l.X, F, T, K, l.Y + q * 4 * FT, l.wiener + q * 2 * FT, stream)) return e;
+  } else {
+    for (int q = 0; q < P; ++q)
+      if (int e = gccnmf_wiener_apply(h, l.src_mask + q * KT, l.W, l.X, F, T, K, l.Y + q * 4 * FT, l.wiener + q * FT, l.ws_wiener,
+                                      gccnmf_wiener_apply_workspace_bytes(F), stream))
+        return e;
+  }
+  if (int e = gccnmf_istft_frames(h, l.Y, 2 * P, N, T, 0, l.frames, stream)) return e;
+  GCCNMF_LAUNCH(h, ll_src_ola_emit_kernel, dim3(S, P), 256, 0, stream, l.streams, l.head, l.w_syn, l.frames, N, hop, hops, T, l.Q, l.out_ring, out);
+  GCCNMF_LAUNCH(h, ll_src_advance_kernel, S, 256, 0, stream, l.streams, hops, hop, l.stage, l.in_ring, l.R, l.counters);
+  return GCCNMF_OK;
 }
 
 int ll_enqueue(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l, int hops, const float* in, float* out, void* stream) {
@@ -335,6 +513,7 @@ int ll_enqueue(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l,
   const int64_t Lseg = (int64_t)l.R + n;
   if (int e = gccnmf_stft_segments(h, l.stage, (int64_t)S * Lseg, 2, S, hops, Lseg, l.win_a, N, hop, 0, l.X, inf ? l.V : nullptr, stream)) return e;
   if (int e = gccnmf_phat_angspec(h, l.X, F, T, 0, l.E, D, l.coh, l.ang, nullptr, nullptr, 0, stream)) return e;
+  if (l.P) return ll_enqueue_sources(h, cfg, l, hops, out, stream);
   GCCNMF_LAUNCH(h, ll_targets_kernel, S, 128, 0, stream, l.streams, l.ang, l.valid, D, hops, T, l.carry, l.acc, l.targets);
   if (int e = gccnmf_tdoa_argmax(h, l.coh, F, T, l.E, D, l.W, K, l.argmax, l.counters, l.ws_argmax, l.n_argmax, stream)) return e;
   if (int e = gccnmf_tdoa_gccnmf_gated(h, l.coh, F, T, l.E, D, l.W, K, l.argmax, l.counters, gccnmf_tdoa_argmax_refine_capacity(K, T),
@@ -357,19 +536,11 @@ int ll_enqueue(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l,
   return GCCNMF_OK;
 }
 
-}  // namespace
-
-extern "C" {
-
-size_t gccnmf_ll_state_bytes(const gccnmf_ll_config* cfg) {
-  if (ll_check(nullptr, cfg) != 0) return 0;
-  return ll_carve(*cfg, nullptr).bytes;
-}
-
-int gccnmf_ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, const float* W, const double* E, const double* analysis_window,
-                   const double* synthesis_weights, float gain, const float* H0, void* state, size_t state_bytes, void* stream) {
+// ---------------------------------------------------------------------------------------------- entry points (P = 0: gccnmf_ll_*)
+int ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, const float* W, const double* E, const double* analysis_window,
+            const double* synthesis_weights, float gain, const float* H0, void* state, size_t state_bytes, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l);
+  LL_CARVE_OR_FAIL(l, P);
   GCCNMF_REQUIRE(h, W && E && analysis_window && synthesis_weights, "ll_init: NULL pointer");
   GCCNMF_REQUIRE(h, cfg->inference_iterations == 0 || H0 != nullptr, "ll_init: inference needs H0");
   cudaStream_t s = (cudaStream_t)stream;
@@ -395,23 +566,28 @@ int gccnmf_ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, const float* W
     GCCNMF_LAUNCH(h, ll_dict_kernel, (l.K + 127) / 128, 128, 0, stream, l.W, l.F, l.K, l.WT, l.colsumW);
   }
   GCCNMF_LAUNCH(h, ll_header_kernel, 1, 1, 0, stream, l.head, l.w_syn, l.N, gain);
-  GCCNMF_LAUNCH(h, ll_reset_kernel, l.S, 256, 0, stream, l.streams, 0, l.S, l.in_ring, l.out_ring, l.carry, l.R, l.N, l.D, 1);
+  // with sources the P output rings of a stream are zeroed by ll_src_reset_kernel (N = 0 here: no single ring)
+  GCCNMF_LAUNCH(h, ll_reset_kernel, l.S, 256, 0, stream, l.streams, 0, l.S, l.in_ring, l.out_ring, l.carry, l.R, P ? 0 : l.N, l.D, 1);
+  if (P)
+    GCCNMF_LAUNCH(h, ll_src_reset_kernel, l.S, 256, 0, stream, 0, l.S, P, l.D, l.N, l.out_ring, l.src_targets, l.src_override, l.src_status, 1);
   return GCCNMF_OK;
 }
 
-int gccnmf_ll_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int first, int count, void* stream) {
+int ll_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* state, size_t state_bytes, int first, int count, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l);
+  LL_CARVE_OR_FAIL(l, P);
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "ll_reset_streams: streams [%d, %d + %d) outside [0, %d)", first,
                  first, count, l.S);
-  GCCNMF_LAUNCH(h, ll_reset_kernel, count, 256, 0, stream, l.streams, first, count, l.in_ring, l.out_ring, l.carry, l.R, l.N, l.D, 0);
+  GCCNMF_LAUNCH(h, ll_reset_kernel, count, 256, 0, stream, l.streams, first, count, l.in_ring, l.out_ring, l.carry, l.R, P ? 0 : l.N, l.D, 0);
+  if (P)
+    GCCNMF_LAUNCH(h, ll_src_reset_kernel, count, 256, 0, stream, first, count, P, l.D, l.N, l.out_ring, l.src_targets, l.src_override, l.src_status, 0);
   return GCCNMF_OK;
 }
 
-int gccnmf_ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int first, int count,
-                         const gccnmf_ll_stream_params* params_host, void* stream) {
+int ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* state, size_t state_bytes, int first, int count,
+                  const gccnmf_ll_stream_params* params_host, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l);
+  LL_CARVE_OR_FAIL(l, P);
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "ll_set_params: streams [%d, %d + %d) outside [0, %d)", first,
                  first, count, l.S);
   GCCNMF_REQUIRE(h, params_host != nullptr, "ll_set_params: NULL parameters");
@@ -429,29 +605,23 @@ int gccnmf_ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* st
   return GCCNMF_OK;
 }
 
-int gccnmf_ll_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, const float* in, float* out,
-                      void* stream) {
-  GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l);
-  return ll_enqueue(h, cfg, l, hops, in, out, stream);
-}
-
-int gccnmf_ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, float* in, float* out,
-                           const float* in_host, float* out_host, void** graph_exec, void* stream) {
+int ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* state, size_t state_bytes, int hops, float* in, float* out,
+                    const float* in_host, float* out_host, void** graph_exec, void* stream) {
   GCCNMF_ENTER(h);
   GCCNMF_REQUIRE(h, graph_exec != nullptr && stream != nullptr, "ll_graph_create: needs a non-default stream and an output slot");
   *graph_exec = nullptr;
-  LL_CARVE_OR_FAIL(l);
+  LL_CARVE_OR_FAIL(l, P);
   GCCNMF_REQUIRE(h, hops >= 1 && hops <= l.C, "ll_graph_create: hops must be in [1, %d] (got %d)", l.C, hops);
   GCCNMF_REQUIRE(h, in && out, "ll_graph_create: NULL pointer");
   if (int st = gccnmf_get_twiddles(h, l.N, nullptr, nullptr)) return st;
   cudaStream_t s = (cudaStream_t)stream;
   const size_t bytes = (size_t)l.S * 2 * hops * l.hop * sizeof(float);
+  const size_t out_bytes = bytes * (P ? P : 1);
   GCCNMF_CHECK_CUDA(h, cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
   int st = GCCNMF_OK;
   if (in_host && cudaMemcpyAsync(in, in_host, bytes, cudaMemcpyHostToDevice, s) != cudaSuccess) st = GCCNMF_ERR_CUDA;
   if (st == GCCNMF_OK) st = ll_enqueue(h, cfg, l, hops, in, out, stream);
-  if (st == GCCNMF_OK && out_host && cudaMemcpyAsync(out_host, out, bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess) st = GCCNMF_ERR_CUDA;
+  if (st == GCCNMF_OK && out_host && cudaMemcpyAsync(out_host, out, out_bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess) st = GCCNMF_ERR_CUDA;
   cudaGraph_t graph = nullptr;
   const cudaError_t end = cudaStreamEndCapture(s, &graph);
   if (st != GCCNMF_OK || end != cudaSuccess) {
@@ -467,35 +637,158 @@ int gccnmf_ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* 
   return GCCNMF_OK;
 }
 
-int gccnmf_ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, int what, void* dst, void* stream) {
+int ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* state, size_t state_bytes, int hops, int what, void* dst, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l);
+  LL_CARVE_OR_FAIL(l, P);
   GCCNMF_REQUIRE(h, dst != nullptr, "ll_export: NULL destination");
   GCCNMF_REQUIRE(h, hops >= 1 && hops <= l.C, "ll_export: hops must be in [1, %d] (got %d)", l.C, hops);
   const bool inf = cfg->inference_iterations > 0;
-  const size_t T = (size_t)l.S * hops, F = l.F, K = l.K, D = l.D;
+  const size_t T = (size_t)l.S * hops, F = l.F, K = l.K, D = l.D, Ps = P;
   const void* src = nullptr;
   size_t bytes = 0;
-  switch (what) {
-    case 0: src = l.X; bytes = 2 * F * T * 8; break;
-    case 1: src = l.coh; bytes = F * T * 8; break;
-    case 2: src = l.ang; bytes = D * T * 8; break;
-    case 3: src = l.acc; bytes = D * T * 8; break;
-    case 4: src = l.targets; bytes = T * 4; break;
-    case 5: src = l.argmax; bytes = K * T * 4; break;
-    case 6: src = l.mask; bytes = K * T * 4; break;
-    case 7: src = l.wiener; bytes = (inf ? 2 : 1) * F * T * 4; break;
-    case 8: src = l.Y; bytes = 2 * F * T * 8; break;
-    case 9: src = l.counters; bytes = 4; break;
-    case 10: src = l.counters + 1; bytes = 4; break;
-    case 11: if (inf) { src = l.H; bytes = K * 2 * T * 4; } break;
-    case 12: src = l.valid; bytes = T * 4; break;
-    case 13: src = l.carry; bytes = (size_t)l.S * D * 8; break;
-    default: break;
+  if (P) {   // the items of the single-target chain that this mode does not compute are refused
+    switch (what) {
+      case 0: case 1: case 2: case 3: case 11: case 12: case 13: break;
+      case GCCNMF_LLSEP_EXPORT_TARGETS: src = l.col_targets; bytes = T * Ps * 4; break;
+      case GCCNMF_LLSEP_EXPORT_VALUES: src = l.values; bytes = Ps * K * T * 4; break;
+      case GCCNMF_LLSEP_EXPORT_MASKS: src = l.src_mask; bytes = Ps * K * T * 4; break;
+      case GCCNMF_LLSEP_EXPORT_WIENER: src = l.wiener; bytes = Ps * (inf ? 2 : 1) * F * T * 4; break;
+      case GCCNMF_LLSEP_EXPORT_Y: src = l.Y; bytes = Ps * 2 * F * T * 8; break;
+      case GCCNMF_LLSEP_EXPORT_STREAM_STATUS: src = l.src_status; bytes = (size_t)l.S * 4; break;
+      case GCCNMF_LLSEP_EXPORT_CARRIED_TARGETS:
+        GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync(dst, Ps * 4, l.src_targets, kLLMaxSources * 4, Ps * 4, l.S, cudaMemcpyDefault, (cudaStream_t)stream));
+        return GCCNMF_OK;
+      case GCCNMF_LLSEP_EXPORT_CALL_STATUS: src = l.counters + 3; bytes = 4; break;
+      default: return gccnmf_fail(h, GCCNMF_ERR_INVALID_ARGUMENT, "llsep_export: item %d is not computed with sources", what);
+    }
+  }
+  if (!src) {
+    switch (what) {
+      case 0: src = l.X; bytes = 2 * F * T * 8; break;
+      case 1: src = l.coh; bytes = F * T * 8; break;
+      case 2: src = l.ang; bytes = D * T * 8; break;
+      case 3: src = l.acc; bytes = D * T * 8; break;
+      case 4: src = l.targets; bytes = T * 4; break;
+      case 5: src = l.argmax; bytes = K * T * 4; break;
+      case 6: src = l.mask; bytes = K * T * 4; break;
+      case 7: src = l.wiener; bytes = (inf ? 2 : 1) * F * T * 4; break;
+      case 8: src = l.Y; bytes = 2 * F * T * 8; break;
+      case 9: src = l.counters; bytes = 4; break;
+      case 10: src = l.counters + 1; bytes = 4; break;
+      case 11: if (inf) { src = l.H; bytes = K * 2 * T * 4; } break;
+      case 12: src = l.valid; bytes = T * 4; break;
+      case 13: src = l.carry; bytes = (size_t)l.S * D * 8; break;
+      default: break;
+    }
   }
   if (!src) return gccnmf_fail(h, GCCNMF_ERR_INVALID_ARGUMENT, "ll_export: unknown item %d", what);
   GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, (cudaStream_t)stream));
   return GCCNMF_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t gccnmf_ll_state_bytes(const gccnmf_ll_config* cfg) {
+  if (ll_check(nullptr, cfg, 0) != 0) return 0;
+  return ll_carve(*cfg, 0, nullptr).bytes;
+}
+
+int gccnmf_ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, const float* W, const double* E, const double* analysis_window,
+                   const double* synthesis_weights, float gain, const float* H0, void* state, size_t state_bytes, void* stream) {
+  return ll_init(h, cfg, 0, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
+}
+
+int gccnmf_ll_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int first, int count, void* stream) {
+  return ll_reset_streams(h, cfg, 0, state, state_bytes, first, count, stream);
+}
+
+int gccnmf_ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int first, int count,
+                         const gccnmf_ll_stream_params* params_host, void* stream) {
+  return ll_set_params(h, cfg, 0, state, state_bytes, first, count, params_host, stream);
+}
+
+int gccnmf_ll_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, const float* in, float* out,
+                      void* stream) {
+  GCCNMF_ENTER(h);
+  LL_CARVE_OR_FAIL(l, 0);
+  return ll_enqueue(h, cfg, l, hops, in, out, stream);
+}
+
+int gccnmf_ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, float* in, float* out,
+                           const float* in_host, float* out_host, void** graph_exec, void* stream) {
+  return ll_graph_create(h, cfg, 0, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
+}
+
+int gccnmf_ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, int what, void* dst, void* stream) {
+  return ll_export(h, cfg, 0, state, state_bytes, hops, what, dst, stream);
+}
+
+// ---- sources (2 <= num_sources <= 8)
+size_t gccnmf_llsep_state_bytes(const gccnmf_ll_config* cfg, int num_sources) {
+  if (num_sources == 0 || ll_check(nullptr, cfg, num_sources) != 0) return 0;
+  return ll_carve(*cfg, num_sources, nullptr).bytes;
+}
+
+int gccnmf_llsep_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, const float* W, const double* E,
+                      const double* analysis_window, const double* synthesis_weights, float gain, const float* H0, void* state,
+                      size_t state_bytes, void* stream) {
+  GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
+  return ll_init(h, cfg, num_sources, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
+}
+
+int gccnmf_llsep_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
+                               int count, void* stream) {
+  GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
+  return ll_reset_streams(h, cfg, num_sources, state, state_bytes, first, count, stream);
+}
+
+int gccnmf_llsep_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
+                            int count, const gccnmf_ll_stream_params* params_host, void* stream) {
+  GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
+  return ll_set_params(h, cfg, num_sources, state, state_bytes, first, count, params_host, stream);
+}
+
+int gccnmf_llsep_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
+                             int count, const int32_t* targets_host, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
+  const int P = num_sources;
+  LL_CARVE_OR_FAIL(l, P);
+  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "llsep_set_targets: streams [%d, %d + %d) outside [0, %d)",
+                 first, first, count, l.S);
+  GCCNMF_REQUIRE(h, targets_host != nullptr, "llsep_set_targets: NULL targets");
+  for (int i = 0; i < count * P; ++i)
+    GCCNMF_REQUIRE(h, targets_host[i] >= -1 && targets_host[i] < l.D, "llsep_set_targets: stream %d source %d: target %d outside [0, %d) (or -1)",
+                   first + i / P, i % P, targets_host[i], l.D);
+  for (int i0 = 0; i0 < count; i0 += kLLParamsPerLaunch) {
+    const int n = count - i0 < kLLParamsPerLaunch ? count - i0 : kLLParamsPerLaunch;
+    LLTargetsBatch b{};
+    memcpy(b.t, targets_host + (size_t)i0 * P, (size_t)n * P * sizeof(int32_t));
+    GCCNMF_LAUNCH(h, ll_src_override_kernel, 1, kLLParamsPerLaunch, 0, stream, l.src_override, first + i0, n, P, b);
+  }
+  return GCCNMF_OK;
+}
+
+int gccnmf_llsep_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int hops,
+                         const float* in, float* out, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
+  LL_CARVE_OR_FAIL(l, num_sources);
+  return ll_enqueue(h, cfg, l, hops, in, out, stream);
+}
+
+int gccnmf_llsep_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int hops,
+                              float* in, float* out, const float* in_host, float* out_host, void** graph_exec, void* stream) {
+  GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
+  return ll_graph_create(h, cfg, num_sources, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
+}
+
+int gccnmf_llsep_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int hops, int what,
+                        void* dst, void* stream) {
+  GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
+  return ll_export(h, cfg, num_sources, state, state_bytes, hops, what, dst, stream);
 }
 
 }  // extern "C"

@@ -13,6 +13,12 @@ The synthesis is a weight vector w applied to every frame in the overlap-add and
 with gainFactor = 2 hop / N.  The latency is Q hop - hop - z samples, Q = ceil(N / hop) and z the first nonzero index of w; when hop
 divides N that is N - hop for the first two, and 2m - hop - 1 for the asymmetric synthesis window of
 lowLatencySpeechEnhancement.ipynb:382-392 (its first weight is zero).
+
+Sources (`numSources` = P in [2, 8], `gccnmf_llsep_*`): every stream is separated into P sources, one per target TDOA index (the
+reference's multi-target rule, gccNMFFunctions.py:94-143, per frame).  The targets of a frame are the P largest strict local
+maxima of its running maximum (held, with status bit 0, when there are fewer), or the overrides of `set_targets`; each atom goes
+to the target with the largest float32 GCC-NMF value (numpy.nanargmax), and source q is the single-target filter and synthesis fed
+that mask.  `process` then returns (S, P, 2, n).  The boxcar epsilon and the single target override play no part.
 """
 import ctypes
 
@@ -24,6 +30,11 @@ SYNTHESIS_MODES = ('online', 'lowlatency', 'windowed')
 
 EXPORT_X, EXPORT_COHERENCE, EXPORT_ANGULAR, EXPORT_ACC_MAX, EXPORT_TARGETS, EXPORT_ARGMAX, EXPORT_MASKS, EXPORT_WIENER, EXPORT_Y, \
     EXPORT_REFINED, EXPORT_STATUS, EXPORT_H, EXPORT_VALID, EXPORT_CARRY = range(14)
+# export items of an engine with sources (gccnmf_llsep_export); items 4 .. 10 are then refused
+EXPORT_SOURCE_TARGETS, EXPORT_SOURCE_VALUES, EXPORT_SOURCE_MASKS, EXPORT_SOURCE_WIENER, EXPORT_SOURCE_Y, EXPORT_STREAM_STATUS, \
+    EXPORT_CARRIED_TARGETS, EXPORT_CALL_STATUS = range(14, 22)
+STATUS_FEW_PEAKS, STATUS_ALL_NAN = 1, 2
+MAX_SOURCES = 8
 
 
 def synthesisWeights(mode, synthesisWindow, hopSize):
@@ -57,7 +68,10 @@ def batchArguments(mode):
 
 class LowLatencyEngine(object):
     def __init__(self, W, expJOmegaTau, analysisWindow, synthesisWindow, hopSize, numStreams=1, hopsPerCall=1, synthesis='lowlatency',
-                 targetTDOAEpsilon=1.0, numInferenceIterations=0, sparsityAlpha=0.0, epsilon=1e-16, seedValue=0, device=0):
+                 targetTDOAEpsilon=1.0, numInferenceIterations=0, sparsityAlpha=0.0, epsilon=1e-16, seedValue=0, device=0, numSources=0):
+        self.P = int(numSources)
+        if self.P != 0 and not 2 <= self.P <= MAX_SOURCES:
+            raise ValueError('numSources must be 0 (one enhanced target) or in [2, %d] (got %d)' % (MAX_SOURCES, self.P))
         self.h = default_handle(device)
         torch = self.torch = self.h.torch
         W = np.ascontiguousarray(W, dtype=np.float32)
@@ -74,7 +88,8 @@ class LowLatencyEngine(object):
         if self.latency < 0:
             raise ValueError('the synthesis weights start less than a hop before the end of the frame')
         self.cfg = LLConfig(N, self.hop, self.C, K, self.D, self.S, int(numInferenceIterations), float(sparsityAlpha), float(epsilon))
-        self.state_bytes = int(self.h.lib.gccnmf_ll_state_bytes(ctypes.byref(self.cfg)))
+        self.state_bytes = int(self.h.lib.gccnmf_llsep_state_bytes(ctypes.byref(self.cfg), self.P) if self.P else
+                               self.h.lib.gccnmf_ll_state_bytes(ctypes.byref(self.cfg)))
         if self.state_bytes == 0:
             raise ValueError('invalid low-latency configuration (N a power of two in [32, 4096], 1 <= hop <= N, 1 <= hopsPerCall <= 64, '
                              'D a power of two in [4, 128], 1 <= numStreams <= 4096)')
@@ -91,6 +106,7 @@ class LowLatencyEngine(object):
         self._eps = np.full(self.S, float(targetTDOAEpsilon), np.float32)
         self._active = np.ones(self.S, np.int32)
         self._override = np.full(self.S, -1, np.int32)
+        self._targets = np.full((self.S, max(self.P, 1)), -1, np.int32)
         self._io = {}
         self._graphs = {}
         self._exports = {}
@@ -98,14 +114,26 @@ class LowLatencyEngine(object):
         self.h.torch.cuda.current_stream(self.h.device).synchronize()
         c = self._const
         with torch.cuda.stream(self.stream):
-            self._check(self.h.lib.gccnmf_ll_init(self.h.h, ctypes.byref(self.cfg), c[0].data_ptr(), c[1].data_ptr(), c[2].data_ptr(),
-                                                  c[3].data_ptr(), float(self.gain), c[4].data_ptr() if c[4] is not None else None,
-                                                  self.state.data_ptr(), self.state_bytes, self.stream.cuda_stream))
+            self._check(self._fn('init')(self.h.h, ctypes.byref(self.cfg), *self._p, c[0].data_ptr(), c[1].data_ptr(), c[2].data_ptr(),
+                                         c[3].data_ptr(), float(self.gain), c[4].data_ptr() if c[4] is not None else None,
+                                         self.state.data_ptr(), self.state_bytes, self.stream.cuda_stream))
         self._send_params(0, self.S)
         self.stream.synchronize()
 
     def _check(self, status):
         self.h.check(status)
+
+    @property
+    def _p(self):
+        """The num_sources argument of the gccnmf_llsep_* entries (none for gccnmf_ll_*)."""
+        return (self.P,) if self.P else ()
+
+    def _fn(self, name):
+        return getattr(self.h.lib, ('gccnmf_llsep_' if self.P else 'gccnmf_ll_') + name)
+
+    def _state(self, name, *args):
+        """gccnmf_ll_<name>(h, cfg, state, state_bytes, *args), or gccnmf_llsep_<name>(h, cfg, P, state, state_bytes, *args)."""
+        self._check(self._fn(name)(self.h.h, ctypes.byref(self.cfg), *self._p, self.state.data_ptr(), self.state_bytes, *args))
 
     def _streams(self, streams):
         if streams is None:
@@ -120,8 +148,7 @@ class LowLatencyEngine(object):
         for i in range(count):
             s = first + i
             arr[i] = LLStreamParams(float(self._eps[s]), int(self._active[s]), int(self._override[s]))
-        self._check(self.h.lib.gccnmf_ll_set_params(self.h.h, ctypes.byref(self.cfg), self.state.data_ptr(), self.state_bytes, first, count,
-                                                    arr, self.stream.cuda_stream))
+        self._state('set_params', first, count, arr, self.stream.cuda_stream)
 
     def _send_streams(self, idx):
         lo, hi = int(idx.min()), int(idx.max())
@@ -141,6 +168,21 @@ class LowLatencyEngine(object):
             self._override[idx] = o
         self._send_streams(idx)
 
+    def set_targets(self, streams, targets):
+        """Sources only: per stream P target TDOA indexes that replace the localised ones, -1 for a source that follows the
+        localisation.  targets broadcasts to (len(streams), P)."""
+        if not self.P:
+            raise ValueError('set_targets needs numSources >= 2')
+        idx = self._streams(streams)
+        t = np.broadcast_to(np.asarray(targets, dtype=np.int64), (len(idx), self.P))
+        if t.min() < -1 or t.max() >= self.D:
+            raise ValueError('targets outside [0, %d) (or -1)' % self.D)
+        self._targets[idx] = t
+        lo, hi = int(idx.min()), int(idx.max())
+        arr = np.ascontiguousarray(self._targets[lo:hi + 1], dtype=np.int32)
+        self._state('set_targets', lo, hi - lo + 1, arr.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), self.stream.cuda_stream)
+        self.stream.synchronize()
+
     def set_active(self, streams, active):
         """An inactive stream outputs zeros and its state does not change."""
         idx = self._streams(streams)
@@ -152,8 +194,7 @@ class LowLatencyEngine(object):
         idx = np.unique(self._streams(streams))
         breaks = np.flatnonzero(np.diff(idx) != 1) + 1          # one call per contiguous run of streams
         for run in np.split(idx, breaks):
-            self._check(self.h.lib.gccnmf_ll_reset_streams(self.h.h, ctypes.byref(self.cfg), self.state.data_ptr(), self.state_bytes,
-                                                           int(run[0]), len(run), self.stream.cuda_stream))
+            self._state('reset_streams', int(run[0]), len(run), self.stream.cuda_stream)
         self.stream.synchronize()
 
     # ------------------------------------------------------------------ per-call work
@@ -162,9 +203,10 @@ class LowLatencyEngine(object):
         if b is None:
             torch = self.torch
             shape = (self.S, 2, hops * self.hop)
-            b = self._io[hops] = (torch.zeros(shape, dtype=torch.float32).pin_memory(), torch.zeros(shape, dtype=torch.float32).pin_memory(),
+            oshape = (self.S, self.P, 2, hops * self.hop) if self.P else shape
+            b = self._io[hops] = (torch.zeros(shape, dtype=torch.float32).pin_memory(), torch.zeros(oshape, dtype=torch.float32).pin_memory(),
                                   torch.zeros(shape, dtype=torch.float32, device=self.h.device),
-                                  torch.zeros(shape, dtype=torch.float32, device=self.h.device))
+                                  torch.zeros(oshape, dtype=torch.float32, device=self.h.device))
         return b
 
     def build_graph(self, hops=None):
@@ -174,14 +216,13 @@ class LowLatencyEngine(object):
         if g is None:
             in_host, out_host, in_dev, out_dev = self._buffers(hops)
             g = ctypes.c_void_p()
-            self._check(self.h.lib.gccnmf_ll_graph_create(self.h.h, ctypes.byref(self.cfg), self.state.data_ptr(), self.state_bytes, hops,
-                                                          in_dev.data_ptr(), out_dev.data_ptr(), in_host.data_ptr(), out_host.data_ptr(),
-                                                          ctypes.byref(g), self.stream.cuda_stream))
+            self._state('graph_create', hops, in_dev.data_ptr(), out_dev.data_ptr(), in_host.data_ptr(), out_host.data_ptr(), ctypes.byref(g),
+                        self.stream.cuda_stream)
             self._graphs[hops] = g
         return g
 
     def process(self, x, use_graph=True):
-        """x (S, 2, hops * hop) float32 -> (S, 2, hops * hop) float32 (a copy)."""
+        """x (S, 2, hops * hop) float32 -> (S, 2, hops * hop) float32, or (S, P, 2, hops * hop) with sources (a copy)."""
         x = np.asarray(x, dtype=np.float32)
         if x.ndim != 3 or x.shape[0] != self.S or x.shape[1] != 2 or x.shape[2] % self.hop != 0:
             raise ValueError('x must be (%d, 2, hops * %d)' % (self.S, self.hop))
@@ -195,15 +236,15 @@ class LowLatencyEngine(object):
         else:
             with self.torch.cuda.stream(self.stream):
                 in_dev.copy_(in_host, non_blocking=True)
-                self._check(self.h.lib.gccnmf_ll_process(self.h.h, ctypes.byref(self.cfg), self.state.data_ptr(), self.state_bytes, hops,
-                                                         in_dev.data_ptr(), out_dev.data_ptr(), self.stream.cuda_stream))
+                self._state('process', hops, in_dev.data_ptr(), out_dev.data_ptr(), self.stream.cuda_stream)
                 out_host.copy_(out_dev, non_blocking=True)
         self.stream.synchronize()
         self.last_hops = hops
         return out_host.numpy().copy()
 
     def export(self, what):
-        """Host copy of one item of the last call (see gccnmf_ll_export); T = S hops columns, column s hops + i = frame i of stream s."""
+        """Host copy of one item of the last call (see gccnmf_ll_export / gccnmf_llsep_export); T = S hops columns, column s hops + i =
+        frame i of stream s."""
         if self.last_hops is None:
             raise RuntimeError('no call yet')
         torch = self.torch
@@ -213,13 +254,19 @@ class LowLatencyEngine(object):
                   EXPORT_MASKS: ((K, T), torch.float32), EXPORT_WIENER: (((2, F, T) if self.inference else (F, T)), torch.float32),
                   EXPORT_Y: ((2, F, T), torch.complex64), EXPORT_REFINED: ((1,), torch.int32), EXPORT_STATUS: ((1,), torch.int32),
                   EXPORT_H: ((K, 2 * T), torch.float32), EXPORT_VALID: ((T,), torch.int32), EXPORT_CARRY: ((self.S, D), torch.float64)}
+        P = self.P
+        if P:
+            shapes.update({EXPORT_SOURCE_TARGETS: ((T, P), torch.int32), EXPORT_SOURCE_VALUES: ((P, K, T), torch.float32),
+                           EXPORT_SOURCE_MASKS: ((P, K, T), torch.float32),
+                           EXPORT_SOURCE_WIENER: (((P, 2, F, T) if self.inference else (P, F, T)), torch.float32),
+                           EXPORT_SOURCE_Y: ((P, 2, F, T), torch.complex64), EXPORT_STREAM_STATUS: ((self.S,), torch.int32),
+                           EXPORT_CARRIED_TARGETS: ((self.S, P), torch.int32), EXPORT_CALL_STATUS: ((1,), torch.int32)})
         shape, dtype = shapes[what]
         key = (what, shape)
         buf = self._exports.get(key)
         if buf is None:
             buf = self._exports[key] = torch.zeros(shape, dtype=dtype).pin_memory()
-        self._check(self.h.lib.gccnmf_ll_export(self.h.h, ctypes.byref(self.cfg), self.state.data_ptr(), self.state_bytes, self.last_hops,
-                                                int(what), buf.data_ptr(), self.stream.cuda_stream))
+        self._state('export', self.last_hops, int(what), buf.data_ptr(), self.stream.cuda_stream)
         self.stream.synchronize()
         return buf.numpy().copy()
 
@@ -237,20 +284,21 @@ class LowLatencyEngine(object):
 
 
 def streamSignals(signals, W, expJOmegaTau, analysisWindow, synthesisWindow, hopSize, hopsPerCall=1, synthesis='lowlatency',
-                  targetTDOAEpsilon=1.0, numInferenceIterations=0, use_graph=True, device=0, **kwargs):
+                  targetTDOAEpsilon=1.0, numInferenceIterations=0, use_graph=True, device=0, numSources=0, **kwargs):
     """Streams a list of stereo signals (2, n_i) through one engine, one stream each, hopsPerCall hops per call, and returns the
-    outputs aligned with the input: out_i[:, p] = output sample p + latency (the batch function's targetEstimateSamplesOLA), each
-    (2, n_i).  Shorter signals are followed by silence; the engine is flushed with `latency` samples of silence at the end."""
+    outputs aligned with the input: out_i[..., p] = output sample p + latency (the batch function's targetEstimateSamplesOLA), each
+    (2, n_i), or (P, 2, n_i) with numSources = P.  Shorter signals are followed by silence; the engine is flushed with `latency`
+    samples of silence at the end."""
     sig = [np.asarray(s, dtype=np.float32) for s in signals]
     eng = LowLatencyEngine(W, expJOmegaTau, analysisWindow, synthesisWindow, hopSize, numStreams=len(sig), hopsPerCall=hopsPerCall,
                            synthesis=synthesis, targetTDOAEpsilon=targetTDOAEpsilon, numInferenceIterations=numInferenceIterations,
-                           device=device, **kwargs)
+                           device=device, numSources=numSources, **kwargs)
     step = eng.hop * eng.C
     total = max(s.shape[1] for s in sig) + eng.latency
     total = -(-total // step) * step
     x = np.zeros((len(sig), 2, total), np.float32)
     for i, s in enumerate(sig):
         x[i, :, :s.shape[1]] = s
-    y = np.concatenate([eng.process(x[:, :, p:p + step], use_graph=use_graph) for p in range(0, total, step)], axis=2)
+    y = np.concatenate([eng.process(x[:, :, p:p + step], use_graph=use_graph) for p in range(0, total, step)], axis=-1)
     eng.close()
-    return [y[i, :, eng.latency:eng.latency + s.shape[1]] for i, s in enumerate(sig)]
+    return [y[i, ..., eng.latency:eng.latency + s.shape[1]] for i, s in enumerate(sig)]

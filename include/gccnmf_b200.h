@@ -576,6 +576,60 @@ GCCNMF_API int gccnmf_ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* 
 GCCNMF_API int gccnmf_ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, int what,
                      void* dst, void* stream);
 
+/* ---- a11 streamed, each stream separated into P sources: one output per target TDOA (TARGET_MODE_MULTIPLE) --------------
+ * The multi-target rule of gccNMFFunctions.py:94-143 per frame of the gccnmf_ll_* loop.  A stream has P target TDOA indexes
+ * tau_0 .. tau_{P-1} in [0, D), 2 <= P <= 8.  Per whole frame t of a call:
+ * - targets: the running maximum is carried as in gccnmf_ll_*; the P largest strict local maxima of the frame's running maximum,
+ *   ascending (estimateTargetTDOAIndexesFromAngularSpectrum), become the stream's targets.  With fewer than P peaks the targets
+ *   stay and status bit GCCNMF_LLSEP_STATUS_FEW_PEAKS of the stream is set (sticky until reset).  After init / reset the
+ *   targets are floor((2 q + 1) D / (2 P)).  A source's override (gccnmf_llsep_set_targets, >= 0) replaces its target.  Frames
+ *   before the stream's first sample and inactive streams change nothing.
+ * - values[q][k][t] = float32 of the float64 sum_f W[f][k] Re(coh[f][t] E[f][tau_q(t)]): the bits gccnmf_tdoa_gccnmf writes at
+ *   (tau_q(t), k, t).  masks = gccnmf_coeff_mask of the values (numpy.nanargmax; ties go to the lower source); a (k, t) whose
+ *   values are all NaN belongs to no source and sets bit GCCNMF_LLSEP_STATUS_ALL_NAN of the call's status.
+ * - source q: the single-target Wiener filter with mask_q (with inference, on the H inferred once per frame and shared by the
+ *   sources), inverse FFT, overlap-add into its own N-sample output ring and emit, at the latency and gain of gccnmf_ll_*.
+ * Where no value is NaN the masks partition the atoms, so the P outputs add up to the output with every atom kept.  The epsilon
+ * and target_override of gccnmf_ll_stream_params play no part; `active` does (an inactive stream outputs zeros).
+ * Buffers: in (S, 2, hops hop), out (S, P, 2, hops hop).  Launch / destroy graphs with gccnmf_rt_graph_launch / _destroy.
+ * Export: items 0 .. 3 and 11 .. 13 as gccnmf_ll_export, plus 14 column targets (T, P) i32, 15 values (P, K, T) f32, 16 masks
+ * (P, K, T) f32, 17 Wiener filters (P, F, T) f32 or (P, 2, F, T) with inference, 18 Y (P, 2, F, T) c64, 19 stream status (S) i32,
+ * 20 carried targets (S, P) i32, 21 the call's status (1) i32.  Items 4 .. 10 (the single-target chain) are refused.
+ * num_sources outside [2, 8], overrides outside [0, D) other than -1, and T P or P K T (T = S hops_per_call) at or above 2^31
+ * fail before anything is enqueued. */
+#define GCCNMF_LLSEP_MAX_SOURCES 8
+#define GCCNMF_LLSEP_STATUS_FEW_PEAKS 1
+#define GCCNMF_LLSEP_STATUS_ALL_NAN 2
+#define GCCNMF_LLSEP_EXPORT_TARGETS 14
+#define GCCNMF_LLSEP_EXPORT_VALUES 15
+#define GCCNMF_LLSEP_EXPORT_MASKS 16
+#define GCCNMF_LLSEP_EXPORT_WIENER 17
+#define GCCNMF_LLSEP_EXPORT_Y 18
+#define GCCNMF_LLSEP_EXPORT_STREAM_STATUS 19
+#define GCCNMF_LLSEP_EXPORT_CARRIED_TARGETS 20
+#define GCCNMF_LLSEP_EXPORT_CALL_STATUS 21
+/* Host only; 0 for an invalid configuration or num_sources.  Larger than gccnmf_ll_state_bytes of the same configuration. */
+GCCNMF_API size_t gccnmf_llsep_state_bytes(const gccnmf_ll_config* cfg, int num_sources);
+/* As gccnmf_ll_init; every stream also starts on the default targets with no overrides. */
+GCCNMF_API int gccnmf_llsep_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, const float* W, const double* E,
+                      const double* analysis_window, const double* synthesis_weights, float gain, const float* H0, void* state,
+                      size_t state_bytes, void* stream);
+/* As gccnmf_ll_reset_streams; targets back to the defaults and status cleared, overrides stay. */
+GCCNMF_API int gccnmf_llsep_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes,
+                               int first, int count, void* stream);
+GCCNMF_API int gccnmf_llsep_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes,
+                            int first, int count, const gccnmf_ll_stream_params* params_host, void* stream);
+/* targets_host: count x P host array, consumed before the call returns; -1: the source follows the localisation. */
+GCCNMF_API int gccnmf_llsep_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes,
+                             int first, int count, const int32_t* targets_host, void* stream);
+GCCNMF_API int gccnmf_llsep_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes,
+                         int hops, const float* in, float* out, void* stream);
+GCCNMF_API int gccnmf_llsep_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes,
+                              int hops, float* in, float* out, const float* in_host, float* out_host, void** graph_exec,
+                              void* stream);
+GCCNMF_API int gccnmf_llsep_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes,
+                        int hops, int what, void* dst, void* stream);
+
 /*
  * The building block the KL-NMF loop runs on (klnmf_tma.cu): the same 3-product contraction, TMA-fed, over operands
  * that are pre-split into bf16 hi/lo planes and kept in ONE orientation each; an operand contracted over its
