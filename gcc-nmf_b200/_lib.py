@@ -186,7 +186,22 @@ SIGNATURES.update({
     'gccnmf_llsep_process': (c_int, [_H, _LC, c_int, _P, c_size_t, c_int, _P, _P, _S]),
     'gccnmf_llsep_graph_create': (c_int, [_H, _LC, c_int, _P, c_size_t, c_int, _P, _P, _P, _P, ctypes.POINTER(c_void_p), _S]),
     'gccnmf_llsep_export': (c_int, [_H, _LC, c_int, _P, c_size_t, c_int, c_int, c_void_p, _S]),
+    'gccnmf_llrec_record_bytes': (c_size_t, [_LC, c_int]),
+    'gccnmf_llrec_workspace_bytes': (c_size_t, [_LC, c_int, c_int]),
+    'gccnmf_llrec_save_streams': (c_int, [_H, _LC, c_int, _P, c_size_t, c_int, c_int, c_void_p, c_size_t, _P, c_size_t, _S]),
+    'gccnmf_llrec_load_streams': (c_int, [_H, _LC, c_int, _P, c_size_t, c_int, c_int, c_void_p, c_size_t, _P, c_size_t, _S]),
 })
+
+
+class RecordHeader(ctypes.Structure):
+    """gccnmf_record_header (include/gccnmf_b200.h): the first bytes of every stream record."""
+    _fields_ = [('magic', ctypes.c_uint32), ('abi_version', c_int32), ('kind', c_int32), ('num_sources', c_int32),
+                ('payload_bytes', ctypes.c_uint64), ('synthesis_digest', ctypes.c_uint64), ('config', c_int32 * 16)]
+
+
+RECORD_MAGIC = 0x52534347
+RECORD_KIND_LL = 2
+RECORD_HEADER_BYTES = 256
 
 
 _lib = None

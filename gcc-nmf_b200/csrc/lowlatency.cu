@@ -686,6 +686,160 @@ int ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* state,
   return GCCNMF_OK;
 }
 
+// ---------------------------------------------------------------------------------------------- stream records
+// The persistent state of stream s is every byte a later call reads that an earlier call or a setting wrote:
+//   streams[s]        hops (frame validity, ring positions), epsilon, active, target_override       (ll_push, ll_mask, ll_*emit)
+//   carry[s]          D running maxima                                                               (ll_running_max)
+//   in_ring[s]        the last R samples of both channels                                            (ll_push <- ll_advance)
+//   out_ring[s]       the N-sample overlap-add ring of both channels, P of them with sources         (ll_ola_emit)
+//   src_targets[s], src_override[s], src_status[s]    (sources only)                                (ll_src_targets_kernel)
+// Everything else is either shared by the streams (header, windows, E, W and what init derives from it) or rewritten by every call
+// before it is read (stage, valid, X ... frames, counters).  A region is a strided array in the state: stream s's bytes are
+// [offset + s stride, + bytes), and they go to [rec_offset, + bytes) of the stream's record payload.  Rings are copied whole: their
+// positions derive from hops, which travels with them.
+struct RecordRegion { size_t offset, stride, rec_offset, bytes; };
+constexpr int kRecordMaxRegions = 8;
+struct RecordMap {
+  RecordRegion r[kRecordMaxRegions];
+  int n;
+  size_t payload;                        // payload bytes of one stream (16-aligned): the staging stride
+};
+constexpr size_t kRecordHeaderBytes = GCCNMF_RECORD_HEADER_BYTES;
+static_assert(sizeof(gccnmf_record_header) <= kRecordHeaderBytes, "record header");
+
+RecordMap ll_record_map(const gccnmf_ll_config& c, int P) {
+  char* const base = reinterpret_cast<char*>(256);
+  const LLLayout l = ll_carve(c, P, base);
+  const size_t N = l.N, R = l.R, D = l.D, Pm = P > 0 ? P : 1;
+  RecordMap m{};
+  size_t at = 0;
+  auto add = [&](const void* p, size_t bytes) {
+    if (bytes == 0) return;              // R = 0 when hop = N
+    m.r[m.n++] = RecordRegion{(size_t)((const char*)p - base), bytes, at, bytes};
+    at = align_up(at + bytes, 16);
+  };
+  add(l.streams, sizeof(LLStream));
+  add(l.carry, D * sizeof(double));
+  add(l.in_ring, 2 * R * sizeof(float));
+  add(l.out_ring, Pm * 2 * N * sizeof(float));
+  if (P) {
+    add(l.src_targets, kLLMaxSources * sizeof(int32_t));
+    add(l.src_override, kLLMaxSources * sizeof(int32_t));
+    add(l.src_status, sizeof(int32_t));
+  }
+  m.payload = at;
+  return m;
+}
+
+size_t ll_record_bytes(const gccnmf_ll_config& c, int P) { return kRecordHeaderBytes + align_up(ll_record_map(c, P).payload, 256); }
+
+// Grid (count, regions): CTA (i, g) copies region g of stream first + i between the state and payload i of the staging buffer,
+// in 16-byte words where both ends and the length allow it (every carve region is 256-aligned; LLStream and odd ring lengths
+// are not), else in 4-byte words (every region is a whole number of them).
+__global__ void __launch_bounds__(256)
+ll_record_copy_kernel(char* __restrict__ state, int first, RecordMap m, char* __restrict__ staging, int to_staging) {
+  const RecordRegion g = m.r[blockIdx.y];
+  char* slot = state + g.offset + (size_t)(first + blockIdx.x) * g.stride;
+  char* rec = staging + (size_t)blockIdx.x * m.payload + g.rec_offset;
+  const char* src = to_staging ? slot : rec;
+  char* dst = to_staging ? rec : slot;
+  if ((((uintptr_t)src | (uintptr_t)dst | g.bytes) & 15) == 0) {
+    for (size_t i = threadIdx.x; i < g.bytes / 16; i += blockDim.x)
+      reinterpret_cast<uint4*>(dst)[i] = reinterpret_cast<const uint4*>(src)[i];
+  } else {
+    for (size_t i = threadIdx.x; i < g.bytes / 4; i += blockDim.x)
+      reinterpret_cast<uint32_t*>(dst)[i] = reinterpret_cast<const uint32_t*>(src)[i];
+  }
+}
+
+// What a record must agree on, from the host arguments alone: magic, ABI version, kind, P, payload size and the configuration without
+// S and C.  The synthesis digest is left 0: see ll_synthesis_digest.
+gccnmf_record_header ll_record_header(const gccnmf_ll_config& cfg, int P) {
+  gccnmf_record_header r{};
+  r.magic = GCCNMF_RECORD_MAGIC;
+  r.abi_version = GCCNMF_ABI_VERSION;
+  r.kind = GCCNMF_RECORD_KIND_LL;
+  r.num_sources = P;
+  r.payload_bytes = ll_record_map(cfg, P).payload;
+  gccnmf_ll_config c = cfg;
+  c.num_streams = 0;
+  c.hops_per_call = 0;
+  static_assert(sizeof(c) <= sizeof(r.config), "record config");
+  memcpy(r.config, &c, sizeof(c));
+  return r;
+}
+
+// FNV-1a 64 of the synthesis weights' bytes followed by the gain's.  Both live only in the state, so they are read back on the
+// stream and waited for, as init reads the weights.
+int ll_synthesis_digest(gccnmf_handle* h, const LLLayout& l, uint64_t* digest, void* stream) {
+  const size_t wb = (size_t)l.N * sizeof(double);
+  unsigned char* w = new unsigned char[wb + sizeof(LLHeader)];
+  cudaStream_t s = (cudaStream_t)stream;
+  cudaError_t err = cudaMemcpyAsync(w, l.w_syn, wb, cudaMemcpyDeviceToHost, s);
+  if (err == cudaSuccess) err = cudaMemcpyAsync(w + wb, l.head, sizeof(LLHeader), cudaMemcpyDeviceToHost, s);
+  if (err == cudaSuccess) err = cudaStreamSynchronize(s);
+  uint64_t d = 1469598103934665603ull;
+  for (size_t i = 0; i < wb + sizeof(float); ++i) d = (d ^ w[i]) * 1099511628211ull;    // the weights, then LLHeader::gain
+  delete[] w;
+  GCCNMF_CHECK_CUDA(h, err);
+  *digest = d;
+  return GCCNMF_OK;
+}
+
+#define LL_RECORD_ARGS_OR_FAIL(what)                                                                                               \
+  LL_CARVE_OR_FAIL(l, P);                                                                                                            \
+  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, what ": streams [%d, %d + %d) outside [0, %d)", \
+                 first, first, count, l.S);                                                                                          \
+  const RecordMap m = ll_record_map(*cfg, P);                                                                                        \
+  const size_t rec_bytes = ll_record_bytes(*cfg, P);                                                                                 \
+  GCCNMF_REQUIRE(h, record != nullptr && record_bytes >= (size_t)count * rec_bytes, what ": record needs %zu bytes for %d streams",  \
+                 (size_t)count * rec_bytes, count);                                                                                  \
+  if (workspace == nullptr || workspace_bytes < (size_t)count * m.payload || ((uintptr_t)workspace & 3) != 0)                        \
+    return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, what ": workspace needs %zu bytes, 4-byte aligned", (size_t)count * m.payload);
+
+int ll_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* state, size_t state_bytes, int first, int count, void* record,
+                    size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
+  GCCNMF_ENTER(h);
+  LL_RECORD_ARGS_OR_FAIL("ll_save_streams");
+  gccnmf_record_header head = ll_record_header(*cfg, P);
+  if (int st = ll_synthesis_digest(h, l, &head.synthesis_digest, stream)) return st;
+  for (int i = 0; i < count; ++i) memcpy((char*)record + (size_t)i * rec_bytes, &head, sizeof(head));
+  GCCNMF_LAUNCH(h, ll_record_copy_kernel, dim3(count, m.n), 256, 0, stream, (char*)state, first, m, (char*)workspace, 1);
+  GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync((char*)record + kRecordHeaderBytes, rec_bytes, workspace, m.payload, m.payload, count,
+                                         cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  return GCCNMF_OK;
+}
+
+int ll_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* state, size_t state_bytes, int first, int count, const void* record,
+                    size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
+  GCCNMF_ENTER(h);
+  LL_RECORD_ARGS_OR_FAIL("ll_load_streams");
+  const gccnmf_record_header want = ll_record_header(*cfg, P);
+  for (int i = 0; i < count; ++i) {      // everything but the digest, before the device is touched
+    gccnmf_record_header got;
+    memcpy(&got, (const char*)record + (size_t)i * rec_bytes, sizeof(got));
+    GCCNMF_REQUIRE(h, got.magic == want.magic, "ll_load_streams: record %d: not a stream record (magic 0x%08x)", i, got.magic);
+    GCCNMF_REQUIRE(h, got.abi_version == want.abi_version, "ll_load_streams: record %d: ABI version %d, this library is %d", i, got.abi_version,
+                   want.abi_version);
+    GCCNMF_REQUIRE(h, got.kind == want.kind, "ll_load_streams: record %d: kind %d is not a low-latency stream", i, got.kind);
+    GCCNMF_REQUIRE(h, got.num_sources == P, "ll_load_streams: record %d: %d sources, this engine has %d", i, got.num_sources, P);
+    GCCNMF_REQUIRE(h, got.payload_bytes == want.payload_bytes, "ll_load_streams: record %d: payload of %llu bytes, expected %llu", i,
+                   (unsigned long long)got.payload_bytes, (unsigned long long)want.payload_bytes);
+    GCCNMF_REQUIRE(h, memcmp(got.config, want.config, sizeof(want.config)) == 0, "ll_load_streams: record %d: another configuration", i);
+  }
+  uint64_t digest = 0;
+  if (int st = ll_synthesis_digest(h, l, &digest, stream)) return st;
+  for (int i = 0; i < count; ++i) {
+    gccnmf_record_header got;
+    memcpy(&got, (const char*)record + (size_t)i * rec_bytes, sizeof(got));
+    GCCNMF_REQUIRE(h, got.synthesis_digest == digest, "ll_load_streams: record %d: other synthesis weights or gain", i);
+  }
+  GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync(workspace, m.payload, (const char*)record + kRecordHeaderBytes, rec_bytes, m.payload, count,
+                                         cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  GCCNMF_LAUNCH(h, ll_record_copy_kernel, dim3(count, m.n), 256, 0, stream, (char*)state, first, m, (char*)workspace, 0);
+  return GCCNMF_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -789,6 +943,27 @@ int gccnmf_llsep_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_s
                         void* dst, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
   return ll_export(h, cfg, num_sources, state, state_bytes, hops, what, dst, stream);
+}
+
+// ---- stream records (0 <= num_sources <= 8)
+size_t gccnmf_llrec_record_bytes(const gccnmf_ll_config* cfg, int num_sources) {
+  if (ll_check(nullptr, cfg, num_sources) != 0) return 0;
+  return ll_record_bytes(*cfg, num_sources);
+}
+
+size_t gccnmf_llrec_workspace_bytes(const gccnmf_ll_config* cfg, int num_sources, int count) {
+  if (ll_check(nullptr, cfg, num_sources) != 0 || count < 1) return 0;
+  return (size_t)count * ll_record_map(*cfg, num_sources).payload;
+}
+
+int gccnmf_llrec_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
+                              int count, void* record, size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
+  return ll_save_streams(h, cfg, num_sources, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes, stream);
+}
+
+int gccnmf_llrec_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
+                              int count, const void* record, size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
+  return ll_load_streams(h, cfg, num_sources, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

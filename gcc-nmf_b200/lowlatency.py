@@ -24,7 +24,7 @@ import ctypes
 
 import numpy as np
 
-from ._lib import LLConfig, LLStreamParams, default_handle
+from ._lib import RECORD_KIND_LL, RECORD_MAGIC, LLConfig, LLStreamParams, ParameterError, RecordHeader, default_handle
 
 SYNTHESIS_MODES = ('online', 'lowlatency', 'windowed')
 
@@ -110,6 +110,8 @@ class LowLatencyEngine(object):
         self._io = {}
         self._graphs = {}
         self._exports = {}
+        self._staging = None                                      # device staging of stream records
+        self._header = None                                       # their header, once computed
         self.last_hops = None
         self.h.torch.cuda.current_stream(self.h.device).synchronize()
         c = self._const
@@ -269,6 +271,80 @@ class LowLatencyEngine(object):
         self._state('export', self.last_hops, int(what), buf.data_ptr(), self.stream.cuda_stream)
         self.stream.synchronize()
         return buf.numpy().copy()
+
+    # ------------------------------------------------------------------ stream records (gccnmf_llrec_*)
+    @property
+    def record_bytes(self):
+        """Bytes of one stream's record."""
+        return int(self.h.lib.gccnmf_llrec_record_bytes(ctypes.byref(self.cfg), self.P))
+
+    def _record_runs(self, streams):
+        """(first, count, first record row) of each run of consecutive stream indexes, in the order given."""
+        idx = self._streams(streams)
+        if len(np.unique(idx)) != len(idx):
+            raise ValueError('a stream is listed twice')
+        row = 0
+        for run in np.split(idx, np.flatnonzero(np.diff(idx) != 1) + 1):
+            yield int(run[0]), len(run), row
+            row += len(run)
+
+    def _record_call(self, name, streams, rec):
+        rb = self.record_bytes
+        for first, count, row in self._record_runs(streams):
+            n = int(self.h.lib.gccnmf_llrec_workspace_bytes(ctypes.byref(self.cfg), self.P, count))
+            if self._staging is None or self._staging.numel() < n:
+                self._staging = self.torch.empty(n, dtype=self.torch.uint8, device=self.h.device)
+            self._check(getattr(self.h.lib, 'gccnmf_llrec_' + name)(
+                self.h.h, ctypes.byref(self.cfg), self.P, self.state.data_ptr(), self.state_bytes, first, count, rec.data[row].data_ptr(),
+                count * rb, self._staging.data_ptr(), self._staging.numel(), self.stream.cuda_stream))
+        self.stream.synchronize()
+
+    def save_streams(self, streams=None):
+        """The persistent state of `streams` (default: all, in order) between calls -> a StreamRecord, one record per stream.  The
+        streams go on unchanged."""
+        from .records import StreamRecord
+        idx = self._streams(streams)
+        rec = StreamRecord(RECORD_KIND_LL, self.P, self.torch.zeros((len(idx), self.record_bytes), dtype=self.torch.uint8).pin_memory(),
+                           dict(eps=self._eps[idx].copy(), active=self._active[idx].copy(), override=self._override[idx].copy(),
+                                targets=self._targets[idx].copy()))
+        self._record_call('save_streams', idx, rec)
+        return rec
+
+    def _record_header(self):
+        """The header this engine's records carry (gccnmf_record_header), computed on the host: the library writes the same."""
+        cfg = LLConfig.from_buffer_copy(bytes(self.cfg))
+        cfg.num_streams = cfg.hops_per_call = 0
+        head = RecordHeader(magic=RECORD_MAGIC, abi_version=self.h.lib.gccnmf_abi_version(), kind=RECORD_KIND_LL, num_sources=self.P,
+                            payload_bytes=int(self.h.lib.gccnmf_llrec_workspace_bytes(ctypes.byref(self.cfg), self.P, 1)))
+        ctypes.memmove(head.config, bytes(cfg), ctypes.sizeof(cfg))
+        d = 1469598103934665603                                    # FNV-1a 64 of the weights' bytes, then the gain's
+        for b in np.ascontiguousarray(self.weights, np.float64).tobytes() + np.float32(self.gain).tobytes():
+            d = ((d ^ b) * 1099511628211) & 0xFFFFFFFFFFFFFFFF
+        head.synthesis_digest = d
+        return head
+
+    def load_streams(self, streams, record):
+        """Record i replaces the state and settings of streams[i] from the next call on.  The record must come from an engine with
+        the same configuration other than numStreams and hopsPerCall, the same synthesis and numSources.  Every record is checked on
+        the host before anything is loaded, so a refusal leaves the engine and the device untouched.  Each run of consecutive
+        streams is one library call (one wait for the synthesis weights, one copy, one kernel)."""
+        idx = self._streams(streams)
+        if record.kind != RECORD_KIND_LL or record.count != len(idx):
+            raise ValueError('a low-latency record of %d streams is needed (got kind %d, %d streams)' % (len(idx), record.kind, record.count))
+        if record.data.shape[1] != self.record_bytes:
+            raise ParameterError('records of %d bytes do not fit this engine (%d bytes)' % (record.data.shape[1], self.record_bytes))
+        if self._header is None:
+            self._header = self._record_header()
+        want = self._header
+        head = np.frombuffer(bytes(want), np.uint8)
+        for i in np.flatnonzero((record.data.numpy()[:, :len(head)] != head).any(axis=1))[:1]:
+            got = record.header(int(i))
+            value = lambda h, f: bytes(h.config) if f == 'config' else getattr(h, f)       # noqa: E731
+            bad = [f for f, _ in RecordHeader._fields_ if value(got, f) != value(want, f)]
+            raise ParameterError('record %d does not fit this engine: %s differ' % (i, ', '.join(bad)))
+        self._record_call('load_streams', idx, record)
+        m = record.mirrors
+        self._eps[idx], self._active[idx], self._override[idx], self._targets[idx] = m['eps'], m['active'], m['override'], m['targets']
 
     def close(self):
         if self.h.h:

@@ -630,6 +630,48 @@ GCCNMF_API int gccnmf_llsep_graph_create(gccnmf_handle* h, const gccnmf_ll_confi
 GCCNMF_API int gccnmf_llsep_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes,
                         int hops, int what, void* dst, void* stream);
 
+/* ---- stream records: move a live stream to another stream index, engine, device or process -----------------------------------
+ * A record is the persistent state of one stream (its counters and parameters, running maximum, input ring, output ring(s) and,
+ * with sources, its targets, overrides and status) behind a header.  It does not depend on num_streams, hops_per_call, the
+ * stream index or the device.  A stream saved after a call and loaded anywhere compatible produces, from the next call on, the
+ * bytes it would have produced had it never moved.  Compatible: the same gccnmf_ll_config fields other than num_streams and
+ * hops_per_call (compared bit for bit), the same num_sources, the same synthesis weights and gain.
+ * These entries are the low-latency engine's, one family for both of its forms (num_sources 0 for gccnmf_ll_*, 2 .. 8 for
+ * gccnmf_llsep_*).
+ * Records live in a caller-owned HOST buffer (pinned for asynchronous copies): `count` records of gccnmf_llrec_record_bytes
+ * each, record i for stream first + i.  `workspace` is device staging of gccnmf_llrec_workspace_bytes(count) bytes, at least
+ * 4-byte aligned (16-byte aligned for the fast copy).
+ * save: reads the engine's synthesis weights and gain back on `stream` and waits for them (their digest goes into the header),
+ *   then one copy kernel into the staging and one device-to-host copy; the host buffer is complete when `stream` reaches it.
+ *   The streams are not changed (reset or deactivate them afterwards if they are to stop here).
+ * load: checks magic, ABI version, kind, num_sources, payload size and configuration of every record on the host, without
+ *   touching the device.  Only when all of them match does it read the synthesis weights and gain back (one wait on `stream`)
+ *   to check the digest.  Then one host-to-device copy and one copy kernel; the streams' state is replaced from the next call on.
+ *   Other streams, the graphs and the shared state are untouched.  A refused record enqueues no kernel and no host-to-device
+ *   copy. */
+#define GCCNMF_RECORD_MAGIC 0x52534347u   /* "GCSR" */
+#define GCCNMF_RECORD_KIND_LL 2
+#define GCCNMF_RECORD_HEADER_BYTES 256    /* the payload starts here in every record */
+typedef struct gccnmf_record_header {
+  uint32_t magic;
+  int32_t abi_version;                    /* GCCNMF_ABI_VERSION of the library that wrote it */
+  int32_t kind;
+  int32_t num_sources;                    /* 0: gccnmf_ll_* */
+  uint64_t payload_bytes;
+  uint64_t synthesis_digest;              /* FNV-1a 64 of the synthesis weights' bytes followed by the gain's */
+  int32_t config[16];                     /* the config struct's fields in order (num_streams and hops_per_call 0), then 0 */
+} gccnmf_record_header;
+/* num_sources: 0 for a gccnmf_ll_* engine, else the gccnmf_llsep_* engine's.  Host only; 0 for an invalid configuration or
+ * num_sources, or count < 1. */
+GCCNMF_API size_t gccnmf_llrec_record_bytes(const gccnmf_ll_config* cfg, int num_sources);
+GCCNMF_API size_t gccnmf_llrec_workspace_bytes(const gccnmf_ll_config* cfg, int num_sources, int count);
+GCCNMF_API int gccnmf_llrec_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes,
+                              int first, int count, void* record, size_t record_bytes, void* workspace, size_t workspace_bytes,
+                              void* stream);
+GCCNMF_API int gccnmf_llrec_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes,
+                              int first, int count, const void* record, size_t record_bytes, void* workspace,
+                              size_t workspace_bytes, void* stream);
+
 /*
  * The building block the KL-NMF loop runs on (klnmf_tma.cu): the same 3-product contraction, TMA-fed, over operands
  * that are pre-split into bf16 hi/lo planes and kept in ONE orientation each; an operand contracted over its
