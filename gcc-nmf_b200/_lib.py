@@ -203,6 +203,25 @@ RECORD_MAGIC = 0x52534347
 RECORD_KIND_LL = 2
 RECORD_HEADER_BYTES = 256
 
+SIGNATURES.update({
+    'gccnmf_rtrec_record_bytes': (c_size_t, [_C, c_int]),
+    'gccnmf_rtrec_workspace_bytes': (c_size_t, [_C, c_int, c_int, c_int, c_int, c_int]),
+    'gccnmf_rtrec_save_slots': (c_int, _BANK + [c_int, c_int, c_void_p, c_size_t, _P, c_size_t, _S]),
+    'gccnmf_rtrec_load_slots': (c_int, _BANK + [c_int, c_int, c_void_p, c_size_t, _P, c_size_t, _S]),
+})
+
+
+class RtRecordHeader(ctypes.Structure):
+    """gccnmf_rtrec_header (include/gccnmf_b200.h): the header of a real-time slot's record; its first 24 bytes are those of
+    RecordHeader."""
+    _fields_ = [('magic', ctypes.c_uint32), ('abi_version', c_int32), ('kind', c_int32), ('num_sources', c_int32),
+                ('payload_bytes', ctypes.c_uint64), ('windows_digest', ctypes.c_uint64), ('dictionary_digest', ctypes.c_uint64),
+                ('steering_digest', ctypes.c_uint64), ('dictionary_atoms', c_int32), ('reserved', c_int32), ('config', c_int32 * 16)]
+
+
+RECORD_KIND_RT = 1
+RTREC_DIGEST_CHUNK_WORDS = 1024
+
 
 _lib = None
 

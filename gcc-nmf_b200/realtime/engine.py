@@ -11,12 +11,17 @@ import ctypes
 import numpy as np
 
 from .._lib import RtConfig, default_handle
+from . import slotrecords
 
 EXPORT_GCCPHAT, EXPORT_TARGET, EXPORT_ATOM_MASK, EXPORT_INPUT_SPEC, EXPORT_OUTPUT_SPEC, EXPORT_ARGMAX, EXPORT_H, EXPORT_HISTORY, \
     EXPORT_HISTORY_INDEX = range(9)
 
+# gccNMFProcessor.py:190-199 -- what gccnmf_rt_init, gccnmf_rtm_init and gccnmf_rtm_reset_slots leave in a slot
+DEFAULT_SLOT_PARAMS = dict(targetTDOAIndex=10.0, epsilon=2.0, beta=1.0, noiseFloor=0.0, mode=1, separationEnabled=True,
+                           localizationEnabled=False, localizationWindowSize=6, active=True)
 
-class RealtimeEngine(object):
+
+class RealtimeEngine(slotrecords.SlotRecords):
     def __init__(self, W, expJOmegaTau, analysisWindow, synthesisWindow, hopSize, blockSize, windowsPerBlock, historyLength=128,
                  numInferenceIterations=0, sparsityAlpha=0.0, epsilon=1e-16, seedValue=0, device=0):
         self.h = default_handle(device)
@@ -55,6 +60,8 @@ class RealtimeEngine(object):
         self.frames_out_dev = torch.zeros((2, N, self.nT), dtype=torch.float32, device=self.h.device)
         self._graph = None
         self._exports = {}
+        self._record_digests = (slotrecords.windows_digest(analysisWindow, synthesisWindow), [(slotrecords.dictionary_digest(W, H0), K)],
+                                [slotrecords.steering_digest(E)])
         self.reset()
 
     # ------------------------------------------------------------------ state
@@ -71,15 +78,43 @@ class RealtimeEngine(object):
                                                   c[3].data_ptr(), c[4].data_ptr() if c[4] is not None else None,
                                                   self.state.data_ptr(), self.state_bytes, self.stream.cuda_stream))
         self.stream.synchronize()
+        self._params = [dict(DEFAULT_SLOT_PARAMS)]
 
     def set_params(self, targetTDOAIndex=None, epsilon=2.0, beta=1.0, noiseFloor=0.0, mode=1, separationEnabled=True,
                    localizationEnabled=False, localizationWindowSize=6):
         """targetTDOAIndex=None keeps the device-resident index (loop-carried by the localisation)."""
+        self._params[0].update(targetTDOAIndex=targetTDOAIndex, epsilon=epsilon, beta=beta, noiseFloor=noiseFloor, mode=mode,
+                               separationEnabled=separationEnabled, localizationEnabled=localizationEnabled,
+                               localizationWindowSize=localizationWindowSize)
         self._check(self.h.lib.gccnmf_rt_set_params(self.h.h, ctypes.byref(self.cfg), self.state.data_ptr(), self.state_bytes,
                                                     float(targetTDOAIndex if targetTDOAIndex is not None else 0.0),
                                                     0 if targetTDOAIndex is None else 1, float(epsilon), float(beta), float(noiseFloor), int(mode),
                                                     1 if separationEnabled else 0, 1 if localizationEnabled else 0, int(localizationWindowSize),
                                                     self.stream.cuda_stream))
+
+    # ------------------------------------------------------------------ stream records (gccnmf_rtrec_*, slotrecords.SlotRecords)
+    P = 0
+    _record_dims = (1, 0, 0, 0)
+
+    def _slots(self, slots):
+        out = [int(s) for s in (slots if np.ndim(slots) else [slots])]
+        if any(s != 0 for s in out):
+            raise IndexError('a RealtimeEngine has the one slot 0')
+        return out
+
+    def save_streams(self):
+        """The persistent state of the stream between blocks -> a StreamRecord of one record, which any real-time engine with
+        this configuration (other than K_max), numSources 0, these windows and an entry holding this W, H0 and expJOmegaTau
+        can load into a slot."""
+        return slotrecords.SlotRecords.save_streams(self, [0])
+
+    def load_streams(self, record):
+        """The stream continues from a record of one real-time slot (of any engine form) from the next block on.  The record's
+        dictionary, H0 and steering table must be this engine's."""
+        return slotrecords.SlotRecords.load_streams(self, [0], record)
+
+    def _records_loaded(self, slots, entries):
+        pass
 
     # ------------------------------------------------------------------ per-block work
     def build_graph(self):

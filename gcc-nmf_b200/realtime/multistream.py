@@ -27,7 +27,8 @@ import ctypes
 import numpy as np
 
 from .._lib import RtConfig, RtmSlotParams, default_handle
-from .engine import (EXPORT_ARGMAX, EXPORT_ATOM_MASK, EXPORT_GCCPHAT, EXPORT_H, EXPORT_HISTORY, EXPORT_HISTORY_INDEX,  # noqa: F401
+from . import slotrecords
+from .engine import (DEFAULT_SLOT_PARAMS, EXPORT_ARGMAX, EXPORT_ATOM_MASK, EXPORT_GCCPHAT, EXPORT_H, EXPORT_HISTORY, EXPORT_HISTORY_INDEX,  # noqa: F401
                      EXPORT_INPUT_SPEC, EXPORT_OUTPUT_SPEC, EXPORT_TARGET)
 
 # export items of an engine with sources (gccnmf_rtsep_export); EXPORT_ATOM_MASK and EXPORT_OUTPUT_SPEC are then source 0's
@@ -41,9 +42,6 @@ MAX_SOURCES = 8
 EXPORT_ASSIGNMENT = 14               # (2,) int32 (dictionary, steering) entries of a slot of a bank engine
 MAX_BANK_ENTRIES = 64
 
-# gccNMFProcessor.py:190-199 -- what gccnmf_rtm_init and gccnmf_rtm_reset_slots leave in a slot
-DEFAULT_SLOT_PARAMS = dict(targetTDOAIndex=10.0, epsilon=2.0, beta=1.0, noiseFloor=0.0, mode=1, separationEnabled=True,
-                           localizationEnabled=False, localizationWindowSize=6, active=True)
 
 
 def check_bank_entries(values, count, num_entries, name):
@@ -75,7 +73,7 @@ def check_bank_index(index, num_entries, name):
     return int(index)
 
 
-class MultiStreamRealtimeEngine(object):
+class MultiStreamRealtimeEngine(slotrecords.SlotRecords):
     def __init__(self, W, expJOmegaTau, analysisWindow, synthesisWindow, hopSize, blockSize, windowsPerBlock, numStreams, historyLength=128,
                  numInferenceIterations=0, sparsityAlpha=0.0, epsilon=1e-16, seedValue=0, device=0, numSources=0):
         self.P = int(numSources)
@@ -121,6 +119,10 @@ class MultiStreamRealtimeEngine(object):
         if self.bank:                           # device copies of every entry, read by init
             self._dicts = [(dev(w), dev(self._h0(w.shape[1])) if H0 is not None else None) for w in Ws]
             self._steers = [dev(e.view(np.float32).reshape(F, 2 * self.D)) for e in Es]
+        # content digests of the windows and of every entry, which stream records name their entries by
+        self._record_digests = (slotrecords.windows_digest(analysisWindow, synthesisWindow),
+                                [(slotrecords.dictionary_digest(w, self._h0(w.shape[1])), w.shape[1]) for w in Ws],
+                                [slotrecords.steering_digest(e) for e in Es])
         S = self.S
         per_slot = (self.P,) if self.P else ()          # outputs: (S, [P,] 2, ...)
         self.in_host = torch.zeros((S, 2, self.B), dtype=torch.float32).pin_memory()
@@ -319,6 +321,7 @@ class MultiStreamRealtimeEngine(object):
         self.stream.synchronize()
         self._dicts[index] = entry
         self.dictionaryAtoms[index] = W.shape[1]
+        self._record_digests[1][index] = (slotrecords.dictionary_digest(W, H0), W.shape[1])
 
     def load_steering(self, index, expJOmegaTau):
         """Replaces steering entry `index` by expJOmegaTau (F, D) from the next block on.  The graph is kept."""
@@ -332,6 +335,18 @@ class MultiStreamRealtimeEngine(object):
         self._abi('load_steering', int(index), entry.data_ptr(), self.stream.cuda_stream)
         self.stream.synchronize()
         self._steers[index] = entry
+        self._record_digests[2][index] = slotrecords.steering_digest(E)
+
+    # ------------------------------------------------------------------ stream records (gccnmf_rtrec_*, slotrecords.SlotRecords)
+    @property
+    def _record_dims(self):
+        return (self.S, self.P, self.Qd, self.Qe)
+
+    def _records_loaded(self, slots, entries):
+        """After a load: the slots are on the entries the records mapped to.  _block_atoms stays: K-shaped exports describe the
+        destination slot's last block until the next one."""
+        for s, e in zip(slots, entries):
+            self._assign[s] = list(e)
 
     # ------------------------------------------------------------------ per-block work
     def build_graph(self):

@@ -672,6 +672,61 @@ GCCNMF_API int gccnmf_llrec_load_streams(gccnmf_handle* h, const gccnmf_ll_confi
                               int first, int count, const void* record, size_t record_bytes, void* workspace,
                               size_t workspace_bytes, void* stream);
 
+/* ---- real-time stream records: move a live slot to another slot, engine, engine form, device or process ---------------------
+ * One family for every real-time form, with the arguments of gccnmf_rtbank_*: (num_streams, num_sources, num_dictionaries,
+ * num_steerings) = (1, 0, 0, 0) for gccnmf_rt_*, (S, 0, 0, 0) for gccnmf_rtm_*, (S, P, 0, 0) for gccnmf_rtsep_* and
+ * (S, P, Qd, Qe) for a bank.  A record is the persistent state of one slot (its parameters, block counter, history index and
+ * target, GCC-PHAT history, input ring, output ring(s) and, with sources, its targets and status) behind a gccnmf_rtrec_header.
+ * It does not depend on num_streams, the slot index, num_dictionaries, num_steerings, num_atoms (K_max) or the device.  A slot
+ * saved between blocks and loaded into a compatible slot computes, from the next block on, the bytes it would have computed had
+ * it never moved.  Compatible: the same gccnmf_rt_config fields other than num_atoms (compared bit for bit), the same
+ * num_sources, the same windows, and a dictionary entry and a steering entry whose content digests equal the record's.  The
+ * record names its entries by content, not by index: a load puts the slot on the LOWEST destination entry of each kind whose
+ * digest (and, for a dictionary, K_i) matches, and writes that into the slot's bank assignment.  The empty bank (rt, rtm,
+ * rtsep) counts as one dictionary of num_atoms atoms and one steering table.
+ * Content digest (GCCNMF_RTREC_DIGEST_*): the input is a sequence of n 32-bit words cut into chunks of 1024 words; chunk j gets
+ * c_j = FNV-1a 64 over its words (h = (h ^ w) * 0x100000001b3 from 0xcbf29ce484222325); the digest is FNV-1a 64 over the words
+ * (n_lo, n_hi, c_0 lo, c_0 hi, c_1 lo, ...).  It is applied to the windows (analysis then synthesis, 2 N f32), to dictionary
+ * entry i (W_i (F, K_i) f32, then H0_i (K_i, 2) f32 when inference_iterations > 0) and to steering entry j (its stored E^T,
+ * (D, Fp) complex64 with Fp = (F + 3) & ~3, the bins F .. Fp - 1 zero).
+ * Records live in a caller-owned HOST buffer (pinned for asynchronous copies): `count` records of gccnmf_rtrec_record_bytes
+ * each, record i for slot first + i.  `workspace` is device memory of gccnmf_rtrec_workspace_bytes(count) bytes, 16-byte aligned.
+ * save: the digest kernels, one copy kernel that writes `count` whole records (header included) into the workspace, one
+ *   device-to-host copy; no host wait.  The slots are not changed.
+ * load: checks magic, ABI version, kind, num_sources, payload size and configuration of every record on the host (refused: nothing
+ *   enqueued).  Then the digest kernels on the destination, one read-back of the digests and K_i (one wait on `stream`), and the
+ *   mapping of every record's entries (refused: only those read-only kernels ran).  Then one host-to-device copy of the records,
+ *   one copy kernel (which also writes the bank assignment) and, with a bank, the sort of the slots by dictionary.  Other slots,
+ *   the graphs and the shared region are untouched; both entries are stream-ordered and may sit between two graph launches.
+ *   K-shaped exports between a load and the next block still describe the destination slot's last block. */
+#define GCCNMF_RECORD_KIND_RT 1
+#define GCCNMF_RTREC_DIGEST_CHUNK_WORDS 1024
+#define GCCNMF_RTREC_DIGEST_BASIS 0xcbf29ce484222325ull
+#define GCCNMF_RTREC_DIGEST_PRIME 0x100000001b3ull
+typedef struct gccnmf_rtrec_header {
+  uint32_t magic;                         /* the first 24 bytes are those of gccnmf_record_header */
+  int32_t abi_version;
+  int32_t kind;                           /* GCCNMF_RECORD_KIND_RT */
+  int32_t num_sources;                    /* 0 or 2 .. 8 */
+  uint64_t payload_bytes;
+  uint64_t windows_digest;
+  uint64_t dictionary_digest;             /* of the dictionary entry the slot was on */
+  uint64_t steering_digest;               /* of the steering entry the slot was on */
+  int32_t dictionary_atoms;               /* that entry's K_i */
+  int32_t reserved;                       /* 0 */
+  int32_t config[16];                     /* the config struct's fields in order (num_atoms 0), then 0 */
+} gccnmf_rtrec_header;
+/* Host only; 0 for an invalid configuration, num_sources or bank, or count < 1. */
+GCCNMF_API size_t gccnmf_rtrec_record_bytes(const gccnmf_rt_config* cfg, int num_sources);
+GCCNMF_API size_t gccnmf_rtrec_workspace_bytes(const gccnmf_rt_config* cfg, int num_streams, int num_sources, int num_dictionaries,
+                                    int num_steerings, int count);
+GCCNMF_API int gccnmf_rtrec_save_slots(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources,
+                            int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int first, int count,
+                            void* record, size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream);
+GCCNMF_API int gccnmf_rtrec_load_slots(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_streams, int num_sources,
+                            int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int first, int count,
+                            const void* record, size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream);
+
 /*
  * The building block the KL-NMF loop runs on (klnmf_tma.cu): the same 3-product contraction, TMA-fed, over operands
  * that are pre-split into bf16 hi/lo planes and kept in ONE orientation each; an operand contracted over its
