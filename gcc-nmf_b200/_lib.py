@@ -192,6 +192,25 @@ SIGNATURES.update({
     'gccnmf_llrec_load_streams': (c_int, [_H, _LC, c_int, _P, c_size_t, c_int, c_int, c_void_p, c_size_t, _P, c_size_t, _S]),
 })
 
+_HIST = [_H, _LC, c_int, c_int, _P, c_size_t]      # handle, config, num_sources, history_length, state, state_bytes
+SIGNATURES.update({
+    'gccnmf_llhist_state_bytes': (c_size_t, [_LC, c_int, c_int]),
+    'gccnmf_llhist_init': (c_int, [_H, _LC, c_int, c_int, _P, _P, _P, _P, c_float, _P, _P, c_size_t, _S]),
+    'gccnmf_llhist_reset_streams': (c_int, _HIST + [c_int, c_int, _S]),
+    'gccnmf_llhist_set_params': (c_int, _HIST + [c_int, c_int, ctypes.POINTER(LLStreamParams), _S]),
+    'gccnmf_llhist_set_targets': (c_int, _HIST + [c_int, c_int, ctypes.POINTER(c_int32), _S]),
+    'gccnmf_llhist_set_window': (c_int, _HIST + [c_int, c_int, ctypes.POINTER(c_int32), _S]),
+    'gccnmf_llhist_process': (c_int, _HIST + [c_int, _P, _P, _S]),
+    'gccnmf_llhist_graph_create': (c_int, _HIST + [c_int, _P, _P, _P, _P, ctypes.POINTER(c_void_p), _S]),
+    'gccnmf_llhist_export': (c_int, _HIST + [c_int, c_int, c_void_p, _S]),
+    'gccnmf_llhist_record_bytes': (c_size_t, [_LC, c_int, c_int]),
+    'gccnmf_llhist_workspace_bytes': (c_size_t, [_LC, c_int, c_int, c_int]),
+    'gccnmf_llhist_save_streams': (c_int, _HIST + [c_int, c_int, c_void_p, c_size_t, _P, c_size_t, _S]),
+    'gccnmf_llhist_load_streams': (c_int, _HIST + [c_int, c_int, c_void_p, c_size_t, _P, c_size_t, _S]),
+})
+LLHIST_MAX_HISTORY = 1024
+LLHIST_RECORD_CONFIG_HISTORY = 9        # config[9] of a record header: the history length (0 without history)
+
 
 class RecordHeader(ctypes.Structure):
     """gccnmf_record_header (include/gccnmf_b200.h): the first bytes of every stream record."""

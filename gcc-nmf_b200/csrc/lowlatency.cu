@@ -28,6 +28,10 @@
 //   istft frames       one launch over the (P, 2) spectra
 //   ll_src_ola_emit    per (stream, source): ll_ola_emit_kernel's overlap-add and emit into the source's own ring
 //   ll_src_advance     per stream, after every source has emitted: the input ring and the hop count move on
+//
+// With a history of Lh > 0 frames per stream (gccnmf_llhist_*) the targets stage is ll_hist_targets / ll_hist_src_targets instead:
+// the running maximum as above, every valid frame's angular column into the stream's (D, Lh) ring, and for a stream on window
+// w >= 1 the nanmean of its newest w columns in place of the running maximum (rt_localize's rule).  With Lh = 0 nothing changes.
 #include <cmath>
 
 #include "common.cuh"
@@ -71,11 +75,18 @@ struct LLLayout {
   // masks (P, K, T) and the column targets (T, P).  out_ring, wiener, Y and frames then hold P times as much.
   int32_t *src_targets, *src_override, *src_status, *col_targets;
   float *values, *src_mask;
+  // history (gccnmf_llhist_*, Lh > 0): per stream one block of hist_stride bytes, the ring (D, Lh) f64 followed by the ring's write
+  // index, the window w (i32 each) and 8 zero bytes; per call the window means (D, T)
+  int Lh;
+  size_t hist_stride;
+  char* hist;
+  double* means;
 };
 
 bool is_pow2(int x) { return x > 0 && (x & (x - 1)) == 0; }
 constexpr int kLLMaxSources = 8;
 constexpr int kLLInferMaxSmem = 227 * 1024;   // the H100's opt-in dynamic shared memory per block
+constexpr int kLLMaxHistory = 1024;
 
 int ll_check(gccnmf_handle* h, const gccnmf_ll_config* cfg) {
   GCCNMF_REQUIRE(h, cfg != nullptr, "ll: NULL config");
@@ -107,7 +118,15 @@ int ll_check(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P) {
   return 0;
 }
 
-LLLayout ll_carve(const gccnmf_ll_config& c, int P, void* base) {
+// Lh = 0: gccnmf_ll_* / gccnmf_llsep_*; 1 <= Lh <= 1024: a history ring of Lh frames per stream (gccnmf_llhist_*)
+int ll_check(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh) {
+  if (int st = ll_check(h, cfg, P)) return st;
+  GCCNMF_REQUIRE(h, Lh >= 0 && Lh <= kLLMaxHistory, "llhist: history_length must be in [0, %d] (got %d)", kLLMaxHistory, Lh);
+  GCCNMF_REQUIRE(h, (int64_t)cfg->num_streams * cfg->num_tdoas * Lh < ((int64_t)1 << 31), "llhist: S x D x history_length overflows int32");
+  return 0;
+}
+
+LLLayout ll_carve(const gccnmf_ll_config& c, int P, void* base, int Lh = 0) {
   WorkspaceCarver w(base ? base : reinterpret_cast<void*>(256), base ? ~size_t(0) >> 1 : ~size_t(0) >> 1);
   LLLayout l{};
   l.S = c.num_streams; l.N = c.window_size; l.hop = c.hop_size; l.C = c.hops_per_call; l.K = c.num_atoms; l.D = c.num_tdoas;
@@ -154,14 +173,19 @@ LLLayout ll_carve(const gccnmf_ll_config& c, int P, void* base) {
   l.col_targets = w.take<int32_t>(T * Ps);
   l.values = w.take<float>(Ps * K * T);
   l.src_mask = w.take<float>(Ps * K * T);
+  // history: appended last (nothing is taken with Lh = 0, so the layouts above are unchanged)
+  l.Lh = Lh;
+  l.hist_stride = Lh ? D * Lh * sizeof(double) + 16 : 0;
+  l.hist = w.take<char>(S * l.hist_stride);
+  l.means = w.take<double>(Lh ? D * T : 0);
   l.bytes = align_up(w.used, 256);
   return l;
 }
 
-#define LL_CARVE_OR_FAIL(l, P)                                                                                       \
-  if (int st__ = ll_check(h, cfg, P)) return st__;                                                                   \
+#define LL_CARVE_OR_FAIL(l, P, Lh)                                                                                   \
+  if (int st__ = ll_check(h, cfg, P, Lh)) return st__;                                                               \
   GCCNMF_REQUIRE(h, state != nullptr, "ll: NULL state");                                                             \
-  const LLLayout l = ll_carve(*cfg, P, state);                                                                       \
+  const LLLayout l = ll_carve(*cfg, P, state, Lh);                                                                   \
   if (state_bytes < l.bytes) return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "ll: state too small: need %zu bytes", l.bytes);
 
 // ---------------------------------------------------------------------------------------------- kernels
@@ -314,6 +338,121 @@ ll_src_targets_kernel(const LLStream* __restrict__ streams, const double* __rest
     }
   }
   if (d < P) src_targets[(int64_t)s * kLLMaxSources + d] = cur_s[d];
+}
+
+// History (gccnmf_llhist_*), thread d = TDOA of stream s: each valid frame's angular column goes into the ring at the write index,
+// which moves on; then, whatever the frame's validity, means[d][t] = the nanmean of the newest w ring columns, summed newest first
+// in float64 and skipping NaN (rt_localize's loop, restated), NaN when all of them are NaN or w = 0.  The zero columns of a ring
+// that has seen fewer than w frames count in the denominator.  The write index is stored by thread 0 after `__syncthreads`.
+// Returns w (the same in every thread).
+__device__ __forceinline__ int ll_hist_means(const double* __restrict__ ang, const int32_t* __restrict__ valid, int D, int hops, int T, char* hist,
+                                             size_t hist_stride, int Lh, double* __restrict__ means) {
+  const int s = blockIdx.x, d = threadIdx.x;
+  const int t0 = s * hops;
+  double* ring = reinterpret_cast<double*>(hist + (size_t)s * hist_stride);
+  int32_t* slot = reinterpret_cast<int32_t*>(ring + (size_t)D * Lh);      // [0] write index, [1] window
+  int idx = slot[0];
+  const int w = slot[1];
+  if (d < D) {
+    double* row = ring + (size_t)d * Lh;
+    for (int i = 0; i < hops; ++i) {
+      const int t = t0 + i;
+      if (valid[t]) {
+        row[idx] = ang[(int64_t)d * T + t];
+        idx = idx + 1 == Lh ? 0 : idx + 1;
+      }
+      double m = __longlong_as_double(0x7ff8000000000000LL);
+      if (w > 0) {
+        double sum = 0.0;
+        int n = 0;
+        for (int j = 0, p = idx; j < w; ++j) {
+          p = p == 0 ? Lh - 1 : p - 1;
+          const double v = row[p];
+          if (v == v) { sum += v; ++n; }
+        }
+        if (n > 0) m = sum / (double)n;
+      }
+      means[(int64_t)d * T + t] = m;
+    }
+  }
+  __syncthreads();
+  if (d == 0) slot[0] = idx;
+  return w;
+}
+
+// History, one CTA per stream, thread d = TDOA: the running maximum and its carry as ll_targets_kernel, the ring and the window
+// means, then target[t] = argmax over d of the means (w >= 1) or of the running maximum (w = 0), or the stream's override.
+__global__ void __launch_bounds__(128)
+ll_hist_targets_kernel(const LLStream* __restrict__ streams, const double* __restrict__ ang, const int32_t* __restrict__ valid, int D, int hops,
+                       int T, double* __restrict__ carry, double* __restrict__ acc, char* __restrict__ hist, size_t hist_stride, int Lh,
+                       double* __restrict__ means, int32_t* __restrict__ targets) {
+  const int s = blockIdx.x, d = threadIdx.x;
+  ll_running_max(streams, ang, valid, D, hops, T, carry, acc);
+  const int w = ll_hist_means(ang, valid, D, hops, T, hist, hist_stride, Lh, means);
+  if (d < hops) {
+    const double* x = w > 0 ? means : acc;
+    const int t = s * hops + d;
+    double bv = x[t];
+    int bi = 0;
+    for (int e = 1; e < D; ++e) {
+      const double v = x[(int64_t)e * T + t];
+      if (ll_argmax_better(v, e, bv, bi)) { bv = v; bi = e; }
+    }
+    const int o = streams[s].target_override;
+    targets[t] = o >= 0 ? o : bi;
+  }
+}
+
+// History with sources: ll_src_targets_kernel's rule on the window means (w >= 1) or on the running maximum (w = 0).
+__global__ void __launch_bounds__(128)
+ll_hist_src_targets_kernel(const LLStream* __restrict__ streams, const double* __restrict__ ang, const int32_t* __restrict__ valid, int D,
+                           int hops, int T, int P, double* __restrict__ carry, double* __restrict__ acc, char* __restrict__ hist,
+                           size_t hist_stride, int Lh, double* __restrict__ means, int32_t* __restrict__ src_targets,
+                           const int32_t* __restrict__ src_override, int32_t* __restrict__ src_status, int32_t* __restrict__ col_targets) {
+  __shared__ double x_s[128];
+  __shared__ unsigned char peak_s[128], chosen_s[128];
+  __shared__ int num_peaks_s;
+  __shared__ int32_t pick_s[kLLMaxSources], cur_s[kLLMaxSources];
+  const int s = blockIdx.x, d = threadIdx.x;
+  const int t0 = s * hops;
+  ll_running_max(streams, ang, valid, D, hops, T, carry, acc);
+  if (d < P) cur_s[d] = src_targets[(int64_t)s * kLLMaxSources + d];
+  const int w = ll_hist_means(ang, valid, D, hops, T, hist, hist_stride, Lh, means);
+  const double* x = w > 0 ? means : acc;
+  for (int i = 0; i < hops; ++i) {
+    const int t = t0 + i;
+    if (valid[t]) {                      // the same for every thread of the CTA
+      if (d < D) x_s[d] = x[(int64_t)d * T + t];
+      const int peaks = select_peaks(x_s, D, P, peak_s, chosen_s, &num_peaks_s, pick_s);
+      if (d == 0) {
+        if (peaks >= P)
+          for (int q = 0; q < P; ++q) cur_s[q] = pick_s[q];
+        else
+          src_status[s] |= GCCNMF_LLSEP_STATUS_FEW_PEAKS;
+      }
+      __syncthreads();
+    }
+    if (d < P) {
+      const int o = src_override[(int64_t)s * kLLMaxSources + d];
+      col_targets[(int64_t)t * P + d] = o >= 0 ? o : cur_s[d];
+    }
+  }
+  if (d < P) src_targets[(int64_t)s * kLLMaxSources + d] = cur_s[d];
+}
+
+// History: streams [first, first + count) back to a zero ring, write index 0 and window 0 (16-byte words: the stride is a multiple of 16).
+__global__ void ll_hist_reset_kernel(char* __restrict__ hist, size_t hist_stride, int first, int count) {
+  if ((int)blockIdx.x >= count) return;
+  uint4* b = reinterpret_cast<uint4*>(hist + (size_t)(first + blockIdx.x) * hist_stride);
+  for (size_t i = threadIdx.x; i < hist_stride / 16; i += blockDim.x) b[i] = make_uint4(0, 0, 0, 0);
+}
+
+struct LLWindowBatch { int32_t w[kLLParamsPerLaunch]; };
+
+__global__ void ll_hist_window_kernel(char* __restrict__ hist, size_t hist_stride, size_t window_offset, int first, int count, LLWindowBatch b) {
+  const int i = threadIdx.x;
+  if (i >= count) return;
+  *reinterpret_cast<int32_t*>(hist + (size_t)(first + i) * hist_stride + window_offset) = b.w[i];
 }
 
 // mask[k][t] = |argmax[k][t] - target[t]| < epsilon of t's stream   (atom_mask_kernel mode 0)
@@ -477,8 +616,12 @@ __global__ void ll_src_override_kernel(int32_t* __restrict__ src_override, int f
 int ll_enqueue_sources(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l, int hops, float* out, void* stream) {
   const int S = l.S, N = l.N, hop = l.hop, F = l.F, K = l.K, D = l.D, P = l.P, T = S * hops;
   const bool inf = cfg->inference_iterations > 0;
-  GCCNMF_LAUNCH(h, ll_src_targets_kernel, S, 128, 0, stream, l.streams, l.ang, l.valid, D, hops, T, P, l.carry, l.acc, l.src_targets,
-                l.src_override, l.src_status, l.col_targets);
+  if (l.Lh)
+    GCCNMF_LAUNCH(h, ll_hist_src_targets_kernel, S, 128, 0, stream, l.streams, l.ang, l.valid, D, hops, T, P, l.carry, l.acc, l.hist, l.hist_stride,
+                  l.Lh, l.means, l.src_targets, l.src_override, l.src_status, l.col_targets);
+  else
+    GCCNMF_LAUNCH(h, ll_src_targets_kernel, S, 128, 0, stream, l.streams, l.ang, l.valid, D, hops, T, P, l.carry, l.acc, l.src_targets,
+                  l.src_override, l.src_status, l.col_targets);
   if (int e = gccnmf_target_gccnmf(h, l.coh, F, T, l.E, D, l.W, K, l.col_targets, P, l.values, stream)) return e;
   if (int e = gccnmf_coeff_mask(h, l.values, P, K, T, l.src_mask, l.counters + 2, stream)) return e;
   const size_t KT = (size_t)K * T, FT = (size_t)F * T;
@@ -514,7 +657,11 @@ int ll_enqueue(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l,
   if (int e = gccnmf_stft_segments(h, l.stage, (int64_t)S * Lseg, 2, S, hops, Lseg, l.win_a, N, hop, 0, l.X, inf ? l.V : nullptr, stream)) return e;
   if (int e = gccnmf_phat_angspec(h, l.X, F, T, 0, l.E, D, l.coh, l.ang, nullptr, nullptr, 0, stream)) return e;
   if (l.P) return ll_enqueue_sources(h, cfg, l, hops, out, stream);
-  GCCNMF_LAUNCH(h, ll_targets_kernel, S, 128, 0, stream, l.streams, l.ang, l.valid, D, hops, T, l.carry, l.acc, l.targets);
+  if (l.Lh)
+    GCCNMF_LAUNCH(h, ll_hist_targets_kernel, S, 128, 0, stream, l.streams, l.ang, l.valid, D, hops, T, l.carry, l.acc, l.hist, l.hist_stride, l.Lh,
+                  l.means, l.targets);
+  else
+    GCCNMF_LAUNCH(h, ll_targets_kernel, S, 128, 0, stream, l.streams, l.ang, l.valid, D, hops, T, l.carry, l.acc, l.targets);
   if (int e = gccnmf_tdoa_argmax(h, l.coh, F, T, l.E, D, l.W, K, l.argmax, l.counters, l.ws_argmax, l.n_argmax, stream)) return e;
   if (int e = gccnmf_tdoa_gccnmf_gated(h, l.coh, F, T, l.E, D, l.W, K, l.argmax, l.counters, gccnmf_tdoa_argmax_refine_capacity(K, T),
                                        l.counters + 1, stream))
@@ -537,10 +684,10 @@ int ll_enqueue(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l,
 }
 
 // ---------------------------------------------------------------------------------------------- entry points (P = 0: gccnmf_ll_*)
-int ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, const float* W, const double* E, const double* analysis_window,
+int ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, const float* W, const double* E, const double* analysis_window,
             const double* synthesis_weights, float gain, const float* H0, void* state, size_t state_bytes, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P);
+  LL_CARVE_OR_FAIL(l, P, Lh);
   GCCNMF_REQUIRE(h, W && E && analysis_window && synthesis_weights, "ll_init: NULL pointer");
   GCCNMF_REQUIRE(h, cfg->inference_iterations == 0 || H0 != nullptr, "ll_init: inference needs H0");
   cudaStream_t s = (cudaStream_t)stream;
@@ -570,24 +717,27 @@ int ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, const float* W
   GCCNMF_LAUNCH(h, ll_reset_kernel, l.S, 256, 0, stream, l.streams, 0, l.S, l.in_ring, l.out_ring, l.carry, l.R, P ? 0 : l.N, l.D, 1);
   if (P)
     GCCNMF_LAUNCH(h, ll_src_reset_kernel, l.S, 256, 0, stream, 0, l.S, P, l.D, l.N, l.out_ring, l.src_targets, l.src_override, l.src_status, 1);
+  // the history is zeroed by the memset above: ring, write index 0, window 0
   return GCCNMF_OK;
 }
 
-int ll_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* state, size_t state_bytes, int first, int count, void* stream) {
+int ll_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, void* state, size_t state_bytes, int first, int count,
+                     void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P);
+  LL_CARVE_OR_FAIL(l, P, Lh);
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "ll_reset_streams: streams [%d, %d + %d) outside [0, %d)", first,
                  first, count, l.S);
   GCCNMF_LAUNCH(h, ll_reset_kernel, count, 256, 0, stream, l.streams, first, count, l.in_ring, l.out_ring, l.carry, l.R, P ? 0 : l.N, l.D, 0);
   if (P)
     GCCNMF_LAUNCH(h, ll_src_reset_kernel, count, 256, 0, stream, first, count, P, l.D, l.N, l.out_ring, l.src_targets, l.src_override, l.src_status, 0);
+  if (Lh) GCCNMF_LAUNCH(h, ll_hist_reset_kernel, count, 256, 0, stream, l.hist, l.hist_stride, first, count);
   return GCCNMF_OK;
 }
 
-int ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* state, size_t state_bytes, int first, int count,
+int ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, void* state, size_t state_bytes, int first, int count,
                   const gccnmf_ll_stream_params* params_host, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P);
+  LL_CARVE_OR_FAIL(l, P, Lh);
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "ll_set_params: streams [%d, %d + %d) outside [0, %d)", first,
                  first, count, l.S);
   GCCNMF_REQUIRE(h, params_host != nullptr, "ll_set_params: NULL parameters");
@@ -605,12 +755,12 @@ int ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* st
   return GCCNMF_OK;
 }
 
-int ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* state, size_t state_bytes, int hops, float* in, float* out,
+int ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, void* state, size_t state_bytes, int hops, float* in, float* out,
                     const float* in_host, float* out_host, void** graph_exec, void* stream) {
   GCCNMF_ENTER(h);
   GCCNMF_REQUIRE(h, graph_exec != nullptr && stream != nullptr, "ll_graph_create: needs a non-default stream and an output slot");
   *graph_exec = nullptr;
-  LL_CARVE_OR_FAIL(l, P);
+  LL_CARVE_OR_FAIL(l, P, Lh);
   GCCNMF_REQUIRE(h, hops >= 1 && hops <= l.C, "ll_graph_create: hops must be in [1, %d] (got %d)", l.C, hops);
   GCCNMF_REQUIRE(h, in && out, "ll_graph_create: NULL pointer");
   if (int st = gccnmf_get_twiddles(h, l.N, nullptr, nullptr)) return st;
@@ -637,13 +787,30 @@ int ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* 
   return GCCNMF_OK;
 }
 
-int ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* state, size_t state_bytes, int hops, int what, void* dst, void* stream) {
+int ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, void* state, size_t state_bytes, int hops, int what, void* dst,
+              void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P);
+  LL_CARVE_OR_FAIL(l, P, Lh);
   GCCNMF_REQUIRE(h, dst != nullptr, "ll_export: NULL destination");
   GCCNMF_REQUIRE(h, hops >= 1 && hops <= l.C, "ll_export: hops must be in [1, %d] (got %d)", l.C, hops);
   const bool inf = cfg->inference_iterations > 0;
   const size_t T = (size_t)l.S * hops, F = l.F, K = l.K, D = l.D, Ps = P;
+  if (what >= GCCNMF_LLHIST_EXPORT_RING && what <= GCCNMF_LLHIST_EXPORT_MEANS) {
+    GCCNMF_REQUIRE(h, Lh > 0, "ll_export: item %d needs history_length > 0", what);
+    const size_t ring = D * Lh * sizeof(double);
+    cudaStream_t st = (cudaStream_t)stream;
+    switch (what) {
+      case GCCNMF_LLHIST_EXPORT_RING:
+        GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync(dst, ring, l.hist, l.hist_stride, ring, l.S, cudaMemcpyDefault, st));
+        break;
+      case GCCNMF_LLHIST_EXPORT_INDEX: case GCCNMF_LLHIST_EXPORT_WINDOWS:
+        GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync(dst, 4, l.hist + ring + (what == GCCNMF_LLHIST_EXPORT_WINDOWS ? 4 : 0), l.hist_stride, 4, l.S,
+                                               cudaMemcpyDefault, st));
+        break;
+      default: GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(dst, l.means, D * T * sizeof(double), cudaMemcpyDefault, st)); break;
+    }
+    return GCCNMF_OK;
+  }
   const void* src = nullptr;
   size_t bytes = 0;
   if (P) {   // the items of the single-target chain that this mode does not compute are refused
@@ -693,6 +860,7 @@ int ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* state,
 //   in_ring[s]        the last R samples of both channels                                            (ll_push <- ll_advance)
 //   out_ring[s]       the N-sample overlap-add ring of both channels, P of them with sources         (ll_ola_emit)
 //   src_targets[s], src_override[s], src_status[s]    (sources only)                                (ll_src_targets_kernel)
+//   hist[s]           history only: the ring, its write index, the window and 8 zero bytes          (ll_hist_means, set_window)
 // Everything else is either shared by the streams (header, windows, E, W and what init derives from it) or rewritten by every call
 // before it is read (stage, valid, X ... frames, counters).  A region is a strided array in the state: stream s's bytes are
 // [offset + s stride, + bytes), and they go to [rec_offset, + bytes) of the stream's record payload.  Rings are copied whole: their
@@ -707,9 +875,9 @@ struct RecordMap {
 constexpr size_t kRecordHeaderBytes = GCCNMF_RECORD_HEADER_BYTES;
 static_assert(sizeof(gccnmf_record_header) <= kRecordHeaderBytes, "record header");
 
-RecordMap ll_record_map(const gccnmf_ll_config& c, int P) {
+RecordMap ll_record_map(const gccnmf_ll_config& c, int P, int Lh = 0) {
   char* const base = reinterpret_cast<char*>(256);
-  const LLLayout l = ll_carve(c, P, base);
+  const LLLayout l = ll_carve(c, P, base, Lh);
   const size_t N = l.N, R = l.R, D = l.D, Pm = P > 0 ? P : 1;
   RecordMap m{};
   size_t at = 0;
@@ -727,11 +895,14 @@ RecordMap ll_record_map(const gccnmf_ll_config& c, int P) {
     add(l.src_override, kLLMaxSources * sizeof(int32_t));
     add(l.src_status, sizeof(int32_t));
   }
+  add(l.hist, l.hist_stride);            // nothing with Lh = 0: the records of gccnmf_llrec_*
   m.payload = at;
   return m;
 }
 
-size_t ll_record_bytes(const gccnmf_ll_config& c, int P) { return kRecordHeaderBytes + align_up(ll_record_map(c, P).payload, 256); }
+size_t ll_record_bytes(const gccnmf_ll_config& c, int P, int Lh = 0) {
+  return kRecordHeaderBytes + align_up(ll_record_map(c, P, Lh).payload, 256);
+}
 
 // Grid (count, regions): CTA (i, g) copies region g of stream first + i between the state and payload i of the staging buffer,
 // in 16-byte words where both ends and the length allow it (every carve region is 256-aligned; LLStream and odd ring lengths
@@ -753,19 +924,22 @@ ll_record_copy_kernel(char* __restrict__ state, int first, RecordMap m, char* __
 }
 
 // What a record must agree on, from the host arguments alone: magic, ABI version, kind, P, payload size and the configuration without
-// S and C.  The synthesis digest is left 0: see ll_synthesis_digest.
-gccnmf_record_header ll_record_header(const gccnmf_ll_config& cfg, int P) {
+// S and C, followed by the history length (0 without history, so those records are gccnmf_llrec_*'s).  The synthesis digest is left
+// 0: see ll_synthesis_digest.
+constexpr int kRecordConfigHistory = sizeof(gccnmf_ll_config) / sizeof(int32_t);    // config[9]
+gccnmf_record_header ll_record_header(const gccnmf_ll_config& cfg, int P, int Lh = 0) {
   gccnmf_record_header r{};
   r.magic = GCCNMF_RECORD_MAGIC;
   r.abi_version = GCCNMF_ABI_VERSION;
   r.kind = GCCNMF_RECORD_KIND_LL;
   r.num_sources = P;
-  r.payload_bytes = ll_record_map(cfg, P).payload;
+  r.payload_bytes = ll_record_map(cfg, P, Lh).payload;
   gccnmf_ll_config c = cfg;
   c.num_streams = 0;
   c.hops_per_call = 0;
-  static_assert(sizeof(c) <= sizeof(r.config), "record config");
+  static_assert(sizeof(c) + sizeof(int32_t) <= sizeof(r.config), "record config");
   memcpy(r.config, &c, sizeof(c));
+  r.config[kRecordConfigHistory] = Lh;
   return r;
 }
 
@@ -787,21 +961,21 @@ int ll_synthesis_digest(gccnmf_handle* h, const LLLayout& l, uint64_t* digest, v
 }
 
 #define LL_RECORD_ARGS_OR_FAIL(what)                                                                                               \
-  LL_CARVE_OR_FAIL(l, P);                                                                                                            \
+  LL_CARVE_OR_FAIL(l, P, Lh);                                                                                                        \
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, what ": streams [%d, %d + %d) outside [0, %d)", \
                  first, first, count, l.S);                                                                                          \
-  const RecordMap m = ll_record_map(*cfg, P);                                                                                        \
-  const size_t rec_bytes = ll_record_bytes(*cfg, P);                                                                                 \
+  const RecordMap m = ll_record_map(*cfg, P, Lh);                                                                                    \
+  const size_t rec_bytes = ll_record_bytes(*cfg, P, Lh);                                                                             \
   GCCNMF_REQUIRE(h, record != nullptr && record_bytes >= (size_t)count * rec_bytes, what ": record needs %zu bytes for %d streams",  \
                  (size_t)count * rec_bytes, count);                                                                                  \
   if (workspace == nullptr || workspace_bytes < (size_t)count * m.payload || ((uintptr_t)workspace & 3) != 0)                        \
     return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, what ": workspace needs %zu bytes, 4-byte aligned", (size_t)count * m.payload);
 
-int ll_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* state, size_t state_bytes, int first, int count, void* record,
+int ll_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, void* state, size_t state_bytes, int first, int count, void* record,
                     size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
   GCCNMF_ENTER(h);
   LL_RECORD_ARGS_OR_FAIL("ll_save_streams");
-  gccnmf_record_header head = ll_record_header(*cfg, P);
+  gccnmf_record_header head = ll_record_header(*cfg, P, Lh);
   if (int st = ll_synthesis_digest(h, l, &head.synthesis_digest, stream)) return st;
   for (int i = 0; i < count; ++i) memcpy((char*)record + (size_t)i * rec_bytes, &head, sizeof(head));
   GCCNMF_LAUNCH(h, ll_record_copy_kernel, dim3(count, m.n), 256, 0, stream, (char*)state, first, m, (char*)workspace, 1);
@@ -810,11 +984,11 @@ int ll_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* 
   return GCCNMF_OK;
 }
 
-int ll_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* state, size_t state_bytes, int first, int count, const void* record,
+int ll_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, void* state, size_t state_bytes, int first, int count, const void* record,
                     size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
   GCCNMF_ENTER(h);
   LL_RECORD_ARGS_OR_FAIL("ll_load_streams");
-  const gccnmf_record_header want = ll_record_header(*cfg, P);
+  const gccnmf_record_header want = ll_record_header(*cfg, P, Lh);
   for (int i = 0; i < count; ++i) {      // everything but the digest, before the device is touched
     gccnmf_record_header got;
     memcpy(&got, (const char*)record + (size_t)i * rec_bytes, sizeof(got));
@@ -823,6 +997,8 @@ int ll_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* 
                    want.abi_version);
     GCCNMF_REQUIRE(h, got.kind == want.kind, "ll_load_streams: record %d: kind %d is not a low-latency stream", i, got.kind);
     GCCNMF_REQUIRE(h, got.num_sources == P, "ll_load_streams: record %d: %d sources, this engine has %d", i, got.num_sources, P);
+    GCCNMF_REQUIRE(h, got.config[kRecordConfigHistory] == Lh, "ll_load_streams: record %d: history length %d, this engine has %d", i,
+                   got.config[kRecordConfigHistory], Lh);
     GCCNMF_REQUIRE(h, got.payload_bytes == want.payload_bytes, "ll_load_streams: record %d: payload of %llu bytes, expected %llu", i,
                    (unsigned long long)got.payload_bytes, (unsigned long long)want.payload_bytes);
     GCCNMF_REQUIRE(h, memcmp(got.config, want.config, sizeof(want.config)) == 0, "ll_load_streams: record %d: another configuration", i);
@@ -840,76 +1016,10 @@ int ll_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, void* 
   return GCCNMF_OK;
 }
 
-}  // namespace
-
-extern "C" {
-
-size_t gccnmf_ll_state_bytes(const gccnmf_ll_config* cfg) {
-  if (ll_check(nullptr, cfg, 0) != 0) return 0;
-  return ll_carve(*cfg, 0, nullptr).bytes;
-}
-
-int gccnmf_ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, const float* W, const double* E, const double* analysis_window,
-                   const double* synthesis_weights, float gain, const float* H0, void* state, size_t state_bytes, void* stream) {
-  return ll_init(h, cfg, 0, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
-}
-
-int gccnmf_ll_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int first, int count, void* stream) {
-  return ll_reset_streams(h, cfg, 0, state, state_bytes, first, count, stream);
-}
-
-int gccnmf_ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int first, int count,
-                         const gccnmf_ll_stream_params* params_host, void* stream) {
-  return ll_set_params(h, cfg, 0, state, state_bytes, first, count, params_host, stream);
-}
-
-int gccnmf_ll_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, const float* in, float* out,
-                      void* stream) {
+int ll_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, void* state, size_t state_bytes, int first, int count,
+                   const int32_t* targets_host, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, 0);
-  return ll_enqueue(h, cfg, l, hops, in, out, stream);
-}
-
-int gccnmf_ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, float* in, float* out,
-                           const float* in_host, float* out_host, void** graph_exec, void* stream) {
-  return ll_graph_create(h, cfg, 0, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
-}
-
-int gccnmf_ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, int what, void* dst, void* stream) {
-  return ll_export(h, cfg, 0, state, state_bytes, hops, what, dst, stream);
-}
-
-// ---- sources (2 <= num_sources <= 8)
-size_t gccnmf_llsep_state_bytes(const gccnmf_ll_config* cfg, int num_sources) {
-  if (num_sources == 0 || ll_check(nullptr, cfg, num_sources) != 0) return 0;
-  return ll_carve(*cfg, num_sources, nullptr).bytes;
-}
-
-int gccnmf_llsep_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, const float* W, const double* E,
-                      const double* analysis_window, const double* synthesis_weights, float gain, const float* H0, void* state,
-                      size_t state_bytes, void* stream) {
-  GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_init(h, cfg, num_sources, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
-}
-
-int gccnmf_llsep_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
-                               int count, void* stream) {
-  GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_reset_streams(h, cfg, num_sources, state, state_bytes, first, count, stream);
-}
-
-int gccnmf_llsep_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
-                            int count, const gccnmf_ll_stream_params* params_host, void* stream) {
-  GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_set_params(h, cfg, num_sources, state, state_bytes, first, count, params_host, stream);
-}
-
-int gccnmf_llsep_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
-                             int count, const int32_t* targets_host, void* stream) {
-  GCCNMF_ENTER(h);
-  GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  const int P = num_sources;
-  LL_CARVE_OR_FAIL(l, P);
+  LL_CARVE_OR_FAIL(l, P, Lh);
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "llsep_set_targets: streams [%d, %d + %d) outside [0, %d)",
                  first, first, count, l.S);
   GCCNMF_REQUIRE(h, targets_host != nullptr, "llsep_set_targets: NULL targets");
@@ -925,24 +1035,115 @@ int gccnmf_llsep_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int 
   return GCCNMF_OK;
 }
 
+int ll_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, void* state, size_t state_bytes, int first, int count,
+                  const int32_t* windows_host, void* stream) {
+  GCCNMF_ENTER(h);
+  LL_CARVE_OR_FAIL(l, P, Lh);
+  GCCNMF_REQUIRE(h, Lh > 0, "llhist_set_window: needs history_length > 0");
+  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "llhist_set_window: streams [%d, %d + %d) outside [0, %d)",
+                 first, first, count, l.S);
+  GCCNMF_REQUIRE(h, windows_host != nullptr, "llhist_set_window: NULL windows");
+  for (int i = 0; i < count; ++i)
+    GCCNMF_REQUIRE(h, windows_host[i] >= 0 && windows_host[i] <= Lh, "llhist_set_window: stream %d: window %d outside [0, %d]", first + i,
+                   windows_host[i], Lh);
+  for (int i0 = 0; i0 < count; i0 += kLLParamsPerLaunch) {
+    const int n = count - i0 < kLLParamsPerLaunch ? count - i0 : kLLParamsPerLaunch;
+    LLWindowBatch b{};
+    memcpy(b.w, windows_host + i0, (size_t)n * sizeof(int32_t));
+    GCCNMF_LAUNCH(h, ll_hist_window_kernel, 1, kLLParamsPerLaunch, 0, stream, l.hist, l.hist_stride, (size_t)l.D * Lh * sizeof(double) + 4,
+                  first + i0, n, b);
+  }
+  return GCCNMF_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t gccnmf_ll_state_bytes(const gccnmf_ll_config* cfg) {
+  if (ll_check(nullptr, cfg, 0) != 0) return 0;
+  return ll_carve(*cfg, 0, nullptr).bytes;
+}
+
+int gccnmf_ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, const float* W, const double* E, const double* analysis_window,
+                   const double* synthesis_weights, float gain, const float* H0, void* state, size_t state_bytes, void* stream) {
+  return ll_init(h, cfg, 0, 0, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
+}
+
+int gccnmf_ll_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int first, int count, void* stream) {
+  return ll_reset_streams(h, cfg, 0, 0, state, state_bytes, first, count, stream);
+}
+
+int gccnmf_ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int first, int count,
+                         const gccnmf_ll_stream_params* params_host, void* stream) {
+  return ll_set_params(h, cfg, 0, 0, state, state_bytes, first, count, params_host, stream);
+}
+
+int gccnmf_ll_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, const float* in, float* out,
+                      void* stream) {
+  GCCNMF_ENTER(h);
+  LL_CARVE_OR_FAIL(l, 0, 0);
+  return ll_enqueue(h, cfg, l, hops, in, out, stream);
+}
+
+int gccnmf_ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, float* in, float* out,
+                           const float* in_host, float* out_host, void** graph_exec, void* stream) {
+  return ll_graph_create(h, cfg, 0, 0, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
+}
+
+int gccnmf_ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, int what, void* dst, void* stream) {
+  return ll_export(h, cfg, 0, 0, state, state_bytes, hops, what, dst, stream);
+}
+
+// ---- sources (2 <= num_sources <= 8)
+size_t gccnmf_llsep_state_bytes(const gccnmf_ll_config* cfg, int num_sources) {
+  if (num_sources == 0 || ll_check(nullptr, cfg, num_sources) != 0) return 0;
+  return ll_carve(*cfg, num_sources, nullptr).bytes;
+}
+
+int gccnmf_llsep_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, const float* W, const double* E,
+                      const double* analysis_window, const double* synthesis_weights, float gain, const float* H0, void* state,
+                      size_t state_bytes, void* stream) {
+  GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
+  return ll_init(h, cfg, num_sources, 0, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
+}
+
+int gccnmf_llsep_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
+                               int count, void* stream) {
+  GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
+  return ll_reset_streams(h, cfg, num_sources, 0, state, state_bytes, first, count, stream);
+}
+
+int gccnmf_llsep_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
+                            int count, const gccnmf_ll_stream_params* params_host, void* stream) {
+  GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
+  return ll_set_params(h, cfg, num_sources, 0, state, state_bytes, first, count, params_host, stream);
+}
+
+int gccnmf_llsep_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
+                             int count, const int32_t* targets_host, void* stream) {
+  GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
+  return ll_set_targets(h, cfg, num_sources, 0, state, state_bytes, first, count, targets_host, stream);
+}
+
 int gccnmf_llsep_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int hops,
                          const float* in, float* out, void* stream) {
   GCCNMF_ENTER(h);
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  LL_CARVE_OR_FAIL(l, num_sources);
+  LL_CARVE_OR_FAIL(l, num_sources, 0);
   return ll_enqueue(h, cfg, l, hops, in, out, stream);
 }
 
 int gccnmf_llsep_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int hops,
                               float* in, float* out, const float* in_host, float* out_host, void** graph_exec, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_graph_create(h, cfg, num_sources, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
+  return ll_graph_create(h, cfg, num_sources, 0, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
 }
 
 int gccnmf_llsep_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int hops, int what,
                         void* dst, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_export(h, cfg, num_sources, state, state_bytes, hops, what, dst, stream);
+  return ll_export(h, cfg, num_sources, 0, state, state_bytes, hops, what, dst, stream);
 }
 
 // ---- stream records (0 <= num_sources <= 8)
@@ -958,12 +1159,87 @@ size_t gccnmf_llrec_workspace_bytes(const gccnmf_ll_config* cfg, int num_sources
 
 int gccnmf_llrec_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
                               int count, void* record, size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
-  return ll_save_streams(h, cfg, num_sources, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes, stream);
+  return ll_save_streams(h, cfg, num_sources, 0, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes, stream);
 }
 
 int gccnmf_llrec_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
                               int count, const void* record, size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
-  return ll_load_streams(h, cfg, num_sources, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes, stream);
+  return ll_load_streams(h, cfg, num_sources, 0, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes, stream);
+}
+
+// ---- history (0 <= num_sources <= 8, 0 <= history_length <= 1024)
+size_t gccnmf_llhist_state_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length) {
+  if (ll_check(nullptr, cfg, num_sources, history_length) != 0) return 0;
+  return ll_carve(*cfg, num_sources, nullptr, history_length).bytes;
+}
+
+int gccnmf_llhist_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, const float* W, const double* E,
+                       const double* analysis_window, const double* synthesis_weights, float gain, const float* H0, void* state,
+                       size_t state_bytes, void* stream) {
+  return ll_init(h, cfg, num_sources, history_length, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
+}
+
+int gccnmf_llhist_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
+                                size_t state_bytes, int first, int count, void* stream) {
+  return ll_reset_streams(h, cfg, num_sources, history_length, state, state_bytes, first, count, stream);
+}
+
+int gccnmf_llhist_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
+                             size_t state_bytes, int first, int count, const gccnmf_ll_stream_params* params_host, void* stream) {
+  return ll_set_params(h, cfg, num_sources, history_length, state, state_bytes, first, count, params_host, stream);
+}
+
+int gccnmf_llhist_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
+                              size_t state_bytes, int first, int count, const int32_t* targets_host, void* stream) {
+  GCCNMF_REQUIRE(h, num_sources != 0, "llhist_set_targets: needs num_sources in [2, %d] (got 0)", kLLMaxSources);
+  return ll_set_targets(h, cfg, num_sources, history_length, state, state_bytes, first, count, targets_host, stream);
+}
+
+int gccnmf_llhist_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
+                             size_t state_bytes, int first, int count, const int32_t* windows_host, void* stream) {
+  return ll_set_window(h, cfg, num_sources, history_length, state, state_bytes, first, count, windows_host, stream);
+}
+
+int gccnmf_llhist_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state, size_t state_bytes,
+                          int hops, const float* in, float* out, void* stream) {
+  GCCNMF_ENTER(h);
+  LL_CARVE_OR_FAIL(l, num_sources, history_length);
+  return ll_enqueue(h, cfg, l, hops, in, out, stream);
+}
+
+int gccnmf_llhist_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
+                               size_t state_bytes, int hops, float* in, float* out, const float* in_host, float* out_host, void** graph_exec,
+                               void* stream) {
+  return ll_graph_create(h, cfg, num_sources, history_length, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
+}
+
+int gccnmf_llhist_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state, size_t state_bytes,
+                         int hops, int what, void* dst, void* stream) {
+  return ll_export(h, cfg, num_sources, history_length, state, state_bytes, hops, what, dst, stream);
+}
+
+size_t gccnmf_llhist_record_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length) {
+  if (ll_check(nullptr, cfg, num_sources, history_length) != 0) return 0;
+  return ll_record_bytes(*cfg, num_sources, history_length);
+}
+
+size_t gccnmf_llhist_workspace_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int count) {
+  if (ll_check(nullptr, cfg, num_sources, history_length) != 0 || count < 1) return 0;
+  return (size_t)count * ll_record_map(*cfg, num_sources, history_length).payload;
+}
+
+int gccnmf_llhist_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
+                               size_t state_bytes, int first, int count, void* record, size_t record_bytes, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+  return ll_save_streams(h, cfg, num_sources, history_length, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes,
+                         stream);
+}
+
+int gccnmf_llhist_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
+                               size_t state_bytes, int first, int count, const void* record, size_t record_bytes, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+  return ll_load_streams(h, cfg, num_sources, history_length, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes,
+                         stream);
 }
 
 }  // extern "C"

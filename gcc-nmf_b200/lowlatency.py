@@ -19,12 +19,19 @@ reference's multi-target rule, gccNMFFunctions.py:94-143, per frame).  The targe
 maxima of its running maximum (held, with status bit 0, when there are fewer), or the overrides of `set_targets`; each atom goes
 to the target with the largest float32 GCC-NMF value (numpy.nanargmax), and source q is the single-target filter and synthesis fed
 that mask.  `process` then returns (S, P, 2, n).  The boxcar epsilon and the single target override play no part.
+
+Localisation window (`historyLength` = Lh in [1, 1024], `gccnmf_llhist_*`): every stream keeps the angular spectra of its last Lh
+frames in a ring.  `set_localization(streams, window)` with 1 <= window <= Lh makes a stream's target (or its P targets) follow the
+nanmean of its newest `window` frames, the real-time engine's rule, so the target follows a talker who moves and recovers from
+silent frames; window 0 (the default, and after `reset`) is the running maximum above.  With historyLength 0 the engine is the
+plain one.
 """
 import ctypes
 
 import numpy as np
 
-from ._lib import RECORD_KIND_LL, RECORD_MAGIC, LLConfig, LLStreamParams, ParameterError, RecordHeader, default_handle
+from ._lib import (LLHIST_MAX_HISTORY, LLHIST_RECORD_CONFIG_HISTORY, RECORD_KIND_LL, RECORD_MAGIC, LLConfig, LLStreamParams, ParameterError,
+                   RecordHeader, default_handle)
 
 SYNTHESIS_MODES = ('online', 'lowlatency', 'windowed')
 
@@ -33,8 +40,11 @@ EXPORT_X, EXPORT_COHERENCE, EXPORT_ANGULAR, EXPORT_ACC_MAX, EXPORT_TARGETS, EXPO
 # export items of an engine with sources (gccnmf_llsep_export); items 4 .. 10 are then refused
 EXPORT_SOURCE_TARGETS, EXPORT_SOURCE_VALUES, EXPORT_SOURCE_MASKS, EXPORT_SOURCE_WIENER, EXPORT_SOURCE_Y, EXPORT_STREAM_STATUS, \
     EXPORT_CARRIED_TARGETS, EXPORT_CALL_STATUS = range(14, 22)
+# export items of an engine with historyLength > 0 (gccnmf_llhist_export)
+EXPORT_HISTORY, EXPORT_HISTORY_INDEX, EXPORT_WINDOWS, EXPORT_WINDOW_MEANS = range(22, 26)
 STATUS_FEW_PEAKS, STATUS_ALL_NAN = 1, 2
 MAX_SOURCES = 8
+MAX_HISTORY = LLHIST_MAX_HISTORY
 
 
 def synthesisWeights(mode, synthesisWindow, hopSize):
@@ -68,10 +78,14 @@ def batchArguments(mode):
 
 class LowLatencyEngine(object):
     def __init__(self, W, expJOmegaTau, analysisWindow, synthesisWindow, hopSize, numStreams=1, hopsPerCall=1, synthesis='lowlatency',
-                 targetTDOAEpsilon=1.0, numInferenceIterations=0, sparsityAlpha=0.0, epsilon=1e-16, seedValue=0, device=0, numSources=0):
+                 targetTDOAEpsilon=1.0, numInferenceIterations=0, sparsityAlpha=0.0, epsilon=1e-16, seedValue=0, device=0, numSources=0,
+                 historyLength=0):
         self.P = int(numSources)
         if self.P != 0 and not 2 <= self.P <= MAX_SOURCES:
             raise ValueError('numSources must be 0 (one enhanced target) or in [2, %d] (got %d)' % (MAX_SOURCES, self.P))
+        self.Lh = int(historyLength)
+        if not 0 <= self.Lh <= MAX_HISTORY:
+            raise ValueError('historyLength must be in [0, %d] (got %d)' % (MAX_HISTORY, self.Lh))
         self.h = default_handle(device)
         torch = self.torch = self.h.torch
         W = np.ascontiguousarray(W, dtype=np.float32)
@@ -88,8 +102,11 @@ class LowLatencyEngine(object):
         if self.latency < 0:
             raise ValueError('the synthesis weights start less than a hop before the end of the frame')
         self.cfg = LLConfig(N, self.hop, self.C, K, self.D, self.S, int(numInferenceIterations), float(sparsityAlpha), float(epsilon))
-        self.state_bytes = int(self.h.lib.gccnmf_llsep_state_bytes(ctypes.byref(self.cfg), self.P) if self.P else
-                               self.h.lib.gccnmf_ll_state_bytes(ctypes.byref(self.cfg)))
+        if self.Lh:
+            self.state_bytes = int(self.h.lib.gccnmf_llhist_state_bytes(ctypes.byref(self.cfg), self.P, self.Lh))
+        else:
+            self.state_bytes = int(self.h.lib.gccnmf_llsep_state_bytes(ctypes.byref(self.cfg), self.P) if self.P else
+                                   self.h.lib.gccnmf_ll_state_bytes(ctypes.byref(self.cfg)))
         if self.state_bytes == 0:
             raise ValueError('invalid low-latency configuration (N a power of two in [32, 4096], 1 <= hop <= N, 1 <= hopsPerCall <= 64, '
                              'D a power of two in [4, 128], 1 <= numStreams <= 4096)')
@@ -107,6 +124,7 @@ class LowLatencyEngine(object):
         self._active = np.ones(self.S, np.int32)
         self._override = np.full(self.S, -1, np.int32)
         self._targets = np.full((self.S, max(self.P, 1)), -1, np.int32)
+        self._window = np.zeros(self.S, np.int32)
         self._io = {}
         self._graphs = {}
         self._exports = {}
@@ -127,14 +145,16 @@ class LowLatencyEngine(object):
 
     @property
     def _p(self):
-        """The num_sources argument of the gccnmf_llsep_* entries (none for gccnmf_ll_*)."""
-        return (self.P,) if self.P else ()
+        """The num_sources argument of the gccnmf_llsep_* entries, num_sources and history_length of the gccnmf_llhist_* entries (none
+        for gccnmf_ll_*)."""
+        return (self.P, self.Lh) if self.Lh else (self.P,) if self.P else ()
 
     def _fn(self, name):
-        return getattr(self.h.lib, ('gccnmf_llsep_' if self.P else 'gccnmf_ll_') + name)
+        return getattr(self.h.lib, ('gccnmf_llhist_' if self.Lh else 'gccnmf_llsep_' if self.P else 'gccnmf_ll_') + name)
 
     def _state(self, name, *args):
-        """gccnmf_ll_<name>(h, cfg, state, state_bytes, *args), or gccnmf_llsep_<name>(h, cfg, P, state, state_bytes, *args)."""
+        """gccnmf_ll_<name>(h, cfg, state, state_bytes, *args), gccnmf_llsep_<name>(h, cfg, P, state, state_bytes, *args) or
+        gccnmf_llhist_<name>(h, cfg, P, Lh, state, state_bytes, *args)."""
         self._check(self._fn(name)(self.h.h, ctypes.byref(self.cfg), *self._p, self.state.data_ptr(), self.state_bytes, *args))
 
     def _streams(self, streams):
@@ -185,6 +205,21 @@ class LowLatencyEngine(object):
         self._state('set_targets', lo, hi - lo + 1, arr.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), self.stream.cuda_stream)
         self.stream.synchronize()
 
+    def set_localization(self, streams, window):
+        """Per-stream localisation window in frames: 0 is the running maximum (the default), 1 .. historyLength the nanmean of the
+        stream's newest `window` angular spectra.  window broadcasts to len(streams)."""
+        idx = self._streams(streams)
+        w = np.broadcast_to(np.asarray(window, dtype=np.int64), idx.shape)
+        if w.min() < 0 or w.max() > self.Lh:
+            raise ValueError('window outside [0, %d] (historyLength %d)' % (self.Lh, self.Lh))
+        if not self.Lh:
+            return                                                # only window 0: the engine is the plain one
+        self._window[idx] = w
+        lo, hi = int(idx.min()), int(idx.max())
+        arr = np.ascontiguousarray(self._window[lo:hi + 1], dtype=np.int32)
+        self._state('set_window', lo, hi - lo + 1, arr.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), self.stream.cuda_stream)
+        self.stream.synchronize()
+
     def set_active(self, streams, active):
         """An inactive stream outputs zeros and its state does not change."""
         idx = self._streams(streams)
@@ -192,8 +227,10 @@ class LowLatencyEngine(object):
         self._send_streams(idx)
 
     def reset(self, streams=None):
-        """The streams start over (rings zeroed, running maximum -inf, no frames yet); their parameters stay."""
+        """The streams start over (rings zeroed, running maximum -inf, no frames yet, localisation window 0); their other
+        parameters stay."""
         idx = np.unique(self._streams(streams))
+        self._window[idx] = 0
         breaks = np.flatnonzero(np.diff(idx) != 1) + 1          # one call per contiguous run of streams
         for run in np.split(idx, breaks):
             self._state('reset_streams', int(run[0]), len(run), self.stream.cuda_stream)
@@ -263,6 +300,9 @@ class LowLatencyEngine(object):
                            EXPORT_SOURCE_WIENER: (((P, 2, F, T) if self.inference else (P, F, T)), torch.float32),
                            EXPORT_SOURCE_Y: ((P, 2, F, T), torch.complex64), EXPORT_STREAM_STATUS: ((self.S,), torch.int32),
                            EXPORT_CARRIED_TARGETS: ((self.S, P), torch.int32), EXPORT_CALL_STATUS: ((1,), torch.int32)})
+        if self.Lh:
+            shapes.update({EXPORT_HISTORY: ((self.S, D, self.Lh), torch.float64), EXPORT_HISTORY_INDEX: ((self.S,), torch.int32),
+                           EXPORT_WINDOWS: ((self.S,), torch.int32), EXPORT_WINDOW_MEANS: ((D, T), torch.float64)})
         shape, dtype = shapes[what]
         key = (what, shape)
         buf = self._exports.get(key)
@@ -272,11 +312,19 @@ class LowLatencyEngine(object):
         self.stream.synchronize()
         return buf.numpy().copy()
 
-    # ------------------------------------------------------------------ stream records (gccnmf_llrec_*)
+    # ------------------------------------------------------------------ stream records (gccnmf_llrec_*, or gccnmf_llhist_* with history)
+    def _rec(self, name):
+        """gccnmf_llrec_<name> bound to (cfg, P), or gccnmf_llhist_<name> bound to (cfg, P, Lh)."""
+        fn = getattr(self.h.lib, ('gccnmf_llhist_' if self.Lh else 'gccnmf_llrec_') + name)
+        hist = (self.Lh,) if self.Lh else ()
+        if name.endswith('_bytes'):
+            return lambda *a: fn(ctypes.byref(self.cfg), self.P, *hist, *a)
+        return lambda *a: fn(self.h.h, ctypes.byref(self.cfg), self.P, *hist, *a)
+
     @property
     def record_bytes(self):
         """Bytes of one stream's record."""
-        return int(self.h.lib.gccnmf_llrec_record_bytes(ctypes.byref(self.cfg), self.P))
+        return int(self._rec('record_bytes')())
 
     def _record_runs(self, streams):
         """(first, count, first record row) of each run of consecutive stream indexes, in the order given."""
@@ -291,12 +339,11 @@ class LowLatencyEngine(object):
     def _record_call(self, name, streams, rec):
         rb = self.record_bytes
         for first, count, row in self._record_runs(streams):
-            n = int(self.h.lib.gccnmf_llrec_workspace_bytes(ctypes.byref(self.cfg), self.P, count))
+            n = int(self._rec('workspace_bytes')(count))
             if self._staging is None or self._staging.numel() < n:
                 self._staging = self.torch.empty(n, dtype=self.torch.uint8, device=self.h.device)
-            self._check(getattr(self.h.lib, 'gccnmf_llrec_' + name)(
-                self.h.h, ctypes.byref(self.cfg), self.P, self.state.data_ptr(), self.state_bytes, first, count, rec.data[row].data_ptr(),
-                count * rb, self._staging.data_ptr(), self._staging.numel(), self.stream.cuda_stream))
+            self._check(self._rec(name)(self.state.data_ptr(), self.state_bytes, first, count, rec.data[row].data_ptr(), count * rb,
+                                        self._staging.data_ptr(), self._staging.numel(), self.stream.cuda_stream))
         self.stream.synchronize()
 
     def save_streams(self, streams=None):
@@ -304,9 +351,12 @@ class LowLatencyEngine(object):
         streams go on unchanged."""
         from .records import StreamRecord
         idx = self._streams(streams)
+        mirrors = dict(eps=self._eps[idx].copy(), active=self._active[idx].copy(), override=self._override[idx].copy(),
+                       targets=self._targets[idx].copy())
+        if self.Lh:
+            mirrors['window'] = self._window[idx].copy()
         rec = StreamRecord(RECORD_KIND_LL, self.P, self.torch.zeros((len(idx), self.record_bytes), dtype=self.torch.uint8).pin_memory(),
-                           dict(eps=self._eps[idx].copy(), active=self._active[idx].copy(), override=self._override[idx].copy(),
-                                targets=self._targets[idx].copy()))
+                           mirrors)
         self._record_call('save_streams', idx, rec)
         return rec
 
@@ -315,8 +365,9 @@ class LowLatencyEngine(object):
         cfg = LLConfig.from_buffer_copy(bytes(self.cfg))
         cfg.num_streams = cfg.hops_per_call = 0
         head = RecordHeader(magic=RECORD_MAGIC, abi_version=self.h.lib.gccnmf_abi_version(), kind=RECORD_KIND_LL, num_sources=self.P,
-                            payload_bytes=int(self.h.lib.gccnmf_llrec_workspace_bytes(ctypes.byref(self.cfg), self.P, 1)))
+                            payload_bytes=int(self._rec('workspace_bytes')(1)))
         ctypes.memmove(head.config, bytes(cfg), ctypes.sizeof(cfg))
+        head.config[LLHIST_RECORD_CONFIG_HISTORY] = self.Lh
         d = 1469598103934665603                                    # FNV-1a 64 of the weights' bytes, then the gain's
         for b in np.ascontiguousarray(self.weights, np.float64).tobytes() + np.float32(self.gain).tobytes():
             d = ((d ^ b) * 1099511628211) & 0xFFFFFFFFFFFFFFFF
@@ -325,14 +376,16 @@ class LowLatencyEngine(object):
 
     def load_streams(self, streams, record):
         """Record i replaces the state and settings of streams[i] from the next call on.  The record must come from an engine with
-        the same configuration other than numStreams and hopsPerCall, the same synthesis and numSources.  Every record is checked on
-        the host before anything is loaded, so a refusal leaves the engine and the device untouched.  Each run of consecutive
+        the same configuration other than numStreams and hopsPerCall, the same synthesis, numSources and historyLength.  Every record
+        is checked on the host before anything is loaded, so a refusal leaves the engine and the device untouched.  Each run of consecutive
         streams is one library call (one wait for the synthesis weights, one copy, one kernel)."""
         idx = self._streams(streams)
         if record.kind != RECORD_KIND_LL or record.count != len(idx):
             raise ValueError('a low-latency record of %d streams is needed (got kind %d, %d streams)' % (len(idx), record.kind, record.count))
         if record.data.shape[1] != self.record_bytes:
-            raise ParameterError('records of %d bytes do not fit this engine (%d bytes)' % (record.data.shape[1], self.record_bytes))
+            lh = record.header(0).config[LLHIST_RECORD_CONFIG_HISTORY]
+            raise ParameterError('records of %d bytes (history length %d) do not fit this engine (%d bytes, history length %d)'
+                                 % (record.data.shape[1], lh, self.record_bytes, self.Lh))
         if self._header is None:
             self._header = self._record_header()
         want = self._header
@@ -345,6 +398,8 @@ class LowLatencyEngine(object):
         self._record_call('load_streams', idx, record)
         m = record.mirrors
         self._eps[idx], self._active[idx], self._override[idx], self._targets[idx] = m['eps'], m['active'], m['override'], m['targets']
+        if self.Lh:
+            self._window[idx] = m['window']
 
     def close(self):
         if self.h.h:
@@ -360,15 +415,18 @@ class LowLatencyEngine(object):
 
 
 def streamSignals(signals, W, expJOmegaTau, analysisWindow, synthesisWindow, hopSize, hopsPerCall=1, synthesis='lowlatency',
-                  targetTDOAEpsilon=1.0, numInferenceIterations=0, use_graph=True, device=0, numSources=0, **kwargs):
+                  targetTDOAEpsilon=1.0, numInferenceIterations=0, use_graph=True, device=0, numSources=0, historyLength=0,
+                  localizationWindow=0, **kwargs):
     """Streams a list of stereo signals (2, n_i) through one engine, one stream each, hopsPerCall hops per call, and returns the
     outputs aligned with the input: out_i[..., p] = output sample p + latency (the batch function's targetEstimateSamplesOLA), each
     (2, n_i), or (P, 2, n_i) with numSources = P.  Shorter signals are followed by silence; the engine is flushed with `latency`
-    samples of silence at the end."""
+    samples of silence at the end.  historyLength / localizationWindow: every stream localises over its newest
+    localizationWindow frames (see set_localization)."""
     sig = [np.asarray(s, dtype=np.float32) for s in signals]
     eng = LowLatencyEngine(W, expJOmegaTau, analysisWindow, synthesisWindow, hopSize, numStreams=len(sig), hopsPerCall=hopsPerCall,
                            synthesis=synthesis, targetTDOAEpsilon=targetTDOAEpsilon, numInferenceIterations=numInferenceIterations,
-                           device=device, numSources=numSources, **kwargs)
+                           device=device, numSources=numSources, historyLength=historyLength, **kwargs)
+    eng.set_localization(None, localizationWindow)
     step = eng.hop * eng.C
     total = max(s.shape[1] for s in sig) + eng.latency
     total = -(-total // step) * step

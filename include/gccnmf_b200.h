@@ -672,6 +672,64 @@ GCCNMF_API int gccnmf_llrec_load_streams(gccnmf_handle* h, const gccnmf_ll_confi
                               int first, int count, const void* record, size_t record_bytes, void* workspace,
                               size_t workspace_bytes, void* stream);
 
+/* ---- localisation over a sliding window of each stream's recent frames ----------------------------------------------------------
+ * The low-latency engine of gccnmf_ll_* (num_sources 0) or gccnmf_llsep_* (2 .. 8) with a history of history_length = Lh frames per
+ * stream, 0 <= Lh <= 1024.  Every entry takes (num_sources, history_length) after the config and does what its gccnmf_ll_* /
+ * gccnmf_llsep_* namesake does; with Lh = 0 the engine, its state size, its launches and its records are those of the namesakes.
+ * - History ring: every whole frame of an active stream writes its angular spectrum column (export item 2, float64) into the
+ *   stream's (D, Lh) ring at the write index, which then moves on (mod Lh).  The running maximum and its carry advance as before,
+ *   whatever the window.  Frames before the first sample and inactive streams change nothing.  init and reset zero the ring and
+ *   set the write index and the window to 0.
+ * - Window w per stream, 0 <= w <= Lh (gccnmf_llhist_set_window; from the next call, and allowed between launches of a graph):
+ *   w = 0 keeps the running-maximum rule of the namesakes.  w >= 1: per frame, mean[d] = the nanmean of the newest w ring columns,
+ *   summed in float64 newest first, skipping NaN (NaN when all are NaN); the zero columns of a ring that has seen fewer than w
+ *   frames count in the denominator.  This is rt_localize's rule (gccnmf_rt_*).  The target is then the argmax of the mean
+ *   (numpy.argmax's order; target_override still wins), or with sources the P largest strict local maxima of the mean with the
+ *   hold rule, status bit and overrides of gccnmf_llsep_*.  After w frames without NaN, an earlier NaN no longer matters.
+ * - Export: the namesakes' items plus 22 the rings (S, D, Lh) f64, 23 the write indexes (S) i32, 24 the windows (S) i32 and 25 the
+ *   call's window means (D, T) f64 (NaN for the streams with w = 0).  Items 22 .. 25 need Lh > 0.
+ * - Records (gccnmf_llhist_record_bytes / workspace_bytes / save_streams / load_streams): gccnmf_llrec_*'s, with the ring, its
+ *   write index and the window after the other regions, and Lh in config[9] of the header; a load requires an equal Lh.  With
+ *   Lh = 0 the records are byte-identical to gccnmf_llrec_*'s, and each family loads the other's.
+ * Lh outside [0, 1024], a window outside [0, Lh], items 22 .. 25 or set_window with Lh = 0, set_targets with num_sources 0, and
+ * S D Lh at or above 2^31 fail before anything is enqueued. */
+#define GCCNMF_LLHIST_MAX_HISTORY 1024
+#define GCCNMF_LLHIST_EXPORT_RING 22
+#define GCCNMF_LLHIST_EXPORT_INDEX 23
+#define GCCNMF_LLHIST_EXPORT_WINDOWS 24
+#define GCCNMF_LLHIST_EXPORT_MEANS 25
+/* Host only; 0 for an invalid configuration, num_sources or history_length. */
+GCCNMF_API size_t gccnmf_llhist_state_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length);
+GCCNMF_API int gccnmf_llhist_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, const float* W,
+                       const double* E, const double* analysis_window, const double* synthesis_weights, float gain, const float* H0,
+                       void* state, size_t state_bytes, void* stream);
+/* Also zeroes the streams' rings and sets their write index and window to 0. */
+GCCNMF_API int gccnmf_llhist_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
+                                size_t state_bytes, int first, int count, void* stream);
+GCCNMF_API int gccnmf_llhist_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
+                             size_t state_bytes, int first, int count, const gccnmf_ll_stream_params* params_host, void* stream);
+/* num_sources >= 2 only. */
+GCCNMF_API int gccnmf_llhist_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
+                              size_t state_bytes, int first, int count, const int32_t* targets_host, void* stream);
+/* windows_host: count host int32, consumed before the call returns, each in [0, history_length]. */
+GCCNMF_API int gccnmf_llhist_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
+                             size_t state_bytes, int first, int count, const int32_t* windows_host, void* stream);
+GCCNMF_API int gccnmf_llhist_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
+                          size_t state_bytes, int hops, const float* in, float* out, void* stream);
+GCCNMF_API int gccnmf_llhist_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
+                               size_t state_bytes, int hops, float* in, float* out, const float* in_host, float* out_host,
+                               void** graph_exec, void* stream);
+GCCNMF_API int gccnmf_llhist_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
+                         size_t state_bytes, int hops, int what, void* dst, void* stream);
+GCCNMF_API size_t gccnmf_llhist_record_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length);
+GCCNMF_API size_t gccnmf_llhist_workspace_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int count);
+GCCNMF_API int gccnmf_llhist_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
+                               size_t state_bytes, int first, int count, void* record, size_t record_bytes, void* workspace,
+                               size_t workspace_bytes, void* stream);
+GCCNMF_API int gccnmf_llhist_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
+                               size_t state_bytes, int first, int count, const void* record, size_t record_bytes, void* workspace,
+                               size_t workspace_bytes, void* stream);
+
 /* ---- real-time stream records: move a live slot to another slot, engine, engine form, device or process ---------------------
  * One family for every real-time form, with the arguments of gccnmf_rtbank_*: (num_streams, num_sources, num_dictionaries,
  * num_steerings) = (1, 0, 0, 0) for gccnmf_rt_*, (S, 0, 0, 0) for gccnmf_rtm_*, (S, P, 0, 0) for gccnmf_rtsep_* and
