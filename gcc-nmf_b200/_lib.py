@@ -241,6 +241,33 @@ class RtRecordHeader(ctypes.Structure):
 RECORD_KIND_RT = 1
 RTREC_DIGEST_CHUNK_WORDS = 1024
 
+_LLBANK = [_H, _LC, c_int, c_int, c_int, _P, c_size_t]      # handle, config, num_sources, history_length, num_steerings, state, state_bytes
+SIGNATURES.update({
+    'gccnmf_llbank_state_bytes': (c_size_t, [_LC, c_int, c_int, c_int]),
+    'gccnmf_llbank_init': (c_int, [_H, _LC, c_int, c_int, c_int, _P, _P, _P, _P, c_float, _P, _P, c_size_t, _S]),
+    'gccnmf_llbank_load_steering': (c_int, _LLBANK + [c_int, _P, _S]),
+    'gccnmf_llbank_assign': (c_int, _LLBANK + [c_int, c_int, ctypes.POINTER(c_int32), _S]),
+    'gccnmf_llbank_reset_streams': (c_int, _LLBANK + [c_int, c_int, _S]),
+    'gccnmf_llbank_set_params': (c_int, _LLBANK + [c_int, c_int, ctypes.POINTER(LLStreamParams), _S]),
+    'gccnmf_llbank_set_targets': (c_int, _LLBANK + [c_int, c_int, ctypes.POINTER(c_int32), _S]),
+    'gccnmf_llbank_set_window': (c_int, _LLBANK + [c_int, c_int, ctypes.POINTER(c_int32), _S]),
+    'gccnmf_llbank_process': (c_int, _LLBANK + [c_int, _P, _P, _S]),
+    'gccnmf_llbank_graph_create': (c_int, _LLBANK + [c_int, _P, _P, _P, _P, ctypes.POINTER(c_void_p), _S]),
+    'gccnmf_llbank_export': (c_int, _LLBANK + [c_int, c_int, c_void_p, _S]),
+    'gccnmf_llbank_record_bytes': (c_size_t, [_LC, c_int, c_int, c_int]),
+    'gccnmf_llbank_workspace_bytes': (c_size_t, [_LC, c_int, c_int, c_int, c_int]),
+    'gccnmf_llbank_save_streams': (c_int, _LLBANK + [c_int, c_int, c_void_p, c_size_t, _P, c_size_t, _S]),
+    'gccnmf_llbank_load_streams': (c_int, _LLBANK + [c_int, c_int, c_void_p, c_size_t, _P, c_size_t, _S]),
+})
+LLBANK_MAX_STEERINGS = 64
+RECORD_KIND_LLBANK = 3
+
+
+class LLBankRecordHeader(ctypes.Structure):
+    """gccnmf_llbank_record_header (include/gccnmf_b200.h): RecordHeader's fields, then the content digests of the dictionary and of
+    the stream's steering table."""
+    _fields_ = RecordHeader._fields_ + [('dictionary_digest', ctypes.c_uint64), ('steering_digest', ctypes.c_uint64)]
+
 
 _lib = None
 

@@ -120,6 +120,37 @@ struct WorkspaceCarver {
   bool ok() const { return base != nullptr && used <= size; }
 };
 
+// A bank of Qe steering tables for the columns of a low-latency call (gccnmf_llbank_*): table e is E + e F D, (F, D) complex128 as
+// gccnmf_ll_init stores E, and ET + e D Fp its transpose (D, Fp), bins F .. Fp - 1 zero.  Column t = s hops + i (frame i of stream
+// s) is on table assign[s].  order lists the streams by entry, stable, and seg[e] .. seg[e + 1] are entry e's positions in it, so
+// the kernels that reuse a table row across a tile of columns take their tiles from one entry at a time (steer_tile).
+struct SteerBank {
+  const double2 *E, *ET;
+  const int32_t *assign, *order, *seg;
+  int Qe, hops;
+  int64_t Fp;
+  __device__ __forceinline__ int entry(int t) const { return __ldg(assign + t / hops); }
+  __device__ __forceinline__ int column(int u) const { return __ldg(order + u / hops) * hops + u % hops; }   // sorted position -> column
+};
+
+// Tile `cta` of the column tiles of width `tile` cut from each entry's sorted columns in turn: its entry (-1 past the last tile)
+// and sorted positions [u0, u1).  At most ceil(T / tile) + Qe - 1 tiles exist.
+__device__ __forceinline__ int steer_tile(const SteerBank& b, int tile, int cta, int& u0, int& u1) {
+  int first = 0;
+  for (int e = 0; e < b.Qe; ++e) {
+    const int c0 = __ldg(b.seg + e) * b.hops, c1 = __ldg(b.seg + e + 1) * b.hops, n = (c1 - c0 + tile - 1) / tile;
+    if (cta < first + n) {
+      u0 = c0 + (cta - first) * tile;
+      u1 = u0 + tile < c1 ? u0 + tile : c1;
+      return e;
+    }
+    first += n;
+  }
+  u0 = u1 = 0;
+  return -1;
+}
+inline int steer_tiles_max(int T, int tile, int Qe) { return (T + tile - 1) / tile + Qe; }
+
 // scipy.signal.argrelmax(x) (order 1, mode 'clip': strict local maxima, never the end points), then the S largest peaks
 // (gccNMFFunctions.py:100: peakIndexes[argsort(x[peakIndexes])[-numSources:]]) in ascending index order (:113), by every thread of
 // one CTA.  x: D values in shared memory, written before the call; peak / chosen: D bytes of shared scratch.  Thread 0 writes the

@@ -153,6 +153,110 @@ phat_angspec_kernel(const float2* __restrict__ X, int F, int T, int x_is_coheren
     }
 }
 
+// phat_angspec_kernel for a steering bank (gccnmf_llbank_*): a CTA takes 16 columns of one entry in sorted order (steer_tile), so
+// it stages one table's rows as the plain kernel stages E, and every column's sums are the plain kernel's, term for term and in the
+// same order.  Always a spectrogram pair in, coherence and angular spectrum out.
+template <int DPL, int BF>
+__global__ void __launch_bounds__(kAngWarps * 32)
+phat_angspec_bank_kernel(const float2* __restrict__ X, int F, int T, SteerBank bank, int D, float2* __restrict__ coherence,
+                         double* __restrict__ angular) {
+  constexpr int kThreads = kAngWarps * 32;
+  constexpr int kCPerThread = BF * kAngT / kThreads;
+  constexpr int kEPerThread = BF * 32 * DPL / kThreads;
+  static_assert(BF * kAngT % kThreads == 0 && BF % kAngWarps == 0, "chunk shape");
+  __shared__ double2 Cs[BF][kAngT];
+  __shared__ double2 Es[(BF > kAngT / 2 ? BF : kAngT / 2)][32 * DPL];
+  __shared__ int col_s[kAngT];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  int u0, u1;
+  const int entry = steer_tile(bank, kAngT, blockIdx.x, u0, u1);
+  if (entry < 0) return;
+  if (threadIdx.x < kAngT) col_s[threadIdx.x] = u0 + (int)threadIdx.x < u1 ? bank.column(u0 + threadIdx.x) : -1;
+  __syncthreads();
+  const double2* __restrict__ E = bank.E + (int64_t)entry * F * D;
+  double acc[kAngT][DPL];
+#pragma unroll
+  for (int tt = 0; tt < kAngT; ++tt)
+#pragma unroll
+    for (int j = 0; j < DPL; ++j) acc[tt][j] = 0.0;
+
+  float2 xa[kCPerThread], xb[kCPerThread];
+  double2 er[kEPerThread];
+  auto fetch = [&](int f0) {
+#pragma unroll
+    for (int q = 0; q < kCPerThread; ++q) {
+      const int e = threadIdx.x + q * kThreads, f = f0 + e / kAngT, t = col_s[e % kAngT];
+      xa[q] = xb[q] = float2{0.f, 0.f};
+      if (f < F && t >= 0) {
+        xa[q] = X[(int64_t)f * T + t];
+        xb[q] = X[((int64_t)F + f) * T + t];
+      }
+    }
+#pragma unroll
+    for (int q = 0; q < kEPerThread; ++q) {
+      const int e = threadIdx.x + q * kThreads, ff = e / (32 * DPL), d = e % (32 * DPL);
+      er[q] = (f0 + ff < F && d < D) ? E[(int64_t)(f0 + ff) * D + d] : double2{0.0, 0.0};
+    }
+  };
+  auto stash = [&](int f0) {
+#pragma unroll
+    for (int q = 0; q < kCPerThread; ++q) {
+      const int e = threadIdx.x + q * kThreads, ff = e / kAngT, tt = e % kAngT;
+      const int f = f0 + ff, t = col_s[tt];
+      double2 c = double2{0.0, 0.0};
+      if (f < F && t >= 0) {
+        const float2 coh = phat_coherence(xa[q], xb[q]);
+        coherence[(int64_t)f * T + t] = coh;
+        c = double2{(double)coh.x, (double)coh.y};
+      }
+      Cs[ff][tt] = c;
+    }
+#pragma unroll
+    for (int q = 0; q < kEPerThread; ++q) {
+      const int e = threadIdx.x + q * kThreads;
+      Es[e / (32 * DPL)][e % (32 * DPL)] = er[q];
+    }
+  };
+
+  fetch(0);
+  for (int f0 = 0; f0 < F; f0 += BF) {
+    stash(f0);
+    __syncthreads();
+    if (f0 + BF < F) fetch(f0 + BF);
+#pragma unroll
+    for (int i = 0; i < BF / kAngWarps; ++i) {
+      const int ff = w + kAngWarps * i;
+      double2 e[DPL];
+#pragma unroll
+      for (int j = 0; j < DPL; ++j) e[j] = Es[ff][lane + 32 * j];
+#pragma unroll
+      for (int tt = 0; tt < kAngT; ++tt) {
+        const double2 c = Cs[ff][tt];
+#pragma unroll
+        for (int j = 0; j < DPL; ++j) acc[tt][j] += c.x * e[j].x - c.y * e[j].y;   // Re(C * E)
+      }
+    }
+    __syncthreads();
+  }
+  double (*red)[32 * DPL] = reinterpret_cast<double (*)[32 * DPL]>(&Es[0][0]);
+  for (int r = 0; r < kAngWarps; ++r) {
+    if (w == r) {
+#pragma unroll
+      for (int tt = 0; tt < kAngT; ++tt)
+#pragma unroll
+        for (int j = 0; j < DPL; ++j) {
+          const int d = lane + 32 * j;
+          red[tt][d] = r == 0 ? acc[tt][j] : red[tt][d] + acc[tt][j];
+        }
+    }
+    __syncthreads();
+  }
+  for (int e = threadIdx.x; e < kAngT * D; e += blockDim.x) {
+    const int d = e / kAngT, tt = e % kAngT;
+    if (col_s[tt] >= 0) angular[(int64_t)d * T + col_s[tt]] = red[tt][d];
+  }
+}
+
 __global__ void mean_tiles_kernel(const double* __restrict__ tile_sums, int tiles, int D, int T, double* __restrict__ mean) {
   const int d = blockIdx.x * blockDim.x + threadIdx.x;
   if (d >= D) return;
@@ -191,6 +295,26 @@ struct LoadTargetGCC {  // B(n = t * P + q, k = f) = Re(coherence[f][t] * E[f][t
     if (n >= N || f >= F) return 0.0;
     const int t = n / P;
     return re_coh_steer(__ldg(coh + (int64_t)f * T + t), __ldg(E + (int64_t)f * D + __ldg(targets + n)));
+  }
+};
+
+// The two loaders above for a steering bank: column t reads the table of its stream's entry.
+struct LoadRealGCCBank {
+  static constexpr bool kContigK = false;
+  const float2* coh; SteerBank bank; int F, T, D, N;
+  __device__ double operator()(int n, int f) const {
+    if (n >= N || f >= F) return 0.0;
+    const int t = n / D, d = n - t * D;
+    return re_coh_steer(__ldg(coh + (int64_t)f * T + t), __ldg(bank.E + ((int64_t)bank.entry(t) * F + f) * D + d));
+  }
+};
+struct LoadTargetGCCBank {
+  static constexpr bool kContigK = false;
+  const float2* coh; SteerBank bank; const int32_t* targets; int F, T, D, P, N;
+  __device__ double operator()(int n, int f) const {
+    if (n >= N || f >= F) return 0.0;
+    const int t = n / P;
+    return re_coh_steer(__ldg(coh + (int64_t)f * T + t), __ldg(bank.E + ((int64_t)bank.entry(t) * F + f) * D + __ldg(targets + n)));
   }
 };
 
@@ -274,6 +398,75 @@ tdoa_gccnmf_kernel(int K, int N, int F, LoadWAtoms aload, LoadRealGCC bload, int
 template <int BN, int TN>
 __global__ void __launch_bounds__((GM / GTM) * (BN / TN))
 target_gccnmf_kernel(int K, int N, int F, LoadWAtoms aload, LoadTargetGCC bload, int T, int P, float* __restrict__ values) {
+  double acc[GTM][TN];
+  const int m0 = blockIdx.y * GM, n0 = blockIdx.x * BN;
+  gemm_simt_mainloop<double, GM, BN, GK, GTM, TN>(acc, m0, n0, F, aload, bload);
+  constexpr int TX = BN / TN;
+#pragma unroll
+  for (int i = 0; i < GTM; ++i) {
+    const int m = gemm_row<GM, GTM, TX>(m0, i);
+    if (m >= K) continue;
+#pragma unroll
+    for (int j = 0; j < TN; ++j) {
+      const int n = gemm_col<BN, TN, TX>(n0, j);
+      if (n >= N) continue;
+      const int t = n / P, q = n - t * P;
+      values[((int64_t)q * K + m) * T + t] = (float)acc[i][j];
+    }
+  }
+}
+
+// tdoa_gccnmf_kernel<true> (argmax only, optionally gated) and target_gccnmf_kernel for a steering bank: the same main loop and
+// epilogue with LoadRealGCCBank / LoadTargetGCCBank, so a column's values and decisions are the plain kernels' on its table.
+__global__ void __launch_bounds__(kGccThreads)
+tdoa_argmax_bank_kernel(int K, int N, int F, LoadWAtoms aload, LoadRealGCCBank bload, int T, int D, int32_t* __restrict__ argmax,
+                        const int32_t* __restrict__ gate, int gate_capacity, int32_t* __restrict__ ran) {
+  if (gate) {
+    if (*gate <= gate_capacity) return;
+    if (ran && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) *ran = 1;
+  }
+  double acc[GTM][GTN];
+  const int m0 = blockIdx.y * GM, n0 = blockIdx.x * GN;
+  gemm_simt_mainloop<double, GM, GN, GK, GTM, GTN>(acc, m0, n0, F, aload, bload);
+  constexpr int TX = GN / GTN;
+  const int tx = threadIdx.x % TX;
+  const int lanes = min(D / 4, TX);
+#pragma unroll
+  for (int i = 0; i < GTM; ++i) {
+    const int m = gemm_row<GM, GTM, TX>(m0, i);
+    double bv[2];
+    int bi[2];
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      const int d0 = (half * (GN / 2) + tx * (GTN / 2)) % D;
+      bv[half] = acc[i][half * (GTN / 2)];
+      bi[half] = d0;
+#pragma unroll
+      for (int j = 1; j < GTN / 2; ++j) {
+        const double v = acc[i][half * (GTN / 2) + j];
+        if (argmax_better(v, d0 + j, bv[half], bi[half])) { bv[half] = v; bi[half] = d0 + j; }
+      }
+    }
+    if (D == GN) {
+      if (argmax_better(bv[1], bi[1], bv[0], bi[0])) { bv[0] = bv[1]; bi[0] = bi[1]; }
+    }
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      if (D == GN && half == 1) break;
+      for (int o = 1; o < lanes; o <<= 1) {
+        const double ov = __shfl_xor_sync(0xffffffffu, bv[half], o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi[half], o);
+        if (argmax_better(ov, oi, bv[half], bi[half])) { bv[half] = ov; bi[half] = oi; }
+      }
+      const int n_first = n0 + half * (GN / 2) + tx * (GTN / 2);
+      if ((tx % lanes) == 0 && m < K && n_first < N) argmax[(int64_t)m * T + n_first / D] = bi[half];
+    }
+  }
+}
+
+template <int BN, int TN>
+__global__ void __launch_bounds__((GM / GTM) * (BN / TN))
+target_gccnmf_bank_kernel(int K, int N, int F, LoadWAtoms aload, LoadTargetGCCBank bload, int T, int P, float* __restrict__ values) {
   double acc[GTM][TN];
   const int m0 = blockIdx.y * GM, n0 = blockIdx.x * BN;
   gemm_simt_mainloop<double, GM, BN, GK, GTM, TN>(acc, m0, n0, F, aload, bload);
@@ -677,6 +870,57 @@ int gccnmf_target_gccnmf(gccnmf_handle* h, const float* coherence, int F, int T,
   } else {
     constexpr int kBN = 32, kTN = 4;
     auto k = target_gccnmf_kernel<kBN, kTN>;
+    GCCNMF_LAUNCH(h, k, dim3((N + kBN - 1) / kBN, mt), (GM / GTM) * (kBN / kTN), 0, stream, K, N, F, a, b, T, P, values);
+  }
+  return GCCNMF_OK;
+}
+
+// ---- steering banks (gccnmf_llbank_*): the forms above whose column t reads table bank.entry(t)
+// gccnmf_phat_angspec of a spectrogram pair into coherence and angular spectrum; the grid covers the most tiles the entries can
+// cut (fixed for a configuration, so the launch can sit in a graph whatever the assignment).
+int gccnmf_phat_angspec_bank(gccnmf_handle* h, const float* X, int F, int T, const SteerBank& bank, int D, float* coherence, double* angular,
+                             void* stream) {
+  GCCNMF_REQUIRE(h, F > 0 && T > 0 && D > 0 && X && coherence && angular && bank.Qe >= 1, "phat_angspec_bank: bad arguments");
+  if (D > kAngMaxD) return gccnmf_fail(h, GCCNMF_ERR_UNSUPPORTED, "phat_angspec_bank: numTDOAs %d > %d", D, kAngMaxD);
+  const int tiles = steer_tiles_max(T, kAngT, bank.Qe);
+  const float2* Xc = reinterpret_cast<const float2*>(X);
+  float2* Cc = reinterpret_cast<float2*>(coherence);
+  if (D <= 32) GCCNMF_LAUNCH(h, (phat_angspec_bank_kernel<1, 32>), tiles, kAngWarps * 32, 0, stream, Xc, F, T, bank, D, Cc, angular);
+  else if (D <= 64) GCCNMF_LAUNCH(h, (phat_angspec_bank_kernel<2, 16>), tiles, kAngWarps * 32, 0, stream, Xc, F, T, bank, D, Cc, angular);
+  else GCCNMF_LAUNCH(h, (phat_angspec_bank_kernel<4, 8>), tiles, kAngWarps * 32, 0, stream, Xc, F, T, bank, D, Cc, angular);
+  return GCCNMF_OK;
+}
+
+// The float64 all-TDOA argmax (gccnmf_tdoa_gccnmf's, argmax only); with `gate` the graph-safe fallback of gccnmf_tdoa_gccnmf_gated.
+int gccnmf_tdoa_gccnmf_bank(gccnmf_handle* h, const float* coherence, int F, int T, const SteerBank& bank, int D, const float* W, int K,
+                            int32_t* argmax, const int32_t* gate, int capacity, int32_t* ran, void* stream) {
+  GCCNMF_REQUIRE(h, F > 0 && T > 0 && D > 0 && K > 0 && coherence && W && argmax && bank.Qe >= 1, "tdoa_gccnmf_bank: bad arguments");
+  GCCNMF_REQUIRE(h, (int64_t)T * D < (int64_t)1 << 31, "tdoa_gccnmf_bank: T * D overflows int32");
+  if (!(is_pow2(D) && D >= 4 && D <= GN))
+    return gccnmf_fail(h, GCCNMF_ERR_UNSUPPORTED, "tdoa_gccnmf_bank: numTDOAs must be a power of two in [4, %d] (got %d)", GN, D);
+  const int N = T * D;
+  LoadWAtoms a{W, K, F};
+  LoadRealGCCBank b{reinterpret_cast<const float2*>(coherence), bank, F, T, D, N};
+  GCCNMF_LAUNCH(h, tdoa_argmax_bank_kernel, dim3((N + GN - 1) / GN, (K + GM - 1) / GM), kGccThreads, 0, stream, K, N, F, a, b, T, D, argmax, gate,
+                capacity, ran);
+  return GCCNMF_OK;
+}
+
+int gccnmf_target_gccnmf_bank(gccnmf_handle* h, const float* coherence, int F, int T, const SteerBank& bank, int D, const float* W, int K,
+                              const int32_t* targets, int P, float* values, void* stream) {
+  GCCNMF_REQUIRE(h, F > 0 && T > 0 && D > 0 && K > 0 && P > 0 && coherence && W && targets && values && bank.Qe >= 1,
+                 "target_gccnmf_bank: bad arguments");
+  GCCNMF_REQUIRE(h, (int64_t)T * P < (int64_t)1 << 31 && (int64_t)P * K * T < (int64_t)1 << 31, "target_gccnmf_bank: T x P or P x K x T overflows int32");
+  const int N = T * P;
+  LoadWAtoms a{W, K, F};
+  LoadTargetGCCBank b{reinterpret_cast<const float2*>(coherence), bank, targets, F, T, D, P, N};
+  const int mt = (K + GM - 1) / GM;
+  if ((int64_t)((N + GN - 1) / GN) * mt >= h->sm_count) {
+    auto k = target_gccnmf_bank_kernel<GN, GTN>;
+    GCCNMF_LAUNCH(h, k, dim3((N + GN - 1) / GN, mt), (GM / GTM) * (GN / GTN), 0, stream, K, N, F, a, b, T, P, values);
+  } else {
+    constexpr int kBN = 32, kTN = 4;
+    auto k = target_gccnmf_bank_kernel<kBN, kTN>;
     GCCNMF_LAUNCH(h, k, dim3((N + kBN - 1) / kBN, mt), (GM / GTM) * (kBN / kTN), 0, stream, K, N, F, a, b, T, P, values);
   }
   return GCCNMF_OK;

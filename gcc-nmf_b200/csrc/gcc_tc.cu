@@ -80,6 +80,55 @@ build_gcc_planes_kernel(const float2* __restrict__ coh, int F, int T, const doub
   }
 }
 
+// build_gcc_planes_kernel for a steering bank: a CTA takes 32 columns of one entry in sorted order (steer_tile) and reuses that
+// table's rows across them, writing each column's rows where the plain kernel writes them.
+__global__ void __launch_bounds__(256)
+build_gcc_planes_bank_kernel(const float2* __restrict__ coh, int F, int T, SteerBank bank, int D, bf16* __restrict__ G, int64_t pitch, int64_t plane) {
+  __shared__ float2 Cs[64][33];   // [f][tile column]
+  __shared__ int col_s[32];
+  int u0, u1;
+  const int entry = steer_tile(bank, 32, blockIdx.y, u0, u1);
+  if (entry < 0) return;
+  const double2* __restrict__ E = bank.E + (int64_t)entry * F * D;
+  const int f0 = blockIdx.x * 64;
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  if (threadIdx.x < 32) col_s[lane] = u0 + lane < u1 ? bank.column(u0 + lane) : -1;
+  __syncthreads();
+  for (int i = w; i < 64; i += 8) {
+    const int f = f0 + i, t = col_s[lane];
+    Cs[i][lane] = (f < F && t >= 0) ? coh[(int64_t)f * T + t] : float2{0.f, 0.f};
+  }
+  __syncthreads();
+  const int f = f0 + 2 * lane;
+  if (f >= pitch) return;
+  const int t_end = u1 - u0;
+  for (int d0 = w; d0 < D; d0 += 16) {
+    double2 e[2][2];
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        const int d = d0 + 8 * j;
+        e[j][q] = (f + q < F && d < D) ? __ldg(E + (int64_t)(f + q) * D + d) : double2{0.0, 0.0};
+      }
+    for (int tt = 0; tt < t_end; ++tt) {
+      const float2 c0 = Cs[2 * lane][tt], c1 = Cs[2 * lane + 1][tt];
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        if (d0 + 8 * j >= D) break;
+        const float g0 = (float)((double)c0.x * e[j][0].x - (double)c0.y * e[j][0].y);
+        const float g1 = (float)((double)c1.x * e[j][1].x - (double)c1.y * e[j][1].y);
+        bf16 h0, l0, h1, l1;
+        split_bf16(g0, h0, l0);
+        split_bf16(g1, h1, l1);
+        bf16* row = G + ((int64_t)col_s[tt] * D + d0 + 8 * j) * pitch + f;
+        *reinterpret_cast<__nv_bfloat162*>(row) = __nv_bfloat162(h0, h1);
+        *reinterpret_cast<__nv_bfloat162*>(row + plane) = __nv_bfloat162(l0, l1);
+      }
+    }
+  }
+}
+
 // planes[p][i] = split(src[i])  (W as it lies: (F, K) row-major = MN-major operand of the argmax GEMM, K-major of the reconstruction)
 __global__ void split_to_planes_kernel(const float* __restrict__ src, int64_t n, bf16* __restrict__ planes, int64_t plane) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -524,6 +573,82 @@ refine_candidates_kernel(const int2* __restrict__ list, const uint4* __restrict_
   }
 }
 
+// refine_candidates_kernel for a steering bank: a pair reads the transposed table of its column's entry.
+__global__ void __launch_bounds__(256)
+refine_candidates_bank_kernel(const int2* __restrict__ list, const uint4* __restrict__ candidates, const int* __restrict__ count, int capacity,
+                              const float2* __restrict__ cohT, const float* __restrict__ WT, SteerBank bank, int F, int64_t Fp, int D,
+                              int T, int32_t* __restrict__ argmax) {
+  __shared__ double re_s[8][kRefineGroup][33];     // per warp: Re(C E) of 32 bins per candidate (row padded: conflict-free reads)
+  __shared__ double w_s[8][32];                    // per warp: W of the 32 bins
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  double (*re)[33] = re_s[wib];
+  double* wv = w_s[wib];
+  const int warps = gridDim.x * (blockDim.x >> 5);
+  const int n = min(*count, capacity);
+  for (int p = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); p < n; p += warps) {
+    const int k = list[p].x, t = list[p].y;
+    const uint4 c4 = candidates[p];
+    uint32_t bits[4] = {c4.x, c4.y, c4.z, c4.w};
+    const float2* crow = cohT + (int64_t)t * Fp;
+    const float* wrow = WT + (int64_t)k * Fp;
+    const double2* ET = bank.ET + (int64_t)bank.entry(t) * D * Fp;      // the pair's table, transposed
+    double bv = 0.0;
+    int bi = -1;
+    int word = 0;
+    while (true) {
+      int ds[kRefineGroup], nd = 0;                       // the next <= 8 candidate TDOAs, ascending (warp-uniform)
+      while (nd < kRefineGroup && word < 4) {
+        if (bits[word] == 0u) { ++word; continue; }
+        const int b = __ffs(bits[word]) - 1;
+        bits[word] &= bits[word] - 1;
+        ds[nd++] = word * 32 + b;
+      }
+      if (nd == 0) break;
+      double g[kRefineGroup], w = 0.0;                    // this lane's bin of the chunk: Re(C E) per candidate, W
+      auto load = [&](int f0) {
+        const int f = f0 + lane;
+        if (f >= F) return;
+        const float2 c = crow[f];
+        w = (double)wrow[f];
+#pragma unroll
+        for (int j = 0; j < kRefineGroup; ++j)
+          if (j < nd) {
+            const double2 e = ET[(int64_t)ds[j] * Fp + f];
+            g[j] = (double)c.x * e.x - (double)c.y * e.y;
+          }
+      };
+      load(0);
+      double acc = 0.0;                                   // lane j < nd: candidate ds[j]
+      for (int f0 = 0; f0 < F; f0 += 32) {
+#pragma unroll
+        for (int j = 0; j < kRefineGroup; ++j)
+          if (j < nd) re[j][lane] = g[j];
+        wv[lane] = w;
+        __syncwarp();
+        if (f0 + 32 < F) load(f0 + 32);
+        if (lane < nd) {
+          const double* r = re[lane];
+          if (F - f0 >= 32) {
+#pragma unroll 8
+            for (int s = 0; s < 32; ++s) acc = fma(r[s], wv[s], acc);
+          } else {
+            for (int s = 0; s < F - f0; ++s) acc = fma(r[s], wv[s], acc);
+          }
+        }
+        __syncwarp();
+      }
+#pragma unroll
+      for (int j = 0; j < kRefineGroup; ++j) {            // ascending TDOAs: numpy's first-maximum rule
+        if (j < nd) {
+          const double v = __shfl_sync(0xffffffffu, acc, j);
+          if (bi < 0 || argmax_better64(v, ds[j], bv, bi)) { bv = v; bi = ds[j]; }
+        }
+      }
+    }
+    if (lane == 0 && bi >= 0) argmax[(int64_t)k * T + t] = bi;
+  }
+}
+
 // dst (cols, ld) = src (rows, cols)^T for 4-, 8- and 16-byte elements (zero in the pad columns [rows, ld))
 template <typename E>
 __global__ void transpose_pad_kernel(const E* __restrict__ src, int rows, int cols, E* __restrict__ dst, int64_t ld) {
@@ -687,6 +812,10 @@ ReconWorkspace carve_recon(void* ws, size_t bytes, int S, int F, int T, int K) {
 
 }  // namespace
 
+// gcc.cu
+int gccnmf_tdoa_gccnmf_bank(gccnmf_handle* h, const float* coherence, int F, int T, const SteerBank& bank, int D, const float* W, int K,
+                            int32_t* argmax, const int32_t* gate, int capacity, int32_t* ran, void* stream);
+
 bool gccnmf_tdoa_argmax_tc_supported(int F, int T, int D, int K) {
   const bool d_ok = D >= 8 && D <= 128 && (D & (D - 1)) == 0;          // whole frames per 256-column tile; refinement kernels: D <= 128
   return d_ok && K % 8 == 0 && K >= 64 && F >= 32 && (int64_t)T * D >= kArgmaxTile && (int64_t)T * D < ((int64_t)1 << 31);
@@ -703,20 +832,32 @@ size_t gccnmf_tdoa_argmax_workspace_bytes(int F, int T, int D, int K) {
   return argmax_workspace_bytes(F, T, D, K);
 }
 
-int gccnmf_tdoa_argmax(gccnmf_handle* h, const float* coherence, int F, int T, const double* E, int D, const float* W, int K,
+}  // extern "C"
+
+// gccnmf_tdoa_argmax, or with `bank` its form for a steering bank (E unused): only the plane build, the refinement and the float64
+// fallback read the tables; the GEMM and its epilogue see G alone.  A bank always takes the candidate refinement, over the
+// transposed tables it keeps (every refinement form gives the float64 decision).
+static int tdoa_argmax(gccnmf_handle* h, const float* coherence, int F, int T, const double* E, const SteerBank* bank, int D, const float* W, int K,
                        int32_t* argmax, int32_t* overflow_flag, void* workspace, size_t workspace_bytes, void* stream) {
   GCCNMF_ENTER(h);
-  GCCNMF_REQUIRE(h, F > 0 && T > 0 && D > 0 && K > 0 && coherence && E && W && argmax, "tdoa_argmax: bad arguments");
+  GCCNMF_REQUIRE(h, F > 0 && T > 0 && D > 0 && K > 0 && coherence && (E || bank) && W && argmax, "tdoa_argmax: bad arguments");
   if (h->force_simt_nmf || !gccnmf_tdoa_argmax_tc_supported(F, T, D, K)) {
     // exact float64 SIMT kernel: nothing to refine, and the caller must not read an unwritten counter
     if (overflow_flag) GCCNMF_CHECK_CUDA(h, cudaMemsetAsync(overflow_flag, 0, sizeof(int32_t), (cudaStream_t)stream));
+    if (bank) return gccnmf_tdoa_gccnmf_bank(h, coherence, F, T, *bank, D, W, K, argmax, nullptr, 0, nullptr, stream);
     return gccnmf_tdoa_gccnmf(h, coherence, F, T, E, D, W, K, nullptr, argmax, stream);
   }
   ArgmaxWorkspace w = carve_argmax(workspace, workspace_bytes, F, T, D, K);
   if (!w.ok) return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "tdoa_argmax workspace too small: need %zu bytes", gccnmf_tdoa_argmax_workspace_bytes(F, T, D, K));
+  GCCNMF_REQUIRE(h, !bank || bank->Fp == w.Fp, "tdoa_argmax: the bank's transposed tables have %lld bins, the workspace %lld",
+                 (long long)(bank ? bank->Fp : 0), (long long)w.Fp);
   GCCNMF_CHECK_CUDA(h, cudaMemsetAsync(w.count, 0, 16, (cudaStream_t)stream));
-  GCCNMF_LAUNCH(h, build_gcc_planes_kernel, dim3((int)((w.Fp + 63) / 64), (T + 31) / 32), 256, 0, stream,
-                reinterpret_cast<const float2*>(coherence), F, T, reinterpret_cast<const double2*>(E), D, w.Gp, w.Fp, w.plane_g);
+  if (bank)
+    GCCNMF_LAUNCH(h, build_gcc_planes_bank_kernel, dim3((int)((w.Fp + 63) / 64), steer_tiles_max(T, 32, bank->Qe)), 256, 0, stream,
+                  reinterpret_cast<const float2*>(coherence), F, T, *bank, D, w.Gp, w.Fp, w.plane_g);
+  else
+    GCCNMF_LAUNCH(h, build_gcc_planes_kernel, dim3((int)((w.Fp + 63) / 64), (T + 31) / 32), 256, 0, stream,
+                  reinterpret_cast<const float2*>(coherence), F, T, reinterpret_cast<const double2*>(E), D, w.Gp, w.Fp, w.plane_g);
   const int64_t nw = (int64_t)F * K;
   GCCNMF_LAUNCH(h, split_to_planes_kernel, (unsigned)((nw + 255) / 256), 256, 0, stream, W, nw, w.Wp, w.plane_w);
   GCCNMF_LAUNCH(h, abs_colsum_kernel, (K + 127) / 128, 128, 0, stream, W, F, K, w.colsum);
@@ -736,7 +877,14 @@ int gccnmf_tdoa_argmax(gccnmf_handle* h, const float* coherence, int F, int T, c
   } else if (int st = plane_gemm<true, false>(h, kArgmaxTile, Wmn, Gk, K, N, F, 1, false, epi, nullptr, stream, true)) {
     return st;
   }
-  if (h->argmax_refine_shared) {
+  if (bank) {
+    const dim3 tb(32, 8);
+    GCCNMF_LAUNCH(h, transpose_pad_kernel<float2>, dim3((T + 31) / 32, (int)((w.Fp + 31) / 32)), tb, 0, stream, reinterpret_cast<const float2*>(coherence), F,
+                  T, w.cohT, w.Fp);
+    GCCNMF_LAUNCH(h, transpose_pad_kernel<float>, dim3((K + 31) / 32, (int)((w.Fp + 31) / 32)), tb, 0, stream, W, F, K, w.WT, w.Fp);
+    GCCNMF_LAUNCH(h, refine_candidates_bank_kernel, h->sm_count * 8, 256, 0, stream, w.list, w.cand, w.count, w.capacity, w.cohT, w.WT, *bank, F, w.Fp, D,
+                  T, argmax);
+  } else if (h->argmax_refine_shared) {
     // candidate refinement over transposed copies (contiguous loads); argmax_refine_shared = 0 selects the all-TDOA kernels below
     const dim3 tb(32, 8);
     GCCNMF_LAUNCH(h, transpose_pad_kernel<float2>, dim3((T + 31) / 32, (int)((w.Fp + 31) / 32)), tb, 0, stream, reinterpret_cast<const float2*>(coherence), F,
@@ -757,6 +905,13 @@ int gccnmf_tdoa_argmax(gccnmf_handle* h, const float* coherence, int F, int T, c
   // (identical channels) gets there: the two central TDOAs of the symmetric grid tie in nearly every decision.
   if (overflow_flag) GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(overflow_flag, w.count, sizeof(int), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return GCCNMF_OK;
+}
+
+extern "C" {
+
+int gccnmf_tdoa_argmax(gccnmf_handle* h, const float* coherence, int F, int T, const double* E, int D, const float* W, int K,
+                       int32_t* argmax, int32_t* overflow_flag, void* workspace, size_t workspace_bytes, void* stream) {
+  return tdoa_argmax(h, coherence, F, T, E, nullptr, D, W, K, argmax, overflow_flag, workspace, workspace_bytes, stream);
 }
 
 size_t gccnmf_masked_recon_workspace_bytes(int S, int F, int T, int K) {
@@ -788,3 +943,16 @@ int gccnmf_masked_recon_planes(gccnmf_handle* h, const float* masks, const float
 }
 
 }  // extern "C"
+
+// gccnmf_tdoa_argmax for a steering bank (gccnmf_llbank_*): the same workspace, bank.Fp = (F + 7) & ~7.
+int gccnmf_tdoa_argmax_bank(gccnmf_handle* h, const float* coherence, int F, int T, const SteerBank& bank, int D, const float* W, int K,
+                            int32_t* argmax, int32_t* overflow_flag, void* workspace, size_t workspace_bytes, void* stream) {
+  return tdoa_argmax(h, coherence, F, T, nullptr, &bank, D, W, K, argmax, overflow_flag, workspace, workspace_bytes, stream);
+}
+
+// ET (D, Fp) = E (F, D)^T, complex128, bins F .. Fp - 1 zero: the transposed table a bank's refinement reads.
+int gccnmf_steering_transpose(gccnmf_handle* h, const double* E, int F, int D, double* ET, int64_t Fp, void* stream) {
+  GCCNMF_LAUNCH(h, transpose_pad_kernel<double2>, dim3((D + 31) / 32, (int)((Fp + 31) / 32)), dim3(32, 8), 0, stream, reinterpret_cast<const double2*>(E), F,
+                D, reinterpret_cast<double2*>(ET), Fp);
+  return GCCNMF_OK;
+}

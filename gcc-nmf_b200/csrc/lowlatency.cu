@@ -33,6 +33,8 @@
 // the running maximum as above, every valid frame's angular column into the stream's (D, Lh) ring, and for a stream on window
 // w >= 1 the nanmean of its newest w columns in place of the running maximum (rt_localize's rule).  With Lh = 0 nothing changes.
 #include <cmath>
+#include <cstddef>
+#include <vector>
 
 #include "common.cuh"
 
@@ -43,6 +45,15 @@ int gccnmf_tdoa_gccnmf_gated(gccnmf_handle* h, const float* coherence, int F, in
                              int32_t* argmax, const int32_t* gate, int capacity, int32_t* ran, void* stream);
 int gccnmf_target_gccnmf(gccnmf_handle* h, const float* coherence, int F, int T, const double* E, int D, const float* W, int K,
                          const int32_t* targets, int P, float* values, void* stream);
+int gccnmf_phat_angspec_bank(gccnmf_handle* h, const float* X, int F, int T, const SteerBank& bank, int D, float* coherence, double* angular,
+                             void* stream);
+int gccnmf_tdoa_argmax_bank(gccnmf_handle* h, const float* coherence, int F, int T, const SteerBank& bank, int D, const float* W, int K,
+                            int32_t* argmax, int32_t* overflow_flag, void* workspace, size_t workspace_bytes, void* stream);
+int gccnmf_tdoa_gccnmf_bank(gccnmf_handle* h, const float* coherence, int F, int T, const SteerBank& bank, int D, const float* W, int K,
+                            int32_t* argmax, const int32_t* gate, int capacity, int32_t* ran, void* stream);
+int gccnmf_target_gccnmf_bank(gccnmf_handle* h, const float* coherence, int F, int T, const SteerBank& bank, int D, const float* W, int K,
+                              const int32_t* targets, int P, float* values, void* stream);
+int gccnmf_steering_transpose(gccnmf_handle* h, const double* E, int F, int D, double* ET, int64_t Fp, void* stream);
 
 namespace {
 
@@ -81,12 +92,20 @@ struct LLLayout {
   size_t hist_stride;
   char* hist;
   double* means;
+  // steering bank (gccnmf_llbank_*, Qe >= 1): E holds Qe tables (F, D) at a stride of 2 F D doubles; appended last, their
+  // transposes ET (Qe, D, Fp) complex128 for the argmax refinement, the stream -> entry assignment (S), the streams sorted by entry
+  // (S) and each entry's first position in that order (Qe + 1)
+  int Qe;
+  int64_t Fp;
+  double* ET;
+  int32_t *assign, *order, *seg;
 };
 
 bool is_pow2(int x) { return x > 0 && (x & (x - 1)) == 0; }
 constexpr int kLLMaxSources = 8;
 constexpr int kLLInferMaxSmem = 227 * 1024;   // the H100's opt-in dynamic shared memory per block
 constexpr int kLLMaxHistory = 1024;
+constexpr int kLLMaxSteerings = 64;
 
 int ll_check(gccnmf_handle* h, const gccnmf_ll_config* cfg) {
   GCCNMF_REQUIRE(h, cfg != nullptr, "ll: NULL config");
@@ -126,7 +145,14 @@ int ll_check(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh) {
   return 0;
 }
 
-LLLayout ll_carve(const gccnmf_ll_config& c, int P, void* base, int Lh = 0) {
+// Qe = 0: no bank (gccnmf_llhist_*); 1 <= Qe <= 64: a bank of Qe steering tables (gccnmf_llbank_*)
+int ll_check(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe) {
+  if (int st = ll_check(h, cfg, P, Lh)) return st;
+  GCCNMF_REQUIRE(h, Qe >= 0 && Qe <= kLLMaxSteerings, "llbank: num_steerings must be in [0, %d] (got %d)", kLLMaxSteerings, Qe);
+  return 0;
+}
+
+LLLayout ll_carve(const gccnmf_ll_config& c, int P, void* base, int Lh = 0, int Qe = 0) {
   WorkspaceCarver w(base ? base : reinterpret_cast<void*>(256), base ? ~size_t(0) >> 1 : ~size_t(0) >> 1);
   LLLayout l{};
   l.S = c.num_streams; l.N = c.window_size; l.hop = c.hop_size; l.C = c.hops_per_call; l.K = c.num_atoms; l.D = c.num_tdoas;
@@ -140,7 +166,7 @@ LLLayout ll_carve(const gccnmf_ll_config& c, int P, void* base, int Lh = 0) {
   l.counters = w.take<int32_t>(4);
   l.win_a = w.take<double>(N);
   l.w_syn = w.take<double>(N);
-  l.E = w.take<double>(2 * F * D);
+  l.E = w.take<double>((Qe ? Qe : 1) * 2 * F * D);
   l.W = w.take<float>(F * K);
   l.WT = w.take<float>(inf ? K * F : 0);
   l.colsumW = w.take<float>(inf ? K : 0);
@@ -178,15 +204,26 @@ LLLayout ll_carve(const gccnmf_ll_config& c, int P, void* base, int Lh = 0) {
   l.hist_stride = Lh ? D * Lh * sizeof(double) + 16 : 0;
   l.hist = w.take<char>(S * l.hist_stride);
   l.means = w.take<double>(Lh ? D * T : 0);
+  // bank: appended last (nothing is taken with Qe = 0, so the layouts above are unchanged)
+  l.Qe = Qe;
+  l.Fp = (F + 7) & ~size_t(7);                 // gccnmf_tdoa_argmax's padded bin count
+  l.ET = w.take<double>(Qe ? Qe * 2 * D * l.Fp : 0);
+  l.assign = w.take<int32_t>(Qe ? S : 0);
+  l.order = w.take<int32_t>(Qe ? S : 0);
+  l.seg = w.take<int32_t>(Qe ? Qe + 1 : 0);
   l.bytes = align_up(w.used, 256);
   return l;
 }
 
-#define LL_CARVE_OR_FAIL(l, P, Lh)                                                                                   \
-  if (int st__ = ll_check(h, cfg, P, Lh)) return st__;                                                               \
+#define LL_CARVE_OR_FAIL(l, P, Lh, Qe)                                                                               \
+  if (int st__ = ll_check(h, cfg, P, Lh, Qe)) return st__;                                                           \
   GCCNMF_REQUIRE(h, state != nullptr, "ll: NULL state");                                                             \
-  const LLLayout l = ll_carve(*cfg, P, state, Lh);                                                                   \
+  const LLLayout l = ll_carve(*cfg, P, state, Lh, Qe);                                                               \
   if (state_bytes < l.bytes) return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "ll: state too small: need %zu bytes", l.bytes);
+
+SteerBank ll_bank(const LLLayout& l, int hops) {
+  return SteerBank{reinterpret_cast<const double2*>(l.E), reinterpret_cast<const double2*>(l.ET), l.assign, l.order, l.seg, l.Qe, hops, l.Fp};
+}
 
 // ---------------------------------------------------------------------------------------------- kernels
 __global__ void ll_reset_kernel(LLStream* streams, int first, int count, float* in_ring, float* out_ring, double* carry, int R, int N, int D,
@@ -455,6 +492,43 @@ __global__ void ll_hist_window_kernel(char* __restrict__ hist, size_t hist_strid
   *reinterpret_cast<int32_t*>(hist + (size_t)(first + i) * hist_stride + window_offset) = b.w[i];
 }
 
+// Bank: stable counting sort of the S streams by entry, by one warp over chunks of 32 streams: order lists the streams of entry 0
+// in stream order, then those of entry 1, ...; seg[e] is entry e's first position and seg[Qe] = S.
+__global__ void __launch_bounds__(32) ll_sort_streams_kernel(const int32_t* __restrict__ assign, int S, int Qe, int32_t* __restrict__ order,
+                                                            int32_t* __restrict__ seg) {
+  __shared__ int base[kLLMaxSteerings];
+  const int lane = threadIdx.x;
+  for (int i = lane; i < Qe; i += 32) base[i] = 0;
+  __syncwarp();
+  for (int pass = 0; pass < 2; ++pass) {               // 0: count per entry, 1: place
+    for (int s0 = 0; s0 < S; s0 += 32) {
+      const int s = s0 + lane;
+      const int e = s < S ? assign[s] : -1;
+      const unsigned peers = __match_any_sync(0xffffffffu, e);
+      const bool leader = lane == __ffs(peers) - 1;
+      if (pass == 1 && e >= 0) order[base[e] + __popc(peers & ((1u << lane) - 1u))] = s;
+      __syncwarp();
+      if (leader && e >= 0) base[e] += __popc(peers);
+      __syncwarp();
+    }
+    if (pass == 0 && lane == 0)                        // counts -> first positions
+      for (int i = 0, sum = 0; i < Qe; ++i) {
+        const int n = base[i];
+        base[i] = seg[i] = sum;
+        sum += n;
+      }
+    __syncwarp();
+  }
+  if (lane == 0) seg[Qe] = S;
+}
+
+struct LLAssignBatch { int32_t e[kLLParamsPerLaunch]; };
+
+// Bank: streams [first, first + count) onto the entries of the batch, or all of them onto entry 0 (set_zero: init, reset).
+__global__ void ll_assign_kernel(int32_t* __restrict__ assign, int first, int count, LLAssignBatch b, int set_zero) {
+  for (int i = threadIdx.x; i < count; i += blockDim.x) assign[first + i] = set_zero ? 0 : b.e[i];
+}
+
 // mask[k][t] = |argmax[k][t] - target[t]| < epsilon of t's stream   (atom_mask_kernel mode 0)
 __global__ void ll_mask_kernel(const LLStream* __restrict__ streams, const int32_t* __restrict__ argmax, const int32_t* __restrict__ targets, int K,
                                int T, int hops, float* __restrict__ mask) {
@@ -622,7 +696,11 @@ int ll_enqueue_sources(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLa
   else
     GCCNMF_LAUNCH(h, ll_src_targets_kernel, S, 128, 0, stream, l.streams, l.ang, l.valid, D, hops, T, P, l.carry, l.acc, l.src_targets,
                   l.src_override, l.src_status, l.col_targets);
-  if (int e = gccnmf_target_gccnmf(h, l.coh, F, T, l.E, D, l.W, K, l.col_targets, P, l.values, stream)) return e;
+  if (l.Qe) {
+    if (int e = gccnmf_target_gccnmf_bank(h, l.coh, F, T, ll_bank(l, hops), D, l.W, K, l.col_targets, P, l.values, stream)) return e;
+  } else if (int e = gccnmf_target_gccnmf(h, l.coh, F, T, l.E, D, l.W, K, l.col_targets, P, l.values, stream)) {
+    return e;
+  }
   if (int e = gccnmf_coeff_mask(h, l.values, P, K, T, l.src_mask, l.counters + 2, stream)) return e;
   const size_t KT = (size_t)K * T, FT = (size_t)F * T;
   if (inf) {
@@ -655,17 +733,29 @@ int ll_enqueue(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l,
   GCCNMF_LAUNCH(h, ll_push_kernel, dim3(S, 2), 256, 0, stream, l.streams, in, l.in_ring, S, l.R, n, hops, before_first, l.stage, l.valid);
   const int64_t Lseg = (int64_t)l.R + n;
   if (int e = gccnmf_stft_segments(h, l.stage, (int64_t)S * Lseg, 2, S, hops, Lseg, l.win_a, N, hop, 0, l.X, inf ? l.V : nullptr, stream)) return e;
-  if (int e = gccnmf_phat_angspec(h, l.X, F, T, 0, l.E, D, l.coh, l.ang, nullptr, nullptr, 0, stream)) return e;
+  if (l.Qe) {
+    if (int e = gccnmf_phat_angspec_bank(h, l.X, F, T, ll_bank(l, hops), D, l.coh, l.ang, stream)) return e;
+  } else if (int e = gccnmf_phat_angspec(h, l.X, F, T, 0, l.E, D, l.coh, l.ang, nullptr, nullptr, 0, stream)) {
+    return e;
+  }
   if (l.P) return ll_enqueue_sources(h, cfg, l, hops, out, stream);
   if (l.Lh)
     GCCNMF_LAUNCH(h, ll_hist_targets_kernel, S, 128, 0, stream, l.streams, l.ang, l.valid, D, hops, T, l.carry, l.acc, l.hist, l.hist_stride, l.Lh,
                   l.means, l.targets);
   else
     GCCNMF_LAUNCH(h, ll_targets_kernel, S, 128, 0, stream, l.streams, l.ang, l.valid, D, hops, T, l.carry, l.acc, l.targets);
-  if (int e = gccnmf_tdoa_argmax(h, l.coh, F, T, l.E, D, l.W, K, l.argmax, l.counters, l.ws_argmax, l.n_argmax, stream)) return e;
-  if (int e = gccnmf_tdoa_gccnmf_gated(h, l.coh, F, T, l.E, D, l.W, K, l.argmax, l.counters, gccnmf_tdoa_argmax_refine_capacity(K, T),
-                                       l.counters + 1, stream))
-    return e;
+  if (l.Qe) {
+    const SteerBank b = ll_bank(l, hops);
+    if (int e = gccnmf_tdoa_argmax_bank(h, l.coh, F, T, b, D, l.W, K, l.argmax, l.counters, l.ws_argmax, l.n_argmax, stream)) return e;
+    if (int e = gccnmf_tdoa_gccnmf_bank(h, l.coh, F, T, b, D, l.W, K, l.argmax, l.counters, gccnmf_tdoa_argmax_refine_capacity(K, T),
+                                        l.counters + 1, stream))
+      return e;
+  } else {
+    if (int e = gccnmf_tdoa_argmax(h, l.coh, F, T, l.E, D, l.W, K, l.argmax, l.counters, l.ws_argmax, l.n_argmax, stream)) return e;
+    if (int e = gccnmf_tdoa_gccnmf_gated(h, l.coh, F, T, l.E, D, l.W, K, l.argmax, l.counters, gccnmf_tdoa_argmax_refine_capacity(K, T),
+                                         l.counters + 1, stream))
+      return e;
+  }
   const int64_t KT = (int64_t)K * T;
   GCCNMF_LAUNCH(h, ll_mask_kernel, (unsigned)((KT + 255) / 256), 256, 0, stream, l.streams, l.argmax, l.targets, K, T, hops, l.mask);
   if (inf) {
@@ -684,10 +774,10 @@ int ll_enqueue(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l,
 }
 
 // ---------------------------------------------------------------------------------------------- entry points (P = 0: gccnmf_ll_*)
-int ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, const float* W, const double* E, const double* analysis_window,
+int ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, const float* W, const double* E, const double* analysis_window,
             const double* synthesis_weights, float gain, const float* H0, void* state, size_t state_bytes, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P, Lh);
+  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
   GCCNMF_REQUIRE(h, W && E && analysis_window && synthesis_weights, "ll_init: NULL pointer");
   GCCNMF_REQUIRE(h, cfg->inference_iterations == 0 || H0 != nullptr, "ll_init: inference needs H0");
   cudaStream_t s = (cudaStream_t)stream;
@@ -706,7 +796,11 @@ int ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, const 
   GCCNMF_CHECK_CUDA(h, cudaMemsetAsync(state, 0, l.bytes, s));
   GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.win_a, analysis_window, (size_t)l.N * sizeof(double), cudaMemcpyDeviceToDevice, s));
   GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.w_syn, synthesis_weights, (size_t)l.N * sizeof(double), cudaMemcpyDeviceToDevice, s));
-  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.E, E, (size_t)2 * l.F * l.D * sizeof(double), cudaMemcpyDeviceToDevice, s));
+  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.E, E, (size_t)(Qe ? Qe : 1) * 2 * l.F * l.D * sizeof(double), cudaMemcpyDeviceToDevice, s));
+  for (int j = 0; j < Qe; ++j)
+    if (int st = gccnmf_steering_transpose(h, l.E + (size_t)j * 2 * l.F * l.D, l.F, l.D, l.ET + (size_t)j * 2 * l.D * l.Fp, l.Fp, stream)) return st;
+  // with a bank every stream is on entry 0 (the memset above): sorted in stream order
+  if (Qe) GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
   GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.W, W, (size_t)l.F * l.K * sizeof(float), cudaMemcpyDeviceToDevice, s));
   if (cfg->inference_iterations > 0) {
     GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.H0, H0, (size_t)l.K * 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
@@ -721,23 +815,27 @@ int ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, const 
   return GCCNMF_OK;
 }
 
-int ll_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, void* state, size_t state_bytes, int first, int count,
+int ll_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int first, int count,
                      void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P, Lh);
+  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "ll_reset_streams: streams [%d, %d + %d) outside [0, %d)", first,
                  first, count, l.S);
   GCCNMF_LAUNCH(h, ll_reset_kernel, count, 256, 0, stream, l.streams, first, count, l.in_ring, l.out_ring, l.carry, l.R, P ? 0 : l.N, l.D, 0);
   if (P)
     GCCNMF_LAUNCH(h, ll_src_reset_kernel, count, 256, 0, stream, first, count, P, l.D, l.N, l.out_ring, l.src_targets, l.src_override, l.src_status, 0);
   if (Lh) GCCNMF_LAUNCH(h, ll_hist_reset_kernel, count, 256, 0, stream, l.hist, l.hist_stride, first, count);
+  if (Qe) {
+    GCCNMF_LAUNCH(h, ll_assign_kernel, 1, 256, 0, stream, l.assign, first, count, LLAssignBatch{}, 1);
+    GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
+  }
   return GCCNMF_OK;
 }
 
-int ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, void* state, size_t state_bytes, int first, int count,
+int ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int first, int count,
                   const gccnmf_ll_stream_params* params_host, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P, Lh);
+  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "ll_set_params: streams [%d, %d + %d) outside [0, %d)", first,
                  first, count, l.S);
   GCCNMF_REQUIRE(h, params_host != nullptr, "ll_set_params: NULL parameters");
@@ -755,12 +853,12 @@ int ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, 
   return GCCNMF_OK;
 }
 
-int ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, void* state, size_t state_bytes, int hops, float* in, float* out,
+int ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int hops, float* in, float* out,
                     const float* in_host, float* out_host, void** graph_exec, void* stream) {
   GCCNMF_ENTER(h);
   GCCNMF_REQUIRE(h, graph_exec != nullptr && stream != nullptr, "ll_graph_create: needs a non-default stream and an output slot");
   *graph_exec = nullptr;
-  LL_CARVE_OR_FAIL(l, P, Lh);
+  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
   GCCNMF_REQUIRE(h, hops >= 1 && hops <= l.C, "ll_graph_create: hops must be in [1, %d] (got %d)", l.C, hops);
   GCCNMF_REQUIRE(h, in && out, "ll_graph_create: NULL pointer");
   if (int st = gccnmf_get_twiddles(h, l.N, nullptr, nullptr)) return st;
@@ -787,14 +885,19 @@ int ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh
   return GCCNMF_OK;
 }
 
-int ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, void* state, size_t state_bytes, int hops, int what, void* dst,
+int ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int hops, int what, void* dst,
               void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P, Lh);
+  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
   GCCNMF_REQUIRE(h, dst != nullptr, "ll_export: NULL destination");
   GCCNMF_REQUIRE(h, hops >= 1 && hops <= l.C, "ll_export: hops must be in [1, %d] (got %d)", l.C, hops);
   const bool inf = cfg->inference_iterations > 0;
   const size_t T = (size_t)l.S * hops, F = l.F, K = l.K, D = l.D, Ps = P;
+  if (what == GCCNMF_LLBANK_EXPORT_ASSIGNMENT) {
+    GCCNMF_REQUIRE(h, Qe > 0, "ll_export: item %d needs num_steerings > 0", what);
+    GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(dst, l.assign, (size_t)l.S * sizeof(int32_t), cudaMemcpyDefault, (cudaStream_t)stream));
+    return GCCNMF_OK;
+  }
   if (what >= GCCNMF_LLHIST_EXPORT_RING && what <= GCCNMF_LLHIST_EXPORT_MEANS) {
     GCCNMF_REQUIRE(h, Lh > 0, "ll_export: item %d needs history_length > 0", what);
     const size_t ring = D * Lh * sizeof(double);
@@ -875,9 +978,10 @@ struct RecordMap {
 constexpr size_t kRecordHeaderBytes = GCCNMF_RECORD_HEADER_BYTES;
 static_assert(sizeof(gccnmf_record_header) <= kRecordHeaderBytes, "record header");
 
-RecordMap ll_record_map(const gccnmf_ll_config& c, int P, int Lh = 0) {
+// A bank (Qe >= 1) moves the regions' offsets in the state (E holds Qe tables), not the payload.
+RecordMap ll_record_map(const gccnmf_ll_config& c, int P, int Lh = 0, int Qe = 0) {
   char* const base = reinterpret_cast<char*>(256);
-  const LLLayout l = ll_carve(c, P, base, Lh);
+  const LLLayout l = ll_carve(c, P, base, Lh, Qe);
   const size_t N = l.N, R = l.R, D = l.D, Pm = P > 0 ? P : 1;
   RecordMap m{};
   size_t at = 0;
@@ -927,11 +1031,13 @@ ll_record_copy_kernel(char* __restrict__ state, int first, RecordMap m, char* __
 // S and C, followed by the history length (0 without history, so those records are gccnmf_llrec_*'s).  The synthesis digest is left
 // 0: see ll_synthesis_digest.
 constexpr int kRecordConfigHistory = sizeof(gccnmf_ll_config) / sizeof(int32_t);    // config[9]
-gccnmf_record_header ll_record_header(const gccnmf_ll_config& cfg, int P, int Lh = 0) {
+// With a bank (Qe >= 1) the kind is GCCNMF_RECORD_KIND_LLBANK and a gccnmf_llbank_record_header follows the same fields with the
+// content digests of the dictionary and of the stream's steering table.
+gccnmf_record_header ll_record_header(const gccnmf_ll_config& cfg, int P, int Lh = 0, int Qe = 0) {
   gccnmf_record_header r{};
   r.magic = GCCNMF_RECORD_MAGIC;
   r.abi_version = GCCNMF_ABI_VERSION;
-  r.kind = GCCNMF_RECORD_KIND_LL;
+  r.kind = Qe ? GCCNMF_RECORD_KIND_LLBANK : GCCNMF_RECORD_KIND_LL;
   r.num_sources = P;
   r.payload_bytes = ll_record_map(cfg, P, Lh).payload;
   gccnmf_ll_config c = cfg;
@@ -960,36 +1066,138 @@ int ll_synthesis_digest(gccnmf_handle* h, const LLLayout& l, uint64_t* digest, v
   return GCCNMF_OK;
 }
 
+// ---- bank records: content digests (GCCNMF_RTREC_DIGEST_*, the real-time records' function, restated) of item 0, the dictionary
+// (W (F, K) f32 then, with inference, H0 (K, 2) f32), and items 1 .. Qe, the steering tables as stored ((F, D) complex128).  The
+// workspace holds the records' payloads, then one chunk digest per 1024-word chunk of each item, then the 1 + Qe item digests.
+static_assert(offsetof(gccnmf_llbank_record_header, config) == offsetof(gccnmf_record_header, config), "shared prefix");
+static_assert(sizeof(gccnmf_llbank_record_header) <= kRecordHeaderBytes, "record header");
+constexpr int kDigestChunk = GCCNMF_RTREC_DIGEST_CHUNK_WORDS;
+struct LLDigestItems {
+  const uint32_t *W, *H0, *E;
+  size_t nw, nh, ne;                       // words of W, of H0 (0 without inference) and of one table
+  int Qe, cd, ce;                          // chunks of the dictionary and of one table
+};
+
+LLDigestItems ll_digest_items(const LLLayout& l, bool inf) {
+  LLDigestItems d;
+  d.W = reinterpret_cast<const uint32_t*>(l.W);
+  d.H0 = reinterpret_cast<const uint32_t*>(l.H0);
+  d.E = reinterpret_cast<const uint32_t*>(l.E);
+  d.nw = (size_t)l.F * l.K;
+  d.nh = inf ? (size_t)2 * l.K : 0;
+  d.ne = (size_t)4 * l.F * l.D;
+  d.Qe = l.Qe;
+  d.cd = (int)((d.nw + d.nh + kDigestChunk - 1) / kDigestChunk);
+  d.ce = (int)((d.ne + kDigestChunk - 1) / kDigestChunk);
+  return d;
+}
+
+// The workspace of `count` records: payloads, then (bank only) chunk digests and item digests, each 256-aligned.
+size_t ll_record_workspace_bytes(const gccnmf_ll_config& c, int P, int Lh, int Qe, int count) {
+  const size_t payloads = (size_t)count * ll_record_map(c, P, Lh).payload;
+  if (!Qe) return payloads;
+  const LLDigestItems d = ll_digest_items(ll_carve(c, P, nullptr, Lh, Qe), c.inference_iterations > 0);
+  return align_up(payloads, 256) + align_up((size_t)(d.cd + Qe * d.ce) * sizeof(uint64_t), 256) + (size_t)(1 + Qe) * sizeof(uint64_t);
+}
+
+__device__ __forceinline__ uint64_t ll_fnv(uint64_t h, uint32_t w) { return (h ^ w) * GCCNMF_RTREC_DIGEST_PRIME; }
+
+__device__ __forceinline__ void ll_digest_item(const LLDigestItems& d, int item, const uint32_t*& a, size_t& na, const uint32_t*& b, size_t& nb) {
+  if (item == 0) {
+    a = d.W; na = d.nw; b = d.H0; nb = d.nh;
+  } else {
+    a = d.E + (size_t)(item - 1) * d.ne; na = d.ne; b = nullptr; nb = 0;
+  }
+}
+
+// One thread per chunk: FNV-1a 64 over the chunk's words.
+__global__ void __launch_bounds__(128) ll_digest_chunks_kernel(LLDigestItems d, uint64_t* __restrict__ chunks) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= d.cd + d.Qe * d.ce) return;
+  const int item = t < d.cd ? 0 : 1 + (t - d.cd) / d.ce, j = t < d.cd ? t : (t - d.cd) % d.ce;
+  const uint32_t *a, *b;
+  size_t na, nb;
+  ll_digest_item(d, item, a, na, b, nb);
+  const size_t n = na + nb, w0 = (size_t)j * kDigestChunk, w1 = w0 + kDigestChunk < n ? w0 + kDigestChunk : n;
+  uint64_t h = GCCNMF_RTREC_DIGEST_BASIS;
+  for (size_t w = w0; w < (w1 < na ? w1 : na); ++w) h = ll_fnv(h, __ldg(a + w));
+  for (size_t w = w0 > na ? w0 : na; w < w1; ++w) h = ll_fnv(h, __ldg(b + (w - na)));
+  chunks[t] = h;
+}
+
+// One thread per item: FNV-1a 64 over (n_lo, n_hi, c_0 lo, c_0 hi, ...).
+__global__ void __launch_bounds__(128) ll_digest_fold_kernel(LLDigestItems d, const uint64_t* __restrict__ chunks, uint64_t* __restrict__ digest) {
+  const int item = blockIdx.x * blockDim.x + threadIdx.x;
+  if (item > d.Qe) return;
+  const size_t n = item == 0 ? d.nw + d.nh : d.ne;
+  const int c0 = item == 0 ? 0 : d.cd + (item - 1) * d.ce, nc = item == 0 ? d.cd : d.ce;
+  uint64_t h = ll_fnv(ll_fnv(GCCNMF_RTREC_DIGEST_BASIS, (uint32_t)n), (uint32_t)(n >> 32));
+  for (int j = 0; j < nc; ++j) {
+    const uint64_t c = chunks[c0 + j];
+    h = ll_fnv(ll_fnv(h, (uint32_t)c), (uint32_t)(c >> 32));
+  }
+  digest[item] = h;
+}
+
+// The dictionary digest and the Qe table digests of this state (digest[0], digest[1 ..]) into the workspace and back to the host, with
+// the entries of streams [first, first + count) when `entries` is not NULL: one wait on the stream.
+int ll_bank_digests(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l, int count, char* workspace, int first, uint64_t* digest,
+                    int32_t* entries, void* stream) {
+  const LLDigestItems d = ll_digest_items(l, cfg->inference_iterations > 0);
+  uint64_t* chunks = reinterpret_cast<uint64_t*>(workspace + align_up((size_t)count * ll_record_map(*cfg, l.P, l.Lh).payload, 256));
+  uint64_t* dev = chunks + align_up((size_t)(d.cd + l.Qe * d.ce) * sizeof(uint64_t), 256) / sizeof(uint64_t);
+  const int chunk_count = d.cd + l.Qe * d.ce;
+  GCCNMF_LAUNCH(h, ll_digest_chunks_kernel, (chunk_count + 127) / 128, 128, 0, stream, d, chunks);
+  GCCNMF_LAUNCH(h, ll_digest_fold_kernel, (l.Qe + 1 + 127) / 128, 128, 0, stream, d, chunks, dev);
+  cudaStream_t s = (cudaStream_t)stream;
+  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(digest, dev, (size_t)(1 + l.Qe) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+  if (entries) GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(entries, l.assign + first, (size_t)count * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  GCCNMF_CHECK_CUDA(h, cudaStreamSynchronize(s));
+  return GCCNMF_OK;
+}
+
 #define LL_RECORD_ARGS_OR_FAIL(what)                                                                                               \
-  LL_CARVE_OR_FAIL(l, P, Lh);                                                                                                        \
+  LL_CARVE_OR_FAIL(l, P, Lh, Qe);                                                                                                        \
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, what ": streams [%d, %d + %d) outside [0, %d)", \
                  first, first, count, l.S);                                                                                          \
-  const RecordMap m = ll_record_map(*cfg, P, Lh);                                                                                    \
+  const RecordMap m = ll_record_map(*cfg, P, Lh, Qe);                                                                                \
   const size_t rec_bytes = ll_record_bytes(*cfg, P, Lh);                                                                             \
   GCCNMF_REQUIRE(h, record != nullptr && record_bytes >= (size_t)count * rec_bytes, what ": record needs %zu bytes for %d streams",  \
                  (size_t)count * rec_bytes, count);                                                                                  \
-  if (workspace == nullptr || workspace_bytes < (size_t)count * m.payload || ((uintptr_t)workspace & 3) != 0)                        \
-    return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, what ": workspace needs %zu bytes, 4-byte aligned", (size_t)count * m.payload);
+  const size_t ws_need = ll_record_workspace_bytes(*cfg, P, Lh, Qe, count);                                                          \
+  if (workspace == nullptr || workspace_bytes < ws_need || ((uintptr_t)workspace & (Qe ? 7 : 3)) != 0)                               \
+    return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, what ": workspace needs %zu bytes, %d-byte aligned", ws_need, Qe ? 8 : 4);
 
-int ll_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, void* state, size_t state_bytes, int first, int count, void* record,
+int ll_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int first, int count, void* record,
                     size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
   GCCNMF_ENTER(h);
   LL_RECORD_ARGS_OR_FAIL("ll_save_streams");
-  gccnmf_record_header head = ll_record_header(*cfg, P, Lh);
+  gccnmf_record_header head = ll_record_header(*cfg, P, Lh, Qe);
   if (int st = ll_synthesis_digest(h, l, &head.synthesis_digest, stream)) return st;
   for (int i = 0; i < count; ++i) memcpy((char*)record + (size_t)i * rec_bytes, &head, sizeof(head));
+  if (Qe) {                              // the bank header: the dictionary's digest and that of each stream's table
+    uint64_t digest[1 + kLLMaxSteerings];
+    std::vector<int32_t> entries(count);
+    const int st = ll_bank_digests(h, cfg, l, count, (char*)workspace, first, digest, entries.data(), stream);
+    for (int i = 0; i < count && st == GCCNMF_OK; ++i) {
+      gccnmf_llbank_record_header* r = reinterpret_cast<gccnmf_llbank_record_header*>((char*)record + (size_t)i * rec_bytes);
+      r->dictionary_digest = digest[0];
+      r->steering_digest = digest[1 + entries[i]];
+    }
+    if (st) return st;
+  }
   GCCNMF_LAUNCH(h, ll_record_copy_kernel, dim3(count, m.n), 256, 0, stream, (char*)state, first, m, (char*)workspace, 1);
   GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync((char*)record + kRecordHeaderBytes, rec_bytes, workspace, m.payload, m.payload, count,
                                          cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   return GCCNMF_OK;
 }
 
-int ll_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, void* state, size_t state_bytes, int first, int count, const void* record,
+int ll_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int first, int count, const void* record,
                     size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
   GCCNMF_ENTER(h);
   LL_RECORD_ARGS_OR_FAIL("ll_load_streams");
-  const gccnmf_record_header want = ll_record_header(*cfg, P, Lh);
-  for (int i = 0; i < count; ++i) {      // everything but the digest, before the device is touched
+  const gccnmf_record_header want = ll_record_header(*cfg, P, Lh, Qe);
+  for (int i = 0; i < count; ++i) {      // everything but the digests, before the device is touched
     gccnmf_record_header got;
     memcpy(&got, (const char*)record + (size_t)i * rec_bytes, sizeof(got));
     GCCNMF_REQUIRE(h, got.magic == want.magic, "ll_load_streams: record %d: not a stream record (magic 0x%08x)", i, got.magic);
@@ -1010,16 +1218,42 @@ int ll_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh
     memcpy(&got, (const char*)record + (size_t)i * rec_bytes, sizeof(got));
     GCCNMF_REQUIRE(h, got.synthesis_digest == digest, "ll_load_streams: record %d: other synthesis weights or gain", i);
   }
+  // bank: the same dictionary, and the lowest entry whose table has the record's content (only the read-only digest kernels have run
+  // when this refuses)
+  std::vector<int32_t> entries(Qe ? count : 0);
+  if (Qe) {
+    uint64_t bank[1 + kLLMaxSteerings];
+    if (int st = ll_bank_digests(h, cfg, l, count, (char*)workspace, first, bank, nullptr, stream)) return st;
+    for (int i = 0; i < count; ++i) {
+      gccnmf_llbank_record_header got;
+      memcpy(&got, (const char*)record + (size_t)i * rec_bytes, sizeof(got));
+      GCCNMF_REQUIRE(h, got.dictionary_digest == bank[0], "ll_load_streams: record %d: another dictionary", i);
+      int e = -1;
+      for (int j = Qe - 1; j >= 0; --j)
+        if (bank[1 + j] == got.steering_digest) e = j;
+      GCCNMF_REQUIRE(h, e >= 0, "ll_load_streams: record %d: no steering entry of this engine has the stream's table", i);
+      entries[i] = e;
+    }
+  }
   GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync(workspace, m.payload, (const char*)record + kRecordHeaderBytes, rec_bytes, m.payload, count,
                                          cudaMemcpyHostToDevice, (cudaStream_t)stream));
   GCCNMF_LAUNCH(h, ll_record_copy_kernel, dim3(count, m.n), 256, 0, stream, (char*)state, first, m, (char*)workspace, 0);
+  if (Qe) {
+    for (int i0 = 0; i0 < count; i0 += kLLParamsPerLaunch) {
+      const int n = count - i0 < kLLParamsPerLaunch ? count - i0 : kLLParamsPerLaunch;
+      LLAssignBatch b{};
+      memcpy(b.e, entries.data() + i0, (size_t)n * sizeof(int32_t));
+      GCCNMF_LAUNCH(h, ll_assign_kernel, 1, kLLParamsPerLaunch, 0, stream, l.assign, first + i0, n, b, 0);
+    }
+    GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
+  }
   return GCCNMF_OK;
 }
 
-int ll_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, void* state, size_t state_bytes, int first, int count,
+int ll_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int first, int count,
                    const int32_t* targets_host, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P, Lh);
+  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "llsep_set_targets: streams [%d, %d + %d) outside [0, %d)",
                  first, first, count, l.S);
   GCCNMF_REQUIRE(h, targets_host != nullptr, "llsep_set_targets: NULL targets");
@@ -1035,10 +1269,10 @@ int ll_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh,
   return GCCNMF_OK;
 }
 
-int ll_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, void* state, size_t state_bytes, int first, int count,
+int ll_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int first, int count,
                   const int32_t* windows_host, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P, Lh);
+  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
   GCCNMF_REQUIRE(h, Lh > 0, "llhist_set_window: needs history_length > 0");
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "llhist_set_window: streams [%d, %d + %d) outside [0, %d)",
                  first, first, count, l.S);
@@ -1056,6 +1290,38 @@ int ll_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, 
   return GCCNMF_OK;
 }
 
+// Bank: table j <- E (F, D) complex128 on the device, and its transpose; stream-ordered, from the next call on.
+int ll_load_steering(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int entry,
+                     const double* E, void* stream) {
+  GCCNMF_ENTER(h);
+  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
+  GCCNMF_REQUIRE(h, entry >= 0 && entry < Qe, "llbank_load_steering: entry %d outside [0, %d)", entry, Qe);
+  GCCNMF_REQUIRE(h, E != nullptr, "llbank_load_steering: NULL table");
+  double* dst = l.E + (size_t)entry * 2 * l.F * l.D;
+  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(dst, E, (size_t)2 * l.F * l.D * sizeof(double), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return gccnmf_steering_transpose(h, dst, l.F, l.D, l.ET + (size_t)entry * 2 * l.D * l.Fp, l.Fp, stream);
+}
+
+// Bank: streams [first, first + count) onto entries_host[0 .. count), then the streams sorted again; stream-ordered.
+int ll_assign(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int first, int count,
+              const int32_t* entries_host, void* stream) {
+  GCCNMF_ENTER(h);
+  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
+  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "llbank_assign: streams [%d, %d + %d) outside [0, %d)", first,
+                 first, count, l.S);
+  GCCNMF_REQUIRE(h, entries_host != nullptr, "llbank_assign: NULL entries");
+  for (int i = 0; i < count; ++i)
+    GCCNMF_REQUIRE(h, entries_host[i] >= 0 && entries_host[i] < Qe, "llbank_assign: stream %d: entry %d outside [0, %d)", first + i, entries_host[i], Qe);
+  for (int i0 = 0; i0 < count; i0 += kLLParamsPerLaunch) {
+    const int n = count - i0 < kLLParamsPerLaunch ? count - i0 : kLLParamsPerLaunch;
+    LLAssignBatch b{};
+    memcpy(b.e, entries_host + i0, (size_t)n * sizeof(int32_t));
+    GCCNMF_LAUNCH(h, ll_assign_kernel, 1, kLLParamsPerLaunch, 0, stream, l.assign, first + i0, n, b, 0);
+  }
+  GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
+  return GCCNMF_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1067,32 +1333,32 @@ size_t gccnmf_ll_state_bytes(const gccnmf_ll_config* cfg) {
 
 int gccnmf_ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, const float* W, const double* E, const double* analysis_window,
                    const double* synthesis_weights, float gain, const float* H0, void* state, size_t state_bytes, void* stream) {
-  return ll_init(h, cfg, 0, 0, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
+  return ll_init(h, cfg, 0, 0, 0, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
 }
 
 int gccnmf_ll_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int first, int count, void* stream) {
-  return ll_reset_streams(h, cfg, 0, 0, state, state_bytes, first, count, stream);
+  return ll_reset_streams(h, cfg, 0, 0, 0, state, state_bytes, first, count, stream);
 }
 
 int gccnmf_ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int first, int count,
                          const gccnmf_ll_stream_params* params_host, void* stream) {
-  return ll_set_params(h, cfg, 0, 0, state, state_bytes, first, count, params_host, stream);
+  return ll_set_params(h, cfg, 0, 0, 0, state, state_bytes, first, count, params_host, stream);
 }
 
 int gccnmf_ll_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, const float* in, float* out,
                       void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, 0, 0);
+  LL_CARVE_OR_FAIL(l, 0, 0, 0);
   return ll_enqueue(h, cfg, l, hops, in, out, stream);
 }
 
 int gccnmf_ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, float* in, float* out,
                            const float* in_host, float* out_host, void** graph_exec, void* stream) {
-  return ll_graph_create(h, cfg, 0, 0, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
+  return ll_graph_create(h, cfg, 0, 0, 0, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
 }
 
 int gccnmf_ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, int what, void* dst, void* stream) {
-  return ll_export(h, cfg, 0, 0, state, state_bytes, hops, what, dst, stream);
+  return ll_export(h, cfg, 0, 0, 0, state, state_bytes, hops, what, dst, stream);
 }
 
 // ---- sources (2 <= num_sources <= 8)
@@ -1105,45 +1371,45 @@ int gccnmf_llsep_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sou
                       const double* analysis_window, const double* synthesis_weights, float gain, const float* H0, void* state,
                       size_t state_bytes, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_init(h, cfg, num_sources, 0, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
+  return ll_init(h, cfg, num_sources, 0, 0, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
 }
 
 int gccnmf_llsep_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
                                int count, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_reset_streams(h, cfg, num_sources, 0, state, state_bytes, first, count, stream);
+  return ll_reset_streams(h, cfg, num_sources, 0, 0, state, state_bytes, first, count, stream);
 }
 
 int gccnmf_llsep_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
                             int count, const gccnmf_ll_stream_params* params_host, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_set_params(h, cfg, num_sources, 0, state, state_bytes, first, count, params_host, stream);
+  return ll_set_params(h, cfg, num_sources, 0, 0, state, state_bytes, first, count, params_host, stream);
 }
 
 int gccnmf_llsep_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
                              int count, const int32_t* targets_host, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_set_targets(h, cfg, num_sources, 0, state, state_bytes, first, count, targets_host, stream);
+  return ll_set_targets(h, cfg, num_sources, 0, 0, state, state_bytes, first, count, targets_host, stream);
 }
 
 int gccnmf_llsep_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int hops,
                          const float* in, float* out, void* stream) {
   GCCNMF_ENTER(h);
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  LL_CARVE_OR_FAIL(l, num_sources, 0);
+  LL_CARVE_OR_FAIL(l, num_sources, 0, 0);
   return ll_enqueue(h, cfg, l, hops, in, out, stream);
 }
 
 int gccnmf_llsep_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int hops,
                               float* in, float* out, const float* in_host, float* out_host, void** graph_exec, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_graph_create(h, cfg, num_sources, 0, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
+  return ll_graph_create(h, cfg, num_sources, 0, 0, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
 }
 
 int gccnmf_llsep_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int hops, int what,
                         void* dst, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_export(h, cfg, num_sources, 0, state, state_bytes, hops, what, dst, stream);
+  return ll_export(h, cfg, num_sources, 0, 0, state, state_bytes, hops, what, dst, stream);
 }
 
 // ---- stream records (0 <= num_sources <= 8)
@@ -1159,12 +1425,12 @@ size_t gccnmf_llrec_workspace_bytes(const gccnmf_ll_config* cfg, int num_sources
 
 int gccnmf_llrec_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
                               int count, void* record, size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
-  return ll_save_streams(h, cfg, num_sources, 0, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes, stream);
+  return ll_save_streams(h, cfg, num_sources, 0, 0, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes, stream);
 }
 
 int gccnmf_llrec_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
                               int count, const void* record, size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
-  return ll_load_streams(h, cfg, num_sources, 0, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes, stream);
+  return ll_load_streams(h, cfg, num_sources, 0, 0, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes, stream);
 }
 
 // ---- history (0 <= num_sources <= 8, 0 <= history_length <= 1024)
@@ -1176,46 +1442,46 @@ size_t gccnmf_llhist_state_bytes(const gccnmf_ll_config* cfg, int num_sources, i
 int gccnmf_llhist_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, const float* W, const double* E,
                        const double* analysis_window, const double* synthesis_weights, float gain, const float* H0, void* state,
                        size_t state_bytes, void* stream) {
-  return ll_init(h, cfg, num_sources, history_length, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
+  return ll_init(h, cfg, num_sources, history_length, 0, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
 }
 
 int gccnmf_llhist_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
                                 size_t state_bytes, int first, int count, void* stream) {
-  return ll_reset_streams(h, cfg, num_sources, history_length, state, state_bytes, first, count, stream);
+  return ll_reset_streams(h, cfg, num_sources, history_length, 0, state, state_bytes, first, count, stream);
 }
 
 int gccnmf_llhist_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
                              size_t state_bytes, int first, int count, const gccnmf_ll_stream_params* params_host, void* stream) {
-  return ll_set_params(h, cfg, num_sources, history_length, state, state_bytes, first, count, params_host, stream);
+  return ll_set_params(h, cfg, num_sources, history_length, 0, state, state_bytes, first, count, params_host, stream);
 }
 
 int gccnmf_llhist_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
                               size_t state_bytes, int first, int count, const int32_t* targets_host, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llhist_set_targets: needs num_sources in [2, %d] (got 0)", kLLMaxSources);
-  return ll_set_targets(h, cfg, num_sources, history_length, state, state_bytes, first, count, targets_host, stream);
+  return ll_set_targets(h, cfg, num_sources, history_length, 0, state, state_bytes, first, count, targets_host, stream);
 }
 
 int gccnmf_llhist_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
                              size_t state_bytes, int first, int count, const int32_t* windows_host, void* stream) {
-  return ll_set_window(h, cfg, num_sources, history_length, state, state_bytes, first, count, windows_host, stream);
+  return ll_set_window(h, cfg, num_sources, history_length, 0, state, state_bytes, first, count, windows_host, stream);
 }
 
 int gccnmf_llhist_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state, size_t state_bytes,
                           int hops, const float* in, float* out, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, num_sources, history_length);
+  LL_CARVE_OR_FAIL(l, num_sources, history_length, 0);
   return ll_enqueue(h, cfg, l, hops, in, out, stream);
 }
 
 int gccnmf_llhist_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
                                size_t state_bytes, int hops, float* in, float* out, const float* in_host, float* out_host, void** graph_exec,
                                void* stream) {
-  return ll_graph_create(h, cfg, num_sources, history_length, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
+  return ll_graph_create(h, cfg, num_sources, history_length, 0, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
 }
 
 int gccnmf_llhist_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state, size_t state_bytes,
                          int hops, int what, void* dst, void* stream) {
-  return ll_export(h, cfg, num_sources, history_length, state, state_bytes, hops, what, dst, stream);
+  return ll_export(h, cfg, num_sources, history_length, 0, state, state_bytes, hops, what, dst, stream);
 }
 
 size_t gccnmf_llhist_record_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length) {
@@ -1231,15 +1497,100 @@ size_t gccnmf_llhist_workspace_bytes(const gccnmf_ll_config* cfg, int num_source
 int gccnmf_llhist_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
                                size_t state_bytes, int first, int count, void* record, size_t record_bytes, void* workspace,
                                size_t workspace_bytes, void* stream) {
-  return ll_save_streams(h, cfg, num_sources, history_length, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes,
+  return ll_save_streams(h, cfg, num_sources, history_length, 0, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes,
                          stream);
 }
 
 int gccnmf_llhist_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
                                size_t state_bytes, int first, int count, const void* record, size_t record_bytes, void* workspace,
                                size_t workspace_bytes, void* stream) {
-  return ll_load_streams(h, cfg, num_sources, history_length, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes,
+  return ll_load_streams(h, cfg, num_sources, history_length, 0, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes,
                          stream);
+}
+
+// ---- steering bank (0 <= num_sources <= 8, 0 <= history_length <= 1024, 0 <= num_steerings <= 64)
+size_t gccnmf_llbank_state_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings) {
+  if (ll_check(nullptr, cfg, num_sources, history_length, num_steerings) != 0) return 0;
+  return ll_carve(*cfg, num_sources, nullptr, history_length, num_steerings).bytes;
+}
+
+int gccnmf_llbank_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, const float* W,
+                       const double* E, const double* analysis_window, const double* synthesis_weights, float gain, const float* H0, void* state,
+                       size_t state_bytes, void* stream) {
+  return ll_init(h, cfg, num_sources, history_length, num_steerings, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
+}
+
+int gccnmf_llbank_load_steering(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
+                                size_t state_bytes, int entry, const double* E, void* stream) {
+  return ll_load_steering(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, entry, E, stream);
+}
+
+int gccnmf_llbank_assign(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
+                         size_t state_bytes, int first, int count, const int32_t* entries_host, void* stream) {
+  return ll_assign(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, first, count, entries_host, stream);
+}
+
+int gccnmf_llbank_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
+                                size_t state_bytes, int first, int count, void* stream) {
+  return ll_reset_streams(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, first, count, stream);
+}
+
+int gccnmf_llbank_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
+                             size_t state_bytes, int first, int count, const gccnmf_ll_stream_params* params_host, void* stream) {
+  return ll_set_params(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, first, count, params_host, stream);
+}
+
+int gccnmf_llbank_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
+                              size_t state_bytes, int first, int count, const int32_t* targets_host, void* stream) {
+  GCCNMF_REQUIRE(h, num_sources != 0, "llbank_set_targets: needs num_sources in [2, %d] (got 0)", kLLMaxSources);
+  return ll_set_targets(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, first, count, targets_host, stream);
+}
+
+int gccnmf_llbank_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
+                             size_t state_bytes, int first, int count, const int32_t* windows_host, void* stream) {
+  return ll_set_window(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, first, count, windows_host, stream);
+}
+
+int gccnmf_llbank_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
+                          size_t state_bytes, int hops, const float* in, float* out, void* stream) {
+  GCCNMF_ENTER(h);
+  LL_CARVE_OR_FAIL(l, num_sources, history_length, num_steerings);
+  return ll_enqueue(h, cfg, l, hops, in, out, stream);
+}
+
+int gccnmf_llbank_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
+                               size_t state_bytes, int hops, float* in, float* out, const float* in_host, float* out_host, void** graph_exec,
+                               void* stream) {
+  return ll_graph_create(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
+}
+
+int gccnmf_llbank_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
+                         size_t state_bytes, int hops, int what, void* dst, void* stream) {
+  return ll_export(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, hops, what, dst, stream);
+}
+
+size_t gccnmf_llbank_record_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings) {
+  if (ll_check(nullptr, cfg, num_sources, history_length, num_steerings) != 0) return 0;
+  return ll_record_bytes(*cfg, num_sources, history_length);
+}
+
+size_t gccnmf_llbank_workspace_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, int count) {
+  if (ll_check(nullptr, cfg, num_sources, history_length, num_steerings) != 0 || count < 1) return 0;
+  return ll_record_workspace_bytes(*cfg, num_sources, history_length, num_steerings, count);
+}
+
+int gccnmf_llbank_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
+                               size_t state_bytes, int first, int count, void* record, size_t record_bytes, void* workspace, size_t workspace_bytes,
+                               void* stream) {
+  return ll_save_streams(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, first, count, record, record_bytes, workspace,
+                         workspace_bytes, stream);
+}
+
+int gccnmf_llbank_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
+                               size_t state_bytes, int first, int count, const void* record, size_t record_bytes, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+  return ll_load_streams(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, first, count, record, record_bytes, workspace,
+                         workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -25,13 +25,18 @@ frames in a ring.  `set_localization(streams, window)` with 1 <= window <= Lh ma
 nanmean of its newest `window` frames, the real-time engine's rule, so the target follows a talker who moves and recovers from
 silent frames; window 0 (the default, and after `reset`) is the running maximum above.  With historyLength 0 the engine is the
 plain one.
+
+Steering bank (`expJOmegaTau` a sequence of Qe tables, 1 <= Qe <= 64, `gccnmf_llbank_*`): each stream is on one table, its
+client's microphone spacing; `assign_steering(streams, entries)` moves streams between tables and `load_steering(entry, E)` replaces
+a table, both from the next call on and keeping everything else of the streams.  A stream on table j computes, bit for bit, what an
+engine built with that table alone computes.  `init` and `reset` put streams on table 0.
 """
 import ctypes
 
 import numpy as np
 
-from ._lib import (LLHIST_MAX_HISTORY, LLHIST_RECORD_CONFIG_HISTORY, RECORD_KIND_LL, RECORD_MAGIC, LLConfig, LLStreamParams, ParameterError,
-                   RecordHeader, default_handle)
+from ._lib import (LLBANK_MAX_STEERINGS, LLHIST_MAX_HISTORY, LLHIST_RECORD_CONFIG_HISTORY, RECORD_KIND_LL, RECORD_KIND_LLBANK, RECORD_MAGIC,
+                   LLConfig, LLStreamParams, ParameterError, RecordHeader, default_handle)
 
 SYNTHESIS_MODES = ('online', 'lowlatency', 'windowed')
 
@@ -42,9 +47,11 @@ EXPORT_SOURCE_TARGETS, EXPORT_SOURCE_VALUES, EXPORT_SOURCE_MASKS, EXPORT_SOURCE_
     EXPORT_CARRIED_TARGETS, EXPORT_CALL_STATUS = range(14, 22)
 # export items of an engine with historyLength > 0 (gccnmf_llhist_export)
 EXPORT_HISTORY, EXPORT_HISTORY_INDEX, EXPORT_WINDOWS, EXPORT_WINDOW_MEANS = range(22, 26)
+EXPORT_ASSIGNMENT = 26                                          # an engine with a steering bank (gccnmf_llbank_export)
 STATUS_FEW_PEAKS, STATUS_ALL_NAN = 1, 2
 MAX_SOURCES = 8
 MAX_HISTORY = LLHIST_MAX_HISTORY
+MAX_STEERINGS = LLBANK_MAX_STEERINGS
 
 
 def synthesisWeights(mode, synthesisWindow, hopSize):
@@ -86,15 +93,22 @@ class LowLatencyEngine(object):
         self.Lh = int(historyLength)
         if not 0 <= self.Lh <= MAX_HISTORY:
             raise ValueError('historyLength must be in [0, %d] (got %d)' % (MAX_HISTORY, self.Lh))
+        # a sequence of tables (or a (Qe, F, D) array) is a steering bank; one (F, D) table is the plain engine
+        bank = isinstance(expJOmegaTau, (list, tuple)) or np.ndim(expJOmegaTau) == 3
+        self.Qe = len(expJOmegaTau) if bank else 0
+        if bank and not 1 <= self.Qe <= MAX_STEERINGS:
+            raise ValueError('a steering bank holds 1 .. %d tables (got %d)' % (MAX_STEERINGS, self.Qe))
+        if bank and len({np.shape(e) for e in expJOmegaTau}) != 1:
+            raise ValueError('the tables of a steering bank must all be (F, D)')
         self.h = default_handle(device)
         torch = self.torch = self.h.torch
         W = np.ascontiguousarray(W, dtype=np.float32)
-        E = np.ascontiguousarray(expJOmegaTau, dtype=np.complex128)
+        E = np.ascontiguousarray(np.stack(list(expJOmegaTau)) if bank else expJOmegaTau, dtype=np.complex128)
         F, K = W.shape
         N = len(analysisWindow)
-        if N != 2 * (F - 1) or E.shape[0] != F or len(synthesisWindow) != N:
+        if N != 2 * (F - 1) or E.shape[-2] != F or len(synthesisWindow) != N:
             raise ValueError('W (F, K), expJOmegaTau (F, D) and the windows (N = 2 (F - 1)) do not agree')
-        self.F, self.K, self.N, self.D = F, K, N, E.shape[1]
+        self.F, self.K, self.N, self.D = F, K, N, E.shape[-1]
         self.hop, self.S, self.C = int(hopSize), int(numStreams), int(hopsPerCall)
         self.synthesis = synthesis
         self.weights, self.gain = synthesisWeights(synthesis, synthesisWindow, self.hop)
@@ -102,7 +116,9 @@ class LowLatencyEngine(object):
         if self.latency < 0:
             raise ValueError('the synthesis weights start less than a hop before the end of the frame')
         self.cfg = LLConfig(N, self.hop, self.C, K, self.D, self.S, int(numInferenceIterations), float(sparsityAlpha), float(epsilon))
-        if self.Lh:
+        if self.Qe:
+            self.state_bytes = int(self.h.lib.gccnmf_llbank_state_bytes(ctypes.byref(self.cfg), self.P, self.Lh, self.Qe))
+        elif self.Lh:
             self.state_bytes = int(self.h.lib.gccnmf_llhist_state_bytes(ctypes.byref(self.cfg), self.P, self.Lh))
         else:
             self.state_bytes = int(self.h.lib.gccnmf_llsep_state_bytes(ctypes.byref(self.cfg), self.P) if self.P else
@@ -118,13 +134,18 @@ class LowLatencyEngine(object):
             np.random.seed(seedValue)                                 # gccNMFFunctions.py:70,73, as online.py draws it
             H0 = (np.random.random((K, 2)).astype(np.float32) + epsilon).astype(np.float32)
         dev = lambda a: torch.as_tensor(np.ascontiguousarray(a)).to(self.h.device)      # noqa: E731
-        self._const = [dev(W), dev(E.view(np.float64).reshape(F, 2 * self.D)), dev(np.asarray(analysisWindow, np.float64)),
+        self._const = [dev(W), dev(E.view(np.float64).reshape(-1, F, 2 * self.D)), dev(np.asarray(analysisWindow, np.float64)),
                        dev(self.weights), dev(H0) if H0 is not None else None]
         self._eps = np.full(self.S, float(targetTDOAEpsilon), np.float32)
         self._active = np.ones(self.S, np.int32)
         self._override = np.full(self.S, -1, np.int32)
         self._targets = np.full((self.S, max(self.P, 1)), -1, np.int32)
         self._window = np.zeros(self.S, np.int32)
+        self._assign = np.zeros(self.S, np.int32)                 # bank: each stream's table
+        if self.Qe:                                               # content digests of the dictionary and the tables (bank records)
+            from .records import content_digest
+            self._dict_digest = content_digest(W, H0) if H0 is not None else content_digest(W)
+            self._steer_digests = [content_digest(e) for e in E]
         self._io = {}
         self._graphs = {}
         self._exports = {}
@@ -147,14 +168,15 @@ class LowLatencyEngine(object):
     def _p(self):
         """The num_sources argument of the gccnmf_llsep_* entries, num_sources and history_length of the gccnmf_llhist_* entries (none
         for gccnmf_ll_*)."""
-        return (self.P, self.Lh) if self.Lh else (self.P,) if self.P else ()
+        return (self.P, self.Lh, self.Qe) if self.Qe else (self.P, self.Lh) if self.Lh else (self.P,) if self.P else ()
 
     def _fn(self, name):
-        return getattr(self.h.lib, ('gccnmf_llhist_' if self.Lh else 'gccnmf_llsep_' if self.P else 'gccnmf_ll_') + name)
+        prefix = 'gccnmf_llbank_' if self.Qe else 'gccnmf_llhist_' if self.Lh else 'gccnmf_llsep_' if self.P else 'gccnmf_ll_'
+        return getattr(self.h.lib, prefix + name)
 
     def _state(self, name, *args):
         """gccnmf_ll_<name>(h, cfg, state, state_bytes, *args), gccnmf_llsep_<name>(h, cfg, P, state, state_bytes, *args) or
-        gccnmf_llhist_<name>(h, cfg, P, Lh, state, state_bytes, *args)."""
+        gccnmf_llhist_<name>(h, cfg, P, Lh, state, state_bytes, *args), gccnmf_llbank_<name>(h, cfg, P, Lh, Qe, state, ...)."""
         self._check(self._fn(name)(self.h.h, ctypes.byref(self.cfg), *self._p, self.state.data_ptr(), self.state_bytes, *args))
 
     def _streams(self, streams):
@@ -220,6 +242,36 @@ class LowLatencyEngine(object):
         self._state('set_window', lo, hi - lo + 1, arr.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), self.stream.cuda_stream)
         self.stream.synchronize()
 
+    def assign_steering(self, streams, entries):
+        """Steering bank: the streams use tables `entries` (broadcast to len(streams)) from the next call on; everything else of
+        them stays."""
+        if not self.Qe:
+            raise ValueError('assign_steering needs a steering bank (expJOmegaTau a sequence of tables)')
+        idx = self._streams(streams)
+        e = np.broadcast_to(np.asarray(entries, dtype=np.int64), idx.shape)
+        if e.min() < 0 or e.max() >= self.Qe:
+            raise ValueError('steering entries outside [0, %d)' % self.Qe)
+        self._assign[idx] = e
+        lo, hi = int(idx.min()), int(idx.max())
+        arr = np.ascontiguousarray(self._assign[lo:hi + 1], dtype=np.int32)
+        self._state('assign', lo, hi - lo + 1, arr.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), self.stream.cuda_stream)
+        self.stream.synchronize()
+
+    def load_steering(self, entry, expJOmegaTau):
+        """Steering bank: table `entry` becomes expJOmegaTau (F, D) from the next call on, for every stream on it."""
+        if not self.Qe:
+            raise ValueError('load_steering needs a steering bank (expJOmegaTau a sequence of tables)')
+        if not 0 <= int(entry) < self.Qe:
+            raise ValueError('steering entry outside [0, %d)' % self.Qe)
+        E = np.ascontiguousarray(expJOmegaTau, dtype=np.complex128)
+        if E.shape != (self.F, self.D):
+            raise ValueError('expJOmegaTau must be (%d, %d)' % (self.F, self.D))
+        from .records import content_digest
+        t = self.torch.as_tensor(E.view(np.float64)).to(self.h.device)
+        self._state('load_steering', int(entry), t.data_ptr(), self.stream.cuda_stream)
+        self.stream.synchronize()
+        self._steer_digests[int(entry)] = content_digest(E)
+
     def set_active(self, streams, active):
         """An inactive stream outputs zeros and its state does not change."""
         idx = self._streams(streams)
@@ -231,6 +283,7 @@ class LowLatencyEngine(object):
         parameters stay."""
         idx = np.unique(self._streams(streams))
         self._window[idx] = 0
+        self._assign[idx] = 0
         breaks = np.flatnonzero(np.diff(idx) != 1) + 1          # one call per contiguous run of streams
         for run in np.split(idx, breaks):
             self._state('reset_streams', int(run[0]), len(run), self.stream.cuda_stream)
@@ -300,6 +353,8 @@ class LowLatencyEngine(object):
                            EXPORT_SOURCE_WIENER: (((P, 2, F, T) if self.inference else (P, F, T)), torch.float32),
                            EXPORT_SOURCE_Y: ((P, 2, F, T), torch.complex64), EXPORT_STREAM_STATUS: ((self.S,), torch.int32),
                            EXPORT_CARRIED_TARGETS: ((self.S, P), torch.int32), EXPORT_CALL_STATUS: ((1,), torch.int32)})
+        if self.Qe:
+            shapes[EXPORT_ASSIGNMENT] = ((self.S,), torch.int32)
         if self.Lh:
             shapes.update({EXPORT_HISTORY: ((self.S, D, self.Lh), torch.float64), EXPORT_HISTORY_INDEX: ((self.S,), torch.int32),
                            EXPORT_WINDOWS: ((self.S,), torch.int32), EXPORT_WINDOW_MEANS: ((D, T), torch.float64)})
@@ -314,9 +369,10 @@ class LowLatencyEngine(object):
 
     # ------------------------------------------------------------------ stream records (gccnmf_llrec_*, or gccnmf_llhist_* with history)
     def _rec(self, name):
-        """gccnmf_llrec_<name> bound to (cfg, P), or gccnmf_llhist_<name> bound to (cfg, P, Lh)."""
-        fn = getattr(self.h.lib, ('gccnmf_llhist_' if self.Lh else 'gccnmf_llrec_') + name)
-        hist = (self.Lh,) if self.Lh else ()
+        """gccnmf_llrec_<name> bound to (cfg, P), gccnmf_llhist_<name> bound to (cfg, P, Lh) or gccnmf_llbank_<name> bound to
+        (cfg, P, Lh, Qe)."""
+        fn = getattr(self.h.lib, ('gccnmf_llbank_' if self.Qe else 'gccnmf_llhist_' if self.Lh else 'gccnmf_llrec_') + name)
+        hist = (self.Lh, self.Qe) if self.Qe else (self.Lh,) if self.Lh else ()
         if name.endswith('_bytes'):
             return lambda *a: fn(ctypes.byref(self.cfg), self.P, *hist, *a)
         return lambda *a: fn(self.h.h, ctypes.byref(self.cfg), self.P, *hist, *a)
@@ -355,7 +411,7 @@ class LowLatencyEngine(object):
                        targets=self._targets[idx].copy())
         if self.Lh:
             mirrors['window'] = self._window[idx].copy()
-        rec = StreamRecord(RECORD_KIND_LL, self.P, self.torch.zeros((len(idx), self.record_bytes), dtype=self.torch.uint8).pin_memory(),
+        rec = StreamRecord(RECORD_KIND_LLBANK if self.Qe else RECORD_KIND_LL, self.P, self.torch.zeros((len(idx), self.record_bytes), dtype=self.torch.uint8).pin_memory(),
                            mirrors)
         self._record_call('save_streams', idx, rec)
         return rec
@@ -364,8 +420,9 @@ class LowLatencyEngine(object):
         """The header this engine's records carry (gccnmf_record_header), computed on the host: the library writes the same."""
         cfg = LLConfig.from_buffer_copy(bytes(self.cfg))
         cfg.num_streams = cfg.hops_per_call = 0
-        head = RecordHeader(magic=RECORD_MAGIC, abi_version=self.h.lib.gccnmf_abi_version(), kind=RECORD_KIND_LL, num_sources=self.P,
-                            payload_bytes=int(self._rec('workspace_bytes')(1)))
+        head = RecordHeader(magic=RECORD_MAGIC, abi_version=self.h.lib.gccnmf_abi_version(), kind=RECORD_KIND_LLBANK if self.Qe else RECORD_KIND_LL,
+                            num_sources=self.P,
+                            payload_bytes=int(self.h.lib.gccnmf_llhist_workspace_bytes(ctypes.byref(self.cfg), self.P, self.Lh, 1)))
         ctypes.memmove(head.config, bytes(cfg), ctypes.sizeof(cfg))
         head.config[LLHIST_RECORD_CONFIG_HISTORY] = self.Lh
         d = 1469598103934665603                                    # FNV-1a 64 of the weights' bytes, then the gain's
@@ -378,9 +435,12 @@ class LowLatencyEngine(object):
         """Record i replaces the state and settings of streams[i] from the next call on.  The record must come from an engine with
         the same configuration other than numStreams and hopsPerCall, the same synthesis, numSources and historyLength.  Every record
         is checked on the host before anything is loaded, so a refusal leaves the engine and the device untouched.  Each run of consecutive
-        streams is one library call (one wait for the synthesis weights, one copy, one kernel)."""
+        streams is one library call (one wait for the synthesis weights, one copy, one kernel).  With a steering bank the record must
+        come from a bank engine with the same dictionary, and each stream goes onto the lowest table of this engine with the content of
+        the table it was on."""
         idx = self._streams(streams)
-        if record.kind != RECORD_KIND_LL or record.count != len(idx):
+        kind = RECORD_KIND_LLBANK if self.Qe else RECORD_KIND_LL
+        if record.kind != kind or record.count != len(idx):
             raise ValueError('a low-latency record of %d streams is needed (got kind %d, %d streams)' % (len(idx), record.kind, record.count))
         if record.data.shape[1] != self.record_bytes:
             lh = record.header(0).config[LLHIST_RECORD_CONFIG_HISTORY]
@@ -395,7 +455,18 @@ class LowLatencyEngine(object):
             value = lambda h, f: bytes(h.config) if f == 'config' else getattr(h, f)       # noqa: E731
             bad = [f for f, _ in RecordHeader._fields_ if value(got, f) != value(want, f)]
             raise ParameterError('record %d does not fit this engine: %s differ' % (i, ', '.join(bad)))
+        if self.Qe:
+            entries = np.empty(len(idx), np.int32)
+            for i in range(len(idx)):
+                got = record.header(i)
+                if got.dictionary_digest != self._dict_digest:
+                    raise ParameterError('record %d: another dictionary' % i)
+                if got.steering_digest not in self._steer_digests:
+                    raise ParameterError('record %d: no steering entry of this engine has the stream\'s table' % i)
+                entries[i] = self._steer_digests.index(got.steering_digest)
         self._record_call('load_streams', idx, record)
+        if self.Qe:
+            self._assign[idx] = entries
         m = record.mirrors
         self._eps[idx], self._active[idx], self._override[idx], self._targets[idx] = m['eps'], m['active'], m['override'], m['targets']
         if self.Lh:
@@ -416,17 +487,20 @@ class LowLatencyEngine(object):
 
 def streamSignals(signals, W, expJOmegaTau, analysisWindow, synthesisWindow, hopSize, hopsPerCall=1, synthesis='lowlatency',
                   targetTDOAEpsilon=1.0, numInferenceIterations=0, use_graph=True, device=0, numSources=0, historyLength=0,
-                  localizationWindow=0, **kwargs):
+                  localizationWindow=0, steeringEntries=None, **kwargs):
     """Streams a list of stereo signals (2, n_i) through one engine, one stream each, hopsPerCall hops per call, and returns the
     outputs aligned with the input: out_i[..., p] = output sample p + latency (the batch function's targetEstimateSamplesOLA), each
     (2, n_i), or (P, 2, n_i) with numSources = P.  Shorter signals are followed by silence; the engine is flushed with `latency`
     samples of silence at the end.  historyLength / localizationWindow: every stream localises over its newest
-    localizationWindow frames (see set_localization)."""
+    localizationWindow frames (see set_localization).  With a steering bank (expJOmegaTau a sequence of tables), steeringEntries
+    gives each signal's table (default: table 0)."""
     sig = [np.asarray(s, dtype=np.float32) for s in signals]
     eng = LowLatencyEngine(W, expJOmegaTau, analysisWindow, synthesisWindow, hopSize, numStreams=len(sig), hopsPerCall=hopsPerCall,
                            synthesis=synthesis, targetTDOAEpsilon=targetTDOAEpsilon, numInferenceIterations=numInferenceIterations,
                            device=device, numSources=numSources, historyLength=historyLength, **kwargs)
     eng.set_localization(None, localizationWindow)
+    if steeringEntries is not None:
+        eng.assign_steering(None, steeringEntries)
     step = eng.hop * eng.C
     total = max(s.shape[1] for s in sig) + eng.latency
     total = -(-total // step) * step

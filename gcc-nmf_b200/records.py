@@ -6,15 +6,16 @@ A `StreamRecord` holds one record per stream in a pinned host buffer, each a hea
 the stream's state, plus the engine's host copies of the streams' settings (which a load hands to the destination engine, so
 that its later `set_params` / `set_targets` calls rewrite them unchanged).  `save(path)` / `load(path)` keep it in an .npz file.
 
-A real-time record names the dictionary and steering table its slot was on by content: `content_digest` below, which the library
+A real-time record, and a low-latency record of an engine with a steering bank (`gccnmf_llbank_*`), names the dictionary and
+steering table its slot was on by content: `content_digest` below, which the library
 computes on the device and the engines compute on the host for what they were given.
 """
 import numpy as np
 
-from ._lib import (RECORD_HEADER_BYTES, RECORD_KIND_LL, RECORD_KIND_RT, RECORD_MAGIC, RTREC_DIGEST_CHUNK_WORDS, RecordHeader,
-                   RtRecordHeader)
+from ._lib import (RECORD_HEADER_BYTES, RECORD_KIND_LL, RECORD_KIND_LLBANK, RECORD_KIND_RT, RECORD_MAGIC, RTREC_DIGEST_CHUNK_WORDS,
+                   LLBankRecordHeader, RecordHeader, RtRecordHeader)
 
-KINDS = {RECORD_KIND_LL: RecordHeader, RECORD_KIND_RT: RtRecordHeader}
+KINDS = {RECORD_KIND_LL: RecordHeader, RECORD_KIND_RT: RtRecordHeader, RECORD_KIND_LLBANK: LLBankRecordHeader}
 
 _BASIS = np.uint64(0xcbf29ce484222325)
 _PRIME = np.uint64(0x100000001b3)
@@ -57,7 +58,8 @@ class StreamRecord(object):
         return int(self.data.shape[0])
 
     def header(self, i=0):
-        """The library's header of record i: gccnmf_record_header (low-latency) or gccnmf_rtrec_header (real-time)."""
+        """The library's header of record i: gccnmf_record_header (low-latency), gccnmf_llbank_record_header (low-latency with a
+        steering bank) or gccnmf_rtrec_header (real-time)."""
         return KINDS[self.kind].from_buffer_copy(self.data[i, :RECORD_HEADER_BYTES].numpy().tobytes())
 
     def save(self, path):

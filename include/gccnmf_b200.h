@@ -730,6 +730,78 @@ GCCNMF_API int gccnmf_llhist_load_streams(gccnmf_handle* h, const gccnmf_ll_conf
                                size_t state_bytes, int first, int count, const void* record, size_t record_bytes, void* workspace,
                                size_t workspace_bytes, void* stream);
 
+/* ---- a bank of steering tables: each stream on its own microphone spacing ------------------------------------------------------
+ * The engine of gccnmf_llhist_* (num_sources 0 or 2 .. 8, history_length 0 .. 1024) with num_steerings = Qe steering tables,
+ * 0 <= Qe <= 64.  Every entry takes (num_sources, history_length, num_steerings) after the config and does what its gccnmf_llhist_*
+ * namesake does; with Qe = 0 the engine, its state size, its launches and its records are the namesake's.
+ * - Tables: init takes E_0 .. E_{Qe-1} as one device array (Qe, F, D) complex128, each as gccnmf_ll_init takes E.  Stream s is on
+ *   entry assign[s]; init and reset_streams put it on entry 0.  N, hop, D, K, W, H0, the windows, the synthesis, P and Lh are the
+ *   engine's.  A stream on entry j computes, bit for bit, every sample and export item a gccnmf_llhist_* engine with the same
+ *   num_sources and history_length built with E_j computes from the same input and settings.
+ * - load_steering (table j <- a device (F, D) complex128 array) and assign (streams -> entries) act from the next call, may sit between
+ *   launches of a graph, and keep every other part of the streams: rings, running maximum, history, window, targets, overrides, hop
+ *   count and parameters.  Those are indexed by TDOA, so a new table changes only the columns computed from then on.
+ * - Export: the namesake's items plus 26 the assignment (S) i32 (Qe >= 1).
+ * - Records (record_bytes / workspace_bytes / save_streams / load_streams): with Qe = 0 gccnmf_llhist_*'s.  With Qe >= 1 the kind is
+ *   GCCNMF_RECORD_KIND_LLBANK and the header a gccnmf_llbank_record_header: gccnmf_record_header's fields, then the content digests
+ *   (GCCNMF_RTREC_DIGEST_*, computed on the device) of the dictionary (W (F, K) f32, then H0 (K, 2) f32 with inference) and of the
+ *   stream's steering table as stored ((F, D) complex128).  A load checks every host field first (refused: nothing enqueued), then
+ *   the synthesis digest and the destination's digests (one wait on `stream` each); it refuses, with the state unchanged, a record
+ *   whose dictionary differs or whose table no entry holds, and otherwise puts the stream on the LOWEST entry with that table.  The
+ *   workspace must be 8-byte aligned.  Records do not move between bank and non-bank engines.
+ * Qe outside [0, 64], an entry outside [0, Qe), item 26 with Qe = 0 and the namesake's refusals fail before anything is enqueued. */
+#define GCCNMF_LLBANK_MAX_STEERINGS 64
+#define GCCNMF_LLBANK_EXPORT_ASSIGNMENT 26
+#define GCCNMF_RECORD_KIND_LLBANK 3
+typedef struct gccnmf_llbank_record_header {
+  uint32_t magic;                         /* the fields up to config are those of gccnmf_record_header */
+  int32_t abi_version;
+  int32_t kind;                           /* GCCNMF_RECORD_KIND_LLBANK */
+  int32_t num_sources;
+  uint64_t payload_bytes;
+  uint64_t synthesis_digest;
+  int32_t config[16];
+  uint64_t dictionary_digest;
+  uint64_t steering_digest;               /* of the table the stream was on */
+} gccnmf_llbank_record_header;
+/* Host only; 0 for an invalid configuration, num_sources, history_length or num_steerings. */
+GCCNMF_API size_t gccnmf_llbank_state_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings);
+GCCNMF_API int gccnmf_llbank_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings,
+                       const float* W, const double* E, const double* analysis_window, const double* synthesis_weights, float gain,
+                       const float* H0, void* state, size_t state_bytes, void* stream);
+/* E: one (F, D) complex128 DEVICE table for entry `entry`. */
+GCCNMF_API int gccnmf_llbank_load_steering(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length,
+                                int num_steerings, void* state, size_t state_bytes, int entry, const double* E, void* stream);
+/* entries_host: count host int32 in [0, num_steerings), consumed before the call returns. */
+GCCNMF_API int gccnmf_llbank_assign(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings,
+                         void* state, size_t state_bytes, int first, int count, const int32_t* entries_host, void* stream);
+GCCNMF_API int gccnmf_llbank_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length,
+                                int num_steerings, void* state, size_t state_bytes, int first, int count, void* stream);
+GCCNMF_API int gccnmf_llbank_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings,
+                             void* state, size_t state_bytes, int first, int count, const gccnmf_ll_stream_params* params_host,
+                             void* stream);
+GCCNMF_API int gccnmf_llbank_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length,
+                              int num_steerings, void* state, size_t state_bytes, int first, int count, const int32_t* targets_host,
+                              void* stream);
+GCCNMF_API int gccnmf_llbank_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings,
+                             void* state, size_t state_bytes, int first, int count, const int32_t* windows_host, void* stream);
+GCCNMF_API int gccnmf_llbank_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings,
+                          void* state, size_t state_bytes, int hops, const float* in, float* out, void* stream);
+GCCNMF_API int gccnmf_llbank_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length,
+                               int num_steerings, void* state, size_t state_bytes, int hops, float* in, float* out,
+                               const float* in_host, float* out_host, void** graph_exec, void* stream);
+GCCNMF_API int gccnmf_llbank_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings,
+                         void* state, size_t state_bytes, int hops, int what, void* dst, void* stream);
+GCCNMF_API size_t gccnmf_llbank_record_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings);
+GCCNMF_API size_t gccnmf_llbank_workspace_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings,
+                                     int count);
+GCCNMF_API int gccnmf_llbank_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length,
+                               int num_steerings, void* state, size_t state_bytes, int first, int count, void* record,
+                               size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream);
+GCCNMF_API int gccnmf_llbank_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length,
+                               int num_steerings, void* state, size_t state_bytes, int first, int count, const void* record,
+                               size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- real-time stream records: move a live slot to another slot, engine, engine form, device or process ---------------------
  * One family for every real-time form, with the arguments of gccnmf_rtbank_*: (num_streams, num_sources, num_dictionaries,
  * num_steerings) = (1, 0, 0, 0) for gccnmf_rt_*, (S, 0, 0, 0) for gccnmf_rtm_*, (S, P, 0, 0) for gccnmf_rtsep_* and
