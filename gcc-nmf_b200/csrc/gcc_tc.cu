@@ -162,12 +162,12 @@ struct EpiArgmaxTile {
       const int ml = p & (tgemm::kBM - 1), j = p / tgemm::kBM;
       const int m = m0 + ml;
       if (m >= K) continue;
-      const float* col = tile + (size_t)(j * D) * tgemm::kBM + ml;
+      const float* col = tile + (size_t)(j * D) * tgemm::kTileLd + ml;
       float best = -INFINITY, second = -INFINITY;
       int idx = 0, nan = 0;
 #pragma unroll 8
       for (int d = 0; d < D; ++d) {
-        const float x = col[(size_t)d * tgemm::kBM];
+        const float x = col[(size_t)d * tgemm::kTileLd];
         if (x != x) nan = 1;                 // NaN anywhere: let float64 decide with numpy's NaN rules
         if (x > best) { second = best; best = x; idx = d; }
         else if (x > second) second = x;
@@ -179,7 +179,7 @@ struct EpiArgmaxTile {
         // the TDOAs that can still be the float64 maximum: every value within the margin of the best (all of them after a NaN)
         uint32_t bits[4] = {0u, 0u, 0u, 0u};
         for (int d = 0; d < D; ++d) {
-          const float x = col[(size_t)d * tgemm::kBM];
+          const float x = col[(size_t)d * tgemm::kTileLd];
           if (nan || !(best - x > margin)) bits[d >> 5] |= 1u << (d & 31);
         }
         const int slot = atomicAdd(count, 1);

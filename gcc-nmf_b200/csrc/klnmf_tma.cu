@@ -78,8 +78,13 @@ struct EpiRatioPlanes {   // RT[n][m] = split(VT[n][m] / acc)     G1 / G3 (m = f
   static constexpr int kRowValues = 0;
   static constexpr bool kPrefetch = false;   // V^T is read twice per iteration and stays in L2 (96 % hit rate measured)
   static constexpr bool kDualN = true;       // 2 MMAs per k-step, N = BN and N = 2 BN (the three hi / lo products), see tma_gemm.cuh
-  static constexpr bool kPreloadOperands = true;   // V^T of the thread's columns is fetched while the main loop runs
+  static constexpr bool kPreloadOperands = true;   // V^T of the thread's columns is fetched while the main loop runs (wide tiles)
+  static constexpr bool kSmemOperand = true;       // V^T tile by TMA into shared memory where the tile leaves room for it
   const float* __restrict__ VT; bf16* __restrict__ RT; int64_t ld, plane; int M, N; bool vec;
+  CUtensorMap operand_map;                         // (encoded by the launcher)
+  const float* operand() const { return VT; }
+  int64_t operand_ld() const { return ld; }
+  int operand_cols() const { return N; }
   __device__ void prefetch(int, int) const {}
   __device__ void row_values(int, float*) const {}
   __device__ void init(State&, int, const float*) const {}
@@ -696,9 +701,9 @@ __global__ void tma_reduce_pull_kernel(PeerSet peers, float* reduced_local, int6
 // Cost model of the planner, in SM cycles of one 128-row CTA, from the per-CTA phase stamps of tools/nmf_phases.py at the benchmark
 // shape (H100 SXM, DESIGN.md 4.1).  Per 16-deep k-step the dual-N loop issues MMAs of N = bn and N = 2 bn, the plain loop three of
 // N = bn; an MMA costs 1.1 - 1.2 cycles per column of N (both warpgroups; G1 - G4 main loops at widths 120 - 256).  The epilogue
-// costs about 100 cycles per column for the ratio (G1 / G3) and the H update (G2), 42 for the plain store of the W-update numerator
-// (G4); the fill, the launch and the gaps about 8 k cycles per wave.
-constexpr double kEpiRatioCycles = 100.0, kEpiUpdateHCycles = 100.0, kEpiStoreCycles = 42.0;
+// costs about 95 cycles per column for the ratio (G1 / G3), 93 for the H update (G2), 33 for the plain store of the W-update
+// numerator (G4); the fill, the launch and the gaps about 8 k cycles per wave.
+constexpr double kEpiRatioCycles = 95.0, kEpiUpdateHCycles = 93.0, kEpiStoreCycles = 33.0;
 double mma_cycles(int n) { return 1.2 * n; }
 double kstep_cycles(int bn, bool dual) { return (dual && 2 * bn <= 256) ? mma_cycles(2 * bn) + mma_cycles(bn) : 3.0 * mma_cycles(bn); }
 double epilogue_cycles(int bn, double per_column) { return per_column * bn; }

@@ -42,6 +42,10 @@ constexpr int kThreads = (1 + kMmaWarpgroups) * 128;
 constexpr int kColumnsInFlight = 8;        // epilogue: independent column loads per thread before the first dependent store
 constexpr int kMaxRowValues = 4;           // per-row values an epilogue functor may stage in shared memory
 constexpr int kSmemBudget = 216 * 1024;    // stages; + barriers + epilogue scratch + alignment slack stays under the 227 KB per-CTA limit
+// Leading dimension (floats) of the staged accumulator tile [BN][kTileLd]: the four lanes of a wgmma fragment quad hold one row at
+// columns c, c + 2, c + 4, c + 6, and the 4-word pad puts those columns 8 banks apart, so a warp's 32 staging stores hit 32 distinct
+// banks (with 128 they all land on the bank of their row: 4-way conflicts); a column stays 16-byte aligned for the float4 reads.
+constexpr int kTileLd = kBM + 4;
 
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
@@ -52,6 +56,13 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
+// One 2-D box (inner, rows) -> shared memory of this CTA, completion signalled on `bar`; out-of-range elements are zero-filled.
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
 // Same, delivered to the same shared-memory offset (and signalled on the same barrier offset) of every CTA of the cluster in `mask`.
@@ -140,7 +151,10 @@ struct PlaneGemmArgs {
 };
 
 
-template <int BN, int KB, bool A_MN, bool B_MN, int NACC = 1>     // NACC = 2: dual-N mode, two BN-column accumulator halves
+// WANT_OPERAND: the epilogue takes its float32 operand tile [BN][128] in shared memory (see wants_smem_operand); it gets it when
+// at least kMinStagesWithOperand pipeline stages remain beside it, else the operand is read from global memory as before.
+constexpr int kMinStagesWithOperand = 4;
+template <int BN, int KB, bool A_MN, bool B_MN, int NACC = 1, bool WANT_OPERAND = false>   // NACC = 2: dual-N mode, two BN-column accumulator halves
 struct Config {
   static_assert(KB == 32 || KB == 64, "k-block of 32 (SWIZZLE_64B K-major rows) or 64 (SWIZZLE_128B)");
   static_assert(BN % 8 == 0 && BN >= 16 && BN * NACC <= 256, "wgmma N (= BN, or 2 BN in the dual-N loop)");
@@ -151,14 +165,18 @@ struct Config {
   static constexpr int kBBytes = B_MN ? kBAtoms * kAtomBytes : 2 * BN * KB * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
   static_assert(kABytes % 1024 == 0 && kBBytes % 1024 == 0, "operand blocks must keep 1024-byte alignment");
-  static constexpr int kStagesRaw = kSmemBudget / kStageBytes;
+  static constexpr int kOperandWant = BN * kBM * 4;
+  static constexpr bool kOperandFits = (kSmemBudget - kOperandWant) / kStageBytes >= kMinStagesWithOperand &&
+                                       ((kSmemBudget - kOperandWant) / kStageBytes) * kStageBytes >= BN * kTileLd * 4;
+  static constexpr int kOperandBytes = (WANT_OPERAND && kOperandFits) ? kOperandWant : 0;   // behind the stages, never aliased
+  static constexpr int kStagesRaw = (kSmemBudget - kOperandBytes) / kStageBytes;
   static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
   static_assert(kStages >= 2, "tile too large for a 2-stage pipeline");
   static constexpr int kAccCols = BN * NACC;                      // wgmma N; each thread holds kAccCols / 2 floats
   static constexpr int kBarrierBytes = 256;
   static constexpr int kScratchBytes = kMaxRowValues * kBM * 4 + (kThreads / 32) * 32 * 16;
-  static constexpr int kTotal = kStages * kStageBytes + kBarrierBytes + kScratchBytes + 1024;   // + alignment slack
-  static_assert(kStages * kStageBytes >= BN * kBM * 4, "the epilogue stages the accumulator tile in the pipeline buffers");
+  static constexpr int kTotal = kStages * kStageBytes + kOperandBytes + kBarrierBytes + kScratchBytes + 1024;   // + alignment slack
+  static_assert(kStages * kStageBytes >= BN * kTileLd * 4, "the epilogue stages the accumulator tile in the pipeline buffers");
   static_assert(kTotal <= 227 * 1024, "shared memory per CTA");
 };
 
@@ -204,7 +222,7 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[N / 2], uint32_t a_base,
 }
 
 // Epilogues with `static constexpr bool kTileEpilogue = true` take the whole staged tile:
-//   __device__ void tile_epilogue(const float* tile /* [n][128] */, int m0, int n0, int n_valid, int z) const;   (all threads)
+//   __device__ void tile_epilogue(const float* tile /* [n][kTileLd] */, int m0, int n0, int n_valid, int z) const;   (all threads)
 template <class E, class = void>
 struct has_tile_epilogue { static constexpr bool value = false; };
 template <class E>
@@ -215,11 +233,22 @@ struct has_tile_epilogue<E, decltype((void)E::kTileEpilogue)> { static constexpr
 // into two accumulator halves, and one of N = BN adds A_lo . B_hi to the first half: 2 MMAs per k-step compute the three products
 // lo.hi + hi.hi | hi.lo over 3 BN columns, as the plain loop does in three MMAs of BN, and the epilogue adds the two halves.
 // Epilogues with `static constexpr bool kPreloadOperands = true` have their by-column global operands fetched into registers while
-// the main loop runs (opt-in: measured to pay for the ratio epilogue of the W.H contractions, to cost for the H update).
+// the main loop runs (opt-in: measured to pay for the ratio epilogue of the W.H contractions, to cost for the H update; not used
+// where the operand comes into shared memory instead, see wants_smem_operand).
 template <class E, class = void>
 struct wants_preload { static constexpr bool value = false; };
 template <class E>
 struct wants_preload<E, decltype((void)E::kPreloadOperands)> { static constexpr bool value = E::kPreloadOperands; };
+
+// Epilogues with `static constexpr bool kSmemOperand = true` have a by-column operand that is one float32 element per output
+// element, in the output's layout (`Loaded` is that float4):  CUtensorMap operand_map;  const float* operand() const;
+// int64_t operand_ld() const;  int operand_cols() const  (element (m, n) at operand()[n * operand_ld() + m], n < operand_cols()).
+// The launcher encodes operand_map with a box of 128 m x BN n; the producer thread loads the CTA's box with one TMA copy when it
+// has issued its last stage, into shared memory beside the stages, and the epilogue reads its columns from there.
+template <class E, class = void>
+struct wants_smem_operand { static constexpr bool value = false; };
+template <class E>
+struct wants_smem_operand<E, decltype((void)E::kSmemOperand)> { static constexpr bool value = E::kSmemOperand; };
 
 template <class E, class = void>
 struct wants_dual_n { static constexpr bool value = false; };
@@ -238,9 +267,11 @@ struct wants_dual_n<E, decltype((void)E::kDualN)> { static constexpr bool value 
 //   __device__ void elem(int m, int n, float acc, int z) const;          SIMT tail rows (one column per lane)
 template <int BN, int KB, bool A_MN, bool B_MN, int CN, int CM, class Epilogue>
 __global__ void __launch_bounds__(kThreads, 1)
-plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, PlaneGemmArgs args, Epilogue epi) {
+plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, PlaneGemmArgs args,
+                  const __grid_constant__ Epilogue epi) {
   constexpr bool DUAL = wants_dual_n<Epilogue>::value && !B_MN && 2 * BN <= 256;
-  using C = Config<BN, KB, A_MN, B_MN, DUAL ? 2 : 1>;
+  using C = Config<BN, KB, A_MN, B_MN, DUAL ? 2 : 1, wants_smem_operand<Epilogue>::value && !has_tile_epilogue<Epilogue>::value>;
+  constexpr bool OPERAND = C::kOperandBytes > 0;     // the epilogue's operand tile comes into shared memory by TMA
   constexpr int kCluster = CN * CM;
   static_assert((CN == 1 || CN == 2) && (CM == 1 || CM == 2), "cluster of CN n-tiles x CM m-tiles");
   static_assert(A_MN || (kBM / CN) % 8 == 0, "A row slices keep the swizzle atoms whole");
@@ -265,13 +296,15 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   const uint16_t mask_row = (uint16_t)(((1u << CN) - 1u) << (CN * cy));
   const uint16_t mask_col = (uint16_t)((CM > 1 ? ((1u << cx) | (1u << (cx + CN))) : (1u << cx)));
 
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::kStages * C::kStageBytes);
+  const float* operand = reinterpret_cast<const float*>(smem + C::kStages * C::kStageBytes);   // [BN][128] when OPERAND
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::kStages * C::kStageBytes + C::kOperandBytes);
   uint64_t* full = bars;                    // [kStages]  TMA -> MMA
   uint64_t* empty = bars + C::kStages;      // [kStages]  MMA warpgroups (of every CTA that shares a slice with me) -> TMA
+  uint64_t* operand_full = bars + 2 * C::kStages;   // TMA -> epilogue (OPERAND)
   // epilogue scratch behind the barriers (never touched by TMA): per-row functor values, row-sum partials of the 12 warps
-  float* rowvals = reinterpret_cast<float*>(smem + C::kStages * C::kStageBytes + C::kBarrierBytes);   // [kMaxRowValues][128]
+  float* rowvals = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(bars) + C::kBarrierBytes);   // [kMaxRowValues][128]
   float4* red = reinterpret_cast<float4*>(rowvals + kMaxRowValues * kBM);                             // [12 warps][32 lanes]
-  float* tile = reinterpret_cast<float*>(smem);        // epilogue: [BN][128] float32, aliases the pipeline stages
+  float* tile = reinterpret_cast<float*>(smem);        // epilogue: [BN][kTileLd] float32, aliases the pipeline stages
   const int m0 = tile_m * kBM;
 
   const int cta_linear = blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z);
@@ -285,9 +318,11 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       // one release per MMA warpgroup of every CTA whose multicast lands in this stage (incl. myself)
       mbar_init(smem_u32(&empty[s]), kMmaWarpgroups * (CN + CM - 1));
     }
+    if constexpr (OPERAND) mbar_init(smem_u32(operand_full), 1);
     gmma::fence_barrier_init();
     tma_prefetch_descriptor(&map_a);
     tma_prefetch_descriptor(&map_b);
+    if constexpr (OPERAND) tma_prefetch_descriptor(&epi.operand_map);
   }
   if (kCluster > 1) cluster_sync();     // no peer may signal my barriers or write my stages before they are initialised
   else __syncthreads();
@@ -301,7 +336,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   // after the main loop starts with its operands already there; the MMA warpgroups issue theirs as soon as the tile is staged.
   constexpr int kWarpsAll = kThreads / 32;
   constexpr int kLoadedWords = (int)((sizeof(typename Epilogue::Loaded) + 3) / 4);
-  constexpr bool kPreloads = wants_preload<Epilogue>::value && !has_tile_epilogue<Epilogue>::value && !std::is_empty<typename Epilogue::Loaded>::value;
+  constexpr bool kPreloads = !OPERAND && wants_preload<Epilogue>::value && !has_tile_epilogue<Epilogue>::value && !std::is_empty<typename Epilogue::Loaded>::value;
   constexpr int kPreCap = 64 / (kLoadedWords > 0 ? kLoadedWords : 1);                      // register budget: 64 words per thread
   constexpr int kPre = kPreloads ? ((BN + kWarpsAll - 1) / kWarpsAll < kPreCap ? (BN + kWarpsAll - 1) / kWarpsAll : kPreCap) : 0;
   typename Epilogue::Loaded pre[kPre > 0 ? kPre : 1];
@@ -348,6 +383,12 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
           for (int p = 0; p < 2; ++p)
             tma_load_3d_mc<(CM > 1)>(b_dst + p * (BN * KB * 2) + cy * (kRows * KB * 2), &map_b, bar, k0, n0 + cy * kRows, p, mask_col);
         }
+      }
+      if constexpr (OPERAND) {
+        // the epilogue operand tile, issued behind the last stage so that it does not delay the main loop's operands; it arrives
+        // while the MMAs of the last stages run
+        mbar_arrive_expect_tx(smem_u32(operand_full), C::kOperandBytes);
+        tma_load_2d(smem_u32(operand), &epi.operand_map, smem_u32(operand_full), m0, n0);
       }
       if (args.timing) args.timing[cta_linear * 8 + 4] = clock64();   // producer done issuing
     }
@@ -467,7 +508,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       const int col = 8 * (j >> 2) + c0 + (j & 1), row = r0 + 8 * ((j >> 1) & 1);
       float v = acc[j];
       if constexpr (DUAL) v += acc[j + BN / 2];        // + the A_hi . B_lo half: columns BN .. 2 BN - 1
-      tile[(size_t)col * kBM + row] = v;
+      tile[(size_t)col * kTileLd + row] = v;
     }
     preload();
   }
@@ -491,6 +532,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     int n_valid = min(BN, args.N - n0);
     constexpr int U = kColumnsInFlight;
     int c_first = warp;
+    if constexpr (OPERAND) mbar_wait(smem_u32(operand_full), 0);
     if (zc > 1) {                          // my slice of the tile's columns
       const int per = (n_valid + zc - 1) / zc;
       c_first = z * per + warp;
@@ -502,7 +544,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         for (int u = 0; u < kPre; ++u) {
           const int cc = warp + kWarps * u;
           if (cc < n_valid) {
-            const float4 acc = *reinterpret_cast<const float4*>(tile + (size_t)cc * kBM + 4 * lane);
+            const float4 acc = *reinterpret_cast<const float4*>(tile + (size_t)cc * kTileLd + 4 * lane);
             epi.store(m_first, n0 + cc, acc, pre[u], z, st);
           }
         }
@@ -515,7 +557,10 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
 #pragma unroll
       for (int u = 0; u < U; ++u) {
         const int cc = c + kWarps * u;
-        if (cc < n_valid) loaded[u] = epi.load(m_first, n0 + cc);
+        if (cc < n_valid) {
+          if constexpr (OPERAND) loaded[u] = typename Epilogue::Loaded{*reinterpret_cast<const float4*>(operand + (size_t)cc * kBM + 4 * lane)};
+          else loaded[u] = epi.load(m_first, n0 + cc);
+        }
       }
       if (zc > 1) {
         // sum of the k-splits in split order (the order the W update used for the slabs): the distributed-shared-memory loads of ALL
@@ -525,7 +570,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
 #pragma unroll
         for (int u = 0; u < U; ++u) {
           const int cc = c + kWarps * u;
-          const float* src = tile + (size_t)(cc < n_valid ? cc : 0) * kBM + 4 * lane;
+          const float* src = tile + (size_t)(cc < n_valid ? cc : 0) * kTileLd + 4 * lane;
           sum[u] = z == 0 ? *reinterpret_cast<const float4*>(src) : ld_cluster_f32x4(src, 0);
         }
         for (int r = 1; r < zc; ++r) {
@@ -533,7 +578,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
 #pragma unroll
           for (int u = 0; u < U; ++u) {
             const int cc = c + kWarps * u;
-            const float* src = tile + (size_t)(cc < n_valid ? cc : 0) * kBM + 4 * lane;
+            const float* src = tile + (size_t)(cc < n_valid ? cc : 0) * kTileLd + 4 * lane;
             t[u] = r == z ? *reinterpret_cast<const float4*>(src) : ld_cluster_f32x4(src, (uint32_t)r);
           }
 #pragma unroll
@@ -549,7 +594,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         for (int u = 0; u < U; ++u) {
           const int cc = c + kWarps * u;
           if (cc < n_valid) {
-            const float4 acc = *reinterpret_cast<const float4*>(tile + (size_t)cc * kBM + 4 * lane);
+            const float4 acc = *reinterpret_cast<const float4*>(tile + (size_t)cc * kTileLd + 4 * lane);
             epi.store(m_first, n0 + cc, acc, loaded[u], z, st);
           }
         }

@@ -83,6 +83,33 @@ inline int get_tmap(gccnmf_handle* h, const bf16* base, uint64_t inner, uint64_t
   return 0;
 }
 
+// float32 matrix of `cols` rows of `inner` elements (pitch in elements), one box = box_inner x box_rows, no swizzle: the
+// epilogue operand tile of a plane GEMM (tgemm::wants_smem_operand).
+inline int tmap_f32_2d(gccnmf_handle* h, const float* base, uint64_t inner, uint64_t rows, uint64_t pitch_elems, uint32_t box_inner,
+                       uint32_t box_rows, CUtensorMap* out) {
+  if (!h->tmaps) h->tmaps = new gccnmf_tmap_cache();
+  const TmapKey key{base, inner, rows, pitch_elems * 4, 0, box_inner, box_rows, 0};     // (box_planes = 0: not a plane pair)
+  for (auto& e : h->tmaps->entries)
+    if (e.first == key) { *out = e.second; return 0; }
+  EncodeTiledFn encode = encode_tiled_fn();
+  if (!encode) return gccnmf_fail(h, GCCNMF_ERR_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
+  if ((reinterpret_cast<uintptr_t>(base) & 15) || (key.pitch_bytes & 15))
+    return gccnmf_fail(h, GCCNMF_ERR_INVALID_ARGUMENT, "tensor map: base / pitch must be 16-byte aligned");
+  const cuuint64_t dims[2] = {inner, rows};
+  const cuuint64_t strides[1] = {key.pitch_bytes};
+  const cuuint32_t box[2] = {box_inner, box_rows};
+  const cuuint32_t elem_strides[2] = {1, 1};
+  CUtensorMap m;
+  const CUresult r = encode(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, elem_strides,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return gccnmf_fail(h, GCCNMF_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
+  if (h->tmaps->entries.size() > 256) h->tmaps->entries.clear();
+  h->tmaps->entries.emplace_back(key, m);
+  *out = m;
+  return 0;
+}
+
 // K-major operand: rows x kc, k contiguous; one box = one plane of a row slice (box_rows = tile rows / cluster extent).
 inline int tmap_kmajor(gccnmf_handle* h, const bf16* planes, int rows, int kc, int64_t pitch, int64_t plane, int box_rows, CUtensorMap* out) {
   return get_tmap(h, planes, (uint64_t)kc, (uint64_t)rows, (uint64_t)pitch, (uint64_t)plane, kKB, (uint32_t)box_rows, 1, out);
@@ -202,7 +229,7 @@ struct GemmShape {
 template <int BN, bool A_MN, bool B_MN, int CN, int CM, class Epi>
 struct PlaneGemmInstance {
   static constexpr bool kDual = tgemm::wants_dual_n<Epi>::value && !B_MN && 2 * BN <= 256;
-  using C = tgemm::Config<BN, kKB, A_MN, B_MN, kDual ? 2 : 1>;
+  using C = tgemm::Config<BN, kKB, A_MN, B_MN, kDual ? 2 : 1, tgemm::wants_smem_operand<Epi>::value && !tgemm::has_tile_epilogue<Epi>::value>;
   static int max_clusters(gccnmf_handle* h, int* out) {
     static int cached_per_device[kGccnmfMaxDevices];     // 0 = not queried yet, else value + 1 (per device: attribute + occupancy)
     int& slot = cached_per_device[h->device % kGccnmfMaxDevices];
@@ -266,6 +293,10 @@ struct PlaneGemmInstance {
                       : tmap_kmajor(h, A.planes, g.M, g.Kc, A.pitch, A.plane, tgemm::kBM / CN, &map_a)) return st;
     if (int st = B_MN ? tmap_mnmajor(h, B.planes, g.N, g.Kc, B.pitch, B.plane, &map_b)
                       : tmap_kmajor(h, B.planes, g.N, g.Kc, B.pitch, B.plane, BN / CM, &map_b)) return st;
+    Epi e = epi;
+    if constexpr (C::kOperandBytes > 0)
+      if (int st = tmap_f32_2d(h, e.operand(), (uint64_t)e.operand_ld(), (uint64_t)e.operand_cols(), (uint64_t)e.operand_ld(), tgemm::kBM, BN,
+                               &e.operand_map)) return st;
     PlaneGemmArgs args{};
     args.M = g.M; args.N = g.N; args.Kc = g.Kc;
     args.m_tiles = g.m_tiles;
@@ -288,7 +319,7 @@ struct PlaneGemmInstance {
       h->debug_timing_cursor += (size_t)grid.x * grid.y * grid.z * 8;
     }
     return launch_ex(h, "plane_gemm_kernel", kernel, grid, dim3(tgemm::kThreads), (size_t)C::kTotal, stream, h->nmf_pdl,
-                     args.z_cluster > 1 ? dim3(1, 1, args.z_cluster) : (mf ? dim3(CM, 1, 1) : dim3(CN, CM, 1)), map_a, map_b, args, epi);
+                     args.z_cluster > 1 ? dim3(1, 1, args.z_cluster) : (mf ? dim3(CM, 1, 1) : dim3(CN, CM, 1)), map_a, map_b, args, e);
   }
 };
 
