@@ -263,6 +263,29 @@ LLBANK_MAX_STEERINGS = 64
 RECORD_KIND_LLBANK = 3
 
 
+_LLDICT = [_H, _LC, c_int, c_int, c_int, c_int, _P, c_size_t]   # handle, config, num_sources, history_length, num_dictionaries, num_steerings, state, state_bytes
+SIGNATURES.update({
+    'gccnmf_lldict_state_bytes': (c_size_t, [_LC, c_int, c_int, c_int, c_int]),
+    'gccnmf_lldict_init': (c_int, [_H, _LC, c_int, c_int, c_int, c_int, ctypes.POINTER(c_void_p), ctypes.POINTER(c_int), ctypes.POINTER(c_void_p),
+                                   _P, _P, _P, c_float, _P, c_size_t, _S]),
+    'gccnmf_lldict_load_dictionary': (c_int, _LLDICT + [c_int, _P, c_int, _P, _S]),
+    'gccnmf_lldict_load_steering': (c_int, _LLDICT + [c_int, _P, _S]),
+    'gccnmf_lldict_assign': (c_int, _LLDICT + [c_int, c_int, ctypes.POINTER(c_int32), ctypes.POINTER(c_int32), _S]),
+    'gccnmf_lldict_reset_streams': (c_int, _LLDICT + [c_int, c_int, _S]),
+    'gccnmf_lldict_set_params': (c_int, _LLDICT + [c_int, c_int, ctypes.POINTER(LLStreamParams), _S]),
+    'gccnmf_lldict_set_targets': (c_int, _LLDICT + [c_int, c_int, ctypes.POINTER(c_int32), _S]),
+    'gccnmf_lldict_set_window': (c_int, _LLDICT + [c_int, c_int, ctypes.POINTER(c_int32), _S]),
+    'gccnmf_lldict_process': (c_int, _LLDICT + [c_int, _P, _P, _S]),
+    'gccnmf_lldict_graph_create': (c_int, _LLDICT + [c_int, _P, _P, _P, _P, ctypes.POINTER(c_void_p), _S]),
+    'gccnmf_lldict_export': (c_int, _LLDICT + [c_int, c_int, c_void_p, _S]),
+    'gccnmf_lldict_record_bytes': (c_size_t, [_LC, c_int, c_int, c_int, c_int]),
+    'gccnmf_lldict_workspace_bytes': (c_size_t, [_LC, c_int, c_int, c_int, c_int, c_int]),
+    'gccnmf_lldict_save_streams': (c_int, _LLDICT + [c_int, c_int, c_void_p, c_size_t, _P, c_size_t, _S]),
+    'gccnmf_lldict_load_streams': (c_int, _LLDICT + [c_int, c_int, c_void_p, c_size_t, _P, c_size_t, _S]),
+})
+LLDICT_MAX_DICTIONARIES = 64
+
+
 class LLBankRecordHeader(ctypes.Structure):
     """gccnmf_llbank_record_header (include/gccnmf_b200.h): RecordHeader's fields, then the content digests of the dictionary and of
     the stream's steering table."""

@@ -151,6 +151,21 @@ __device__ __forceinline__ int steer_tile(const SteerBank& b, int tile, int cta,
 }
 inline int steer_tiles_max(int T, int tile, int Qe) { return (T + tile - 1) / tile + Qe; }
 
+// A bank of Qd dictionaries for the columns of a low-latency call (gccnmf_lldict_*): entry e has K[e] <= Kmax atoms, W (F, K[e])
+// f32 row-major at W + e wstride, its |W| column sums at colsum + e Kp, its transpose (K[e], Fp) at WT + e Kp Fp, rowsum(W) at
+// rowsum + e F and its bf16 hi / lo planes as columns [e Kp, e Kp + Kp) of two (F, Qd Kp) planes (zero past K[e]).  Column t is on
+// entry assign[t / hops]; order / seg sort the streams by entry as SteerBank's do, and segments() views them for steer_tile.
+struct DictBank {
+  const float *W, *colsum, *WT, *rowsum;
+  const void* planes;
+  const int32_t *K, *assign, *order, *seg;
+  int Qd, hops, Kp, Kmax;
+  int64_t wstride, Fp;
+  __device__ __forceinline__ int entry(int t) const { return __ldg(assign + t / hops); }
+  __device__ __forceinline__ int column(int u) const { return __ldg(order + u / hops) * hops + u % hops; }
+  __device__ __forceinline__ SteerBank segments() const { return SteerBank{nullptr, nullptr, assign, order, seg, Qd, hops, Fp}; }
+};
+
 // scipy.signal.argrelmax(x) (order 1, mode 'clip': strict local maxima, never the end points), then the S largest peaks
 // (gccNMFFunctions.py:100: peakIndexes[argsort(x[peakIndexes])[-numSources:]]) in ascending index order (:113), by every thread of
 // one CTA.  x: D values in shared memory, written before the call; peak / chosen: D bytes of shared scratch.  Thread 0 writes the

@@ -925,3 +925,214 @@ int gccnmf_target_gccnmf_bank(gccnmf_handle* h, const float* coherence, int F, i
   }
   return GCCNMF_OK;
 }
+
+// ---- dictionary banks (gccnmf_lldict_*): the forms above whose CTA takes its columns from one dictionary's segment (steer_tile on the
+// dictionary sort) and contracts over that entry's W and K, so every value is the same fma chain a plain kernel over (W_e, K_e) runs.
+namespace {
+
+// B(n = j D + d, k = f) = Re(coherence[f][t] E_t[f][d]) for frame j of the tile, t = its column, E_t the table of t's stream
+struct LoadRealGCCDict {
+  static constexpr bool kContigK = false;
+  const float2* coh; SteerBank bank; DictBank dict; int F, T, D, u0, N;
+  __device__ double operator()(int n, int f) const {
+    if (n >= N || f >= F) return 0.0;
+    const int j = n / D, d = n - j * D, t = dict.column(u0 + j);
+    return re_coh_steer(__ldg(coh + (int64_t)f * T + t), __ldg(bank.E + ((int64_t)bank.entry(t) * F + f) * D + d));
+  }
+};
+struct LoadTargetGCCDict {
+  static constexpr bool kContigK = false;
+  const float2* coh; SteerBank bank; DictBank dict; const int32_t* targets; int F, T, D, P, u0, N;
+  __device__ double operator()(int n, int f) const {
+    if (n >= N || f >= F) return 0.0;
+    const int j = n / P, q = n - j * P, t = dict.column(u0 + j);
+    return re_coh_steer(__ldg(coh + (int64_t)f * T + t), __ldg(bank.E + ((int64_t)bank.entry(t) * F + f) * D + __ldg(targets + (int64_t)t * P + q)));
+  }
+};
+
+__global__ void __launch_bounds__(kGccThreads)
+tdoa_argmax_dict_kernel(int F, SteerBank bank, DictBank dict, const float2* __restrict__ coh, int T, int D, int32_t* __restrict__ argmax,
+                        const int32_t* __restrict__ gate, int gate_capacity, int32_t* __restrict__ ran) {
+  if (gate) {
+    if (*gate <= gate_capacity) return;
+    if (ran && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) *ran = 1;
+  }
+  int u0, u1;
+  const int e = steer_tile(dict.segments(), GN / D, blockIdx.x, u0, u1);
+  if (e < 0) return;
+  const int K = __ldg(dict.K + e), m0 = blockIdx.y * GM;
+  if (m0 >= K) return;
+  const int N = (u1 - u0) * D;
+  LoadWAtoms a{dict.W + e * dict.wstride, K, F};
+  LoadRealGCCDict b{coh, bank, dict, F, T, D, u0, N};
+  double acc[GTM][GTN];
+  gemm_simt_mainloop<double, GM, GN, GK, GTM, GTN>(acc, m0, 0, F, a, b);
+  constexpr int TX = GN / GTN;
+  const int tx = threadIdx.x % TX;
+  const int lanes = min(D / 4, TX);
+#pragma unroll
+  for (int i = 0; i < GTM; ++i) {
+    const int m = gemm_row<GM, GTM, TX>(m0, i);
+    double bv[2];
+    int bi[2];
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      const int d0 = (half * (GN / 2) + tx * (GTN / 2)) % D;
+      bv[half] = acc[i][half * (GTN / 2)];
+      bi[half] = d0;
+#pragma unroll
+      for (int j = 1; j < GTN / 2; ++j) {
+        const double v = acc[i][half * (GTN / 2) + j];
+        if (argmax_better(v, d0 + j, bv[half], bi[half])) { bv[half] = v; bi[half] = d0 + j; }
+      }
+    }
+    if (D == GN) {
+      if (argmax_better(bv[1], bi[1], bv[0], bi[0])) { bv[0] = bv[1]; bi[0] = bi[1]; }
+    }
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      if (D == GN && half == 1) break;
+      for (int o = 1; o < lanes; o <<= 1) {
+        const double ov = __shfl_xor_sync(0xffffffffu, bv[half], o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi[half], o);
+        if (argmax_better(ov, oi, bv[half], bi[half])) { bv[half] = ov; bi[half] = oi; }
+      }
+      const int n_first = half * (GN / 2) + tx * (GTN / 2);
+      if ((tx % lanes) == 0 && m < K && n_first < N) argmax[(int64_t)m * T + dict.column(u0 + n_first / D)] = bi[half];
+    }
+  }
+}
+
+// values (P, Kmax, T): rows < K_e of each column; the rows above are the caller's to fill
+__global__ void __launch_bounds__(kGccThreads)
+target_gccnmf_dict_kernel(int F, SteerBank bank, DictBank dict, const float2* __restrict__ coh, const int32_t* __restrict__ targets, int T, int D,
+                          int P, float* __restrict__ values) {
+  int u0, u1;
+  const int e = steer_tile(dict.segments(), GN / P, blockIdx.x, u0, u1);
+  if (e < 0) return;
+  const int K = __ldg(dict.K + e), m0 = blockIdx.y * GM;
+  if (m0 >= K) return;
+  const int N = (u1 - u0) * P;
+  LoadWAtoms a{dict.W + e * dict.wstride, K, F};
+  LoadTargetGCCDict b{coh, bank, dict, targets, F, T, D, P, u0, N};
+  double acc[GTM][GTN];
+  gemm_simt_mainloop<double, GM, GN, GK, GTM, GTN>(acc, m0, 0, F, a, b);
+  constexpr int TX = GN / GTN;
+#pragma unroll
+  for (int i = 0; i < GTM; ++i) {
+    const int m = gemm_row<GM, GTM, TX>(m0, i);
+    if (m >= K) continue;
+#pragma unroll
+    for (int j = 0; j < GTN; ++j) {
+      const int n = gemm_col<GN, GTN, TX>(0, j);
+      if (n >= N) continue;
+      const int jj = n / P, q = n - jj * P;
+      values[((int64_t)q * dict.Kmax + m) * T + dict.column(u0 + jj)] = (float)acc[i][j];
+    }
+  }
+}
+
+// B(n, k) of the Wiener filters for tile column n (sorted position u0 + n): mask[k][t] (H == NULL) or H[k][c T + t] (* mask[k][t])
+struct LoadDictCols {
+  static constexpr bool kContigK = false;
+  const float* H; const float* mask; DictBank dict; int K, T, u0, N; int64_t ldh;
+  __device__ float operator()(int n, int k) const {
+    if (n >= N || k >= K) return 0.f;
+    const int t = dict.column(u0 + n);
+    if (!H) return __ldg(mask + (int64_t)k * T + t);
+    const float hv = __ldg(H + (int64_t)k * ldh + t);
+    return mask ? hv * __ldg(mask + (int64_t)k * T + t) : hv;
+  }
+};
+
+// wiener_apply_kernel (H == NULL, rowsum(W_e) from the bank) and wiener_apply_h_kernel (channel c = blockIdx.z) over RN columns of
+// one dictionary segment
+template <bool WITH_H>
+__global__ void __launch_bounds__(kReconThreads, 2)
+wiener_dict_kernel(const float* __restrict__ mask, DictBank dict, const float* __restrict__ H, const float2* __restrict__ X, int F, int T,
+                   float2* __restrict__ Y, float* __restrict__ wiener) {
+  int u0, u1;
+  const int e = steer_tile(dict.segments(), RN, blockIdx.x, u0, u1);
+  if (e < 0) return;
+  const int K = __ldg(dict.K + e), c = blockIdx.z, N = u1 - u0;
+  const int m0 = blockIdx.y * RM;
+  LoadWRows a{dict.W + e * dict.wstride, F, K};
+  float num[RTM][RTN], den[WITH_H ? RTM : 1][WITH_H ? RTN : 1];
+  if constexpr (WITH_H) {
+    LoadDictCols masked{H + (int64_t)c * T, mask, dict, K, T, u0, N, (int64_t)2 * T}, plain{H + (int64_t)c * T, nullptr, dict, K, T, u0, N, (int64_t)2 * T};
+    gemm_simt_mainloop<float, RM, RN, RK, RTM, RTN>(num, m0, 0, K, a, masked);
+    gemm_simt_mainloop<float, RM, RN, RK, RTM, RTN>(den, m0, 0, K, a, plain);
+  } else {
+    LoadDictCols b{nullptr, mask, dict, K, T, u0, N, 0};
+    gemm_simt_mainloop<float, RM, RN, RK, RTM, RTN>(num, m0, 0, K, a, b);
+  }
+#pragma unroll
+  for (int i = 0; i < RTM; ++i) {
+    const int m = gemm_row<RM, RTM, RN / RTN>(m0, i);
+    if (m >= F) continue;
+    const float rs = WITH_H ? 0.f : __ldg(dict.rowsum + (int64_t)e * F + m);
+#pragma unroll
+    for (int j = 0; j < RTN; ++j) {
+      const int n = gemm_col<RN, RTN, RN / RTN>(0, j);
+      if (n >= N) continue;
+      const int t = dict.column(u0 + n);
+      if constexpr (WITH_H) {
+        const float w = num[i][j] / den[i][j];
+        const int64_t o = ((int64_t)c * F + m) * T + t;
+        if (wiener) wiener[o] = w;
+        const float2 x = X[o];
+        Y[o] = float2{w * x.x, w * x.y};
+      } else {
+        const float w = num[i][j] / rs;
+        if (wiener) wiener[(int64_t)m * T + t] = w;
+#pragma unroll
+        for (int cc = 0; cc < 2; ++cc) {
+          const float2 x = X[((int64_t)cc * F + m) * T + t];
+          Y[((int64_t)cc * F + m) * T + t] = float2{w * x.x, w * x.y};
+        }
+      }
+    }
+  }
+}
+
+}  // namespace
+
+int gccnmf_tdoa_gccnmf_dict(gccnmf_handle* h, const float* coherence, int F, int T, const SteerBank& bank, const DictBank& dict, int D,
+                            int32_t* argmax, const int32_t* gate, int capacity, int32_t* ran, void* stream) {
+  GCCNMF_REQUIRE(h, F > 0 && T > 0 && coherence && argmax && bank.Qe >= 1 && dict.Qd >= 1, "tdoa_gccnmf_dict: bad arguments");
+  GCCNMF_REQUIRE(h, (int64_t)T * D < (int64_t)1 << 31, "tdoa_gccnmf_dict: T * D overflows int32");
+  if (!(is_pow2(D) && D >= 4 && D <= GN))
+    return gccnmf_fail(h, GCCNMF_ERR_UNSUPPORTED, "tdoa_gccnmf_dict: numTDOAs must be a power of two in [4, %d] (got %d)", GN, D);
+  GCCNMF_LAUNCH(h, tdoa_argmax_dict_kernel, dim3(steer_tiles_max(T, GN / D, dict.Qd), (dict.Kmax + GM - 1) / GM), kGccThreads, 0, stream, F, bank,
+                dict, reinterpret_cast<const float2*>(coherence), T, D, argmax, gate, capacity, ran);
+  return GCCNMF_OK;
+}
+
+int gccnmf_target_gccnmf_dict(gccnmf_handle* h, const float* coherence, int F, int T, const SteerBank& bank, const DictBank& dict, int D,
+                              const int32_t* targets, int P, float* values, void* stream) {
+  GCCNMF_REQUIRE(h, F > 0 && T > 0 && P > 0 && P <= GN && coherence && targets && values && bank.Qe >= 1 && dict.Qd >= 1,
+                 "target_gccnmf_dict: bad arguments");
+  GCCNMF_LAUNCH(h, target_gccnmf_dict_kernel, dim3(steer_tiles_max(T, GN / P, dict.Qd), (dict.Kmax + GM - 1) / GM), kGccThreads, 0, stream, F, bank,
+                dict, reinterpret_cast<const float2*>(coherence), targets, T, D, P, values);
+  return GCCNMF_OK;
+}
+
+// H == NULL: gccnmf_wiener_apply's filter; else gccnmf_wiener_apply_h's, per column on its dictionary
+int gccnmf_wiener_dict(gccnmf_handle* h, const float* mask, const DictBank& dict, const float* H, const float* X, int F, int T, float* Y, float* wiener,
+                       void* stream) {
+  GCCNMF_REQUIRE(h, mask && X && Y && F > 0 && T > 0 && dict.Qd >= 1, "wiener_dict: bad arguments");
+  const dim3 grid(steer_tiles_max(T, RN, dict.Qd), (F + RM - 1) / RM, H ? 2 : 1);
+  if (H)
+    GCCNMF_LAUNCH(h, wiener_dict_kernel<true>, grid, kReconThreads, 0, stream, mask, dict, H, reinterpret_cast<const float2*>(X), F, T,
+                  reinterpret_cast<float2*>(Y), wiener);
+  else
+    GCCNMF_LAUNCH(h, wiener_dict_kernel<false>, grid, kReconThreads, 0, stream, mask, dict, H, reinterpret_cast<const float2*>(X), F, T,
+                  reinterpret_cast<float2*>(Y), wiener);
+  return GCCNMF_OK;
+}
+
+// rowsum(W) (F) as gccnmf_wiener_apply computes it
+int gccnmf_rowsum_w(gccnmf_handle* h, const float* W, int F, int K, float* rowsum, void* stream) {
+  GCCNMF_LAUNCH(h, rowsum_w_kernel, F, 128, 0, stream, W, F, K, rowsum);
+  return GCCNMF_OK;
+}

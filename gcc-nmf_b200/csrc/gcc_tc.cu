@@ -363,6 +363,173 @@ int launch_argmax_persistent(gccnmf_handle* h, const CUtensorMap& map_a, const C
                    false, dim3(1, 1, 1), map_a, map_b, K, N, F, m_tiles, n_tiles, epi);
 }
 
+// ------------------------------------------------------------------ step 2 for a dictionary bank (gccnmf_lldict_*)
+// argmax_gemm_persistent_kernel over Qd dictionaries in one launch.  An n tile holds up to 256 / D frames of ONE entry's segment in
+// sorted order (steer_tile), an m tile 128 of that entry's atoms; tiles past the last segment or at or above K[e] are skipped by
+// the producer and the consumers alike.  A is the stacked (F, Qd Kp) planes, so entry e's tile starts at column e Kp + m0.  B is
+// gathered: 256 / D boxes of D rows (one frame each) per plane and k-block from G as the plain build lays it out; every box starts
+// on a swizzle-atom boundary (D x 64 bytes), so the stage holds the image one 256-row box would, and the MMA code is the plain
+// kernel's.  A short tile repeats its first frame in the unused slots (the transaction count stays fixed); the epilogue drops them.
+struct EpiArgmaxDict {
+  int32_t* __restrict__ argmax;        // (Kmax, T)
+  int2* __restrict__ list; uint4* __restrict__ candidates; int* __restrict__ count; int capacity;
+  int T; float margin_factor;
+};
+
+template <int D>
+__global__ void __launch_bounds__(tgemm::kThreads, 1)
+argmax_gemm_dict_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, int Kc, int m_tiles, int n_tiles,
+                        DictBank dict, EpiArgmaxDict epi) {
+  using namespace tgemm;
+  static_assert(D >= 32 && D <= 128 && kPersBN % D == 0, "whole frames of at most 128 TDOAs per tile");
+  constexpr int kFrames = kPersBN / D;
+  extern __shared__ unsigned char smem_dyn[];
+  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~uintptr_t(1023));
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kPersStages * kPersStageBytes);
+  uint64_t* full = bars;
+  uint64_t* empty = bars + kPersStages;
+  if (tid == 0) {
+    for (int s = 0; s < kPersStages; ++s) { mbar_init(smem_u32(&full[s]), 1); mbar_init(smem_u32(&empty[s]), kMmaWarpgroups); }
+    gmma::fence_barrier_init();
+    tma_prefetch_descriptor(&map_a);
+    tma_prefetch_descriptor(&map_b);
+  }
+  __syncthreads();
+  const int total_tiles = m_tiles * n_tiles;
+  const int num_kb = (Kc + kPersKB - 1) / kPersKB;
+  const SteerBank segs = dict.segments();
+  // the tile's entry (-1: skipped), first atom and sorted positions [u0, u1)
+  auto decode = [&](int tile, int& m0, int& u0, int& u1) {
+    m0 = (tile % m_tiles) * kBM;
+    const int e = steer_tile(segs, kFrames, tile / m_tiles, u0, u1);
+    return (e >= 0 && m0 < __ldg(dict.K + e)) ? e : -1;
+  };
+
+  if (warp == 0) {
+    if (lane == 0) {
+      uint32_t g = 0;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        int m0, u0, u1;
+        const int e = decode(tile, m0, u0, u1);
+        if (e < 0) continue;
+        int rows[kFrames];
+#pragma unroll
+        for (int j = 0; j < kFrames; ++j) rows[j] = dict.column(u0 + j < u1 ? u0 + j : u0) * D;
+        const int ma = e * dict.Kp + m0;
+        for (int i = 0; i < num_kb; ++i, ++g) {
+          const int s = g % kPersStages;
+          const uint32_t use = g / kPersStages;
+          if (use > 0) mbar_wait(smem_u32(&empty[s]), (use - 1) & 1);
+          const uint32_t bar = smem_u32(&full[s]);
+          const uint32_t a_dst = smem_u32(smem + (size_t)s * kPersStageBytes), b_dst = a_dst + kPersABytes;
+          mbar_arrive_expect_tx(bar, kPersStageBytes);
+          const int k0 = i * kPersKB;
+#pragma unroll
+          for (int a = 0; a < 2; ++a) tma_load_3d(a_dst + a * kPersAtomBytes, &map_a, bar, ma + 64 * a, k0, 0);
+#pragma unroll
+          for (int p = 0; p < 2; ++p)
+#pragma unroll
+            for (int j = 0; j < kFrames; ++j) tma_load_3d(b_dst + p * (kPersBN * kPersKB * 2) + j * (D * kPersKB * 2), &map_b, bar, k0, rows[j], p);
+        }
+      }
+    }
+    __syncwarp();
+  } else if (warp >= 4) {
+    const int g = (warp >> 2) - 1, wt = tid & 127;
+    const int c0 = 2 * (wt & 3);
+    constexpr int kGroups = D / 8, kWords = (D + 31) / 32;
+    uint32_t gk = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      int m0, u0, u1;
+      const int e = decode(tile, m0, u0, u1);
+      if (e < 0) continue;
+      const int K = __ldg(dict.K + e);
+      float acc[kPersBN / 2];
+#pragma unroll
+      for (int j = 0; j < kPersBN / 2; ++j) acc[j] = 0.f;
+      for (int i = 0; i < num_kb; ++i, ++gk) {
+        const int s = gk % kPersStages;
+        mbar_wait(smem_u32(&full[s]), (gk / kPersStages) & 1);
+        const uint32_t a_base = smem_u32(smem + (size_t)s * kPersStageBytes), b_base = a_base + kPersABytes;
+        gmma::fence_regs(acc);
+        gmma::wgmma_fence();
+        mma_kblock<kPersBN, kPersKB, true, false, false>(acc, a_base + g * kPersAtomBytes, b_base, kPersBN * kPersKB * 2);
+        gmma::wgmma_commit();
+        gmma::fence_regs(acc);
+        gmma::wgmma_wait<1>();
+        if (i > 0 && wt == 0) gmma::mbar_arrive(smem_u32(&empty[(gk - 1) % kPersStages]));
+      }
+      gmma::wgmma_wait<0>();
+      gmma::fence_regs(acc);
+      if (num_kb > 0 && wt == 0) gmma::mbar_arrive(smem_u32(&empty[(gk - 1) % kPersStages]));
+
+      const int frames = u1 - u0;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int m = m0 + 64 * g + 16 * (wt >> 5) + ((wt & 31) >> 2) + 8 * h;
+        const float margin = m < K ? epi.margin_factor * __ldg(dict.colsum + (int64_t)e * dict.Kp + m) : 0.f;
+#pragma unroll
+        for (int fr = 0; fr < kFrames; ++fr) {
+          ArgmaxPartial p{-INFINITY, -INFINITY, 0, 0};
+#pragma unroll
+          for (int q = 0; q < kGroups; ++q) {
+            p.scan(acc[4 * (fr * kGroups + q) + 2 * h], 8 * q + c0);
+            p.scan(acc[4 * (fr * kGroups + q) + 2 * h + 1], 8 * q + c0 + 1);
+          }
+          p.merge_xor(1);
+          p.merge_xor(2);
+          const bool valid = m < K && fr < frames;
+          const int t = valid ? dict.column(u0 + fr) : 0;
+          if (valid && (wt & 3) == 0) epi.argmax[(int64_t)m * epi.T + t] = p.idx;
+          const bool near_tie = valid && (p.nan || !(p.best - p.second > margin));
+          if (__any_sync(0xffffffffu, near_tie)) {
+            uint32_t bits[kWords];
+#pragma unroll
+            for (int w = 0; w < kWords; ++w) bits[w] = 0u;
+#pragma unroll
+            for (int q = 0; q < kGroups; ++q)
+#pragma unroll
+              for (int b = 0; b < 2; ++b) {
+                const int d = 8 * q + c0 + b;
+                const float x = acc[4 * (fr * kGroups + q) + 2 * h + b];
+                if (p.nan || !(p.best - x > margin)) bits[d >> 5] |= 1u << (d & 31);
+              }
+#pragma unroll
+            for (int w = 0; w < kWords; ++w) {
+              bits[w] |= __shfl_xor_sync(0xffffffffu, bits[w], 1);
+              bits[w] |= __shfl_xor_sync(0xffffffffu, bits[w], 2);
+            }
+            if (near_tie && (wt & 3) == 0) {
+              const int slot = atomicAdd(epi.count, 1);
+              if (slot < epi.capacity) {
+                uint32_t b4[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+                for (int w = 0; w < kWords; ++w) b4[w] = bits[w];
+                epi.list[slot] = make_int2(m, t);
+                epi.candidates[slot] = make_uint4(b4[0], b4[1], b4[2], b4[3]);
+              }
+            }
+          }
+        }
+      }
+    }
+  }
+}
+
+template <int D>
+int launch_argmax_dict(gccnmf_handle* h, const CUtensorMap& map_a, const CUtensorMap& map_b, int F, int m_tiles, int n_tiles, const DictBank& dict,
+                       const EpiArgmaxDict& epi, void* stream) {
+  static DeviceFlags configured;
+  if (!configured(h)) {
+    GCCNMF_CHECK_CUDA(h, cudaFuncSetAttribute(argmax_gemm_dict_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, kPersSmem));
+    configured(h) = true;
+  }
+  const int ctas = std::min(h->sm_count, m_tiles * n_tiles);
+  return launch_ex(h, "argmax_gemm_dict_kernel", argmax_gemm_dict_kernel<D>, dim3(ctas), dim3(tgemm::kThreads), (size_t)kPersSmem, stream, false,
+                   dim3(1, 1, 1), map_a, map_b, F, m_tiles, n_tiles, dict, epi);
+}
+
 // ------------------------------------------------------------------ step 3: exact float64 recomputation of flagged (atom, frame) pairs
 __device__ __forceinline__ bool argmax_better64(double v, int i, double bv, int bi) {   // numpy.argmax: NaN is a maximum, first wins
   const bool vn = v != v, bn = bv != bv;
@@ -647,6 +814,93 @@ refine_candidates_bank_kernel(const int2* __restrict__ list, const uint4* __rest
     }
     if (lane == 0 && bi >= 0) argmax[(int64_t)k * T + t] = bi;
   }
+}
+
+// refine_candidates_bank_kernel for a dictionary bank: a pair also reads the transposed W of its column's dictionary.
+__global__ void __launch_bounds__(256)
+refine_candidates_dict_kernel(const int2* __restrict__ list, const uint4* __restrict__ candidates, const int* __restrict__ count, int capacity,
+                              const float2* __restrict__ cohT, DictBank dict, SteerBank bank, int F, int64_t Fp, int D, int T,
+                              int32_t* __restrict__ argmax) {
+  __shared__ double re_s[8][kRefineGroup][33];
+  __shared__ double w_s[8][32];
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  double (*re)[33] = re_s[wib];
+  double* wv = w_s[wib];
+  const int warps = gridDim.x * (blockDim.x >> 5);
+  const int n = min(*count, capacity);
+  for (int p = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); p < n; p += warps) {
+    const int k = list[p].x, t = list[p].y;
+    const uint4 c4 = candidates[p];
+    uint32_t bits[4] = {c4.x, c4.y, c4.z, c4.w};
+    const float2* crow = cohT + (int64_t)t * Fp;
+    const float* wrow = dict.WT + ((int64_t)dict.entry(t) * dict.Kp + k) * Fp;
+    const double2* ET = bank.ET + (int64_t)bank.entry(t) * D * Fp;
+    double bv = 0.0;
+    int bi = -1;
+    int word = 0;
+    while (true) {
+      int ds[kRefineGroup], nd = 0;
+      while (nd < kRefineGroup && word < 4) {
+        if (bits[word] == 0u) { ++word; continue; }
+        const int b = __ffs(bits[word]) - 1;
+        bits[word] &= bits[word] - 1;
+        ds[nd++] = word * 32 + b;
+      }
+      if (nd == 0) break;
+      double g[kRefineGroup], w = 0.0;
+      auto load = [&](int f0) {
+        const int f = f0 + lane;
+        if (f >= F) return;
+        const float2 c = crow[f];
+        w = (double)wrow[f];
+#pragma unroll
+        for (int j = 0; j < kRefineGroup; ++j)
+          if (j < nd) {
+            const double2 e = ET[(int64_t)ds[j] * Fp + f];
+            g[j] = (double)c.x * e.x - (double)c.y * e.y;
+          }
+      };
+      load(0);
+      double acc = 0.0;
+      for (int f0 = 0; f0 < F; f0 += 32) {
+#pragma unroll
+        for (int j = 0; j < kRefineGroup; ++j)
+          if (j < nd) re[j][lane] = g[j];
+        wv[lane] = w;
+        __syncwarp();
+        if (f0 + 32 < F) load(f0 + 32);
+        if (lane < nd) {
+          const double* r = re[lane];
+          if (F - f0 >= 32) {
+#pragma unroll 8
+            for (int s = 0; s < 32; ++s) acc = fma(r[s], wv[s], acc);
+          } else {
+            for (int s = 0; s < F - f0; ++s) acc = fma(r[s], wv[s], acc);
+          }
+        }
+        __syncwarp();
+      }
+#pragma unroll
+      for (int j = 0; j < kRefineGroup; ++j) {
+        if (j < nd) {
+          const double v = __shfl_sync(0xffffffffu, acc, j);
+          if (bi < 0 || argmax_better64(v, ds[j], bv, bi)) { bv = v; bi = ds[j]; }
+        }
+      }
+    }
+    if (lane == 0 && bi >= 0) argmax[(int64_t)k * T + t] = bi;
+  }
+}
+
+// A dictionary's bf16 planes: columns [e Kp, e Kp + Kp) of the (F, Qd Kp) planes, W (F, K) as it lies, zero past K.
+__global__ void split_dict_planes_kernel(const float* __restrict__ W, int F, int K, int Kp, int64_t ld, bf16* __restrict__ planes, int64_t plane) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)F * Kp) return;
+  const int f = (int)(i / Kp), k = (int)(i - (int64_t)f * Kp);
+  bf16 hi, lo;
+  split_bf16(k < K ? W[(int64_t)f * K + k] : 0.f, hi, lo);
+  planes[(int64_t)f * ld + k] = hi;
+  planes[plane + (int64_t)f * ld + k] = lo;
 }
 
 // dst (cols, ld) = src (rows, cols)^T for 4-, 8- and 16-byte elements (zero in the pad columns [rows, ld))
@@ -954,5 +1208,64 @@ int gccnmf_tdoa_argmax_bank(gccnmf_handle* h, const float* coherence, int F, int
 int gccnmf_steering_transpose(gccnmf_handle* h, const double* E, int F, int D, double* ET, int64_t Fp, void* stream) {
   GCCNMF_LAUNCH(h, transpose_pad_kernel<double2>, dim3((D + 31) / 32, (int)((Fp + 31) / 32)), dim3(32, 8), 0, stream, reinterpret_cast<const double2*>(E), F,
                 D, reinterpret_cast<double2*>(ET), Fp);
+  return GCCNMF_OK;
+}
+
+// ---- dictionary banks (gccnmf_lldict_*)
+// Entry e's derived forms from its W (F, K) f32 on the device: the bf16 planes (zero past K), the |W| column sums and the transpose
+// (K, Fp) the refinement reads.  abs_colsum_kernel and transpose_pad_kernel are the plain argmax's, so the values are its values.
+int gccnmf_lldict_prepare(gccnmf_handle* h, const DictBank& dict, int entry, const float* W, int F, int K, void* stream) {
+  const int64_t ld = (int64_t)dict.Qd * dict.Kp, n = (int64_t)F * dict.Kp;
+  bf16* planes = reinterpret_cast<bf16*>(const_cast<void*>(dict.planes)) + (int64_t)entry * dict.Kp;
+  GCCNMF_LAUNCH(h, split_dict_planes_kernel, (unsigned)((n + 255) / 256), 256, 0, stream, W, F, K, dict.Kp, ld, planes, (int64_t)F * ld);
+  GCCNMF_LAUNCH(h, abs_colsum_kernel, (K + 127) / 128, 128, 0, stream, W, F, K, const_cast<float*>(dict.colsum) + (int64_t)entry * dict.Kp);
+  GCCNMF_LAUNCH(h, transpose_pad_kernel<float>, dim3((K + 31) / 32, (int)((dict.Fp + 31) / 32)), dim3(32, 8), 0, stream, W, F, K,
+                const_cast<float*>(dict.WT) + (int64_t)entry * dict.Kp * dict.Fp, dict.Fp);
+  return GCCNMF_OK;
+}
+
+// gcc.cu
+int gccnmf_tdoa_gccnmf_dict(gccnmf_handle* h, const float* coherence, int F, int T, const SteerBank& bank, const DictBank& dict, int D,
+                            int32_t* argmax, const int32_t* gate, int capacity, int32_t* ran, void* stream);
+
+size_t gccnmf_tdoa_argmax_dict_workspace_bytes(int F, int T, int D, int K) { return argmax_workspace_bytes(F, T, D, K); }
+
+// The tensor-core argmax for a dictionary bank: the plane build of the steering bank, ONE grouped GEMM launch over every entry
+// (argmax_gemm_dict_kernel), then the candidate refinement over the column's table and dictionary.  The workspace is
+// gccnmf_tdoa_argmax's at K = Kmax (its W planes and sums go unused: the bank keeps its own).  Without the tensor path (D < 32,
+// F < 32 or the SIMT option) the float64 SIMT form decides every pair.
+int gccnmf_tdoa_argmax_dict(gccnmf_handle* h, const float* coherence, int F, int T, const SteerBank& bank, const DictBank& dict, int D,
+                            int32_t* argmax, int32_t* overflow_flag, void* workspace, size_t workspace_bytes, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, F > 0 && T > 0 && D > 0 && coherence && argmax && bank.Qe >= 1 && dict.Qd >= 1, "tdoa_argmax_dict: bad arguments");
+  if (h->force_simt_nmf || D < 32 || D > 128 || F < 32 || (int64_t)T * D >= ((int64_t)1 << 31)) {
+    if (overflow_flag) GCCNMF_CHECK_CUDA(h, cudaMemsetAsync(overflow_flag, 0, sizeof(int32_t), (cudaStream_t)stream));
+    return gccnmf_tdoa_gccnmf_dict(h, coherence, F, T, bank, dict, D, argmax, nullptr, 0, nullptr, stream);
+  }
+  const int K = dict.Kmax;
+  const size_t need = argmax_workspace_bytes(F, T, D, K);
+  ArgmaxWorkspace w = carve_argmax(workspace, workspace_bytes, F, T, D, K);
+  if (!w.ok || workspace_bytes < need) return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "tdoa_argmax_dict workspace too small: need %zu bytes", need);
+  GCCNMF_REQUIRE(h, bank.Fp == w.Fp && dict.Fp == w.Fp, "tdoa_argmax_dict: the banks' transposed tables have %lld bins, the workspace %lld",
+                 (long long)bank.Fp, (long long)w.Fp);
+  GCCNMF_CHECK_CUDA(h, cudaMemsetAsync(w.count, 0, 16, (cudaStream_t)stream));
+  GCCNMF_LAUNCH(h, build_gcc_planes_bank_kernel, dim3((int)((w.Fp + 63) / 64), steer_tiles_max(T, 32, bank.Qe)), 256, 0, stream,
+                reinterpret_cast<const float2*>(coherence), F, T, bank, D, w.Gp, w.Fp, w.plane_g);
+  const int64_t ld = (int64_t)dict.Qd * dict.Kp;
+  const bf16* planes = reinterpret_cast<const bf16*>(dict.planes);
+  CUtensorMap map_a, map_b;
+  if (int st = tmap_mnmajor(h, planes, (int)ld, F, ld, (int64_t)F * ld, &map_a)) return st;
+  if (int st = tmap_kmajor(h, w.Gp, T * D, F, w.Fp, w.plane_g, D, &map_b)) return st;
+  const int m_tiles = (K + tgemm::kBM - 1) / tgemm::kBM, n_tiles = steer_tiles_max(T * D, kPersBN, dict.Qd) ;
+  const EpiArgmaxDict epi{argmax, w.list, w.cand, w.count, w.capacity, T, margin_factor(F)};
+  const int st = D == 32 ? launch_argmax_dict<32>(h, map_a, map_b, F, m_tiles, n_tiles, dict, epi, stream)
+               : D == 64 ? launch_argmax_dict<64>(h, map_a, map_b, F, m_tiles, n_tiles, dict, epi, stream)
+                         : launch_argmax_dict<128>(h, map_a, map_b, F, m_tiles, n_tiles, dict, epi, stream);
+  if (st) return st;
+  GCCNMF_LAUNCH(h, transpose_pad_kernel<float2>, dim3((T + 31) / 32, (int)((w.Fp + 31) / 32)), dim3(32, 8), 0, stream,
+                reinterpret_cast<const float2*>(coherence), F, T, w.cohT, w.Fp);
+  GCCNMF_LAUNCH(h, refine_candidates_dict_kernel, h->sm_count * 8, 256, 0, stream, w.list, w.cand, w.count, w.capacity, w.cohT, dict, bank, F, w.Fp,
+                D, T, argmax);
+  if (overflow_flag) GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(overflow_flag, w.count, sizeof(int), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return GCCNMF_OK;
 }

@@ -54,6 +54,17 @@ int gccnmf_tdoa_gccnmf_bank(gccnmf_handle* h, const float* coherence, int F, int
 int gccnmf_target_gccnmf_bank(gccnmf_handle* h, const float* coherence, int F, int T, const SteerBank& bank, int D, const float* W, int K,
                               const int32_t* targets, int P, float* values, void* stream);
 int gccnmf_steering_transpose(gccnmf_handle* h, const double* E, int F, int D, double* ET, int64_t Fp, void* stream);
+int gccnmf_lldict_prepare(gccnmf_handle* h, const DictBank& dict, int entry, const float* W, int F, int K, void* stream);
+int gccnmf_tdoa_argmax_dict(gccnmf_handle* h, const float* coherence, int F, int T, const SteerBank& bank, const DictBank& dict, int D,
+                            int32_t* argmax, int32_t* overflow_flag, void* workspace, size_t workspace_bytes, void* stream);
+size_t gccnmf_tdoa_argmax_dict_workspace_bytes(int F, int T, int D, int K);
+int gccnmf_tdoa_gccnmf_dict(gccnmf_handle* h, const float* coherence, int F, int T, const SteerBank& bank, const DictBank& dict, int D,
+                            int32_t* argmax, const int32_t* gate, int capacity, int32_t* ran, void* stream);
+int gccnmf_target_gccnmf_dict(gccnmf_handle* h, const float* coherence, int F, int T, const SteerBank& bank, const DictBank& dict, int D,
+                              const int32_t* targets, int P, float* values, void* stream);
+int gccnmf_wiener_dict(gccnmf_handle* h, const float* mask, const DictBank& dict, const float* H, const float* X, int F, int T, float* Y, float* wiener,
+                       void* stream);
+int gccnmf_rowsum_w(gccnmf_handle* h, const float* W, int F, int K, float* rowsum, void* stream);
 
 namespace {
 
@@ -99,6 +110,20 @@ struct LLLayout {
   int64_t Fp;
   double* ET;
   int32_t *assign, *order, *seg;
+  // dictionary bank (gccnmf_lldict_*, Qd >= 1, always with Qe >= 1): appended last, per entry e in slots of stride Kp = K rounded up
+  // to 128 (K = Kmax, the largest entry): dW (F, K_e) f32 at e F Kp, packed (row stride K_e, as a plain engine on K_e holds W: the
+  // content digest and the SIMT kernels read it so; only the planes are padded to Kp columns); the bf16 planes dWp, two (F, Qd Kp) arrays, entry e in columns
+  // [e Kp, e Kp + K_e), zero beyond; dcolsum |W| column sums (Kp); dWTr the refinement's transpose (Kp, Fp); dWTi, dcolsumW and dH0
+  // (inference only) ll_dict_kernel's W^T (K_e, F) and column sums, and H0 (K_e, 2); drowsum rowsum(W) (F); then the K_e table (Qd),
+  // the stream -> entry assignment (S), the streams sorted by entry (S) and each entry's first position (Qd + 1)
+  int Qd, Kp;
+  float *dW, *dcolsum, *dWTr, *dWTi, *dcolsumW, *dH0, *drowsum;
+  void* dWp;
+  int32_t *dK, *dassign, *dorder, *dseg;
+  // the grouped argmax's workspace (gccnmf_tdoa_argmax's carve at Kmax, whatever shape the plain argmax supports), when the tensor
+  // path can run (D in [32, 128], F >= 32)
+  void* ws_dict;
+  size_t n_dict;
 };
 
 bool is_pow2(int x) { return x > 0 && (x & (x - 1)) == 0; }
@@ -106,6 +131,7 @@ constexpr int kLLMaxSources = 8;
 constexpr int kLLInferMaxSmem = 227 * 1024;   // the H100's opt-in dynamic shared memory per block
 constexpr int kLLMaxHistory = 1024;
 constexpr int kLLMaxSteerings = 64;
+constexpr int kLLMaxDictionaries = 64;
 
 int ll_check(gccnmf_handle* h, const gccnmf_ll_config* cfg) {
   GCCNMF_REQUIRE(h, cfg != nullptr, "ll: NULL config");
@@ -152,7 +178,16 @@ int ll_check(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Q
   return 0;
 }
 
-LLLayout ll_carve(const gccnmf_ll_config& c, int P, void* base, int Lh = 0, int Qe = 0) {
+// Qd = 0: no dictionary bank; 1 <= Qd <= 64 (gccnmf_lldict_*): a bank of Qd dictionaries, with 1 <= Qe <= 64 steering tables
+int ll_check(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, int Qd) {
+  if (int st = ll_check(h, cfg, P, Lh, Qe)) return st;
+  if (Qd == 0) return 0;
+  GCCNMF_REQUIRE(h, Qd >= 1 && Qd <= kLLMaxDictionaries, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, Qd);
+  GCCNMF_REQUIRE(h, Qe >= 1, "lldict: num_steerings must be in [1, %d] (got %d)", kLLMaxSteerings, Qe);
+  return 0;
+}
+
+LLLayout ll_carve(const gccnmf_ll_config& c, int P, void* base, int Lh = 0, int Qe = 0, int Qd = 0) {
   WorkspaceCarver w(base ? base : reinterpret_cast<void*>(256), base ? ~size_t(0) >> 1 : ~size_t(0) >> 1);
   LLLayout l{};
   l.S = c.num_streams; l.N = c.window_size; l.hop = c.hop_size; l.C = c.hops_per_call; l.K = c.num_atoms; l.D = c.num_tdoas;
@@ -211,18 +246,42 @@ LLLayout ll_carve(const gccnmf_ll_config& c, int P, void* base, int Lh = 0, int 
   l.assign = w.take<int32_t>(Qe ? S : 0);
   l.order = w.take<int32_t>(Qe ? S : 0);
   l.seg = w.take<int32_t>(Qe ? Qe + 1 : 0);
+  // dictionary bank: appended last (nothing is taken with Qd = 0)
+  l.Qd = Qd;
+  l.Kp = (int)((K + 127) / 128 * 128);
+  const size_t Qs = Qd, Kp = l.Kp;
+  l.dW = w.take<float>(Qs * F * Kp);
+  l.dWp = w.take<uint16_t>(2 * F * Qs * Kp);
+  l.dcolsum = w.take<float>(Qs * Kp);
+  l.dWTr = w.take<float>(Qs * Kp * l.Fp);
+  l.dWTi = w.take<float>(inf ? Qs * Kp * F : 0);
+  l.dcolsumW = w.take<float>(inf ? Qs * Kp : 0);
+  l.dH0 = w.take<float>(inf ? Qs * Kp * 2 : 0);
+  l.drowsum = w.take<float>(Qs * F);
+  l.dK = w.take<int32_t>(Qs);
+  l.dassign = w.take<int32_t>(Qd ? S : 0);
+  l.dorder = w.take<int32_t>(Qd ? S : 0);
+  l.dseg = w.take<int32_t>(Qd ? Qd + 1 : 0);
+  l.n_dict = Qd && D >= 32 && D <= 128 && F >= 32 ? gccnmf_tdoa_argmax_dict_workspace_bytes((int)F, (int)T, (int)D, (int)K) : 0;
+  l.ws_dict = w.take<unsigned char>(l.n_dict);
+  // (the plain W, WT, colsumW and H0 regions above stay carved and unused with Qd >= 1, so the llbank offsets hold)
   l.bytes = align_up(w.used, 256);
   return l;
 }
 
-#define LL_CARVE_OR_FAIL(l, P, Lh, Qe)                                                                               \
-  if (int st__ = ll_check(h, cfg, P, Lh, Qe)) return st__;                                                           \
+#define LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd)                                                                          \
+  if (int st__ = ll_check(h, cfg, P, Lh, Qe, Qd)) return st__;                                                       \
   GCCNMF_REQUIRE(h, state != nullptr, "ll: NULL state");                                                             \
-  const LLLayout l = ll_carve(*cfg, P, state, Lh, Qe);                                                               \
+  const LLLayout l = ll_carve(*cfg, P, state, Lh, Qe, Qd);                                                           \
   if (state_bytes < l.bytes) return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "ll: state too small: need %zu bytes", l.bytes);
+#define LL_CARVE_OR_FAIL(l, P, Lh, Qe) LLD_CARVE_OR_FAIL(l, P, Lh, Qe, 0)
 
 SteerBank ll_bank(const LLLayout& l, int hops) {
   return SteerBank{reinterpret_cast<const double2*>(l.E), reinterpret_cast<const double2*>(l.ET), l.assign, l.order, l.seg, l.Qe, hops, l.Fp};
+}
+
+DictBank ll_dict(const LLLayout& l, int hops) {
+  return DictBank{l.dW, l.dcolsum, l.dWTr, l.drowsum, l.dWp, l.dK, l.dassign, l.dorder, l.dseg, l.Qd, hops, l.Kp, l.K, (int64_t)l.F * l.Kp, l.Fp};
 }
 
 // ---------------------------------------------------------------------------------------------- kernels
@@ -685,6 +744,81 @@ __global__ void ll_src_override_kernel(int32_t* __restrict__ src_override, int f
   for (int q = 0; q < P; ++q) src_override[(int64_t)(first + i) * kLLMaxSources + q] = b.t[i * P + q];
 }
 
+// ---- dictionary bank (gccnmf_lldict_*): column t is on entry dassign[t / hops] with K_e atoms
+// ll_mask_kernel's mask on rows k < K_e; rows [K_e, Kmax) get 0
+__global__ void ll_dict_mask_kernel(const LLStream* __restrict__ streams, const int32_t* __restrict__ argmax, const int32_t* __restrict__ targets,
+                                    const int32_t* __restrict__ dK, const int32_t* __restrict__ dassign, int K, int T, int hops,
+                                    float* __restrict__ mask) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)K * T) return;
+  const int t = (int)(i % T), k = (int)(i / T);
+  if (k >= __ldg(dK + __ldg(dassign + t / hops))) { mask[i] = 0.f; return; }
+  const float mu = (float)targets[t];
+  const float dist = fabsf((float)argmax[i] - mu);
+  mask[i] = dist < streams[t / hops].epsilon ? 1.f : 0.f;
+}
+
+// ll_infer_kernel on the column's dictionary: its W, W^T, column sums, H0 and K_e; H (Kmax, 2T) rows < K_e
+__global__ void __launch_bounds__(256)
+ll_dict_infer_kernel(DictBank dict, const float* __restrict__ WT, const float* __restrict__ colsumW, const float* __restrict__ H0,
+                     const float* __restrict__ V, int F, int T, int iterations, float alpha, float eps, float* __restrict__ Hout) {
+  extern __shared__ float sm[];
+  const int t = blockIdx.x, ch = blockIdx.y;
+  const int e = dict.entry(t), K = __ldg(dict.K + e);
+  const float* __restrict__ W = dict.W + e * dict.wstride;
+  WT += (int64_t)e * dict.Kp * F;
+  colsumW += (int64_t)e * dict.Kp;
+  H0 += (int64_t)e * dict.Kp * 2;
+  float* Hs = sm;          // K
+  float* Rs = sm + K;      // F
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = blockDim.x >> 5;
+  const int64_t col = (int64_t)ch * T + t;
+  for (int k = threadIdx.x; k < K; k += blockDim.x) Hs[k] = H0[(int64_t)k * 2 + ch];
+  __syncthreads();
+  for (int it = 0; it < iterations; ++it) {
+    for (int f = warp; f < F; f += warps) {
+      float a = 0.f;
+      for (int k = lane; k < K; k += 32) a = fmaf(W[(int64_t)f * K + k], Hs[k], a);
+      for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+      if (lane == 0) Rs[f] = V[(int64_t)f * (2 * T) + col] / a;
+    }
+    __syncthreads();
+    for (int k = warp; k < K; k += warps) {
+      float a = 0.f;
+      for (int f = lane; f < F; f += 32) a = fmaf(WT[(int64_t)k * F + f], Rs[f], a);
+      for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+      if (lane == 0) Hs[k] = Hs[k] * (a / ((colsumW[k] + alpha) + eps));
+    }
+    __syncthreads();
+  }
+  for (int k = threadIdx.x; k < K; k += blockDim.x) Hout[(int64_t)k * (2 * T) + col] = Hs[k];
+}
+
+// The defined fill of the rows [K_e, Kmax) of column t's K-shaped items (NULL: not touched): argmax -1; values, source masks
+// (P of each, (P, Kmax, T)) and H (Kmax, 2T) 0
+__global__ void ll_dict_fill_kernel(const int32_t* __restrict__ dK, const int32_t* __restrict__ dassign, int K, int T, int hops, int P,
+                                    int32_t* __restrict__ argmax, float* __restrict__ values, float* __restrict__ H) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)K * T) return;
+  const int t = (int)(i % T), k = (int)(i / T);
+  if (k < __ldg(dK + __ldg(dassign + t / hops))) return;
+  if (argmax) argmax[i] = -1;
+  if (values)
+    for (int q = 0; q < P; ++q) values[(int64_t)q * K * T + i] = 0.f;
+  if (H) {
+    H[(int64_t)k * 2 * T + t] = 0.f;
+    H[(int64_t)k * 2 * T + T + t] = 0.f;
+  }
+}
+
+// streams [first, first + count) onto the batch's entries where they are >= 0 (-1 keeps a stream's entry)
+__global__ void ll_dict_assign_kernel(int32_t* __restrict__ assign, int first, int count, LLAssignBatch b) {
+  for (int i = threadIdx.x; i < count; i += blockDim.x)
+    if (b.e[i] >= 0) assign[first + i] = b.e[i];
+}
+
+__global__ void ll_set_int_kernel(int32_t* p, int v) { *p = v; }
+
 // Sources, after the shared front (push, STFT, PHAT / angular): targets, the target contraction, coeff_mask, per source the
 // filter (with inference on the shared H), then one inverse FFT of all (P, 2) spectra, emit per (stream, source), advance.
 int ll_enqueue_sources(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l, int hops, float* out, void* stream) {
@@ -696,14 +830,32 @@ int ll_enqueue_sources(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLa
   else
     GCCNMF_LAUNCH(h, ll_src_targets_kernel, S, 128, 0, stream, l.streams, l.ang, l.valid, D, hops, T, P, l.carry, l.acc, l.src_targets,
                   l.src_override, l.src_status, l.col_targets);
-  if (l.Qe) {
+  const unsigned fill_ctas = (unsigned)(((int64_t)K * T + 255) / 256);
+  if (l.Qd) {
+    if (int e = gccnmf_target_gccnmf_dict(h, l.coh, F, T, ll_bank(l, hops), ll_dict(l, hops), D, l.col_targets, P, l.values, stream)) return e;
+    // rows past a column's dictionary hold 0, so coeff_mask's all-NaN flag comes from real atoms only
+    GCCNMF_LAUNCH(h, ll_dict_fill_kernel, fill_ctas, 256, 0, stream, l.dK, l.dassign, K, T, hops, P, nullptr, l.values, nullptr);
+  } else if (l.Qe) {
     if (int e = gccnmf_target_gccnmf_bank(h, l.coh, F, T, ll_bank(l, hops), D, l.W, K, l.col_targets, P, l.values, stream)) return e;
   } else if (int e = gccnmf_target_gccnmf(h, l.coh, F, T, l.E, D, l.W, K, l.col_targets, P, l.values, stream)) {
     return e;
   }
   if (int e = gccnmf_coeff_mask(h, l.values, P, K, T, l.src_mask, l.counters + 2, stream)) return e;
   const size_t KT = (size_t)K * T, FT = (size_t)F * T;
-  if (inf) {
+  if (l.Qd) {
+    const DictBank dict = ll_dict(l, hops);
+    if (inf) {
+      const size_t smem = (size_t)(K + F) * sizeof(float);
+      if (smem > 48 * 1024) GCCNMF_CHECK_CUDA(h, cudaFuncSetAttribute(ll_dict_infer_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      GCCNMF_LAUNCH(h, ll_dict_infer_kernel, dim3(T, 2), 256, smem, stream, dict, l.dWTi, l.dcolsumW, l.dH0, l.V, F, T, cfg->inference_iterations,
+                    cfg->sparsity_alpha, cfg->epsilon, l.H);
+    }
+    for (int q = 0; q < P; ++q)
+      if (int e = gccnmf_wiener_dict(h, l.src_mask + q * KT, dict, inf ? l.H : nullptr, l.X, F, T, l.Y + q * 4 * FT, l.wiener + q * (inf ? 2 : 1) * FT,
+                                     stream))
+        return e;
+    GCCNMF_LAUNCH(h, ll_dict_fill_kernel, fill_ctas, 256, 0, stream, l.dK, l.dassign, K, T, hops, P, nullptr, l.src_mask, inf ? l.H : nullptr);
+  } else if (inf) {
     const size_t smem = (size_t)(K + F) * sizeof(float);
     if (smem > 48 * 1024) GCCNMF_CHECK_CUDA(h, cudaFuncSetAttribute(ll_infer_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     GCCNMF_LAUNCH(h, ll_infer_kernel, dim3(T, 2), 256, smem, stream, l.W, l.WT, l.colsumW, l.H0, l.V, F, K, T, cfg->inference_iterations,
@@ -744,6 +896,29 @@ int ll_enqueue(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l,
                   l.means, l.targets);
   else
     GCCNMF_LAUNCH(h, ll_targets_kernel, S, 128, 0, stream, l.streams, l.ang, l.valid, D, hops, T, l.carry, l.acc, l.targets);
+  if (l.Qd) {
+    const SteerBank b = ll_bank(l, hops);
+    const DictBank dict = ll_dict(l, hops);
+    if (int e = gccnmf_tdoa_argmax_dict(h, l.coh, F, T, b, dict, D, l.argmax, l.counters, l.ws_dict, l.n_dict, stream)) return e;
+    if (int e = gccnmf_tdoa_gccnmf_dict(h, l.coh, F, T, b, dict, D, l.argmax, l.counters, gccnmf_tdoa_argmax_refine_capacity(K, T), l.counters + 1,
+                                        stream))
+      return e;
+    const int64_t KT = (int64_t)K * T;
+    const unsigned ctas = (unsigned)((KT + 255) / 256);
+    GCCNMF_LAUNCH(h, ll_dict_mask_kernel, ctas, 256, 0, stream, l.streams, l.argmax, l.targets, l.dK, l.dassign, K, T, hops, l.mask);
+    if (inf) {
+      const size_t smem = (size_t)(K + F) * sizeof(float);
+      if (smem > 48 * 1024) GCCNMF_CHECK_CUDA(h, cudaFuncSetAttribute(ll_dict_infer_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      GCCNMF_LAUNCH(h, ll_dict_infer_kernel, dim3(T, 2), 256, smem, stream, dict, l.dWTi, l.dcolsumW, l.dH0, l.V, F, T, cfg->inference_iterations,
+                    cfg->sparsity_alpha, cfg->epsilon, l.H);
+    }
+    if (int e = gccnmf_wiener_dict(h, l.mask, dict, inf ? l.H : nullptr, l.X, F, T, l.Y, l.wiener, stream)) return e;
+    GCCNMF_LAUNCH(h, ll_dict_fill_kernel, ctas, 256, 0, stream, l.dK, l.dassign, K, T, hops, 0, l.argmax, nullptr, inf ? l.H : nullptr);
+    if (int e = gccnmf_istft_frames(h, l.Y, 2, N, T, 0, l.frames, stream)) return e;
+    GCCNMF_LAUNCH(h, ll_ola_emit_kernel, S, 256, 0, stream, l.streams, l.head, l.w_syn, l.frames, N, hop, hops, T, before_first, l.out_ring, out,
+                  l.stage, l.in_ring, l.R);
+    return GCCNMF_OK;
+  }
   if (l.Qe) {
     const SteerBank b = ll_bank(l, hops);
     if (int e = gccnmf_tdoa_argmax_bank(h, l.coh, F, T, b, D, l.W, K, l.argmax, l.counters, l.ws_argmax, l.n_argmax, stream)) return e;
@@ -774,12 +949,12 @@ int ll_enqueue(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l,
 }
 
 // ---------------------------------------------------------------------------------------------- entry points (P = 0: gccnmf_ll_*)
-int ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, const float* W, const double* E, const double* analysis_window,
+int ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, int Qd, const float* W, const double* E, const double* analysis_window,
             const double* synthesis_weights, float gain, const float* H0, void* state, size_t state_bytes, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
-  GCCNMF_REQUIRE(h, W && E && analysis_window && synthesis_weights, "ll_init: NULL pointer");
-  GCCNMF_REQUIRE(h, cfg->inference_iterations == 0 || H0 != nullptr, "ll_init: inference needs H0");
+  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
+  GCCNMF_REQUIRE(h, (W || Qd) && E && analysis_window && synthesis_weights, "ll_init: NULL pointer");
+  GCCNMF_REQUIRE(h, cfg->inference_iterations == 0 || H0 != nullptr || Qd, "ll_init: inference needs H0");
   cudaStream_t s = (cudaStream_t)stream;
   // the synthesis weights decide the latency: read them here, before anything is enqueued
   double* wh = new double[l.N];
@@ -801,8 +976,8 @@ int ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe
     if (int st = gccnmf_steering_transpose(h, l.E + (size_t)j * 2 * l.F * l.D, l.F, l.D, l.ET + (size_t)j * 2 * l.D * l.Fp, l.Fp, stream)) return st;
   // with a bank every stream is on entry 0 (the memset above): sorted in stream order
   if (Qe) GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
-  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.W, W, (size_t)l.F * l.K * sizeof(float), cudaMemcpyDeviceToDevice, s));
-  if (cfg->inference_iterations > 0) {
+  if (!Qd) GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.W, W, (size_t)l.F * l.K * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  if (!Qd && cfg->inference_iterations > 0) {
     GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.H0, H0, (size_t)l.K * 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
     GCCNMF_LAUNCH(h, ll_dict_kernel, (l.K + 127) / 128, 128, 0, stream, l.W, l.F, l.K, l.WT, l.colsumW);
   }
@@ -815,10 +990,10 @@ int ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe
   return GCCNMF_OK;
 }
 
-int ll_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int first, int count,
+int ll_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, int Qd, void* state, size_t state_bytes, int first, int count,
                      void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
+  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "ll_reset_streams: streams [%d, %d + %d) outside [0, %d)", first,
                  first, count, l.S);
   GCCNMF_LAUNCH(h, ll_reset_kernel, count, 256, 0, stream, l.streams, first, count, l.in_ring, l.out_ring, l.carry, l.R, P ? 0 : l.N, l.D, 0);
@@ -829,13 +1004,17 @@ int ll_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int L
     GCCNMF_LAUNCH(h, ll_assign_kernel, 1, 256, 0, stream, l.assign, first, count, LLAssignBatch{}, 1);
     GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
   }
+  if (Qd) {
+    GCCNMF_LAUNCH(h, ll_assign_kernel, 1, 256, 0, stream, l.dassign, first, count, LLAssignBatch{}, 1);
+    GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.dassign, l.S, Qd, l.dorder, l.dseg);
+  }
   return GCCNMF_OK;
 }
 
-int ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int first, int count,
+int ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, int Qd, void* state, size_t state_bytes, int first, int count,
                   const gccnmf_ll_stream_params* params_host, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
+  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "ll_set_params: streams [%d, %d + %d) outside [0, %d)", first,
                  first, count, l.S);
   GCCNMF_REQUIRE(h, params_host != nullptr, "ll_set_params: NULL parameters");
@@ -853,12 +1032,12 @@ int ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, 
   return GCCNMF_OK;
 }
 
-int ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int hops, float* in, float* out,
+int ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, int Qd, void* state, size_t state_bytes, int hops, float* in, float* out,
                     const float* in_host, float* out_host, void** graph_exec, void* stream) {
   GCCNMF_ENTER(h);
   GCCNMF_REQUIRE(h, graph_exec != nullptr && stream != nullptr, "ll_graph_create: needs a non-default stream and an output slot");
   *graph_exec = nullptr;
-  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
+  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
   GCCNMF_REQUIRE(h, hops >= 1 && hops <= l.C, "ll_graph_create: hops must be in [1, %d] (got %d)", l.C, hops);
   GCCNMF_REQUIRE(h, in && out, "ll_graph_create: NULL pointer");
   if (int st = gccnmf_get_twiddles(h, l.N, nullptr, nullptr)) return st;
@@ -885,10 +1064,10 @@ int ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh
   return GCCNMF_OK;
 }
 
-int ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int hops, int what, void* dst,
+int ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, int Qd, void* state, size_t state_bytes, int hops, int what, void* dst,
               void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
+  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
   GCCNMF_REQUIRE(h, dst != nullptr, "ll_export: NULL destination");
   GCCNMF_REQUIRE(h, hops >= 1 && hops <= l.C, "ll_export: hops must be in [1, %d] (got %d)", l.C, hops);
   const bool inf = cfg->inference_iterations > 0;
@@ -896,6 +1075,13 @@ int ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int 
   if (what == GCCNMF_LLBANK_EXPORT_ASSIGNMENT) {
     GCCNMF_REQUIRE(h, Qe > 0, "ll_export: item %d needs num_steerings > 0", what);
     GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(dst, l.assign, (size_t)l.S * sizeof(int32_t), cudaMemcpyDefault, (cudaStream_t)stream));
+    return GCCNMF_OK;
+  }
+  if (what == GCCNMF_LLDICT_EXPORT_DICTIONARY_ASSIGNMENT || what == GCCNMF_LLDICT_EXPORT_DICTIONARY_ATOMS) {
+    GCCNMF_REQUIRE(h, Qd > 0, "ll_export: item %d needs num_dictionaries > 0", what);
+    const bool atoms = what == GCCNMF_LLDICT_EXPORT_DICTIONARY_ATOMS;
+    GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(dst, atoms ? l.dK : l.dassign, (size_t)(atoms ? Qd : l.S) * sizeof(int32_t), cudaMemcpyDefault,
+                                         (cudaStream_t)stream));
     return GCCNMF_OK;
   }
   if (what >= GCCNMF_LLHIST_EXPORT_RING && what <= GCCNMF_LLHIST_EXPORT_MEANS) {
@@ -1157,7 +1343,7 @@ int ll_bank_digests(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayou
 }
 
 #define LL_RECORD_ARGS_OR_FAIL(what)                                                                                               \
-  LL_CARVE_OR_FAIL(l, P, Lh, Qe);                                                                                                        \
+  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);                                                                                                        \
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, what ": streams [%d, %d + %d) outside [0, %d)", \
                  first, first, count, l.S);                                                                                          \
   const RecordMap m = ll_record_map(*cfg, P, Lh, Qe);                                                                                \
@@ -1168,7 +1354,7 @@ int ll_bank_digests(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayou
   if (workspace == nullptr || workspace_bytes < ws_need || ((uintptr_t)workspace & (Qe ? 7 : 3)) != 0)                               \
     return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, what ": workspace needs %zu bytes, %d-byte aligned", ws_need, Qe ? 8 : 4);
 
-int ll_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int first, int count, void* record,
+int ll_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, int Qd, void* state, size_t state_bytes, int first, int count, void* record,
                     size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
   GCCNMF_ENTER(h);
   LL_RECORD_ARGS_OR_FAIL("ll_save_streams");
@@ -1192,7 +1378,7 @@ int ll_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh
   return GCCNMF_OK;
 }
 
-int ll_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int first, int count, const void* record,
+int ll_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, int Qd, void* state, size_t state_bytes, int first, int count, const void* record,
                     size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
   GCCNMF_ENTER(h);
   LL_RECORD_ARGS_OR_FAIL("ll_load_streams");
@@ -1250,10 +1436,10 @@ int ll_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh
   return GCCNMF_OK;
 }
 
-int ll_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int first, int count,
+int ll_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, int Qd, void* state, size_t state_bytes, int first, int count,
                    const int32_t* targets_host, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
+  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "llsep_set_targets: streams [%d, %d + %d) outside [0, %d)",
                  first, first, count, l.S);
   GCCNMF_REQUIRE(h, targets_host != nullptr, "llsep_set_targets: NULL targets");
@@ -1269,10 +1455,10 @@ int ll_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh,
   return GCCNMF_OK;
 }
 
-int ll_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int first, int count,
+int ll_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, int Qd, void* state, size_t state_bytes, int first, int count,
                   const int32_t* windows_host, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
+  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
   GCCNMF_REQUIRE(h, Lh > 0, "llhist_set_window: needs history_length > 0");
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "llhist_set_window: streams [%d, %d + %d) outside [0, %d)",
                  first, first, count, l.S);
@@ -1291,10 +1477,10 @@ int ll_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, 
 }
 
 // Bank: table j <- E (F, D) complex128 on the device, and its transpose; stream-ordered, from the next call on.
-int ll_load_steering(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int entry,
+int ll_load_steering(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, int Qd, void* state, size_t state_bytes, int entry,
                      const double* E, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
+  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
   GCCNMF_REQUIRE(h, entry >= 0 && entry < Qe, "llbank_load_steering: entry %d outside [0, %d)", entry, Qe);
   GCCNMF_REQUIRE(h, E != nullptr, "llbank_load_steering: NULL table");
   double* dst = l.E + (size_t)entry * 2 * l.F * l.D;
@@ -1303,10 +1489,10 @@ int ll_load_steering(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int L
 }
 
 // Bank: streams [first, first + count) onto entries_host[0 .. count), then the streams sorted again; stream-ordered.
-int ll_assign(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, void* state, size_t state_bytes, int first, int count,
+int ll_assign(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, int Qd, void* state, size_t state_bytes, int first, int count,
               const int32_t* entries_host, void* stream) {
   GCCNMF_ENTER(h);
-  LL_CARVE_OR_FAIL(l, P, Lh, Qe);
+  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "llbank_assign: streams [%d, %d + %d) outside [0, %d)", first,
                  first, count, l.S);
   GCCNMF_REQUIRE(h, entries_host != nullptr, "llbank_assign: NULL entries");
@@ -1322,6 +1508,246 @@ int ll_assign(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int 
   return GCCNMF_OK;
 }
 
+
+// ---- dictionary bank (gccnmf_lldict_*)
+constexpr int kConfigAtoms = offsetof(gccnmf_ll_config, num_atoms) / sizeof(int32_t);
+
+// Entry e <- W (F, K) f32 and, with inference, H0 (K, 2) f32 (device arrays), with every form derived from them; stream-ordered.
+int lld_load_entry(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l, int e, const float* W, int K, const float* H0, void* stream) {
+  cudaStream_t s = (cudaStream_t)stream;
+  float* dst = l.dW + (size_t)e * l.F * l.Kp;
+  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(dst, W, (size_t)l.F * K * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  if (int st = gccnmf_lldict_prepare(h, ll_dict(l, 1), e, dst, l.F, K, stream)) return st;
+  if (int st = gccnmf_rowsum_w(h, dst, l.F, K, l.drowsum + (size_t)e * l.F, stream)) return st;
+  if (cfg->inference_iterations > 0) {
+    GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.dH0 + (size_t)e * l.Kp * 2, H0, (size_t)K * 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    GCCNMF_LAUNCH(h, ll_dict_kernel, (K + 127) / 128, 128, 0, stream, dst, l.F, K, l.dWTi + (size_t)e * l.Kp * l.F, l.dcolsumW + (size_t)e * l.Kp);
+  }
+  GCCNMF_LAUNCH(h, ll_set_int_kernel, 1, 1, 0, stream, l.dK + e, K);
+  return GCCNMF_OK;
+}
+
+int lld_check_entry(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l, int e, const float* W, int K, const float* H0) {
+  GCCNMF_REQUIRE(h, e >= 0 && e < l.Qd, "lldict: dictionary entry %d outside [0, %d)", e, l.Qd);
+  GCCNMF_REQUIRE(h, W != nullptr, "lldict: entry %d: NULL W", e);
+  GCCNMF_REQUIRE(h, K >= 1 && K <= l.K, "lldict: entry %d: num_atoms %d outside [1, %d] (the config's num_atoms)", e, K, l.K);
+  GCCNMF_REQUIRE(h, cfg->inference_iterations == 0 || H0 != nullptr, "lldict: entry %d: inference needs H0", e);
+  return 0;
+}
+
+int lld_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qd, int Qe, const float* const* W, const int* num_atoms, const double* E,
+             const double* analysis_window, const double* synthesis_weights, float gain, const float* const* H0, void* state, size_t state_bytes,
+             void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, Qd >= 1, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, Qd);
+  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
+  GCCNMF_REQUIRE(h, W && num_atoms, "lldict_init: NULL dictionaries");
+  GCCNMF_REQUIRE(h, cfg->inference_iterations == 0 || H0, "lldict_init: inference needs H0");
+  for (int e = 0; e < Qd; ++e)
+    if (int st = lld_check_entry(h, cfg, l, e, W[e], num_atoms[e], H0 ? H0[e] : nullptr)) return st;
+  if (int st = ll_init(h, cfg, P, Lh, Qe, Qd, nullptr, E, analysis_window, synthesis_weights, gain, nullptr, state, state_bytes, stream)) return st;
+  for (int e = 0; e < Qd; ++e)
+    if (int st = lld_load_entry(h, cfg, l, e, W[e], num_atoms[e], H0 ? H0[e] : nullptr, stream)) return st;
+  GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.dassign, l.S, Qd, l.dorder, l.dseg);     // every stream on entry 0
+  return GCCNMF_OK;
+}
+
+int lld_load_dictionary(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qd, int Qe, void* state, size_t state_bytes, int index,
+                        const float* W, int K, const float* H0, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, Qd >= 1, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, Qd);
+  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
+  if (int st = lld_check_entry(h, cfg, l, index, W, K, H0)) return st;
+  return lld_load_entry(h, cfg, l, index, W, K, H0, stream);
+}
+
+// streams [first, first + count) onto dictionary_host[i] / steering_host[i] (-1 or a NULL array: keep), then both sorts; stream-ordered
+int lld_assign(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qd, int Qe, void* state, size_t state_bytes, int first, int count,
+               const int32_t* dictionary_host, const int32_t* steering_host, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, Qd >= 1, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, Qd);
+  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
+  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "lldict_assign: streams [%d, %d + %d) outside [0, %d)", first,
+                 first, count, l.S);
+  for (int i = 0; i < count; ++i) {
+    const int d = dictionary_host ? dictionary_host[i] : -1, e = steering_host ? steering_host[i] : -1;
+    GCCNMF_REQUIRE(h, d >= -1 && d < Qd, "lldict_assign: stream %d: dictionary entry %d outside [0, %d) (or -1)", first + i, d, Qd);
+    GCCNMF_REQUIRE(h, e >= -1 && e < Qe, "lldict_assign: stream %d: steering entry %d outside [0, %d) (or -1)", first + i, e, Qe);
+  }
+  for (int pass = 0; pass < 2; ++pass) {
+    const int32_t* src = pass ? steering_host : dictionary_host;
+    if (!src) continue;
+    int32_t* assign = pass ? l.assign : l.dassign;
+    for (int i0 = 0; i0 < count; i0 += kLLParamsPerLaunch) {
+      const int n = count - i0 < kLLParamsPerLaunch ? count - i0 : kLLParamsPerLaunch;
+      LLAssignBatch b{};
+      memcpy(b.e, src + i0, (size_t)n * sizeof(int32_t));
+      GCCNMF_LAUNCH(h, ll_dict_assign_kernel, 1, kLLParamsPerLaunch, 0, stream, assign, first + i0, n, b);
+    }
+    if (pass) GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
+    else GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.dassign, l.S, Qd, l.dorder, l.dseg);
+  }
+  return GCCNMF_OK;
+}
+
+// Records: the workspace holds the payloads, one chunk digest per 1024-word chunk of the largest dictionary and of each table, then
+// the Qe table digests and the Qd dictionary digests.  Each dictionary's digest is the llbank digest of an engine built with it.
+struct LLDictDigestSizes { int cd, ce; };
+LLDictDigestSizes lld_digest_sizes(const gccnmf_ll_config& c, const LLLayout& l) {
+  const size_t n = (size_t)l.F * l.K + (c.inference_iterations > 0 ? (size_t)2 * l.K : 0), ne = (size_t)4 * l.F * l.D;
+  return LLDictDigestSizes{(int)((n + kDigestChunk - 1) / kDigestChunk), (int)((ne + kDigestChunk - 1) / kDigestChunk)};
+}
+
+size_t lld_record_workspace_bytes(const gccnmf_ll_config& c, int P, int Lh, int Qd, int Qe, int count) {
+  const LLLayout l = ll_carve(c, P, nullptr, Lh, Qe, Qd);
+  const LLDictDigestSizes z = lld_digest_sizes(c, l);
+  return align_up((size_t)count * ll_record_map(c, P, Lh).payload, 256) + align_up((size_t)(z.cd + Qe * z.ce) * sizeof(uint64_t), 256) +
+         (size_t)(Qd + Qe) * sizeof(uint64_t);
+}
+
+// The Qd dictionary digests, the Qe table digests, the K_e table and (entries != NULL) the two entries of streams [first, first + count)
+// back to the host: two waits on the stream.
+int lld_digests(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l, int count, char* workspace, int first, uint64_t* dict_digest,
+                uint64_t* steer_digest, int32_t* K_host, int32_t* dict_entries, int32_t* steer_entries, void* stream) {
+  cudaStream_t s = (cudaStream_t)stream;
+  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(K_host, l.dK, (size_t)l.Qd * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  GCCNMF_CHECK_CUDA(h, cudaStreamSynchronize(s));
+  const bool inf = cfg->inference_iterations > 0;
+  const LLDictDigestSizes z = lld_digest_sizes(*cfg, l);
+  uint64_t* chunks = reinterpret_cast<uint64_t*>(workspace + align_up((size_t)count * ll_record_map(*cfg, l.P, l.Lh).payload, 256));
+  uint64_t* dev = chunks + align_up((size_t)(z.cd + l.Qe * z.ce) * sizeof(uint64_t), 256) / sizeof(uint64_t);
+  for (int e = 0; e < l.Qd; ++e) {
+    const int K = K_host[e];
+    GCCNMF_REQUIRE(h, K >= 1 && K <= l.K, "lldict: dictionary entry %d has %d atoms", e, K);
+    LLDigestItems d = ll_digest_items(l, inf);
+    d.W = reinterpret_cast<const uint32_t*>(l.dW + (size_t)e * l.F * l.Kp);
+    d.H0 = reinterpret_cast<const uint32_t*>(l.dH0 + (size_t)e * l.Kp * 2);
+    d.nw = (size_t)l.F * K;
+    d.nh = inf ? (size_t)2 * K : 0;
+    d.cd = (int)((d.nw + d.nh + kDigestChunk - 1) / kDigestChunk);
+    d.Qe = e == 0 ? l.Qe : 0;                       // the tables once, with entry 0: dev[0] dictionary 0, dev[1 ..] the tables
+    const int n = d.cd + d.Qe * d.ce;
+    GCCNMF_LAUNCH(h, ll_digest_chunks_kernel, (n + 127) / 128, 128, 0, stream, d, chunks);
+    GCCNMF_LAUNCH(h, ll_digest_fold_kernel, (d.Qe + 1 + 127) / 128, 128, 0, stream, d, chunks, dev + (e == 0 ? 0 : l.Qe + e));
+  }
+  std::vector<uint64_t> all((size_t)l.Qd + l.Qe);
+  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(all.data(), dev, all.size() * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+  if (dict_entries) GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(dict_entries, l.dassign + first, (size_t)count * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  if (steer_entries) GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(steer_entries, l.assign + first, (size_t)count * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  GCCNMF_CHECK_CUDA(h, cudaStreamSynchronize(s));
+  dict_digest[0] = all[0];
+  for (int j = 0; j < l.Qe; ++j) steer_digest[j] = all[1 + j];
+  for (int e = 1; e < l.Qd; ++e) dict_digest[e] = all[l.Qe + e];
+  return GCCNMF_OK;
+}
+
+#define LLD_RECORD_ARGS_OR_FAIL(what)                                                                                              \
+  GCCNMF_REQUIRE(h, Qd >= 1, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, Qd);                    \
+  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);                                                                                               \
+  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, what ": streams [%d, %d + %d) outside [0, %d)", \
+                 first, first, count, l.S);                                                                                          \
+  const RecordMap m = ll_record_map(*cfg, P, Lh, Qe);                                                                                \
+  const size_t rec_bytes = ll_record_bytes(*cfg, P, Lh);                                                                             \
+  GCCNMF_REQUIRE(h, record != nullptr && record_bytes >= (size_t)count * rec_bytes, what ": record needs %zu bytes for %d streams",  \
+                 (size_t)count * rec_bytes, count);                                                                                  \
+  const size_t ws_need = lld_record_workspace_bytes(*cfg, P, Lh, Qd, Qe, count);                                                     \
+  if (workspace == nullptr || workspace_bytes < ws_need || ((uintptr_t)workspace & 7) != 0)                                          \
+    return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, what ": workspace needs %zu bytes, 8-byte aligned", ws_need);
+
+int lld_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qd, int Qe, void* state, size_t state_bytes, int first, int count,
+                     void* record, size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
+  GCCNMF_ENTER(h);
+  LLD_RECORD_ARGS_OR_FAIL("lldict_save_streams");
+  gccnmf_record_header head = ll_record_header(*cfg, P, Lh, Qe);
+  if (int st = ll_synthesis_digest(h, l, &head.synthesis_digest, stream)) return st;
+  uint64_t dd[kLLMaxDictionaries], sd[kLLMaxSteerings];
+  int32_t Kh[kLLMaxDictionaries];
+  std::vector<int32_t> de(count), se(count);
+  if (int st = lld_digests(h, cfg, l, count, (char*)workspace, first, dd, sd, Kh, de.data(), se.data(), stream)) return st;
+  for (int i = 0; i < count; ++i) {
+    char* rec = (char*)record + (size_t)i * rec_bytes;
+    memcpy(rec, &head, sizeof(head));
+    gccnmf_llbank_record_header* r = reinterpret_cast<gccnmf_llbank_record_header*>(rec);
+    r->config[kConfigAtoms] = Kh[de[i]];              // the header an llbank engine built with the stream's dictionary writes
+    r->dictionary_digest = dd[de[i]];
+    r->steering_digest = sd[se[i]];
+  }
+  GCCNMF_LAUNCH(h, ll_record_copy_kernel, dim3(count, m.n), 256, 0, stream, (char*)state, first, m, (char*)workspace, 1);
+  GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync((char*)record + kRecordHeaderBytes, rec_bytes, workspace, m.payload, m.payload, count,
+                                         cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  return GCCNMF_OK;
+}
+
+int lld_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qd, int Qe, void* state, size_t state_bytes, int first, int count,
+                     const void* record, size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
+  GCCNMF_ENTER(h);
+  LLD_RECORD_ARGS_OR_FAIL("lldict_load_streams");
+  const gccnmf_record_header want = ll_record_header(*cfg, P, Lh, Qe);
+  for (int i = 0; i < count; ++i) {      // everything but the digests, before the device is touched
+    gccnmf_record_header got;
+    memcpy(&got, (const char*)record + (size_t)i * rec_bytes, sizeof(got));
+    GCCNMF_REQUIRE(h, got.magic == want.magic, "lldict_load_streams: record %d: not a stream record (magic 0x%08x)", i, got.magic);
+    GCCNMF_REQUIRE(h, got.abi_version == want.abi_version, "lldict_load_streams: record %d: ABI version %d, this library is %d", i, got.abi_version,
+                   want.abi_version);
+    GCCNMF_REQUIRE(h, got.kind == want.kind, "lldict_load_streams: record %d: kind %d is not a bank stream", i, got.kind);
+    GCCNMF_REQUIRE(h, got.num_sources == P, "lldict_load_streams: record %d: %d sources, this engine has %d", i, got.num_sources, P);
+    GCCNMF_REQUIRE(h, got.config[kRecordConfigHistory] == Lh, "lldict_load_streams: record %d: history length %d, this engine has %d", i,
+                   got.config[kRecordConfigHistory], Lh);
+    GCCNMF_REQUIRE(h, got.payload_bytes == want.payload_bytes, "lldict_load_streams: record %d: payload of %llu bytes, expected %llu", i,
+                   (unsigned long long)got.payload_bytes, (unsigned long long)want.payload_bytes);
+    const int K = got.config[kConfigAtoms];
+    GCCNMF_REQUIRE(h, K >= 1 && K <= l.K, "lldict_load_streams: record %d: %d atoms, this engine holds at most %d", i, K, l.K);
+    got.config[kConfigAtoms] = want.config[kConfigAtoms];
+    GCCNMF_REQUIRE(h, memcmp(got.config, want.config, sizeof(want.config)) == 0, "lldict_load_streams: record %d: another configuration", i);
+  }
+  uint64_t digest = 0;
+  if (int st = ll_synthesis_digest(h, l, &digest, stream)) return st;
+  for (int i = 0; i < count; ++i) {
+    gccnmf_record_header got;
+    memcpy(&got, (const char*)record + (size_t)i * rec_bytes, sizeof(got));
+    GCCNMF_REQUIRE(h, got.synthesis_digest == digest, "lldict_load_streams: record %d: other synthesis weights or gain", i);
+  }
+  // the lowest entries holding the record's dictionary (same content and K) and table (only read-only kernels have run when this refuses)
+  uint64_t dd[kLLMaxDictionaries], sd[kLLMaxSteerings];
+  int32_t Kh[kLLMaxDictionaries];
+  if (int st = lld_digests(h, cfg, l, count, (char*)workspace, first, dd, sd, Kh, nullptr, nullptr, stream)) return st;
+  std::vector<int32_t> de(count), se(count);
+  for (int i = 0; i < count; ++i) {
+    gccnmf_llbank_record_header got;
+    memcpy(&got, (const char*)record + (size_t)i * rec_bytes, sizeof(got));
+    const int K = got.config[kConfigAtoms];
+    int d = -1, same_content = -1;
+    for (int e = Qd - 1; e >= 0; --e)
+      if (dd[e] == got.dictionary_digest) {
+        same_content = e;
+        if (Kh[e] == K) d = e;
+      }
+    GCCNMF_REQUIRE(h, same_content >= 0, "lldict_load_streams: record %d: no dictionary entry of this engine holds the stream's dictionary", i);
+    GCCNMF_REQUIRE(h, d >= 0, "lldict_load_streams: record %d: the stream's dictionary has %d atoms, the entry holding it %d", i, K, Kh[same_content]);
+    int e = -1;
+    for (int j = Qe - 1; j >= 0; --j)
+      if (sd[j] == got.steering_digest) e = j;
+    GCCNMF_REQUIRE(h, e >= 0, "lldict_load_streams: record %d: no steering entry of this engine has the stream's table", i);
+    de[i] = d;
+    se[i] = e;
+  }
+  GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync(workspace, m.payload, (const char*)record + kRecordHeaderBytes, rec_bytes, m.payload, count,
+                                         cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  GCCNMF_LAUNCH(h, ll_record_copy_kernel, dim3(count, m.n), 256, 0, stream, (char*)state, first, m, (char*)workspace, 0);
+  for (int pass = 0; pass < 2; ++pass) {
+    const std::vector<int32_t>& src = pass ? se : de;
+    for (int i0 = 0; i0 < count; i0 += kLLParamsPerLaunch) {
+      const int n = count - i0 < kLLParamsPerLaunch ? count - i0 : kLLParamsPerLaunch;
+      LLAssignBatch b{};
+      memcpy(b.e, src.data() + i0, (size_t)n * sizeof(int32_t));
+      GCCNMF_LAUNCH(h, ll_assign_kernel, 1, kLLParamsPerLaunch, 0, stream, pass ? l.assign : l.dassign, first + i0, n, b, 0);
+    }
+  }
+  GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
+  GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.dassign, l.S, Qd, l.dorder, l.dseg);
+  return GCCNMF_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1333,16 +1759,16 @@ size_t gccnmf_ll_state_bytes(const gccnmf_ll_config* cfg) {
 
 int gccnmf_ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, const float* W, const double* E, const double* analysis_window,
                    const double* synthesis_weights, float gain, const float* H0, void* state, size_t state_bytes, void* stream) {
-  return ll_init(h, cfg, 0, 0, 0, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
+  return ll_init(h, cfg, 0, 0, 0, 0, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
 }
 
 int gccnmf_ll_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int first, int count, void* stream) {
-  return ll_reset_streams(h, cfg, 0, 0, 0, state, state_bytes, first, count, stream);
+  return ll_reset_streams(h, cfg, 0, 0, 0, 0, state, state_bytes, first, count, stream);
 }
 
 int gccnmf_ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int first, int count,
                          const gccnmf_ll_stream_params* params_host, void* stream) {
-  return ll_set_params(h, cfg, 0, 0, 0, state, state_bytes, first, count, params_host, stream);
+  return ll_set_params(h, cfg, 0, 0, 0, 0, state, state_bytes, first, count, params_host, stream);
 }
 
 int gccnmf_ll_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, const float* in, float* out,
@@ -1354,11 +1780,11 @@ int gccnmf_ll_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state
 
 int gccnmf_ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, float* in, float* out,
                            const float* in_host, float* out_host, void** graph_exec, void* stream) {
-  return ll_graph_create(h, cfg, 0, 0, 0, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
+  return ll_graph_create(h, cfg, 0, 0, 0, 0, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
 }
 
 int gccnmf_ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, void* state, size_t state_bytes, int hops, int what, void* dst, void* stream) {
-  return ll_export(h, cfg, 0, 0, 0, state, state_bytes, hops, what, dst, stream);
+  return ll_export(h, cfg, 0, 0, 0, 0, state, state_bytes, hops, what, dst, stream);
 }
 
 // ---- sources (2 <= num_sources <= 8)
@@ -1371,25 +1797,25 @@ int gccnmf_llsep_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sou
                       const double* analysis_window, const double* synthesis_weights, float gain, const float* H0, void* state,
                       size_t state_bytes, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_init(h, cfg, num_sources, 0, 0, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
+  return ll_init(h, cfg, num_sources, 0, 0, 0, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
 }
 
 int gccnmf_llsep_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
                                int count, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_reset_streams(h, cfg, num_sources, 0, 0, state, state_bytes, first, count, stream);
+  return ll_reset_streams(h, cfg, num_sources, 0, 0, 0, state, state_bytes, first, count, stream);
 }
 
 int gccnmf_llsep_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
                             int count, const gccnmf_ll_stream_params* params_host, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_set_params(h, cfg, num_sources, 0, 0, state, state_bytes, first, count, params_host, stream);
+  return ll_set_params(h, cfg, num_sources, 0, 0, 0, state, state_bytes, first, count, params_host, stream);
 }
 
 int gccnmf_llsep_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
                              int count, const int32_t* targets_host, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_set_targets(h, cfg, num_sources, 0, 0, state, state_bytes, first, count, targets_host, stream);
+  return ll_set_targets(h, cfg, num_sources, 0, 0, 0, state, state_bytes, first, count, targets_host, stream);
 }
 
 int gccnmf_llsep_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int hops,
@@ -1403,13 +1829,13 @@ int gccnmf_llsep_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_
 int gccnmf_llsep_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int hops,
                               float* in, float* out, const float* in_host, float* out_host, void** graph_exec, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_graph_create(h, cfg, num_sources, 0, 0, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
+  return ll_graph_create(h, cfg, num_sources, 0, 0, 0, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
 }
 
 int gccnmf_llsep_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int hops, int what,
                         void* dst, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llsep: num_sources must be in [2, %d] (got 0)", kLLMaxSources);
-  return ll_export(h, cfg, num_sources, 0, 0, state, state_bytes, hops, what, dst, stream);
+  return ll_export(h, cfg, num_sources, 0, 0, 0, state, state_bytes, hops, what, dst, stream);
 }
 
 // ---- stream records (0 <= num_sources <= 8)
@@ -1425,12 +1851,12 @@ size_t gccnmf_llrec_workspace_bytes(const gccnmf_ll_config* cfg, int num_sources
 
 int gccnmf_llrec_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
                               int count, void* record, size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
-  return ll_save_streams(h, cfg, num_sources, 0, 0, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes, stream);
+  return ll_save_streams(h, cfg, num_sources, 0, 0, 0, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes, stream);
 }
 
 int gccnmf_llrec_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
                               int count, const void* record, size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
-  return ll_load_streams(h, cfg, num_sources, 0, 0, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes, stream);
+  return ll_load_streams(h, cfg, num_sources, 0, 0, 0, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes, stream);
 }
 
 // ---- history (0 <= num_sources <= 8, 0 <= history_length <= 1024)
@@ -1442,28 +1868,28 @@ size_t gccnmf_llhist_state_bytes(const gccnmf_ll_config* cfg, int num_sources, i
 int gccnmf_llhist_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, const float* W, const double* E,
                        const double* analysis_window, const double* synthesis_weights, float gain, const float* H0, void* state,
                        size_t state_bytes, void* stream) {
-  return ll_init(h, cfg, num_sources, history_length, 0, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
+  return ll_init(h, cfg, num_sources, history_length, 0, 0, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
 }
 
 int gccnmf_llhist_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
                                 size_t state_bytes, int first, int count, void* stream) {
-  return ll_reset_streams(h, cfg, num_sources, history_length, 0, state, state_bytes, first, count, stream);
+  return ll_reset_streams(h, cfg, num_sources, history_length, 0, 0, state, state_bytes, first, count, stream);
 }
 
 int gccnmf_llhist_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
                              size_t state_bytes, int first, int count, const gccnmf_ll_stream_params* params_host, void* stream) {
-  return ll_set_params(h, cfg, num_sources, history_length, 0, state, state_bytes, first, count, params_host, stream);
+  return ll_set_params(h, cfg, num_sources, history_length, 0, 0, state, state_bytes, first, count, params_host, stream);
 }
 
 int gccnmf_llhist_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
                               size_t state_bytes, int first, int count, const int32_t* targets_host, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llhist_set_targets: needs num_sources in [2, %d] (got 0)", kLLMaxSources);
-  return ll_set_targets(h, cfg, num_sources, history_length, 0, state, state_bytes, first, count, targets_host, stream);
+  return ll_set_targets(h, cfg, num_sources, history_length, 0, 0, state, state_bytes, first, count, targets_host, stream);
 }
 
 int gccnmf_llhist_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
                              size_t state_bytes, int first, int count, const int32_t* windows_host, void* stream) {
-  return ll_set_window(h, cfg, num_sources, history_length, 0, state, state_bytes, first, count, windows_host, stream);
+  return ll_set_window(h, cfg, num_sources, history_length, 0, 0, state, state_bytes, first, count, windows_host, stream);
 }
 
 int gccnmf_llhist_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state, size_t state_bytes,
@@ -1476,12 +1902,12 @@ int gccnmf_llhist_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num
 int gccnmf_llhist_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
                                size_t state_bytes, int hops, float* in, float* out, const float* in_host, float* out_host, void** graph_exec,
                                void* stream) {
-  return ll_graph_create(h, cfg, num_sources, history_length, 0, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
+  return ll_graph_create(h, cfg, num_sources, history_length, 0, 0, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
 }
 
 int gccnmf_llhist_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state, size_t state_bytes,
                          int hops, int what, void* dst, void* stream) {
-  return ll_export(h, cfg, num_sources, history_length, 0, state, state_bytes, hops, what, dst, stream);
+  return ll_export(h, cfg, num_sources, history_length, 0, 0, state, state_bytes, hops, what, dst, stream);
 }
 
 size_t gccnmf_llhist_record_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length) {
@@ -1497,14 +1923,14 @@ size_t gccnmf_llhist_workspace_bytes(const gccnmf_ll_config* cfg, int num_source
 int gccnmf_llhist_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
                                size_t state_bytes, int first, int count, void* record, size_t record_bytes, void* workspace,
                                size_t workspace_bytes, void* stream) {
-  return ll_save_streams(h, cfg, num_sources, history_length, 0, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes,
+  return ll_save_streams(h, cfg, num_sources, history_length, 0, 0, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes,
                          stream);
 }
 
 int gccnmf_llhist_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
                                size_t state_bytes, int first, int count, const void* record, size_t record_bytes, void* workspace,
                                size_t workspace_bytes, void* stream) {
-  return ll_load_streams(h, cfg, num_sources, history_length, 0, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes,
+  return ll_load_streams(h, cfg, num_sources, history_length, 0, 0, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes,
                          stream);
 }
 
@@ -1517,38 +1943,38 @@ size_t gccnmf_llbank_state_bytes(const gccnmf_ll_config* cfg, int num_sources, i
 int gccnmf_llbank_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, const float* W,
                        const double* E, const double* analysis_window, const double* synthesis_weights, float gain, const float* H0, void* state,
                        size_t state_bytes, void* stream) {
-  return ll_init(h, cfg, num_sources, history_length, num_steerings, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
+  return ll_init(h, cfg, num_sources, history_length, num_steerings, 0, W, E, analysis_window, synthesis_weights, gain, H0, state, state_bytes, stream);
 }
 
 int gccnmf_llbank_load_steering(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
                                 size_t state_bytes, int entry, const double* E, void* stream) {
-  return ll_load_steering(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, entry, E, stream);
+  return ll_load_steering(h, cfg, num_sources, history_length, num_steerings, 0, state, state_bytes, entry, E, stream);
 }
 
 int gccnmf_llbank_assign(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
                          size_t state_bytes, int first, int count, const int32_t* entries_host, void* stream) {
-  return ll_assign(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, first, count, entries_host, stream);
+  return ll_assign(h, cfg, num_sources, history_length, num_steerings, 0, state, state_bytes, first, count, entries_host, stream);
 }
 
 int gccnmf_llbank_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
                                 size_t state_bytes, int first, int count, void* stream) {
-  return ll_reset_streams(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, first, count, stream);
+  return ll_reset_streams(h, cfg, num_sources, history_length, num_steerings, 0, state, state_bytes, first, count, stream);
 }
 
 int gccnmf_llbank_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
                              size_t state_bytes, int first, int count, const gccnmf_ll_stream_params* params_host, void* stream) {
-  return ll_set_params(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, first, count, params_host, stream);
+  return ll_set_params(h, cfg, num_sources, history_length, num_steerings, 0, state, state_bytes, first, count, params_host, stream);
 }
 
 int gccnmf_llbank_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
                               size_t state_bytes, int first, int count, const int32_t* targets_host, void* stream) {
   GCCNMF_REQUIRE(h, num_sources != 0, "llbank_set_targets: needs num_sources in [2, %d] (got 0)", kLLMaxSources);
-  return ll_set_targets(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, first, count, targets_host, stream);
+  return ll_set_targets(h, cfg, num_sources, history_length, num_steerings, 0, state, state_bytes, first, count, targets_host, stream);
 }
 
 int gccnmf_llbank_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
                              size_t state_bytes, int first, int count, const int32_t* windows_host, void* stream) {
-  return ll_set_window(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, first, count, windows_host, stream);
+  return ll_set_window(h, cfg, num_sources, history_length, num_steerings, 0, state, state_bytes, first, count, windows_host, stream);
 }
 
 int gccnmf_llbank_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
@@ -1561,12 +1987,12 @@ int gccnmf_llbank_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num
 int gccnmf_llbank_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
                                size_t state_bytes, int hops, float* in, float* out, const float* in_host, float* out_host, void** graph_exec,
                                void* stream) {
-  return ll_graph_create(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
+  return ll_graph_create(h, cfg, num_sources, history_length, num_steerings, 0, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
 }
 
 int gccnmf_llbank_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
                          size_t state_bytes, int hops, int what, void* dst, void* stream) {
-  return ll_export(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, hops, what, dst, stream);
+  return ll_export(h, cfg, num_sources, history_length, num_steerings, 0, state, state_bytes, hops, what, dst, stream);
 }
 
 size_t gccnmf_llbank_record_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings) {
@@ -1582,15 +2008,121 @@ size_t gccnmf_llbank_workspace_bytes(const gccnmf_ll_config* cfg, int num_source
 int gccnmf_llbank_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
                                size_t state_bytes, int first, int count, void* record, size_t record_bytes, void* workspace, size_t workspace_bytes,
                                void* stream) {
-  return ll_save_streams(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, first, count, record, record_bytes, workspace,
+  return ll_save_streams(h, cfg, num_sources, history_length, num_steerings, 0, state, state_bytes, first, count, record, record_bytes, workspace,
                          workspace_bytes, stream);
 }
 
 int gccnmf_llbank_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
                                size_t state_bytes, int first, int count, const void* record, size_t record_bytes, void* workspace,
                                size_t workspace_bytes, void* stream) {
-  return ll_load_streams(h, cfg, num_sources, history_length, num_steerings, state, state_bytes, first, count, record, record_bytes, workspace,
+  return ll_load_streams(h, cfg, num_sources, history_length, num_steerings, 0, state, state_bytes, first, count, record, record_bytes, workspace,
                          workspace_bytes, stream);
 }
+
+// ---- dictionary bank (0 <= num_sources <= 8, 0 <= history_length <= 1024, 1 <= num_dictionaries <= 64, 1 <= num_steerings <= 64)
+#define LLD_ARGS cfg, num_sources, history_length, num_steerings, num_dictionaries
+size_t gccnmf_lldict_state_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries, int num_steerings) {
+  if (num_dictionaries < 1 || ll_check(nullptr, LLD_ARGS) != 0) return 0;
+  return ll_carve(*cfg, num_sources, nullptr, history_length, num_steerings, num_dictionaries).bytes;
+}
+
+int gccnmf_lldict_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries, int num_steerings,
+                       const float* const* W, const int* num_atoms, const float* const* H0, const double* E, const double* analysis_window,
+                       const double* synthesis_weights, float gain, void* state, size_t state_bytes, void* stream) {
+  return lld_init(h, cfg, num_sources, history_length, num_dictionaries, num_steerings, W, num_atoms, E, analysis_window, synthesis_weights, gain, H0,
+                  state, state_bytes, stream);
+}
+
+int gccnmf_lldict_load_dictionary(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
+                                  int num_steerings, void* state, size_t state_bytes, int index, const float* W, int num_atoms, const float* H0,
+                                  void* stream) {
+  return lld_load_dictionary(h, cfg, num_sources, history_length, num_dictionaries, num_steerings, state, state_bytes, index, W, num_atoms, H0, stream);
+}
+
+int gccnmf_lldict_load_steering(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
+                                int num_steerings, void* state, size_t state_bytes, int index, const double* E, void* stream) {
+  GCCNMF_REQUIRE(h, num_dictionaries >= 1, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, num_dictionaries);
+  return ll_load_steering(h, LLD_ARGS, state, state_bytes, index, E, stream);
+}
+
+int gccnmf_lldict_assign(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries, int num_steerings,
+                         void* state, size_t state_bytes, int first, int count, const int32_t* dictionary_host, const int32_t* steering_host,
+                         void* stream) {
+  return lld_assign(h, cfg, num_sources, history_length, num_dictionaries, num_steerings, state, state_bytes, first, count, dictionary_host,
+                    steering_host, stream);
+}
+
+int gccnmf_lldict_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
+                                int num_steerings, void* state, size_t state_bytes, int first, int count, void* stream) {
+  GCCNMF_REQUIRE(h, num_dictionaries >= 1, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, num_dictionaries);
+  return ll_reset_streams(h, LLD_ARGS, state, state_bytes, first, count, stream);
+}
+
+int gccnmf_lldict_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
+                             int num_steerings, void* state, size_t state_bytes, int first, int count, const gccnmf_ll_stream_params* params_host,
+                             void* stream) {
+  GCCNMF_REQUIRE(h, num_dictionaries >= 1, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, num_dictionaries);
+  return ll_set_params(h, LLD_ARGS, state, state_bytes, first, count, params_host, stream);
+}
+
+int gccnmf_lldict_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
+                              int num_steerings, void* state, size_t state_bytes, int first, int count, const int32_t* targets_host, void* stream) {
+  GCCNMF_REQUIRE(h, num_dictionaries >= 1, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, num_dictionaries);
+  GCCNMF_REQUIRE(h, num_sources != 0, "lldict_set_targets: needs num_sources in [2, %d] (got 0)", kLLMaxSources);
+  return ll_set_targets(h, LLD_ARGS, state, state_bytes, first, count, targets_host, stream);
+}
+
+int gccnmf_lldict_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
+                             int num_steerings, void* state, size_t state_bytes, int first, int count, const int32_t* windows_host, void* stream) {
+  GCCNMF_REQUIRE(h, num_dictionaries >= 1, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, num_dictionaries);
+  return ll_set_window(h, LLD_ARGS, state, state_bytes, first, count, windows_host, stream);
+}
+
+int gccnmf_lldict_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries, int num_steerings,
+                          void* state, size_t state_bytes, int hops, const float* in, float* out, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, num_dictionaries >= 1, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, num_dictionaries);
+  LLD_CARVE_OR_FAIL(l, num_sources, history_length, num_steerings, num_dictionaries);
+  return ll_enqueue(h, cfg, l, hops, in, out, stream);
+}
+
+int gccnmf_lldict_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
+                               int num_steerings, void* state, size_t state_bytes, int hops, float* in, float* out, const float* in_host,
+                               float* out_host, void** graph_exec, void* stream) {
+  GCCNMF_REQUIRE(h, num_dictionaries >= 1, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, num_dictionaries);
+  return ll_graph_create(h, LLD_ARGS, state, state_bytes, hops, in, out, in_host, out_host, graph_exec, stream);
+}
+
+int gccnmf_lldict_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries, int num_steerings,
+                         void* state, size_t state_bytes, int hops, int what, void* dst, void* stream) {
+  GCCNMF_REQUIRE(h, num_dictionaries >= 1, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, num_dictionaries);
+  return ll_export(h, LLD_ARGS, state, state_bytes, hops, what, dst, stream);
+}
+
+size_t gccnmf_lldict_record_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries, int num_steerings) {
+  if (num_dictionaries < 1 || ll_check(nullptr, LLD_ARGS) != 0) return 0;
+  return ll_record_bytes(*cfg, num_sources, history_length);
+}
+
+size_t gccnmf_lldict_workspace_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries, int num_steerings,
+                                     int count) {
+  if (num_dictionaries < 1 || ll_check(nullptr, LLD_ARGS) != 0 || count < 1) return 0;
+  return lld_record_workspace_bytes(*cfg, num_sources, history_length, num_dictionaries, num_steerings, count);
+}
+
+int gccnmf_lldict_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
+                               int num_steerings, void* state, size_t state_bytes, int first, int count, void* record, size_t record_bytes,
+                               void* workspace, size_t workspace_bytes, void* stream) {
+  return lld_save_streams(h, cfg, num_sources, history_length, num_dictionaries, num_steerings, state, state_bytes, first, count, record, record_bytes,
+                          workspace, workspace_bytes, stream);
+}
+
+int gccnmf_lldict_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
+                               int num_steerings, void* state, size_t state_bytes, int first, int count, const void* record, size_t record_bytes,
+                               void* workspace, size_t workspace_bytes, void* stream) {
+  return lld_load_streams(h, cfg, num_sources, history_length, num_dictionaries, num_steerings, state, state_bytes, first, count, record, record_bytes,
+                          workspace, workspace_bytes, stream);
+}
+#undef LLD_ARGS
 
 }  // extern "C"

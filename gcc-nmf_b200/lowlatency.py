@@ -35,7 +35,7 @@ import ctypes
 
 import numpy as np
 
-from ._lib import (LLBANK_MAX_STEERINGS, LLHIST_MAX_HISTORY, LLHIST_RECORD_CONFIG_HISTORY, RECORD_KIND_LL, RECORD_KIND_LLBANK, RECORD_MAGIC,
+from ._lib import (LLDICT_MAX_DICTIONARIES, LLBANK_MAX_STEERINGS, LLHIST_MAX_HISTORY, LLHIST_RECORD_CONFIG_HISTORY, RECORD_KIND_LL, RECORD_KIND_LLBANK, RECORD_MAGIC,
                    LLConfig, LLStreamParams, ParameterError, RecordHeader, default_handle)
 
 SYNTHESIS_MODES = ('online', 'lowlatency', 'windowed')
@@ -47,11 +47,15 @@ EXPORT_SOURCE_TARGETS, EXPORT_SOURCE_VALUES, EXPORT_SOURCE_MASKS, EXPORT_SOURCE_
     EXPORT_CARRIED_TARGETS, EXPORT_CALL_STATUS = range(14, 22)
 # export items of an engine with historyLength > 0 (gccnmf_llhist_export)
 EXPORT_HISTORY, EXPORT_HISTORY_INDEX, EXPORT_WINDOWS, EXPORT_WINDOW_MEANS = range(22, 26)
+EXPORT_DICTIONARY_ASSIGNMENT = 27                               # an engine with a dictionary bank (gccnmf_lldict_export)
+EXPORT_DICTIONARY_ATOMS = 28
+ATOMS_OFFSET = RecordHeader.config.offset + 4 * 3                # a record header's config.num_atoms
 EXPORT_ASSIGNMENT = 26                                          # an engine with a steering bank (gccnmf_llbank_export)
 STATUS_FEW_PEAKS, STATUS_ALL_NAN = 1, 2
 MAX_SOURCES = 8
 MAX_HISTORY = LLHIST_MAX_HISTORY
 MAX_STEERINGS = LLBANK_MAX_STEERINGS
+MAX_DICTIONARIES = LLDICT_MAX_DICTIONARIES
 
 
 def synthesisWeights(mode, synthesisWindow, hopSize):
@@ -100,9 +104,18 @@ class LowLatencyEngine(object):
             raise ValueError('a steering bank holds 1 .. %d tables (got %d)' % (MAX_STEERINGS, self.Qe))
         if bank and len({np.shape(e) for e in expJOmegaTau}) != 1:
             raise ValueError('the tables of a steering bank must all be (F, D)')
+        # a sequence of dictionaries is a dictionary bank (gccnmf_lldict_*, always with a steering bank): K = the largest K_i
+        self.Qd = len(W) if isinstance(W, (list, tuple)) else 0
+        if isinstance(W, (list, tuple)) and not 1 <= self.Qd <= MAX_DICTIONARIES:
+            raise ValueError('a dictionary bank holds 1 .. %d dictionaries (got %d)' % (MAX_DICTIONARIES, self.Qd))
+        if self.Qd and not bank:
+            bank, expJOmegaTau, self.Qe = True, [expJOmegaTau], 1
+        Ws = [np.ascontiguousarray(w, dtype=np.float32) for w in W] if self.Qd else None
+        if self.Qd and (any(w.ndim != 2 or w.shape[0] != Ws[0].shape[0] or w.shape[1] < 1 for w in Ws)):
+            raise ValueError('the dictionaries of a bank must all be (F, K_i) with K_i >= 1')
         self.h = default_handle(device)
         torch = self.torch = self.h.torch
-        W = np.ascontiguousarray(W, dtype=np.float32)
+        W = Ws[int(np.argmax([w.shape[1] for w in Ws]))] if self.Qd else np.ascontiguousarray(W, dtype=np.float32)
         E = np.ascontiguousarray(np.stack(list(expJOmegaTau)) if bank else expJOmegaTau, dtype=np.complex128)
         F, K = W.shape
         N = len(analysisWindow)
@@ -116,7 +129,9 @@ class LowLatencyEngine(object):
         if self.latency < 0:
             raise ValueError('the synthesis weights start less than a hop before the end of the frame')
         self.cfg = LLConfig(N, self.hop, self.C, K, self.D, self.S, int(numInferenceIterations), float(sparsityAlpha), float(epsilon))
-        if self.Qe:
+        if self.Qd:
+            self.state_bytes = int(self.h.lib.gccnmf_lldict_state_bytes(ctypes.byref(self.cfg), self.P, self.Lh, self.Qd, self.Qe))
+        elif self.Qe:
             self.state_bytes = int(self.h.lib.gccnmf_llbank_state_bytes(ctypes.byref(self.cfg), self.P, self.Lh, self.Qe))
         elif self.Lh:
             self.state_bytes = int(self.h.lib.gccnmf_llhist_state_bytes(ctypes.byref(self.cfg), self.P, self.Lh))
@@ -130,6 +145,7 @@ class LowLatencyEngine(object):
         self.stream = torch.cuda.Stream(device=self.h.device)      # a capturable stream of its own
         self.state = torch.empty(self.state_bytes, dtype=torch.uint8, device=self.h.device)
         H0 = None
+        self._seed, self._epsilon = seedValue, epsilon
         if self.inference:
             np.random.seed(seedValue)                                 # gccNMFFunctions.py:70,73, as online.py draws it
             H0 = (np.random.random((K, 2)).astype(np.float32) + epsilon).astype(np.float32)
@@ -142,9 +158,11 @@ class LowLatencyEngine(object):
         self._targets = np.full((self.S, max(self.P, 1)), -1, np.int32)
         self._window = np.zeros(self.S, np.int32)
         self._assign = np.zeros(self.S, np.int32)                 # bank: each stream's table
+        self._dassign = np.zeros(self.S, np.int32)                # dictionary bank: each stream's dictionary
         if self.Qe:                                               # content digests of the dictionary and the tables (bank records)
             from .records import content_digest
-            self._dict_digest = content_digest(W, H0) if H0 is not None else content_digest(W)
+            # (a dictionary bank keeps one digest per entry, below)
+            self._dict_digest = None if self.Qd else content_digest(W, H0) if H0 is not None else content_digest(W)
             self._steer_digests = [content_digest(e) for e in E]
         self._io = {}
         self._graphs = {}
@@ -154,6 +172,21 @@ class LowLatencyEngine(object):
         self.last_hops = None
         self.h.torch.cuda.current_stream(self.h.device).synchronize()
         c = self._const
+        if self.Qd:
+            self._dicts = [dev(w) for w in Ws]
+            self._h0s = [dev(self._draw_h0(w.shape[1])) for w in Ws] if self.inference else None
+            self._atoms = [w.shape[1] for w in Ws]
+            from .records import content_digest
+            self._dict_digests = [content_digest(w, self._draw_h0(w.shape[1])) if self.inference else content_digest(w) for w in Ws]
+            with torch.cuda.stream(self.stream):
+                ptr = lambda ts: (ctypes.c_void_p * self.Qd)(*[t.data_ptr() for t in ts])       # noqa: E731
+                self._check(self.h.lib.gccnmf_lldict_init(self.h.h, ctypes.byref(self.cfg), self.P, self.Lh, self.Qd, self.Qe, ptr(self._dicts),
+                                                          (ctypes.c_int * self.Qd)(*self._atoms), ptr(self._h0s) if self._h0s else None,
+                                                          c[1].data_ptr(), c[2].data_ptr(), c[3].data_ptr(), float(self.gain), self.state.data_ptr(),
+                                                          self.state_bytes, self.stream.cuda_stream))
+            self._send_params(0, self.S)
+            self.stream.synchronize()
+            return
         with torch.cuda.stream(self.stream):
             self._check(self._fn('init')(self.h.h, ctypes.byref(self.cfg), *self._p, c[0].data_ptr(), c[1].data_ptr(), c[2].data_ptr(),
                                          c[3].data_ptr(), float(self.gain), c[4].data_ptr() if c[4] is not None else None,
@@ -164,14 +197,21 @@ class LowLatencyEngine(object):
     def _check(self, status):
         self.h.check(status)
 
+    def _draw_h0(self, K):
+        """H0 (K, 2) as the plain engine with K atoms draws it."""
+        np.random.seed(self._seed)
+        return (np.random.random((K, 2)).astype(np.float32) + self._epsilon).astype(np.float32)
+
     @property
     def _p(self):
         """The num_sources argument of the gccnmf_llsep_* entries, num_sources and history_length of the gccnmf_llhist_* entries (none
         for gccnmf_ll_*)."""
+        if self.Qd:
+            return (self.P, self.Lh, self.Qd, self.Qe)
         return (self.P, self.Lh, self.Qe) if self.Qe else (self.P, self.Lh) if self.Lh else (self.P,) if self.P else ()
 
     def _fn(self, name):
-        prefix = 'gccnmf_llbank_' if self.Qe else 'gccnmf_llhist_' if self.Lh else 'gccnmf_llsep_' if self.P else 'gccnmf_ll_'
+        prefix = 'gccnmf_lldict_' if self.Qd else 'gccnmf_llbank_' if self.Qe else 'gccnmf_llhist_' if self.Lh else 'gccnmf_llsep_' if self.P else 'gccnmf_ll_'
         return getattr(self.h.lib, prefix + name)
 
     def _state(self, name, *args):
@@ -252,10 +292,50 @@ class LowLatencyEngine(object):
         if e.min() < 0 or e.max() >= self.Qe:
             raise ValueError('steering entries outside [0, %d)' % self.Qe)
         self._assign[idx] = e
+        self._send_assign(idx)
+
+    def _send_assign(self, idx):
         lo, hi = int(idx.min()), int(idx.max())
         arr = np.ascontiguousarray(self._assign[lo:hi + 1], dtype=np.int32)
-        self._state('assign', lo, hi - lo + 1, arr.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), self.stream.cuda_stream)
+        ptr = lambda a: a.ctypes.data_as(ctypes.POINTER(ctypes.c_int32))       # noqa: E731
+        if self.Qd:
+            darr = np.ascontiguousarray(self._dassign[lo:hi + 1], dtype=np.int32)
+            self._state('assign', lo, hi - lo + 1, ptr(darr), ptr(arr), self.stream.cuda_stream)
+        else:
+            self._state('assign', lo, hi - lo + 1, ptr(arr), self.stream.cuda_stream)
         self.stream.synchronize()
+
+    def assign_dictionary(self, streams, entries):
+        """Dictionary bank: the streams use dictionaries `entries` (broadcast to len(streams)) from the next call on; everything else
+        of them stays."""
+        if not self.Qd:
+            raise ValueError('assign_dictionary needs a dictionary bank (W a sequence of dictionaries)')
+        idx = self._streams(streams)
+        e = np.broadcast_to(np.asarray(entries, dtype=np.int64), idx.shape)
+        if e.min() < 0 or e.max() >= self.Qd:
+            raise ValueError('dictionary entries outside [0, %d)' % self.Qd)
+        self._dassign[idx] = e
+        self._send_assign(idx)
+
+    def load_dictionary(self, entry, W):
+        """Dictionary bank: dictionary `entry` becomes W (F, K), K <= numAtoms of the largest entry at construction, from the next call
+        on, for every stream on it; with inference its H0 is drawn as the plain engine with K atoms draws it."""
+        if not self.Qd:
+            raise ValueError('load_dictionary needs a dictionary bank (W a sequence of dictionaries)')
+        if not 0 <= int(entry) < self.Qd:
+            raise ValueError('dictionary entry outside [0, %d)' % self.Qd)
+        W = np.ascontiguousarray(W, dtype=np.float32)
+        if W.ndim != 2 or W.shape[0] != self.F or not 1 <= W.shape[1] <= self.K:
+            raise ValueError('W must be (%d, K) with 1 <= K <= %d' % (self.F, self.K))
+        t = self.torch.as_tensor(W).to(self.h.device)
+        h0 = self.torch.as_tensor(self._draw_h0(W.shape[1])).to(self.h.device) if self.inference else None
+        self._state('load_dictionary', int(entry), t.data_ptr(), W.shape[1], h0.data_ptr() if h0 is not None else None, self.stream.cuda_stream)
+        self.stream.synchronize()
+        from .records import content_digest
+        self._dicts[int(entry)], self._atoms[int(entry)] = t, W.shape[1]
+        self._dict_digests[int(entry)] = content_digest(W, h0.cpu().numpy()) if h0 is not None else content_digest(W)
+        if h0 is not None:
+            self._h0s[int(entry)] = h0
 
     def load_steering(self, entry, expJOmegaTau):
         """Steering bank: table `entry` becomes expJOmegaTau (F, D) from the next call on, for every stream on it."""
@@ -284,6 +364,7 @@ class LowLatencyEngine(object):
         idx = np.unique(self._streams(streams))
         self._window[idx] = 0
         self._assign[idx] = 0
+        self._dassign[idx] = 0
         breaks = np.flatnonzero(np.diff(idx) != 1) + 1          # one call per contiguous run of streams
         for run in np.split(idx, breaks):
             self._state('reset_streams', int(run[0]), len(run), self.stream.cuda_stream)
@@ -355,6 +436,9 @@ class LowLatencyEngine(object):
                            EXPORT_CARRIED_TARGETS: ((self.S, P), torch.int32), EXPORT_CALL_STATUS: ((1,), torch.int32)})
         if self.Qe:
             shapes[EXPORT_ASSIGNMENT] = ((self.S,), torch.int32)
+        if self.Qd:
+            shapes[EXPORT_DICTIONARY_ASSIGNMENT] = ((self.S,), torch.int32)
+            shapes[EXPORT_DICTIONARY_ATOMS] = ((self.Qd,), torch.int32)
         if self.Lh:
             shapes.update({EXPORT_HISTORY: ((self.S, D, self.Lh), torch.float64), EXPORT_HISTORY_INDEX: ((self.S,), torch.int32),
                            EXPORT_WINDOWS: ((self.S,), torch.int32), EXPORT_WINDOW_MEANS: ((D, T), torch.float64)})
@@ -371,8 +455,8 @@ class LowLatencyEngine(object):
     def _rec(self, name):
         """gccnmf_llrec_<name> bound to (cfg, P), gccnmf_llhist_<name> bound to (cfg, P, Lh) or gccnmf_llbank_<name> bound to
         (cfg, P, Lh, Qe)."""
-        fn = getattr(self.h.lib, ('gccnmf_llbank_' if self.Qe else 'gccnmf_llhist_' if self.Lh else 'gccnmf_llrec_') + name)
-        hist = (self.Lh, self.Qe) if self.Qe else (self.Lh,) if self.Lh else ()
+        fn = getattr(self.h.lib, ('gccnmf_lldict_' if self.Qd else 'gccnmf_llbank_' if self.Qe else 'gccnmf_llhist_' if self.Lh else 'gccnmf_llrec_') + name)
+        hist = (self.Lh, self.Qd, self.Qe) if self.Qd else (self.Lh, self.Qe) if self.Qe else (self.Lh,) if self.Lh else ()
         if name.endswith('_bytes'):
             return lambda *a: fn(ctypes.byref(self.cfg), self.P, *hist, *a)
         return lambda *a: fn(self.h.h, ctypes.byref(self.cfg), self.P, *hist, *a)
@@ -450,12 +534,31 @@ class LowLatencyEngine(object):
             self._header = self._record_header()
         want = self._header
         head = np.frombuffer(bytes(want), np.uint8)
-        for i in np.flatnonzero((record.data.numpy()[:, :len(head)] != head).any(axis=1))[:1]:
+        data = record.data.numpy()[:, :len(head)].copy()
+        if self.Qd:
+            # a dictionary bank's records carry the stream's K_i in the header's num_atoms: compared below, with the dictionary
+            atoms = data[:, ATOMS_OFFSET:ATOMS_OFFSET + 4].copy().view(np.int32).ravel()
+            data[:, ATOMS_OFFSET:ATOMS_OFFSET + 4] = head[ATOMS_OFFSET:ATOMS_OFFSET + 4]
+        for i in np.flatnonzero((data != head).any(axis=1))[:1]:
             got = record.header(int(i))
             value = lambda h, f: bytes(h.config) if f == 'config' else getattr(h, f)       # noqa: E731
             bad = [f for f, _ in RecordHeader._fields_ if value(got, f) != value(want, f)]
             raise ParameterError('record %d does not fit this engine: %s differ' % (i, ', '.join(bad)))
-        if self.Qe:
+        if self.Qd:
+            dentries, entries = np.empty(len(idx), np.int32), np.empty(len(idx), np.int32)
+            for i in range(len(idx)):
+                got = record.header(i)
+                K = int(atoms[i])
+                same = [e for e in range(self.Qd) if self._dict_digests[e] == got.dictionary_digest]
+                if not same:
+                    raise ParameterError('record %d: no dictionary entry of this engine holds the stream\'s dictionary' % i)
+                fit = [e for e in same if self._atoms[e] == K]
+                if not fit:
+                    raise ParameterError('record %d: the stream\'s dictionary has %d atoms, the entry holding it %d' % (i, K, self._atoms[same[0]]))
+                if got.steering_digest not in self._steer_digests:
+                    raise ParameterError('record %d: no steering entry of this engine has the stream\'s table' % i)
+                dentries[i], entries[i] = fit[0], self._steer_digests.index(got.steering_digest)
+        elif self.Qe:
             entries = np.empty(len(idx), np.int32)
             for i in range(len(idx)):
                 got = record.header(i)
@@ -467,10 +570,19 @@ class LowLatencyEngine(object):
         self._record_call('load_streams', idx, record)
         if self.Qe:
             self._assign[idx] = entries
+        if self.Qd:
+            self._dassign[idx] = dentries
         m = record.mirrors
         self._eps[idx], self._active[idx], self._override[idx], self._targets[idx] = m['eps'], m['active'], m['override'], m['targets']
         if self.Lh:
             self._window[idx] = m['window']
+
+    def _export_now(self, what):
+        """A per-stream assignment item (S) i32 as the device holds it, outside a call."""
+        buf = self.torch.zeros((self.S,), dtype=self.torch.int32).pin_memory()
+        self._state('export', 1, int(what), buf.data_ptr(), self.stream.cuda_stream)
+        self.stream.synchronize()
+        return buf.numpy().copy()
 
     def close(self):
         if self.h.h:
@@ -487,7 +599,7 @@ class LowLatencyEngine(object):
 
 def streamSignals(signals, W, expJOmegaTau, analysisWindow, synthesisWindow, hopSize, hopsPerCall=1, synthesis='lowlatency',
                   targetTDOAEpsilon=1.0, numInferenceIterations=0, use_graph=True, device=0, numSources=0, historyLength=0,
-                  localizationWindow=0, steeringEntries=None, **kwargs):
+                  localizationWindow=0, steeringEntries=None, dictionaryEntries=None, **kwargs):
     """Streams a list of stereo signals (2, n_i) through one engine, one stream each, hopsPerCall hops per call, and returns the
     outputs aligned with the input: out_i[..., p] = output sample p + latency (the batch function's targetEstimateSamplesOLA), each
     (2, n_i), or (P, 2, n_i) with numSources = P.  Shorter signals are followed by silence; the engine is flushed with `latency`
@@ -501,6 +613,8 @@ def streamSignals(signals, W, expJOmegaTau, analysisWindow, synthesisWindow, hop
     eng.set_localization(None, localizationWindow)
     if steeringEntries is not None:
         eng.assign_steering(None, steeringEntries)
+    if dictionaryEntries is not None:
+        eng.assign_dictionary(None, dictionaryEntries)
     step = eng.hop * eng.C
     total = max(s.shape[1] for s in sig) + eng.latency
     total = -(-total // step) * step

@@ -802,6 +802,72 @@ GCCNMF_API int gccnmf_llbank_load_streams(gccnmf_handle* h, const gccnmf_ll_conf
                                int num_steerings, void* state, size_t state_bytes, int first, int count, const void* record,
                                size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- a bank of dictionaries: each stream on its own dictionary and steering table ------------------------------------------------
+ * The engine of gccnmf_llbank_* with num_dictionaries = Qd dictionaries, 1 <= Qd <= 64, and 1 <= Qe <= 64 steering tables.  Every
+ * entry takes (num_sources, history_length, num_dictionaries, num_steerings) after the config.  cfg.num_atoms is Kmax, the most
+ * atoms an entry may hold.  Stream s is on dictionary entry dictionary[s] and steering entry steering[s]; init and reset_streams put it
+ * on (0, 0).  A stream on dictionary i (W_i with K_i atoms) and table j computes, bit for bit, every sample and export item (rows
+ * < K_i of the K-shaped ones) a gccnmf_llhist_* engine with the same num_sources and history_length built with (W_i, E_j) computes.
+ * - init takes W as Qd DEVICE pointers to (F, K_i) f32, num_atoms as Qd host K_i in [1, Kmax] and, with inference, H0 as Qd device
+ *   pointers to (K_i, 2) f32; E as gccnmf_llbank_init takes it.  load_dictionary(index, W, num_atoms, H0) replaces one entry.
+ * - assign(first, count, dictionary_host, steering_host): -1 (or a NULL array) keeps a stream's entry.  assign and both load_* calls
+ *   are stream-ordered, act from the next call, may sit between launches of a graph and keep every other part of the streams.
+ * - Export: the llbank items plus 27 the dictionary assignment (S) i32 and 28 the K_i table (Qd) i32.  K-shaped items keep Kmax rows;
+ *   rows >= K_i of a column are argmax -1 and masks, values, source masks and H 0.
+ * - Records: GCCNMF_RECORD_KIND_LLBANK with a gccnmf_llbank_record_header whose config.num_atoms is the stream's K_i and whose
+ *   dictionary digest is that of W_i (F, K_i) (then H0_i (K_i, 2) with inference): the record a gccnmf_llbank_* engine built with W_i
+ *   writes, so records move both ways between the two families.  A load puts the stream on the lowest entries holding its dictionary
+ *   (same digest and K) and its table, and refuses, with the state unchanged, a dictionary no entry holds or a K mismatch.
+ * K_i outside [1, Kmax], an entry outside the bank, Qd or Qe outside [1, 64], (Kmax + F) x 4 bytes over 227 KB with inference and the
+ * llbank refusals fail before anything is enqueued. */
+#define GCCNMF_LLDICT_MAX_DICTIONARIES 64
+#define GCCNMF_LLDICT_EXPORT_DICTIONARY_ASSIGNMENT 27
+#define GCCNMF_LLDICT_EXPORT_DICTIONARY_ATOMS 28
+/* Host only; 0 for an invalid configuration or argument. */
+GCCNMF_API size_t gccnmf_lldict_state_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
+                                 int num_steerings);
+GCCNMF_API int gccnmf_lldict_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
+                       int num_steerings, const float* const* W, const int* num_atoms, const float* const* H0, const double* E,
+                       const double* analysis_window, const double* synthesis_weights, float gain, void* state, size_t state_bytes,
+                       void* stream);
+GCCNMF_API int gccnmf_lldict_load_dictionary(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length,
+                                  int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int index, const float* W,
+                                  int num_atoms, const float* H0, void* stream);
+GCCNMF_API int gccnmf_lldict_load_steering(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length,
+                                int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int index, const double* E,
+                                void* stream);
+GCCNMF_API int gccnmf_lldict_assign(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
+                         int num_steerings, void* state, size_t state_bytes, int first, int count, const int32_t* dictionary_host,
+                         const int32_t* steering_host, void* stream);
+GCCNMF_API int gccnmf_lldict_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length,
+                                int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int first, int count, void* stream);
+GCCNMF_API int gccnmf_lldict_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length,
+                             int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int first, int count,
+                             const gccnmf_ll_stream_params* params_host, void* stream);
+GCCNMF_API int gccnmf_lldict_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length,
+                              int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int first, int count,
+                              const int32_t* targets_host, void* stream);
+GCCNMF_API int gccnmf_lldict_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length,
+                             int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int first, int count,
+                             const int32_t* windows_host, void* stream);
+GCCNMF_API int gccnmf_lldict_process(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
+                          int num_steerings, void* state, size_t state_bytes, int hops, const float* in, float* out, void* stream);
+GCCNMF_API int gccnmf_lldict_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length,
+                               int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int hops, float* in, float* out,
+                               const float* in_host, float* out_host, void** graph_exec, void* stream);
+GCCNMF_API int gccnmf_lldict_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
+                         int num_steerings, void* state, size_t state_bytes, int hops, int what, void* dst, void* stream);
+GCCNMF_API size_t gccnmf_lldict_record_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
+                                  int num_steerings);
+GCCNMF_API size_t gccnmf_lldict_workspace_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
+                                     int num_steerings, int count);
+GCCNMF_API int gccnmf_lldict_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length,
+                               int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int first, int count, void* record,
+                               size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream);
+GCCNMF_API int gccnmf_lldict_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length,
+                               int num_dictionaries, int num_steerings, void* state, size_t state_bytes, int first, int count,
+                               const void* record, size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- real-time stream records: move a live slot to another slot, engine, engine form, device or process ---------------------
  * One family for every real-time form, with the arguments of gccnmf_rtbank_*: (num_streams, num_sources, num_dictionaries,
  * num_steerings) = (1, 0, 0, 0) for gccnmf_rt_*, (S, 0, 0, 0) for gccnmf_rtm_*, (S, P, 0, 0) for gccnmf_rtsep_* and
