@@ -48,6 +48,8 @@ SIGNATURES = {
     'gccnmf_klnmf_workspace_bytes': (c_size_t, [c_int, c_int, c_int]),
     'gccnmf_klnmf_uses_tensor_cores': (c_int, [_H, c_int, c_int, c_int]),
     'gccnmf_klnmf': (c_int, [_H, _P, c_int, c_int, _P, _P, c_int, c_int, c_float, c_float, c_int, _P, c_size_t, _S]),
+    'gccnmf_klnmf_batched_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),
+    'gccnmf_klnmf_batched': (c_int, [_H, _P, c_int64, c_int64, c_int, c_int, c_int, _P, _P, c_int, c_int, c_float, c_float, c_int, _P, c_size_t, _S]),
     'gccnmf_klnmf_begin': (c_int, [_H, _P, c_int, c_int, _P, _P, c_int, _P, c_size_t, _S]),
     'gccnmf_klnmf_step_numer': (c_int, [_H, _P, c_int, c_int, _P, _P, c_int, c_float, c_float, c_int, _P, _P, c_size_t, _S]),
     'gccnmf_klnmf_step_apply': (c_int, [_H, c_int, c_int, _P, _P, c_int, _P, _P, c_size_t, _S]),
@@ -417,8 +419,9 @@ class Handle(object):
         return t.contiguous().to(self.device, non_blocking=True)
 
     # ------------------------------------------------------------------ ops (device tensors in / out)
-    def stft(self, samples, window, n_fft, hop, conjugate=True, want_V=False, out_key=None):
-        """samples (C, n) f32 cuda, window (n_fft) f64 cuda -> X (C, F, T) c64 [, V (F, C*T) f32]."""
+    def stft(self, samples, window, n_fft, hop, conjugate=True, want_V=False, out_key=None, out=None):
+        """samples (C, n) f32 cuda, window (n_fft) f64 cuda -> X (C, F, T) c64 [, V (F, C*T) f32].  out: (X, V) to write into
+        (contiguous, of those shapes; V may be None)."""
         torch = self.torch
         C, n = samples.shape
         T = self.lib.gccnmf_stft_num_frames(n, n_fft, hop)
@@ -427,8 +430,13 @@ class Handle(object):
                 raise ParameterError('Invalid hop_length: %d' % hop)
             raise ParameterError('Buffer is too short (n=%d) for frame_length=%d' % (n, n_fft))
         F = n_fft // 2 + 1
-        X = self._out(out_key, 'X', (C, F, T), torch.complex64)
-        V = self._out(out_key, 'V', (F, C * T), torch.float32) if want_V else None
+        if out is not None:
+            X, V = out
+            if tuple(X.shape) != (C, F, T) or (V is not None and tuple(V.shape) != (F, C * T)):
+                raise ParameterError('stft: out shapes %s do not match (%d, %d, %d)' % ([tuple(t.shape) for t in out if t is not None], C, F, T))
+        else:
+            X = self._out(out_key, 'X', (C, F, T), torch.complex64)
+            V = self._out(out_key, 'V', (F, C * T), torch.float32) if want_V else None
         self.check(self.lib.gccnmf_stft(self.h, _ptr(samples), samples.stride(0), C, n, _ptr(window), n_fft, hop,
                                         1 if conjugate else 0, _ptr(X), _ptr(V), self.stream))
         return (X, V) if want_V else X
@@ -454,6 +462,21 @@ class Handle(object):
         self.check(self.lib.gccnmf_klnmf(self.h, _ptr(V), F, T2, _ptr(W), _ptr(H), K, int(iterations),
                                          float(sparsity_alpha), float(epsilon), 1 if update_W else 0, _ptr(ws),
                                          ws.numel(), self.stream))
+        return W, H
+
+    def klnmf_batched(self, V, W, H, iterations, sparsity_alpha=0.0, epsilon=1e-16, update_W=True):
+        """B clips in one call, in place on W (B, F, K), H (B, K, T2) f32 cuda.  V (B, F, T2) f32 cuda may be a strided view
+        (unit stride along T2), e.g. clips side by side in the columns of one (F, B T2) matrix, read in place.  Clip b ends bit-identical to klnmf on it alone."""
+        B, F, T2 = V.shape
+        K = W.shape[2]
+        if V.stride(2) != 1 or not V.is_cuda:
+            raise ParameterError('klnmf_batched: V must be a cuda tensor with unit stride along T2')
+        if tuple(W.shape) != (B, F, K) or tuple(H.shape) != (B, K, T2):
+            raise ParameterError('klnmf_batched: W %s / H %s do not match V %s' % (tuple(W.shape), tuple(H.shape), tuple(V.shape)))
+        ws = self.workspace('klnmf_batched', self.lib.gccnmf_klnmf_batched_workspace_bytes(B, F, T2, K))
+        self.check(self.lib.gccnmf_klnmf_batched(self.h, V.data_ptr() if V.numel() else None, V.stride(1), V.stride(0), B, F, T2, _ptr(W), _ptr(H), K,
+                                                 int(iterations), float(sparsity_alpha), float(epsilon), 1 if update_W else 0, _ptr(ws),
+                                                 ws.numel(), self.stream))
         return W, H
 
     def _klnmf_ws(self, F, T2, K):

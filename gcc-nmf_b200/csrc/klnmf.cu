@@ -232,8 +232,11 @@ int apply_W_impl(gccnmf_handle* h, int F, int T2, float* W, float* H, int K, con
 // tensor-core path: TMA-fed plane GEMM (klnmf_tma.cu)
 bool gccnmf_klnmf_tma_supported(int F, int T2, int K);
 size_t gccnmf_klnmf_tma_workspace_bytes(int F, int T2, int K);
-int gccnmf_klnmf_tma_prepare(gccnmf_handle* h, const float* V, int F, int T2, const float* W, const float* H, int K, void* workspace,
+int gccnmf_klnmf_tma_prepare(gccnmf_handle* h, const float* V, int64_t ld_v, int F, int T2, const float* W, const float* H, int K, void* workspace,
                              size_t workspace_bytes, bool need_vt, bool need_w, bool need_ht, void* stream);
+bool gccnmf_klnmf_tma_batch_supported(gccnmf_handle* h, int F, int T2, int K);
+int gccnmf_klnmf_tma_batched(gccnmf_handle* h, const float* V, int64_t ld_v, int64_t clip_stride_v, int B, int F, int T2, float* W, float* H, int K,
+                             int iterations, float alpha, float eps, bool update_W, void* workspace, size_t clip_bytes, void* stream);
 int gccnmf_klnmf_tma_update_H(gccnmf_handle* h, const float* V, int F, int T2, const float* W, float* H, int K, float alpha, float eps,
                               void* workspace, size_t workspace_bytes, int colsum_state, bool pending_norms, void* stream);
 int gccnmf_klnmf_tma_partial_W(gccnmf_handle* h, const float* V, int F, int T2, const float* W, const float* H, int K, void* workspace,
@@ -270,12 +273,7 @@ bool gccnmf_klnmf_tma_pull_fused_ok(gccnmf_handle* h, int F, int K);
 
 static bool use_tc(const gccnmf_handle* h, int F, int T2, int K) { return !h->force_simt_nmf && gccnmf_klnmf_tma_supported(F, T2, K); }
 
-extern "C" {
-
-int gccnmf_klnmf_uses_tensor_cores(const gccnmf_handle* h, int F, int T2, int K) { return h && use_tc(h, F, T2, K) ? 1 : 0; }
-
-size_t gccnmf_klnmf_workspace_bytes(int F, int T2, int K) {
-  if (F <= 0 || T2 <= 0 || K <= 0) return 0;
+static size_t simt_workspace_bytes(int F, int T2, int K) {
   size_t n = 0;
   auto add = [&](size_t count) { n = align_up(n, 256) + count * sizeof(float); };
   add((size_t)F * T2);
@@ -283,7 +281,60 @@ size_t gccnmf_klnmf_workspace_bytes(int F, int T2, int K) {
   add((size_t)F * K + K);
   add(K);
   add(K);
-  n = align_up(n, 256);
+  return align_up(n, 256);
+}
+
+// The whole loop on the tensor-core path; V is read at row pitch ld_v.
+static int klnmf_tc(gccnmf_handle* h, const float* V, int64_t ld_v, int F, int T2, float* W, float* H, int K, int iterations, float sparsity_alpha,
+                    float epsilon, int update_W, void* workspace, size_t workspace_bytes, void* stream) {
+  if (int st = gccnmf_klnmf_tma_prepare(h, V, ld_v, F, T2, W, H, K, workspace, workspace_bytes, true, true, true, stream)) return st;
+  if (int st = gccnmf_klnmf_tma_l2_window(h, F, T2, K, true, workspace, workspace_bytes)) return st;
+  struct WindowGuard { gccnmf_handle* h; ~WindowGuard() { h->l2_window_base = nullptr; h->l2_window_bytes = 0; } } guard{h};
+  for (int it = 0; it < iterations; ++it) {
+    // colsum(W) comes out of the previous W update; with a fixed dictionary it is computed once
+    // (in the (U, G) gauge nothing is rescaled inside the loop: see klnmf_tma.cu)
+    if (int st = gccnmf_klnmf_tma_update_H(h, V, F, T2, W, H, K, sparsity_alpha, epsilon, workspace, workspace_bytes,
+                                          it == 0 ? 0 : (update_W ? 2 : 1), update_W && it > 0, stream)) return st;
+    if (!update_W) continue;
+    if (int st = gccnmf_klnmf_tma_partial_W(h, V, F, T2, W, H, K, workspace, workspace_bytes, true, stream)) return st;
+    if (int st = gccnmf_klnmf_tma_apply_W(h, F, T2, W, K, nullptr, false, workspace, workspace_bytes, stream)) return st;
+  }
+  if (int st = gccnmf_klnmf_tma_finish(h, F, T2, H, K, update_W != 0, workspace, workspace_bytes, stream)) return st;
+  if (update_W) return gccnmf_klnmf_tma_finish_W(h, F, T2, W, K, workspace, workspace_bytes, stream);
+  return GCCNMF_OK;
+}
+
+// The whole loop on the float32 SIMT path (V at pitch T2).
+static int klnmf_simt(gccnmf_handle* h, const float* V, int F, int T2, float* W, float* H, int K, int iterations, float sparsity_alpha, float epsilon,
+                      int update_W, void* workspace, size_t workspace_bytes, void* stream) {
+  Workspace w = carve(workspace, workspace_bytes, F, T2, K);
+  for (int it = 0; it < iterations; ++it) {
+    // with a fixed dictionary colsum(W) only has to be computed once
+    int st = update_H_impl(h, V, F, T2, W, H, K, sparsity_alpha, epsilon, w, !update_W && it > 0, stream);
+    if (st) return st;
+    if (!update_W) continue;
+    st = partial_W_impl(h, V, F, T2, W, H, K, w.numer, w, stream);
+    if (st) return st;
+    st = apply_W_impl(h, F, T2, W, H, K, w.numer, w, stream);
+    if (st) return st;
+  }
+  return GCCNMF_OK;
+}
+
+// Per-clip region of a batched run's workspace: the single-clip workspace, or -- when larger -- the float32 path's workspace plus a
+// packed copy of the clip's V (that path reads V at pitch T2; at tensor-core shapes the copy fits inside the single-clip size).
+static size_t batch_clip_bytes(int F, int T2, int K) {
+  return std::max(gccnmf_klnmf_workspace_bytes(F, T2, K), simt_workspace_bytes(F, T2, K) + align_up((size_t)F * T2 * sizeof(float), 256));
+}
+constexpr int kMaxBatchClips = 65535 / 8;     // grid z of a batched contraction = clips x k-splits (at most 8)
+
+extern "C" {
+
+int gccnmf_klnmf_uses_tensor_cores(const gccnmf_handle* h, int F, int T2, int K) { return h && use_tc(h, F, T2, K) ? 1 : 0; }
+
+size_t gccnmf_klnmf_workspace_bytes(int F, int T2, int K) {
+  if (F <= 0 || T2 <= 0 || K <= 0) return 0;
+  size_t n = simt_workspace_bytes(F, T2, K);
   if (gccnmf_klnmf_tma_supported(F, T2, K)) n = std::max(n, gccnmf_klnmf_tma_workspace_bytes(F, T2, K));
   return n;
 }
@@ -295,7 +346,7 @@ int gccnmf_klnmf_begin(gccnmf_handle* h, const float* V, int F, int T2, const fl
   if (!workspace || workspace_bytes < gccnmf_klnmf_workspace_bytes(F, T2, K))
     return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "klnmf workspace too small: need %zu bytes", gccnmf_klnmf_workspace_bytes(F, T2, K));
   if (use_tc(h, F, T2, K)) {
-    if (int st = gccnmf_klnmf_tma_prepare(h, V, F, T2, W, H, K, workspace, workspace_bytes, true, true, true, stream)) return st;
+    if (int st = gccnmf_klnmf_tma_prepare(h, V, (int64_t)T2, F, T2, W, H, K, workspace, workspace_bytes, true, true, true, stream)) return st;
     return gccnmf_klnmf_tma_l2_window(h, F, T2, K, true, workspace, workspace_bytes);      // cleared by gccnmf_klnmf_end
   }
   return GCCNMF_OK;
@@ -447,33 +498,52 @@ int gccnmf_klnmf(gccnmf_handle* h, const float* V, int F, int T2, float* W, floa
   if (!workspace || workspace_bytes < gccnmf_klnmf_workspace_bytes(F, T2, K))
     return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "klnmf workspace too small: need %zu bytes", gccnmf_klnmf_workspace_bytes(F, T2, K));
   if (iterations == 0) return GCCNMF_OK;
+  if (use_tc(h, F, T2, K))
+    return klnmf_tc(h, V, (int64_t)T2, F, T2, W, H, K, iterations, sparsity_alpha, epsilon, update_W, workspace, workspace_bytes, stream);
+  return klnmf_simt(h, V, F, T2, W, H, K, iterations, sparsity_alpha, epsilon, update_W, workspace, workspace_bytes, stream);
+}
+
+size_t gccnmf_klnmf_batched_workspace_bytes(int B, int F, int T2, int K) {
+  if (B < 1 || B > kMaxBatchClips || F <= 0 || T2 <= 0 || K <= 0) return 0;
+  return (size_t)B * batch_clip_bytes(F, T2, K);
+}
+
+int gccnmf_klnmf_batched(gccnmf_handle* h, const float* V, int64_t ld_v, int64_t clip_stride_v, int B, int F, int T2, float* W, float* H, int K,
+                         int iterations, float sparsity_alpha, float epsilon, int update_W, void* workspace, size_t workspace_bytes, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, B >= 1 && B <= kMaxBatchClips, "klnmf_batched: B must be 1 .. %d (got %d)", kMaxBatchClips, B);
+  if (int st = check_dims(h, F, T2, K)) return st;
+  GCCNMF_REQUIRE(h, V && W && H, "klnmf_batched: NULL V, W or H");
+  GCCNMF_REQUIRE(h, ld_v >= T2 && clip_stride_v >= 0, "klnmf_batched: V pitch %lld < T2 %d or negative clip stride %lld", (long long)ld_v, T2,
+                 (long long)clip_stride_v);
+  GCCNMF_REQUIRE(h, iterations >= 0, "klnmf_batched: iterations must be >= 0 (got %d)", iterations);
+  const size_t clip_bytes = batch_clip_bytes(F, T2, K);
+  if (!workspace || workspace_bytes < (size_t)B * clip_bytes)
+    return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "klnmf_batched workspace too small: need %zu bytes", (size_t)B * clip_bytes);
+  if (iterations == 0) return GCCNMF_OK;
+  char* ws = static_cast<char*>(workspace);
+  const int64_t fk = (int64_t)F * K, kt = (int64_t)K * T2;
   if (use_tc(h, F, T2, K)) {
-    if (int st = gccnmf_klnmf_tma_prepare(h, V, F, T2, W, H, K, workspace, workspace_bytes, true, true, true, stream)) return st;
-    if (int st = gccnmf_klnmf_tma_l2_window(h, F, T2, K, true, workspace, workspace_bytes)) return st;
-    struct WindowGuard { gccnmf_handle* h; ~WindowGuard() { h->l2_window_base = nullptr; h->l2_window_bytes = 0; } } guard{h};
-    for (int it = 0; it < iterations; ++it) {
-      // colsum(W) comes out of the previous W update; with a fixed dictionary it is computed once
-      // (in the (U, G) gauge nothing is rescaled inside the loop: see klnmf_tma.cu)
-      if (int st = gccnmf_klnmf_tma_update_H(h, V, F, T2, W, H, K, sparsity_alpha, epsilon, workspace, workspace_bytes,
-                                            it == 0 ? 0 : (update_W ? 2 : 1), update_W && it > 0, stream)) return st;
-      if (!update_W) continue;
-      if (int st = gccnmf_klnmf_tma_partial_W(h, V, F, T2, W, H, K, workspace, workspace_bytes, true, stream)) return st;
-      if (int st = gccnmf_klnmf_tma_apply_W(h, F, T2, W, K, nullptr, false, workspace, workspace_bytes, stream)) return st;
-    }
-    if (int st = gccnmf_klnmf_tma_finish(h, F, T2, H, K, update_W != 0, workspace, workspace_bytes, stream)) return st;
-    if (update_W) return gccnmf_klnmf_tma_finish_W(h, F, T2, W, K, workspace, workspace_bytes, stream);
+    if (gccnmf_klnmf_tma_batch_supported(h, F, T2, K))
+      return gccnmf_klnmf_tma_batched(h, V, ld_v, clip_stride_v, B, F, T2, W, H, K, iterations, sparsity_alpha, epsilon, update_W != 0, workspace,
+                                      clip_bytes, stream);
+    for (int b = 0; b < B; ++b)       // an option the batch form leaves out: the solo path, one clip at a time
+      if (int st = klnmf_tc(h, V + b * clip_stride_v, ld_v, F, T2, W + b * fk, H + b * kt, K, iterations, sparsity_alpha, epsilon, update_W,
+                            ws + b * clip_bytes, clip_bytes, stream)) return st;
     return GCCNMF_OK;
   }
-  Workspace w = carve(workspace, workspace_bytes, F, T2, K);
-  for (int it = 0; it < iterations; ++it) {
-    // with a fixed dictionary colsum(W) only has to be computed once
-    int st = update_H_impl(h, V, F, T2, W, H, K, sparsity_alpha, epsilon, w, !update_W && it > 0, stream);
-    if (st) return st;
-    if (!update_W) continue;
-    st = partial_W_impl(h, V, F, T2, W, H, K, w.numer, w, stream);
-    if (st) return st;
-    st = apply_W_impl(h, F, T2, W, H, K, w.numer, w, stream);
-    if (st) return st;
+  // float32 SIMT path (tiny or odd shapes, force_simt_nmf), one clip at a time
+  const size_t simt_bytes = simt_workspace_bytes(F, T2, K);
+  for (int b = 0; b < B; ++b) {
+    const float* Vb = V + b * clip_stride_v;
+    if (ld_v != T2) {
+      float* packed = reinterpret_cast<float*>(ws + b * clip_bytes + simt_bytes);
+      GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync(packed, (size_t)T2 * sizeof(float), Vb, (size_t)ld_v * sizeof(float), (size_t)T2 * sizeof(float), F,
+                                             cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+      Vb = packed;
+    }
+    if (int st = klnmf_simt(h, Vb, F, T2, W + b * fk, H + b * kt, K, iterations, sparsity_alpha, epsilon, update_W, ws + b * clip_bytes, simt_bytes,
+                            stream)) return st;
   }
   return GCCNMF_OK;
 }

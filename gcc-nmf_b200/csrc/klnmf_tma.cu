@@ -47,6 +47,11 @@ constexpr int kApplyTile = 32;
 
 // ------------------------------------------------------------------------------------------------ epilogues
 // (concept: tma_gemm.cuh)  A warp owns column n; the lane holds rows m .. m + 3, contiguous in every output below.
+// at_offset(bytes): the same functor with every buffer pointer moved `bytes` on (the clip of a batched launch, tgemm::Clips).
+template <class T>
+__device__ __forceinline__ T* byte_offset(T* p, int64_t bytes) {
+  return p ? reinterpret_cast<T*>(reinterpret_cast<typename std::conditional<std::is_const<T>::value, const char, char>::type*>(p) + bytes) : p;
+}
 struct EpiStoreT {   // DT[z][n][m] = acc.  G4 partials (m = atom, n = f) and the test entry.
   struct State {};
   struct Loaded {};
@@ -62,6 +67,7 @@ struct EpiStoreT {   // DT[z][n][m] = acc.  G4 partials (m = atom, n = f) and th
   __device__ float4 row_partial(const State&) const { return make_float4(0.f, 0.f, 0.f, 0.f); }
   __device__ void row_total(int, int, float) const {}
   __device__ void elem(int m, int n, float acc, int z) const { DT[(int64_t)z * slab + (int64_t)n * ld + m] = acc; }
+  __device__ EpiStoreT at_offset(int64_t bytes) const { EpiStoreT e = *this; e.DT = byte_offset(DT, bytes); return e; }
   __device__ Loaded load(int, int) const { return Loaded{}; }
   __device__ void store(int m, int n, const float4& acc, const Loaded&, int z, State&) const {
     const int valid = min(4, M - m);
@@ -83,6 +89,12 @@ struct EpiRatioPlanes {   // RT[n][m] = split(VT[n][m] / acc)     G1 / G3 (m = f
   const float* __restrict__ VT; bf16* __restrict__ RT; int64_t ld, plane; int M, N; bool vec;
   CUtensorMap operand_map;                         // (encoded by the launcher)
   const float* operand() const { return VT; }
+  __device__ EpiRatioPlanes at_offset(int64_t bytes) const {
+    EpiRatioPlanes e;
+    e.VT = byte_offset(VT, bytes); e.RT = byte_offset(RT, bytes);
+    e.ld = ld; e.plane = plane; e.M = M; e.N = N; e.vec = vec;
+    return e;
+  }
   int64_t operand_ld() const { return ld; }
   int operand_cols() const { return N; }
   __device__ void prefetch(int, int) const {}
@@ -121,6 +133,12 @@ struct EpiUpdateH {
   }
   float* __restrict__ HT; bf16* __restrict__ HTp; const float* __restrict__ colsum_part; const float* __restrict__ sumsq_part;
   float* __restrict__ rowsum_part; float alpha, eps; int64_t ld, plane; int M, N; int slots; bool vec;
+  __device__ EpiUpdateH at_offset(int64_t bytes) const {
+    EpiUpdateH e = *this;
+    e.HT = byte_offset(HT, bytes); e.HTp = byte_offset(HTp, bytes); e.colsum_part = byte_offset(colsum_part, bytes);
+    e.sumsq_part = byte_offset(sumsq_part, bytes); e.rowsum_part = byte_offset(rowsum_part, bytes);
+    return e;
+  }
   __device__ void row_values(int m, float* v) const {
     v[0] = 1.f;
     if (m >= M) return;
@@ -168,8 +186,10 @@ struct EpiUpdateH {
 
 // ------------------------------------------------------------------------------------------------ small kernels
 // dst32 (cols, ld32) = src (rows, cols; ld_src)^T, zero in the pad columns [rows, ld32); optional hi/lo planes (cols, ldp).
-__global__ void tma_transpose_split_kernel(const float* __restrict__ src, int rows, int cols, int64_t ld_src, float* __restrict__ dst32,
-                                           int64_t ld32, bf16* __restrict__ planes, int64_t ldp, int64_t plane) {
+// Each small kernel below has a `_clips` form for batched runs (gccnmf_klnmf_batched): the clip comes from the last grid index, the
+// caller's matrices of clip c lie c clip strides on, and its workspace buffers c * ws_clip_bytes on (one carve per clip).
+__device__ __forceinline__ void transpose_split(const float* __restrict__ src, int rows, int cols, int64_t ld_src, float* __restrict__ dst32,
+                                                int64_t ld32, bf16* __restrict__ planes, int64_t ldp, int64_t plane) {
   __shared__ float tile[32][33];
   const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
   for (int i = threadIdx.y; i < 32; i += blockDim.y) {
@@ -190,14 +210,30 @@ __global__ void tma_transpose_split_kernel(const float* __restrict__ src, int ro
     }
   }
 }
+__global__ void tma_transpose_split_kernel(const float* __restrict__ src, int rows, int cols, int64_t ld_src, float* __restrict__ dst32,
+                                           int64_t ld32, bf16* __restrict__ planes, int64_t ldp, int64_t plane) {
+  transpose_split(src, rows, cols, ld_src, dst32, ld32, planes, ldp, plane);
+}
+__global__ void tma_transpose_split_clips_kernel(const float* __restrict__ src, int rows, int cols, int64_t ld_src, int64_t src_clip,
+                                                 float* __restrict__ dst32, int64_t ld32, bf16* __restrict__ planes, int64_t ldp, int64_t plane,
+                                                 int64_t ws_clip_bytes) {
+  const int64_t c = blockIdx.z;
+  transpose_split(src + c * src_clip, rows, cols, ld_src, byte_offset(dst32, c * ws_clip_bytes), ld32, byte_offset(planes, c * ws_clip_bytes),
+                  ldp, plane);
+}
 
-__global__ void tma_split_kernel(const float* __restrict__ src, int64_t n, bf16* __restrict__ planes, int64_t plane) {
+__device__ __forceinline__ void split_planes(const float* __restrict__ src, int64_t n, bf16* __restrict__ planes, int64_t plane) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   bf16 hi, lo;
   split_bf16(src[i], hi, lo);
   planes[i] = hi;
   planes[plane + i] = lo;
+}
+__global__ void tma_split_kernel(const float* __restrict__ src, int64_t n, bf16* __restrict__ planes, int64_t plane) { split_planes(src, n, planes, plane); }
+__global__ void tma_split_clips_kernel(const float* __restrict__ src, int64_t n, bf16* __restrict__ planes, int64_t plane, int64_t ws_clip_bytes) {
+  const int64_t c = blockIdx.y;
+  split_planes(src + c * n, n, byte_offset(planes, c * ws_clip_bytes), plane);
 }
 
 // planes (rows, pitch) = split(src (rows, inner)) row by row (pitch >= inner; pad columns are left as they are).
@@ -211,12 +247,17 @@ __global__ void tma_split_rows_kernel(const float* src, int rows, int inner, bf1
   planes[plane + (int64_t)r * pitch + col] = lo;
 }
 
-__global__ void tma_colsum_kernel(const float* W, int F, int K, float* colsum) {
+__device__ __forceinline__ void column_sums(const float* W, int F, int K, float* colsum) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= K) return;
   float s = 0.f;
   for (int f = 0; f < F; ++f) s += W[(int64_t)f * K + k];   // row order like numpy.sum(W, axis=0)
   colsum[k] = s;
+}
+__global__ void tma_colsum_kernel(const float* W, int F, int K, float* colsum) { column_sums(W, F, K, colsum); }
+__global__ void tma_colsum_clips_kernel(const float* W, int F, int K, float* colsum, int64_t ws_clip_bytes) {
+  const int64_t c = blockIdx.y;
+  column_sums(W + c * F * K, F, K, byte_offset(colsum, c * ws_clip_bytes));
 }
 
 // Cross-rank sum read straight from the NVSwitch: p is the multicast address of a symmetric buffer, every rank's copy of the
@@ -254,10 +295,10 @@ __device__ __forceinline__ float4 ld_sys_f32x4(const float* p) {      // strong 
   return v;
 }
 template <int MODE>
-__global__ void __launch_bounds__(256)
-tma_apply_w_kernel(float* __restrict__ U, bf16* __restrict__ Up, int64_t plane, const float* __restrict__ partial, int splits,
-                   const float* __restrict__ rowsum, int rowsum_slots, int F, int K, float* __restrict__ sumsq_part, float* __restrict__ colsum_part,
-                   const unsigned* arrival_counter, unsigned arrivals_expected, unsigned long long* stamp, PeerSet peers) {
+__device__ __forceinline__ void
+apply_w(float* __restrict__ U, bf16* __restrict__ Up, int64_t plane, const float* __restrict__ partial, int splits,
+        const float* __restrict__ rowsum, int rowsum_slots, int F, int K, float* __restrict__ sumsq_part, float* __restrict__ colsum_part,
+        const unsigned* arrival_counter, unsigned arrivals_expected, unsigned long long* stamp, const PeerSet& peers) {
   constexpr bool MULTIMEM = MODE == kApplyMultimem;
   constexpr bool PULL = MODE == kApplyPull || MODE == kApplyPullOwner;
   __shared__ float4 part[2][8][32];
@@ -374,6 +415,22 @@ tma_apply_w_kernel(float* __restrict__ U, bf16* __restrict__ Up, int64_t plane, 
     *reinterpret_cast<float4*>((g == 0 ? sumsq_part : colsum_part) + (int64_t)blockIdx.y * K + k) = s;
   }
   if (stamping) stamp[7] = tgemm::globaltimer_ns();
+}
+template <int MODE>
+__global__ void __launch_bounds__(256)
+tma_apply_w_kernel(float* __restrict__ U, bf16* __restrict__ Up, int64_t plane, const float* __restrict__ partial, int splits,
+                   const float* __restrict__ rowsum, int rowsum_slots, int F, int K, float* __restrict__ sumsq_part, float* __restrict__ colsum_part,
+                   const unsigned* arrival_counter, unsigned arrivals_expected, unsigned long long* stamp, PeerSet peers) {
+  apply_w<MODE>(U, Up, plane, partial, splits, rowsum, rowsum_slots, F, K, sumsq_part, colsum_part, arrival_counter, arrivals_expected, stamp, peers);
+}
+// The single-GPU W update of every clip of a batch (this GPU's k-split slabs and row-sum slots), clip = blockIdx.z.
+__global__ void __launch_bounds__(256)
+tma_apply_w_clips_kernel(float* __restrict__ U, bf16* __restrict__ Up, int64_t plane, const float* __restrict__ partial, int splits,
+                         const float* __restrict__ rowsum, int rowsum_slots, int F, int K, float* __restrict__ sumsq_part,
+                         float* __restrict__ colsum_part, int64_t ws_clip_bytes) {
+  const int64_t c = blockIdx.z, o = c * ws_clip_bytes;
+  apply_w<kApplyLocal>(U + c * F * K, byte_offset(Up, o), plane, byte_offset(partial, o), splits, byte_offset(rowsum, o), rowsum_slots, F, K,
+                       byte_offset(sumsq_part, o), byte_offset(colsum_part, o), nullptr, 0u, nullptr, PeerSet{});
 }
 
 // W update with the cross-rank exchange INSIDE it, tile by tile (frame-sharded runs, gccnmf_klnmf_step_pull form 2): the CTA that
@@ -517,16 +574,24 @@ __device__ __forceinline__ float column_norm(const float* __restrict__ sumsq_par
   for (int b = 0; b < row_blocks; ++b) q += sumsq_part[(int64_t)b * K + k];
   return sqrtf(q);
 }
-__global__ void tma_finish_w_kernel(float* __restrict__ W, int F, int K, const float* __restrict__ sumsq_part, int row_blocks) {
+__device__ __forceinline__ void finish_w(float* __restrict__ W, int F, int K, const float* __restrict__ sumsq_part, int row_blocks) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= K) return;
   const float nrm = column_norm(sumsq_part, row_blocks, K, k);
   for (int f = blockIdx.y; f < F; f += gridDim.y) W[(int64_t)f * K + k] = W[(int64_t)f * K + k] / nrm;      // W /= norms (:80)
 }
+__global__ void tma_finish_w_kernel(float* __restrict__ W, int F, int K, const float* __restrict__ sumsq_part, int row_blocks) {
+  finish_w(W, F, K, sumsq_part, row_blocks);
+}
+__global__ void tma_finish_w_clips_kernel(float* __restrict__ W, int F, int K, const float* __restrict__ sumsq_part, int row_blocks,
+                                          int64_t ws_clip_bytes) {
+  const int64_t c = blockIdx.z;
+  finish_w(W + c * F * K, F, K, byte_offset(sumsq_part, c * ws_clip_bytes), row_blocks);
+}
 
 // H (K, T2; caller) = HT32 (T2, K)^T * c (H *= norms, :81) -- or a plain transpose when there was no W update.
-__global__ void tma_finish_h_kernel(const float* __restrict__ HT, int T2, int K, const float* __restrict__ sumsq_part, int row_blocks,
-                                    float* __restrict__ H) {
+__device__ __forceinline__ void finish_h(const float* __restrict__ HT, int T2, int K, const float* __restrict__ sumsq_part, int row_blocks,
+                                         float* __restrict__ H) {
   __shared__ float tile[32][33];
   __shared__ float nrm_s[32];
   const int k0 = blockIdx.x * 32, t0 = blockIdx.y * 32;
@@ -543,6 +608,15 @@ __global__ void tma_finish_h_kernel(const float* __restrict__ HT, int T2, int K,
       H[(int64_t)k * T2 + t] = sumsq_part ? v * nrm_s[i] : v;
     }
   }
+}
+__global__ void tma_finish_h_kernel(const float* __restrict__ HT, int T2, int K, const float* __restrict__ sumsq_part, int row_blocks,
+                                    float* __restrict__ H) {
+  finish_h(HT, T2, K, sumsq_part, row_blocks, H);
+}
+__global__ void tma_finish_h_clips_kernel(const float* __restrict__ HT, int T2, int K, const float* __restrict__ sumsq_part, int row_blocks,
+                                          float* __restrict__ H, int64_t ws_clip_bytes) {
+  const int64_t c = blockIdx.z, o = c * ws_clip_bytes;
+  finish_h(byte_offset(HT, o), T2, K, byte_offset(sumsq_part, o), row_blocks, H + c * K * T2);
 }
 
 // numer = [sum_z partial[z] (F*K) | sum_s rowsum_part[s] (K)] for the cross-rank sum.
@@ -842,14 +916,14 @@ bool w_cluster_reduce(gccnmf_handle* h, const Plan& p, int F, int K) {
 bool gccnmf_klnmf_tma_supported(int F, int T2, int K) { return K % 8 == 0 && F >= 128 && T2 >= 128 && K >= 32; }
 size_t gccnmf_klnmf_tma_workspace_bytes(int F, int T2, int K) { return tma_workspace_bytes(F, T2, K); }
 
-// Builds the operand set from the caller's V, W, H: V^T, planes of W, H^T (float32 + planes).
-int gccnmf_klnmf_tma_prepare(gccnmf_handle* h, const float* V, int F, int T2, const float* W, const float* H, int K,
+// Builds the operand set from the caller's V (row pitch ld_v), W, H: V^T, planes of W, H^T (float32 + planes).
+int gccnmf_klnmf_tma_prepare(gccnmf_handle* h, const float* V, int64_t ld_v, int F, int T2, const float* W, const float* H, int K,
                              void* workspace, size_t workspace_bytes, bool need_vt, bool need_w, bool need_ht, void* stream) {
   TMA_CARVE_OR_FAIL(w);
   const dim3 block(32, 8);
   GCCNMF_CHECK_CUDA(h, cudaMemsetAsync(w.done, 0, 16, (cudaStream_t)stream));
   if (need_vt)
-    GCCNMF_LAUNCH(h, tma_transpose_split_kernel, dim3((T2 + 31) / 32, (int)((w.Fp + 31) / 32)), block, 0, stream, V, F, T2, (int64_t)T2, w.VT, w.Fp,
+    GCCNMF_LAUNCH(h, tma_transpose_split_kernel, dim3((T2 + 31) / 32, (int)((w.Fp + 31) / 32)), block, 0, stream, V, F, T2, ld_v, w.VT, w.Fp,
                   (bf16*)nullptr, (int64_t)0, (int64_t)0);
   if (need_w) {
     const int64_t n = (int64_t)F * K;
@@ -1127,6 +1201,56 @@ int gccnmf_klnmf_tma_l2_window(gccnmf_handle* h, int F, int T2, int K, bool enab
   }
   h->l2_window_base = w.HT;
   h->l2_window_bytes = bytes;
+  return 0;
+}
+
+// ---- batched runs (gccnmf_klnmf_batched): B clips of one shape.  Clip b's workspace is the single-clip carve at
+// workspace + b * clip_bytes; every launch of an iteration covers all clips (clip from the grid), and each clip runs the tile plan
+// of a solo run on its shape, so its W and H carry the bits of gccnmf_klnmf on it alone.  The W-update numerator is always
+// written as k-split slabs and summed by the W update in split order, the sum the cluster-reduced form makes in the same order:
+// the cluster form needs all of a launch's clusters resident, which B clips can break.
+
+// The options the batch form leaves out (the L2 access-policy window, the split W.H contractions): the caller runs such a clip set
+// one clip at a time by the solo path.
+bool gccnmf_klnmf_tma_batch_supported(gccnmf_handle* h, int F, int T2, int K) { return h->l2_persist <= 0 && !wh_split2(h, F, T2, K); }
+
+int gccnmf_klnmf_tma_batched(gccnmf_handle* h, const float* V, int64_t ld_v, int64_t clip_stride_v, int B, int F, int T2, float* W, float* H, int K,
+                             int iterations, float alpha, float eps, bool update_W, void* workspace, size_t clip_bytes, void* stream) {
+  const TmaWorkspace w = tma_carve(workspace, clip_bytes, F, T2, K);      // clip 0; clip b is the same carve b * clip_bytes on
+  if (!w.ok) return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "klnmf_batched: %zu bytes per clip, need %zu", clip_bytes, tma_workspace_bytes(F, T2, K));
+  const int64_t cb = (int64_t)clip_bytes;
+  const Plan p = make_plan(h, F, T2, K);
+  const dim3 block(32, 8);
+  GCCNMF_LAUNCH(h, tma_transpose_split_clips_kernel, dim3((T2 + 31) / 32, (int)((w.Fp + 31) / 32), B), block, 0, stream, V, F, T2, ld_v, clip_stride_v,
+                w.VT, w.Fp, (bf16*)nullptr, (int64_t)0, (int64_t)0, cb);
+  const int64_t fk = (int64_t)F * K;
+  GCCNMF_LAUNCH(h, tma_split_clips_kernel, dim3((unsigned)((fk + 255) / 256), B), 256, 0, stream, (const float*)W, fk, w.Wp, w.plane_w, cb);
+  GCCNMF_LAUNCH(h, tma_transpose_split_clips_kernel, dim3((T2 + 31) / 32, (K + 31) / 32, B), block, 0, stream, (const float*)H, K, T2, (int64_t)T2,
+                (int64_t)K * T2, w.HT, (int64_t)K, w.HTp, (int64_t)K, w.plane_ht, cb);
+  const Operand Wk{w.Wp, (int64_t)K, w.plane_w, false}, Wmn{w.Wp, (int64_t)K, w.plane_w, true};
+  const Operand HTk{w.HTp, (int64_t)K, w.plane_ht, false}, HTmn{w.HTp, (int64_t)K, w.plane_ht, true};
+  const Operand RTk{w.RTp, w.Fp, w.plane_rt, false}, RTmn{w.RTp, w.Fp, w.plane_rt, true};
+  const tgemm::Clips<EpiRatioPlanes> ratio{EpiRatioPlanes{w.VT, w.RTp, w.Fp, w.plane_rt, F, T2, true}, cb, 1};
+  const tgemm::Clips<EpiStoreT> numer{EpiStoreT{w.partial, (int64_t)K, fk, K, F, true, h->gemm_streaming != 0}, cb, p.w.splits};
+  for (int it = 0; it < iterations; ++it) {
+    // (gccnmf_klnmf's loop: colsum(U) computed at the first iteration, then left by the W update, or kept with a fixed dictionary)
+    const int colsum_state = it == 0 ? 0 : (update_W ? 2 : 1);
+    if (int st = plane_gemm_clips<false, false>(h, p.bn_wh, Wk, HTk, F, T2, K, 1, true, ratio, B, stream)) return st;        // G1
+    if (colsum_state == 0) GCCNMF_LAUNCH(h, tma_colsum_clips_kernel, dim3((K + 127) / 128, B), 128, 0, stream, (const float*)W, F, K, w.colsum, cb);
+    const tgemm::Clips<EpiUpdateH> upd{EpiUpdateH{w.HT, w.HTp, w.colsum, colsum_state == 2 ? w.sumsq_part : nullptr, w.rowsum_part, alpha, eps,
+                                                  (int64_t)K, w.plane_ht, K, T2, colsum_state == 2 ? w.row_blocks : 1, true}, cb, 1};
+    if (int st = plane_gemm_clips<true, false>(h, p.bn_h, Wmn, RTk, K, T2, F, 1, false, upd, B, stream)) return st;          // G2
+    if (!update_W) continue;
+    if (int st = plane_gemm_clips<false, false>(h, p.bn_wh, Wk, HTk, F, T2, K, 1, true, ratio, B, stream)) return st;        // G3
+    if (int st = plane_gemm_clips<true, true>(h, p.w.bn, HTmn, RTmn, K, F, T2, p.w.splits, false, numer, B, stream)) return st;  // G4
+    if (int st = launch_ex(h, "tma_apply_w_clips_kernel", tma_apply_w_clips_kernel, dim3((K + kApplyAtoms - 1) / kApplyAtoms, w.row_blocks, B), block,
+                           0, stream, h->nmf_pdl, dim3(1, 1, 1), W, w.Wp, w.plane_w, (const float*)w.partial, p.w.splits, (const float*)w.rowsum_part,
+                           p.rowsum_slots, F, K, w.sumsq_part, w.colsum, cb)) return st;
+  }
+  GCCNMF_LAUNCH(h, tma_finish_h_clips_kernel, dim3((K + 31) / 32, (T2 + 31) / 32, B), block, 0, stream, (const float*)w.HT, T2, K,
+                update_W ? (const float*)w.sumsq_part : (const float*)nullptr, w.row_blocks, H, cb);
+  if (update_W)
+    GCCNMF_LAUNCH(h, tma_finish_w_clips_kernel, dim3((K + 127) / 128, std::min(F, 64), B), 128, 0, stream, W, F, K, (const float*)w.sumsq_part, w.row_blocks, cb);
   return 0;
 }
 

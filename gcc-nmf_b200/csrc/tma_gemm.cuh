@@ -65,6 +65,13 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
+// One 4-D box (inner, rows, planes, clip) -> shared memory of this CTA: the operand maps of a batched launch (Clips).
+__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
 // Same, delivered to the same shared-memory offset (and signalled on the same barrier offset) of every CTA of the cluster in `mask`.
 template <bool MULTICAST>
 __device__ __forceinline__ void tma_load_3d_mc(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, uint16_t mask) {
@@ -255,6 +262,47 @@ struct wants_dual_n { static constexpr bool value = false; };
 template <class E>
 struct wants_dual_n<E, decltype((void)E::kDualN)> { static constexpr bool value = E::kDualN; };
 
+// Batched launch of a by-column epilogue E over C clips of one shape: blockIdx.z = clip * splits + split, so the (1, 1, splits)
+// extent of a clip's k-splits never mixes clips, and clip c's operand planes, epilogue buffers and SIMT-tail operands all lie
+// c * clip_bytes past clip 0's (one per-clip workspace carve repeated C times).  The operand maps carry a fourth, clip dimension
+// with that stride, so TMA zero-fills each clip's ragged edges exactly as in a launch on that clip alone, and the functor a CTA
+// runs is E::at_offset(c * clip_bytes): E with every pointer moved to clip c.  Every tile therefore computes what the same tile of
+// a solo launch computes.  A batched launch runs 1 x 1 clusters and takes the epilogue operand from global memory (no operand
+// map), neither of which changes a result.  The trait makes it a separate instantiation of plane_gemm_kernel.
+template <class E>
+struct Clips {
+  static constexpr bool kBatched = true;
+  static constexpr bool kRowReduce = E::kRowReduce;
+  static constexpr int kRowValues = E::kRowValues;
+  static constexpr bool kPrefetch = E::kPrefetch;
+  static constexpr bool kDualN = wants_dual_n<E>::value;
+  static constexpr bool kPreloadOperands = wants_preload<E>::value;
+  using State = typename E::State;
+  using Loaded = typename E::Loaded;
+  E e;                 // clip 0
+  int64_t clip_bytes;
+  int splits;
+};
+template <class E>
+struct is_batched { static constexpr bool value = false; };
+template <class E>
+struct is_batched<Clips<E>> { static constexpr bool value = true; };
+
+// The functor of this CTA's clip (the launch's own functor when not batched), its clip and its k-split.
+template <class E> __device__ __forceinline__ const E& clip_epilogue(const E& e, int) { return e; }
+template <class E> __device__ __forceinline__ E clip_epilogue(const Clips<E>& c, int clip) { return c.e.at_offset(c.clip_bytes * clip); }
+template <class E> __device__ __forceinline__ int clip_of(const E&) { return 0; }
+template <class E> __device__ __forceinline__ int clip_of(const Clips<E>& c) { return (int)blockIdx.z / c.splits; }
+template <class E> __device__ __forceinline__ int split_of(const E&) { return blockIdx.z; }
+template <class E> __device__ __forceinline__ int split_of(const Clips<E>& c) { return (int)blockIdx.z % c.splits; }
+template <class E> __device__ __forceinline__ int64_t clip_offset(const E&, int) { return 0; }
+template <class E> __device__ __forceinline__ int64_t clip_offset(const Clips<E>& c, int clip) { return c.clip_bytes * clip; }
+template <bool BATCHED, bool MULTICAST>
+__device__ __forceinline__ void tma_load_operand(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int clip, uint16_t mask) {
+  if constexpr (BATCHED) tma_load_4d(dst, map, bar, c0, c1, c2, clip);
+  else tma_load_3d_mc<MULTICAST>(dst, map, bar, c0, c1, c2, mask);
+}
+
 // Epilogue concept (functors in klnmf_tma.cu).  The kernel stages the accumulator tile in shared memory and hands it out by
 // columns: a warp owns column n, lane l rows m .. m + 3 with m = m0 + 4 l (contiguous in every output of the KL-NMF loop).
 //   static constexpr int kRowValues (<= kMaxRowValues);  __device__ void row_values(int m, float* v) const;
@@ -273,6 +321,8 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   using C = Config<BN, KB, A_MN, B_MN, DUAL ? 2 : 1, wants_smem_operand<Epilogue>::value && !has_tile_epilogue<Epilogue>::value>;
   constexpr bool OPERAND = C::kOperandBytes > 0;     // the epilogue's operand tile comes into shared memory by TMA
   constexpr int kCluster = CN * CM;
+  constexpr bool BATCHED = is_batched<Epilogue>::value;
+  static_assert(!BATCHED || kCluster == 1, "a batched launch runs 1 x 1 clusters");
   static_assert((CN == 1 || CN == 2) && (CM == 1 || CM == 2), "cluster of CN n-tiles x CM m-tiles");
   static_assert(A_MN || (kBM / CN) % 8 == 0, "A row slices keep the swizzle atoms whole");
   static_assert(B_MN || (BN / CM) % 8 == 0, "B row slices keep the swizzle atoms whole");
@@ -283,7 +333,9 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   const bool mf = args.m_fastest != 0;
   const int tile_n = mf ? (int)blockIdx.y : (int)blockIdx.x;
   const int tile_m = mf ? (int)blockIdx.x : (int)blockIdx.y;
-  const int z = blockIdx.z;
+  const int z = split_of(epi);
+  const int clip = clip_of(epi);
+  auto&& ep = clip_epilogue(epi, clip);     // the functor of my clip
   const int n0 = tile_n * BN;
   const int total_kblocks = (args.Kc + KB - 1) / KB;
   const int kb_begin = z * args.kblocks_per_split;
@@ -347,7 +399,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
 #pragma unroll
       for (int u = 0; u < kPre; ++u) {
         const int cc = warp + kWarpsAll * u;
-        if (cc < n_valid) pre[u] = epi.load(m0 + 4 * lane, n0 + cc);
+        if (cc < n_valid) pre[u] = ep.load(m0 + 4 * lane, n0 + cc);
       }
     }
   };
@@ -366,22 +418,22 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         if (A_MN) {
 #pragma unroll
           for (int a = 0; a < C::kAAtoms; ++a)
-            if (a % CN == cx) tma_load_3d_mc<(CN > 1)>(a_dst + a * C::kAtomBytes, &map_a, bar, m0 + 64 * a, k0, 0, mask_row);
+            if (a % CN == cx) tma_load_operand<BATCHED, (CN > 1)>(a_dst + a * C::kAtomBytes, &map_a, bar, m0 + 64 * a, k0, 0, clip, mask_row);
         } else {
           constexpr int kRows = kBM / CN;      // my row slice of the A tile, one box per plane
 #pragma unroll
           for (int p = 0; p < 2; ++p)
-            tma_load_3d_mc<(CN > 1)>(a_dst + p * (kBM * KB * 2) + cx * (kRows * KB * 2), &map_a, bar, k0, m0 + cx * kRows, p, mask_row);
+            tma_load_operand<BATCHED, (CN > 1)>(a_dst + p * (kBM * KB * 2) + cx * (kRows * KB * 2), &map_a, bar, k0, m0 + cx * kRows, p, clip, mask_row);
         }
         if (B_MN) {
 #pragma unroll
           for (int a = 0; a < C::kBAtoms; ++a)
-            if (a % CM == cy) tma_load_3d_mc<(CM > 1)>(b_dst + a * C::kAtomBytes, &map_b, bar, n0 + 64 * a, k0, 0, mask_col);
+            if (a % CM == cy) tma_load_operand<BATCHED, (CM > 1)>(b_dst + a * C::kAtomBytes, &map_b, bar, n0 + 64 * a, k0, 0, clip, mask_col);
         } else {
           constexpr int kRows = BN / CM;
 #pragma unroll
           for (int p = 0; p < 2; ++p)
-            tma_load_3d_mc<(CM > 1)>(b_dst + p * (BN * KB * 2) + cy * (kRows * KB * 2), &map_b, bar, k0, n0 + cy * kRows, p, mask_col);
+            tma_load_operand<BATCHED, (CM > 1)>(b_dst + p * (BN * KB * 2) + cy * (kRows * KB * 2), &map_b, bar, k0, n0 + cy * kRows, p, clip, mask_col);
         }
       }
       if constexpr (OPERAND) {
@@ -400,7 +452,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     if (Epilogue::kRowValues > 0) {                      // the functor's per-row values, one row per thread
       for (int r = e * 32 + lane; r < kBM; r += kAuxWarps * 32) {
         float rv[Epilogue::kRowValues > 0 ? Epilogue::kRowValues : 1];
-        epi.row_values(m0 + r, rv);
+        ep.row_values(m0 + r, rv);
 #pragma unroll
         for (int i = 0; i < Epilogue::kRowValues; ++i) rowvals[i * kBM + r] = rv[i];
       }
@@ -410,7 +462,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       // iteration ago and have partly been evicted to HBM since): one prefetch per 128-byte line, 4 lines per column
       const int n_valid = min(BN, args.N - n0);
       if ((lane & 7) == 0)
-        for (int c = e; c < n_valid; c += kAuxWarps) epi.prefetch(m0 + 4 * lane, n0 + c);
+        for (int c = e; c < n_valid; c += kAuxWarps) ep.prefetch(m0 + 4 * lane, n0 + c);
     }
     if (!A_MN && !B_MN && args.tail_rows > 0) {
       // Rows past the last full 128-row tile (F = 513 = 4 x 128 + 1), float32 SIMT from the K-major planes: the m tiles of
@@ -425,8 +477,10 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       const int c_begin = n0 + (z_red ? tile_m * args.z_cluster + z : tile_m) * tcols;
       const int c_end = min(min(args.N, n0 + BN), c_begin + tcols);
       constexpr int kRound = 32 * kAuxWarps;             // columns per round: 16 steps of 2 columns per warp
+      const __nv_bfloat16* tail_a = reinterpret_cast<const __nv_bfloat16*>(reinterpret_cast<const char*>(args.A) + clip_offset(epi, clip));
+      const __nv_bfloat16* tail_b = reinterpret_cast<const __nv_bfloat16*>(reinterpret_cast<const char*>(args.B) + clip_offset(epi, clip));
       for (int m = args.m_tiles * kBM; m < args.M; ++m) {
-        const __nv_bfloat16* a_hi = args.A + (int64_t)m * args.lda;
+        const __nv_bfloat16* a_hi = tail_a + (int64_t)m * args.lda;
         const __nv_bfloat16* a_lo = a_hi + args.a_plane;
 #pragma unroll 1
         for (int c_round = c_begin; c_round < c_end; c_round += kRound) {
@@ -436,7 +490,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
             const int n = c_round + 2 * (e + i * kAuxWarps);
             if (n >= c_end) break;
             const bool two = n + 1 < c_end;
-            const __nv_bfloat16* b_hi = args.B + (int64_t)n * args.ldb;
+            const __nv_bfloat16* b_hi = tail_b + (int64_t)n * args.ldb;
             const __nv_bfloat16* b_lo = b_hi + args.b_plane;
             const int64_t next = two ? args.ldb : 0;
             float acc0 = 0.f, acc1 = 0.f;
@@ -454,7 +508,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
             if (lane == 2 * i + 1) keep = acc1;
           }
           const int n_mine = c_round + 2 * (e + (lane >> 1) * kAuxWarps) + (lane & 1);
-          if (n_mine < c_end) epi.elem(m, n_mine, keep, z_red ? 0 : z);
+          if (n_mine < c_end) ep.elem(m, n_mine, keep, z_red ? 0 : z);
         }
       }
     }
@@ -528,7 +582,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     constexpr int kWarps = kThreads / 32;
     const int m_first = m0 + 4 * lane;
     typename Epilogue::State st;
-    epi.init(st, m_first, rowvals + 4 * lane);
+    ep.init(st, m_first, rowvals + 4 * lane);
     int n_valid = min(BN, args.N - n0);
     constexpr int U = kColumnsInFlight;
     int c_first = warp;
@@ -545,7 +599,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
           const int cc = warp + kWarps * u;
           if (cc < n_valid) {
             const float4 acc = *reinterpret_cast<const float4*>(tile + (size_t)cc * kTileLd + 4 * lane);
-            epi.store(m_first, n0 + cc, acc, pre[u], z, st);
+            ep.store(m_first, n0 + cc, acc, pre[u], z, st);
           }
         }
         c_first = warp + kWarps * kPre;
@@ -559,7 +613,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         const int cc = c + kWarps * u;
         if (cc < n_valid) {
           if constexpr (OPERAND) loaded[u] = typename Epilogue::Loaded{*reinterpret_cast<const float4*>(operand + (size_t)cc * kBM + 4 * lane)};
-          else loaded[u] = epi.load(m_first, n0 + cc);
+          else loaded[u] = ep.load(m_first, n0 + cc);
         }
       }
       if (zc > 1) {
@@ -587,7 +641,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
 #pragma unroll
         for (int u = 0; u < U; ++u) {
           const int cc = c + kWarps * u;
-          if (cc < n_valid) epi.store(m_first, n0 + cc, sum[u], loaded[u], 0, st);
+          if (cc < n_valid) ep.store(m_first, n0 + cc, sum[u], loaded[u], 0, st);
         }
       } else {
 #pragma unroll
@@ -595,20 +649,20 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
           const int cc = c + kWarps * u;
           if (cc < n_valid) {
             const float4 acc = *reinterpret_cast<const float4*>(tile + (size_t)cc * kTileLd + 4 * lane);
-            epi.store(m_first, n0 + cc, acc, loaded[u], z, st);
+            ep.store(m_first, n0 + cc, acc, loaded[u], z, st);
           }
         }
       }
     }
     if constexpr (Epilogue::kRowReduce) {   // per-row sums over the tile's columns: 12 warp partials -> one value per row
-      red[warp * 32 + lane] = epi.row_partial(st);
+      red[warp * 32 + lane] = ep.row_partial(st);
       __syncthreads();
       if (tid < kBM) {
         const float* r = reinterpret_cast<const float*>(red);
         float sum = 0.f;
 #pragma unroll
         for (int w = 0; w < kWarps; ++w) sum += r[w * kBM + tid];
-        epi.row_total(m0 + tid, tile_n, sum);
+        ep.row_total(m0 + tid, tile_n, sum);
       }
     }
     if (args.timing && tid == 64) args.timing[cta_linear * 8 + 6] = clock64();

@@ -42,9 +42,10 @@ struct TmapKey {
   const void* base;
   uint64_t inner, rows, pitch_bytes, plane_bytes;
   uint32_t box_inner, box_rows, box_planes;
+  uint64_t clips, clip_bytes;     // clips > 0: a fourth, clip dimension (batched launches, tgemm::Clips)
   bool operator==(const TmapKey& o) const {
     return base == o.base && inner == o.inner && rows == o.rows && pitch_bytes == o.pitch_bytes && plane_bytes == o.plane_bytes &&
-           box_inner == o.box_inner && box_rows == o.box_rows && box_planes == o.box_planes;
+           box_inner == o.box_inner && box_rows == o.box_rows && box_planes == o.box_planes && clips == o.clips && clip_bytes == o.clip_bytes;
   }
 };
 
@@ -58,23 +59,24 @@ namespace tgemm_host {
 
 // Tensor map over a plane pair [2][rows][pitch] of bf16: dims (inner, rows, 2), box (box_inner, box_rows, box_planes).
 // box_inner * 2 bytes = 64 -> SWIZZLE_64B (K-major k-blocks of 32), 128 -> SWIZZLE_128B (MN-major atoms of 64).
+// clips > 0: `clips` such pairs clip_bytes apart, dims (inner, rows, 2, clips), box of one clip.
 inline int get_tmap(gccnmf_handle* h, const bf16* base, uint64_t inner, uint64_t rows, uint64_t pitch_elems, uint64_t plane_elems,
-             uint32_t box_inner, uint32_t box_rows, uint32_t box_planes, CUtensorMap* out) {
+             uint32_t box_inner, uint32_t box_rows, uint32_t box_planes, CUtensorMap* out, uint64_t clips = 0, uint64_t clip_bytes = 0) {
   if (!h->tmaps) h->tmaps = new gccnmf_tmap_cache();
-  const TmapKey key{base, inner, rows, pitch_elems * 2, plane_elems * 2, box_inner, box_rows, box_planes};
+  const TmapKey key{base, inner, rows, pitch_elems * 2, plane_elems * 2, box_inner, box_rows, box_planes, clips, clips ? clip_bytes : 0};
   for (auto& e : h->tmaps->entries)
     if (e.first == key) { *out = e.second; return 0; }
   EncodeTiledFn encode = encode_tiled_fn();
   if (!encode) return gccnmf_fail(h, GCCNMF_ERR_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
-  if ((reinterpret_cast<uintptr_t>(base) & 15) || (key.pitch_bytes & 15) || (key.plane_bytes & 15))
-    return gccnmf_fail(h, GCCNMF_ERR_INVALID_ARGUMENT, "tensor map: base / pitch / plane stride must be 16-byte aligned");
-  const cuuint64_t dims[3] = {inner, rows, 2};
-  const cuuint64_t strides[2] = {key.pitch_bytes, key.plane_bytes};
-  const cuuint32_t box[3] = {box_inner, box_rows, box_planes};
-  const cuuint32_t elem_strides[3] = {1, 1, 1};
+  if ((reinterpret_cast<uintptr_t>(base) & 15) || (key.pitch_bytes & 15) || (key.plane_bytes & 15) || (key.clip_bytes & 15))
+    return gccnmf_fail(h, GCCNMF_ERR_INVALID_ARGUMENT, "tensor map: base / pitch / plane / clip stride must be 16-byte aligned");
+  const cuuint64_t dims[4] = {inner, rows, 2, clips};
+  const cuuint64_t strides[3] = {key.pitch_bytes, key.plane_bytes, key.clip_bytes};
+  const cuuint32_t box[4] = {box_inner, box_rows, box_planes, 1};
+  const cuuint32_t elem_strides[4] = {1, 1, 1, 1};
   const CUtensorMapSwizzle swz = (box_inner * 2 == 128) ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   CUtensorMap m;
-  const CUresult r = encode(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<bf16*>(base), dims, strides, box, elem_strides,
+  const CUresult r = encode(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, clips ? 4 : 3, const_cast<bf16*>(base), dims, strides, box, elem_strides,
                             CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return gccnmf_fail(h, GCCNMF_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
   if (h->tmaps->entries.size() > 256) h->tmaps->entries.clear();
@@ -88,7 +90,7 @@ inline int get_tmap(gccnmf_handle* h, const bf16* base, uint64_t inner, uint64_t
 inline int tmap_f32_2d(gccnmf_handle* h, const float* base, uint64_t inner, uint64_t rows, uint64_t pitch_elems, uint32_t box_inner,
                        uint32_t box_rows, CUtensorMap* out) {
   if (!h->tmaps) h->tmaps = new gccnmf_tmap_cache();
-  const TmapKey key{base, inner, rows, pitch_elems * 4, 0, box_inner, box_rows, 0};     // (box_planes = 0: not a plane pair)
+  const TmapKey key{base, inner, rows, pitch_elems * 4, 0, box_inner, box_rows, 0, 0, 0};     // (box_planes = 0: not a plane pair)
   for (auto& e : h->tmaps->entries)
     if (e.first == key) { *out = e.second; return 0; }
   EncodeTiledFn encode = encode_tiled_fn();
@@ -111,12 +113,14 @@ inline int tmap_f32_2d(gccnmf_handle* h, const float* base, uint64_t inner, uint
 }
 
 // K-major operand: rows x kc, k contiguous; one box = one plane of a row slice (box_rows = tile rows / cluster extent).
-inline int tmap_kmajor(gccnmf_handle* h, const bf16* planes, int rows, int kc, int64_t pitch, int64_t plane, int box_rows, CUtensorMap* out) {
-  return get_tmap(h, planes, (uint64_t)kc, (uint64_t)rows, (uint64_t)pitch, (uint64_t)plane, kKB, (uint32_t)box_rows, 1, out);
+inline int tmap_kmajor(gccnmf_handle* h, const bf16* planes, int rows, int kc, int64_t pitch, int64_t plane, int box_rows, CUtensorMap* out,
+                       int clips = 0, int64_t clip_bytes = 0) {
+  return get_tmap(h, planes, (uint64_t)kc, (uint64_t)rows, (uint64_t)pitch, (uint64_t)plane, kKB, (uint32_t)box_rows, 1, out, clips, clip_bytes);
 }
 // MN-major operand: stored as kc rows x mn contiguous; one box = one 64-wide atom, both planes.
-inline int tmap_mnmajor(gccnmf_handle* h, const bf16* planes, int mn, int kc, int64_t pitch, int64_t plane, CUtensorMap* out) {
-  return get_tmap(h, planes, (uint64_t)mn, (uint64_t)kc, (uint64_t)pitch, (uint64_t)plane, 64, kKB, 2, out);
+inline int tmap_mnmajor(gccnmf_handle* h, const bf16* planes, int mn, int kc, int64_t pitch, int64_t plane, CUtensorMap* out,
+                        int clips = 0, int64_t clip_bytes = 0) {
+  return get_tmap(h, planes, (uint64_t)mn, (uint64_t)kc, (uint64_t)pitch, (uint64_t)plane, 64, kKB, 2, out, clips, clip_bytes);
 }
 
 // ------------------------------------------------------------------------------------------------ launch helper
@@ -223,6 +227,8 @@ struct GemmShape {
   int z_cluster;        // > 1: the k-splits of a tile form a (1, 1, splits) cluster and are summed through distributed shared memory
   unsigned* done_counter;          // completion signal of the launch to the ranks of a sharded run (see tgemm::PeerSignal)
   tgemm::PeerSignal signal;
+  int clips;                       // > 0: batched launch over `clips` clips clip_bytes apart (tgemm::Clips)
+  int64_t clip_bytes;
 };
 
 // One instantiation: kernel attributes + how many of its clusters can be resident at once (queried once).
@@ -289,10 +295,10 @@ struct PlaneGemmInstance {
     int unused;
     if (int st = max_clusters(h, &unused)) return st;     // (sets the shared-memory attribute on first use)
     CUtensorMap map_a, map_b;
-    if (int st = A_MN ? tmap_mnmajor(h, A.planes, g.M, g.Kc, A.pitch, A.plane, &map_a)
-                      : tmap_kmajor(h, A.planes, g.M, g.Kc, A.pitch, A.plane, tgemm::kBM / CN, &map_a)) return st;
-    if (int st = B_MN ? tmap_mnmajor(h, B.planes, g.N, g.Kc, B.pitch, B.plane, &map_b)
-                      : tmap_kmajor(h, B.planes, g.N, g.Kc, B.pitch, B.plane, BN / CM, &map_b)) return st;
+    if (int st = A_MN ? tmap_mnmajor(h, A.planes, g.M, g.Kc, A.pitch, A.plane, &map_a, g.clips, g.clip_bytes)
+                      : tmap_kmajor(h, A.planes, g.M, g.Kc, A.pitch, A.plane, tgemm::kBM / CN, &map_a, g.clips, g.clip_bytes)) return st;
+    if (int st = B_MN ? tmap_mnmajor(h, B.planes, g.N, g.Kc, B.pitch, B.plane, &map_b, g.clips, g.clip_bytes)
+                      : tmap_kmajor(h, B.planes, g.N, g.Kc, B.pitch, B.plane, BN / CM, &map_b, g.clips, g.clip_bytes)) return st;
     Epi e = epi;
     if constexpr (C::kOperandBytes > 0)
       if (int st = tmap_f32_2d(h, e.operand(), (uint64_t)e.operand_ld(), (uint64_t)e.operand_cols(), (uint64_t)e.operand_ld(), tgemm::kBM, BN,
@@ -313,7 +319,8 @@ struct PlaneGemmInstance {
     args.z_cluster = (CN * CM == 1 && g.z_cluster > 1) ? g.z_cluster : 0;
     args.done_counter = g.done_counter;
     args.signal = g.signal;
-    const dim3 grid = mf ? dim3(g.m_tiles, g.n_tiles, g.splits) : dim3(g.n_tiles, g.m_tiles, g.splits);
+    const int zs = g.splits * std::max(1, g.clips);     // (batched: blockIdx.z = clip * splits + split)
+    const dim3 grid = mf ? dim3(g.m_tiles, g.n_tiles, zs) : dim3(g.n_tiles, g.m_tiles, zs);
     if (!timing && h->debug_timing) {   // diagnostics: every plane GEMM of the KL-NMF loop appends its CTA stamps (8 per CTA)
       args.timing = h->debug_timing + h->debug_timing_cursor;
       h->debug_timing_cursor += (size_t)grid.x * grid.y * grid.z * 8;
@@ -388,6 +395,42 @@ int plane_gemm(gccnmf_handle* h, int bn, const Operand& A, const Operand& B, int
     case 256: return launch_plane_gemm<256, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, timing, stream, m_fastest, prefer_pair);
   }
   return gccnmf_fail(h, GCCNMF_ERR_UNSUPPORTED, "plane gemm: tile width %d (supported: 104, 112, 120, 128, 176, 208, 240, 256)", bn);
+}
+
+// Batched launch (tgemm::Clips) over `clips` clips of one shape, 1 x 1 clusters, k-splits as slabs: the tile plan, tail rows and
+// k-split ranges of every clip are those of launch_plane_gemm on that clip alone.
+template <int BN, bool A_MN, bool B_MN, class Epi>
+int launch_plane_gemm_clips(gccnmf_handle* h, const Operand& A, const Operand& B, int M, int N, int Kc, int splits, bool simt_tail,
+                            const tgemm::Clips<Epi>& epi, int clips, void* stream) {
+  GemmShape g{};
+  g.M = M; g.N = N; g.Kc = Kc; g.splits = splits;
+  const int tail = M % tgemm::kBM;
+  const bool use_tail = simt_tail && !A_MN && !B_MN && tail != 0 && tail <= kTailRowsMax && M > tgemm::kBM && (M / tgemm::kBM) * 128 >= BN;
+  g.m_tiles = use_tail ? M / tgemm::kBM : (M + tgemm::kBM - 1) / tgemm::kBM;
+  g.tail_rows = use_tail ? tail : 0;
+  g.n_tiles = (N + BN - 1) / BN;
+  g.clips = clips;
+  g.clip_bytes = epi.clip_bytes;
+  return PlaneGemmInstance<BN, A_MN, B_MN, 1, 1, tgemm::Clips<Epi>>::launch(h, A, B, g, epi, nullptr, stream);
+}
+template <bool A_MN, bool B_MN, class Epi>
+int plane_gemm_clips(gccnmf_handle* h, int bn, const Operand& A, const Operand& B, int M, int N, int Kc, int splits, bool simt_tail,
+                     const tgemm::Clips<Epi>& epi, int clips, void* stream) {
+  switch (bn) {
+    case 104:
+      if constexpr (tgemm::wants_dual_n<Epi>::value && !B_MN) return launch_plane_gemm_clips<104, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, clips, stream);
+      break;
+    case 120:
+      if constexpr (tgemm::wants_dual_n<Epi>::value && !B_MN) return launch_plane_gemm_clips<120, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, clips, stream);
+      break;
+    case 112: return launch_plane_gemm_clips<112, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, clips, stream);
+    case 128: return launch_plane_gemm_clips<128, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, clips, stream);
+    case 176: return launch_plane_gemm_clips<176, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, clips, stream);
+    case 208: return launch_plane_gemm_clips<208, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, clips, stream);
+    case 240: return launch_plane_gemm_clips<240, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, clips, stream);
+    case 256: return launch_plane_gemm_clips<256, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, clips, stream);
+  }
+  return gccnmf_fail(h, GCCNMF_ERR_UNSUPPORTED, "plane gemm (batched): tile width %d", bn);
 }
 
 // k-splits reduced inside (1, 1, splits) clusters (no slabs): query how many such clusters are resident at once / launch.

@@ -88,6 +88,21 @@ def performKLNMF(V, dictionarySize, numIterations, sparsityAlpha, epsilon=1e-16,
     return W.cpu().numpy(), H.cpu().numpy()
 
 
+def performKLNMFBatch(Vs, dictionarySize, numIterations, sparsityAlpha, epsilon=1e-16, seedValue=0):
+    """performKLNMF on B equal-shape clips in one batched call: Vs (B, F, T2) -> W (B, F, K), H (B, K, T2), clip b equal to
+    performKLNMF(Vs[b], ...).  The reference re-seeds on every call, so every clip starts from the same draw: drawn once here."""
+    Vs = np.asarray(Vs)
+    if Vs.ndim != 3:
+        raise ParameterError('performKLNMFBatch: Vs must be (B, F, T2), got shape %s' % (Vs.shape,))
+    B, F, T2 = Vs.shape
+    W0, H0 = _seededInit(F, T2, dictionarySize, epsilon, seedValue)
+    h = default_handle()
+    W = h.to_device(np.ascontiguousarray(np.broadcast_to(W0, (B,) + W0.shape)))
+    H = h.to_device(np.ascontiguousarray(np.broadcast_to(H0, (B,) + H0.shape)))
+    h.klnmf_batched(h.to_device(np.ascontiguousarray(Vs, dtype=np.float32)), W, H, numIterations, sparsityAlpha, epsilon, update_W=True)
+    return W.cpu().numpy(), H.cpu().numpy()
+
+
 def inferCoefficientsKLNMF(V, W, numIterations, sparsityAlpha, epsilon=1e-16, seedValue=0):
     """The function the notebooks call but the reference never defines
     (onlineSpeechEnhancement.ipynb:433): H-only KL updates (:76) with a fixed dictionary from the

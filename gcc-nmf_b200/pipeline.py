@@ -73,8 +73,12 @@ class GCCNMFPipeline(object):
             self.stage_events.append((name, ev))
 
     def stage_times_ms(self):
+        """Device time per stage in ms (a batch flow runs the per-clip stages once per clip: their times are summed)."""
         ev = self.stage_events
-        return {ev[i + 1][0]: ev[i][1].elapsed_time(ev[i + 1][1]) for i in range(len(ev) - 1)}
+        times = {}
+        for i in range(len(ev) - 1):
+            times[ev[i + 1][0]] = times.get(ev[i + 1][0], 0.0) + ev[i][1].elapsed_time(ev[i + 1][1])
+        return times
 
     # ------------------------------------------------------------------ shared front half
     def _front(self, samples):
@@ -101,14 +105,54 @@ class GCCNMFPipeline(object):
         return dict(X=X, V=V, coherence=coh, angularSpectrogram=ang, meanAngularSpectrum=mean, W=W, H=H,
                     _mean_host=mean_host, _mean_ready=mean_ready)
 
-    def _back(self, r, masks):
+    def _front_batch(self, samples):
+        """_front for B clips (B, 2, n): the STFT of each clip into one (2B, F, T) spectrogram and one (B, F, 2T) V stack (the
+        STFT entry takes one stereo pair per call), the angular spectrum per clip with one event for all B means, one batched
+        KL-NMF over the stack.  Returns one _front dict per clip (views of batch buffers)."""
+        h, torch = self.h, self.torch
+        B, C, n = samples.shape
+        if C != 2:
+            raise ValueError('samples must be (B, 2, n), got %s' % (tuple(samples.shape),))
+        self._mark('start')
+        key = self._token
+        F, T = self.F, self.num_frames(n)
+        X = h.buffer((key, 'batch', 'X'), (2 * B, F, T), torch.complex64)
+        Vs = h.buffer((key, 'batch', 'V'), (B, F, 2 * T), torch.float32)
+        for b in range(B):
+            h.stft(samples[b], self.window, self.N, self.hop, conjugate=True, want_V=True, out=(X[2 * b:2 * b + 2], Vs[b]))
+        self._mark('stft')
+        means_host = getattr(self, '_means_host', None)
+        if means_host is None or means_host.shape[0] != B:
+            means_host = self._means_host = torch.empty((B, self.D), dtype=torch.float64, pin_memory=True)
+        rs = []
+        for b in range(B):
+            Xb = X[2 * b:2 * b + 2]
+            coh, ang, mean = h.phat_angspec(Xb, self.E, out_key=(key, 'clip', b))
+            means_host[b].copy_(mean, non_blocking=True)
+            rs.append(dict(X=Xb, coherence=coh, angularSpectrogram=ang, meanAngularSpectrum=mean, _mean_host=means_host[b]))
+        means_ready = torch.cuda.Event()
+        means_ready.record()
+        self._mark('angular')
+        W0, H0 = self.nmf_init(2 * T)
+        W = h.buffer((key, 'batch', 'W'), (B,) + tuple(W0.shape), W0.dtype)
+        H = h.buffer((key, 'batch', 'H'), (B,) + tuple(H0.shape), H0.dtype)
+        W.copy_(W0.expand_as(W))
+        H.copy_(H0.expand_as(H))
+        h.klnmf_batched(Vs, W, H, self.I, self.alpha, self.eps, update_W=True)
+        self._mark('nmf')
+        for b, r in enumerate(rs):
+            r.update(V=Vs[b], W=W[b], H=H[b], _mean_ready=means_ready)
+        return rs
+
+    def _back(self, r, masks, key=None):
         h = self.h
+        key = self._token if key is None else key
         S = masks.shape[0]
-        est = h.masked_recon_phase(masks, r['X'], r['W'], r['H'], out_key=self._token)
+        est = h.masked_recon_phase(masks, r['X'], r['W'], r['H'], out_key=key)
         self._mark('recon')
         F, T = est.shape[2:]
         y = h.istft_ola(est.reshape(S * 2, F, T), self.synthesisWindow, self.N, self.hop,
-                        gain=np.float32(self.hop / float(self.N) * 2), center=True, conjugate=True, out_key=self._token)
+                        gain=np.float32(self.hop / float(self.N) * 2), center=True, conjugate=True, out_key=key)
         self._mark('istft')
         r['targetCoefficientMasks'] = masks
         r['targetSpectrogramEstimates'] = est
@@ -125,10 +169,12 @@ class GCCNMFPipeline(object):
     # ------------------------------------------------------------------ flows
     def enhance(self, samples, collect_stage_times=False):
         """samples (2, n) f32 cuda -> dict of device tensors (enhancement flow, one target)."""
-        h = self.h
         self.stage_events = [] if collect_stage_times else None
-        r = self._front(samples)
-        argmax, refined = h.tdoa_argmax(r['coherence'], self.E, r['W'], out_key=self._token)
+        return self._enhance_back(self._front(samples), self._token)
+
+    def _enhance_back(self, r, key):
+        h = self.h
+        argmax, refined = h.tdoa_argmax(r['coherence'], self.E, r['W'], out_key=key)
         self._mark('gccnmf')
         target = self._pick_targets(r, 1)[0]
         r['refinedDecisions'] = int(refined.item())
@@ -136,16 +182,18 @@ class GCCNMFPipeline(object):
             _, argmax = h.tdoa_gccnmf(r['coherence'], self.E, r['W'], want_values=False, want_argmax=True)   # exact float64 kernel
         window = (self.hypothesisTDOAs[-1] - self.hypothesisTDOAs[0]) * self.windowPercent
         lut = fn.getTargetTDOALookup(self.hypothesisTDOAs, target, window)
-        mask = h.argmax_mask(argmax, h.to_device(lut.astype(np.uint8)), out_key=self._token)
+        mask = h.argmax_mask(argmax, h.to_device(lut.astype(np.uint8)), out_key=key)
         self._mark('mask')
         r['argMaxGCCNMF'] = argmax
-        return self._back(r, mask[None])
+        return self._back(r, mask[None], key)
 
     def separate(self, samples, numTargets, collect_stage_times=False):
         """samples (2, n) f32 cuda -> dict of device tensors (runGCCNMF.py flow, numTargets sources)."""
-        h = self.h
         self.stage_events = [] if collect_stage_times else None
-        r = self._front(samples)
+        return self._separate_back(self._front(samples), numTargets, self._token)
+
+    def _separate_back(self, r, numTargets, key):
+        h = self.h
         idx = self._pick_targets(r, numTargets)
         E_sel = h.to_device(np.ascontiguousarray(self.E_host[:, idx]))
         values, _ = h.tdoa_gccnmf(r['coherence'], E_sel, r['W'], want_values=True, want_argmax=False)
@@ -154,7 +202,25 @@ class GCCNMFPipeline(object):
         self._mark('mask')
         r['targetTDOAGCCNMFs'] = values
         r['_all_nan_flag'] = flag
-        return self._back(r, masks)
+        return self._back(r, masks, key)
+
+    # ------------------------------------------------------------------ batches of equal-length clips
+    def enhance_batch(self, samples, collect_stage_times=False):
+        """samples (B, 2, n) f32 cuda -> list of B dicts, clip b's bit-identical to enhance(samples[b]).  The STFT and the
+        KL-NMF run once for the whole batch; the later stages run per clip.  Valid until the next batch call."""
+        self.stage_events = [] if collect_stage_times else None
+        rs = self._front_batch(samples)
+        if rs:
+            rs[0]['_mean_ready'].synchronize()          # one host wait for all B means before peak picking
+        return [self._enhance_back(r, (self._token, 'clip', b)) for b, r in enumerate(rs)]
+
+    def separate_batch(self, samples, numTargets, collect_stage_times=False):
+        """samples (B, 2, n) f32 cuda -> list of B dicts, clip b's bit-identical to separate(samples[b], numTargets)."""
+        self.stage_events = [] if collect_stage_times else None
+        rs = self._front_batch(samples)
+        if rs:
+            rs[0]['_mean_ready'].synchronize()
+        return [self._separate_back(r, numTargets, (self._token, 'clip', b)) for b, r in enumerate(rs)]
 
     # ------------------------------------------------------------------ the whole flow as ONE C-ABI call
     def run_fused(self, samples, numTargets=0):

@@ -123,6 +123,18 @@ GCCNMF_API int gccnmf_klnmf(gccnmf_handle* h, const float* V, int F, int T2, flo
                  int iterations, float sparsity_alpha, float epsilon, int update_W,
                  void* workspace, size_t workspace_bytes, void* stream);
 /*
+ * B clips of one shape (F, T2, K) in one call: clip b's W and H come out bit for bit as gccnmf_klnmf on that clip alone would
+ * leave them (same handle, same options).  Clip b's V is read in place at V + b * clip_stride_v with row pitch ld_v (>= T2):
+ * a contiguous (B, F, T2) stack is ld_v = T2, clip_stride_v = F * T2; clips side by side in the columns of one (F, B T2) matrix
+ * are ld_v = B T2, clip_stride_v = T2.  W (B, F, K) and H (B, K, T2) are contiguous clip-major stacks holding the
+ * initial values on entry and the results on return.  On the tensor-core path every launch of an iteration covers all clips; the
+ * workspace grows linearly in B (B x gccnmf_klnmf_workspace_bytes at tensor-core shapes).  B is 1 .. 8191.
+ */
+GCCNMF_API size_t gccnmf_klnmf_batched_workspace_bytes(int B, int F, int T2, int K);
+GCCNMF_API int gccnmf_klnmf_batched(gccnmf_handle* h, const float* V, int64_t ld_v, int64_t clip_stride_v, int B, int F, int T2,
+                         float* W, float* H, int K, int iterations, float sparsity_alpha, float epsilon, int update_W,
+                         void* workspace, size_t workspace_bytes, void* stream);
+/*
  * Frame-sharded dictionary learning (multi-GPU; SURVEY.md section 8e).  A rank holds the columns V_s
  * (F, T2s), H_s (K, T2s) of its frames and a replica of W.  The loop of gccNMFFunctions.py:75-81 becomes
  *
