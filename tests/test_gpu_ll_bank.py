@@ -126,13 +126,14 @@ def test_one_entry_is_the_plain_engine(synthesis, inference, P, Lh):
 
 
 # ---------------------------------------------------------------------------------------------- 2. spread spacings
-SPREAD = [(1, True, None, 0, 0), (3, True, None, 0, 0), (3, False, [1, 3, 2], 0, 0), (1, False, None, 4, 0), (3, True, [2, 1], 4, 64),
-          (1, True, None, 0, 64)]
+# D 32 and 128: the tensor-core argmax over bank-built planes and its refinement over each column's table
+SPREAD = [(1, True, None, 0, 0, 16), (3, True, None, 0, 0, 16), (3, False, [1, 3, 2], 0, 0, 16), (1, False, None, 4, 0, 16),
+          (3, True, [2, 1], 4, 64, 16), (1, True, None, 0, 64, 16), (3, True, [2, 1], 0, 0, 32), (1, False, None, 0, 0, 128)]
 
 
-@pytest.mark.parametrize('C,graph,schedule,P,Lh', SPREAD, ids=['-'.join(map(str, c)) for c in SPREAD])
-def test_spread_entries_equal_plain_engines(C, graph, schedule, P, Lh):
-    p = _setup()
+@pytest.mark.parametrize('C,graph,schedule,P,Lh,D', SPREAD, ids=['-'.join(map(str, c[:5])) + ('-D%d' % c[5] if c[5] != 16 else '') for c in SPREAD])
+def test_spread_entries_equal_plain_engines(C, graph, schedule, P, Lh, D):
+    p = _setup(D=D)
     S, hops = 37, 40
     x = _audio(S, hops, p['hop'])
     entries = np.random.RandomState(5).permutation(np.arange(S) % 8)

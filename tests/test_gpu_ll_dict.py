@@ -2,7 +2,7 @@
 stream on dictionary i and table j against a plain engine built with (W_i, E_j): outputs, the per-column export items on the stream's
 columns and rows < K_i, and the fill of the rows past K_i.
   - a one-entry bank against llhist and llbank engines, every synthesis mode, inference 0 and 5, P 0, 2 and 4, Lh 0 and 64;
-  - K_i in {24, 64, 100, 128, 256} plus a second K = 100 content, unsorted over 37 streams and 3 tables, D = 16 (SIMT), 32 and 128
+  - K_i in {24, 64, 100, 128, 256} plus a second K = 100 content, unsorted over 37 streams and 3 tables, D = 16 (SIMT), 32, 64 and 128
     (grouped tensor-core GEMM), hops per call 1 and 3, mixed schedules, graph and kernel-by-kernel runs of the same case.  K_i = 24
     and 100 make the plain engine take the float64 argmax while the bank takes the tensor path with refinement;
   - 1056 streams over 64 dictionaries and 4 tables;
@@ -150,7 +150,7 @@ def test_one_entry_bank_is_the_plain_engine(synthesis, inference, P, Lh):
         e.close()
 
 
-MIXED = [(D, P, inf, Lh, C) for D in (16, 32, 128) for (P, inf, Lh, C) in ((0, 0, 0, 1), (0, 5, 64, 3), (2, 0, 0, 3), (2, 5, 64, 1))]
+MIXED = [(D, P, inf, Lh, C) for D in (16, 32, 64, 128) for (P, inf, Lh, C) in ((0, 0, 0, 1), (0, 5, 64, 3), (2, 0, 0, 3), (2, 5, 64, 1))]
 
 
 @pytest.mark.parametrize('D,P,inference,Lh,C', MIXED, ids=['-'.join(map(str, c)) for c in MIXED])
