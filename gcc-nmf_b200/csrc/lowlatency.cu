@@ -37,6 +37,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "records.cuh"
 
 int gccnmf_stft_segments(gccnmf_handle* h, const float* samples, int64_t sample_stride, int channels, int segments, int frames_per_seg,
                          int64_t seg_stride, const double* window, int n_fft, int hop, int conjugate, float* X, float* V, void* stream);
@@ -1151,76 +1152,51 @@ int ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int 
 //   src_targets[s], src_override[s], src_status[s]    (sources only)                                (ll_src_targets_kernel)
 //   hist[s]           history only: the ring, its write index, the window and 8 zero bytes          (ll_hist_means, set_window)
 // Everything else is either shared by the streams (header, windows, E, W and what init derives from it) or rewritten by every call
-// before it is read (stage, valid, X ... frames, counters).  A region is a strided array in the state: stream s's bytes are
-// [offset + s stride, + bytes), and they go to [rec_offset, + bytes) of the stream's record payload.  Rings are copied whole: their
+// before it is read (stage, valid, X ... frames, counters).  A region is an array of per-stream blocks in the state (RecordMapBuilder
+// with stride 0), and the payload's padding after each region is zero.  Rings are copied whole: their
 // positions derive from hops, which travels with them.
-struct RecordRegion { size_t offset, stride, rec_offset, bytes; };
-constexpr int kRecordMaxRegions = 8;
-struct RecordMap {
-  RecordRegion r[kRecordMaxRegions];
-  int n;
-  size_t payload;                        // payload bytes of one stream (16-aligned): the staging stride
-};
 constexpr size_t kRecordHeaderBytes = GCCNMF_RECORD_HEADER_BYTES;
-static_assert(sizeof(gccnmf_record_header) <= kRecordHeaderBytes, "record header");
+static_assert(sizeof(gccnmf_llbank_record_header) <= kRecordHeaderBytes, "record header");
+static_assert(offsetof(gccnmf_llbank_record_header, config) == offsetof(gccnmf_record_header, config), "shared prefix");
 
 // A bank (Qe >= 1) moves the regions' offsets in the state (E holds Qe tables), not the payload.
 RecordMap ll_record_map(const gccnmf_ll_config& c, int P, int Lh = 0, int Qe = 0) {
   char* const base = reinterpret_cast<char*>(256);
   const LLLayout l = ll_carve(c, P, base, Lh, Qe);
   const size_t N = l.N, R = l.R, D = l.D, Pm = P > 0 ? P : 1;
-  RecordMap m{};
-  size_t at = 0;
-  auto add = [&](const void* p, size_t bytes) {
-    if (bytes == 0) return;              // R = 0 when hop = N
-    m.r[m.n++] = RecordRegion{(size_t)((const char*)p - base), bytes, at, bytes};
-    at = align_up(at + bytes, 16);
-  };
-  add(l.streams, sizeof(LLStream));
-  add(l.carry, D * sizeof(double));
-  add(l.in_ring, 2 * R * sizeof(float));
-  add(l.out_ring, Pm * 2 * N * sizeof(float));
+  RecordMapBuilder b{base, 0};
+  b.add(l.streams, sizeof(LLStream));
+  b.add(l.carry, D * sizeof(double));
+  b.add(l.in_ring, 2 * R * sizeof(float));  // nothing when hop = N (R = 0)
+  b.add(l.out_ring, Pm * 2 * N * sizeof(float));
   if (P) {
-    add(l.src_targets, kLLMaxSources * sizeof(int32_t));
-    add(l.src_override, kLLMaxSources * sizeof(int32_t));
-    add(l.src_status, sizeof(int32_t));
+    b.add(l.src_targets, kLLMaxSources * sizeof(int32_t));
+    b.add(l.src_override, kLLMaxSources * sizeof(int32_t));
+    b.add(l.src_status, sizeof(int32_t));
   }
-  add(l.hist, l.hist_stride);            // nothing with Lh = 0: the records of gccnmf_llrec_*
-  m.payload = at;
-  return m;
+  b.add(l.hist, l.hist_stride);            // nothing with Lh = 0: the records of gccnmf_llrec_*
+  return b.m;
 }
 
 size_t ll_record_bytes(const gccnmf_ll_config& c, int P, int Lh = 0) {
   return kRecordHeaderBytes + align_up(ll_record_map(c, P, Lh).payload, 256);
 }
 
-// Grid (count, regions): CTA (i, g) copies region g of stream first + i between the state and payload i of the staging buffer,
-// in 16-byte words where both ends and the length allow it (every carve region is 256-aligned; LLStream and odd ring lengths
-// are not), else in 4-byte words (every region is a whole number of them).
+// Grid (count, regions): CTA (i, g) copies region g of stream first + i between the state and payload i of the staging buffer.
 __global__ void __launch_bounds__(256)
 ll_record_copy_kernel(char* __restrict__ state, int first, RecordMap m, char* __restrict__ staging, int to_staging) {
-  const RecordRegion g = m.r[blockIdx.y];
-  char* slot = state + g.offset + (size_t)(first + blockIdx.x) * g.stride;
-  char* rec = staging + (size_t)blockIdx.x * m.payload + g.rec_offset;
-  const char* src = to_staging ? slot : rec;
-  char* dst = to_staging ? rec : slot;
-  if ((((uintptr_t)src | (uintptr_t)dst | g.bytes) & 15) == 0) {
-    for (size_t i = threadIdx.x; i < g.bytes / 16; i += blockDim.x)
-      reinterpret_cast<uint4*>(dst)[i] = reinterpret_cast<const uint4*>(src)[i];
-  } else {
-    for (size_t i = threadIdx.x; i < g.bytes / 4; i += blockDim.x)
-      reinterpret_cast<uint32_t*>(dst)[i] = reinterpret_cast<const uint32_t*>(src)[i];
-  }
+  record_copy_region(state, first + blockIdx.x, m.r[blockIdx.y], staging + (size_t)blockIdx.x * m.payload, to_staging);
 }
 
 // What a record must agree on, from the host arguments alone: magic, ABI version, kind, P, payload size and the configuration without
 // S and C, followed by the history length (0 without history, so those records are gccnmf_llrec_*'s).  The synthesis digest is left
 // 0: see ll_synthesis_digest.
 constexpr int kRecordConfigHistory = sizeof(gccnmf_ll_config) / sizeof(int32_t);    // config[9]
-// With a bank (Qe >= 1) the kind is GCCNMF_RECORD_KIND_LLBANK and a gccnmf_llbank_record_header follows the same fields with the
-// content digests of the dictionary and of the stream's steering table.
-gccnmf_record_header ll_record_header(const gccnmf_ll_config& cfg, int P, int Lh = 0, int Qe = 0) {
-  gccnmf_record_header r{};
+constexpr int kConfigAtoms = offsetof(gccnmf_ll_config, num_atoms) / sizeof(int32_t);
+// With a bank (Qe >= 1) the kind is GCCNMF_RECORD_KIND_LLBANK, and the content digests of the dictionary and of the stream's
+// steering table follow the same fields (gccnmf_llbank_record_header; 0 without a bank).
+gccnmf_llbank_record_header ll_record_header(const gccnmf_ll_config& cfg, int P, int Lh = 0, int Qe = 0) {
+  gccnmf_llbank_record_header r{};
   r.magic = GCCNMF_RECORD_MAGIC;
   r.abi_version = GCCNMF_ABI_VERSION;
   r.kind = Qe ? GCCNMF_RECORD_KIND_LLBANK : GCCNMF_RECORD_KIND_LL;
@@ -1252,187 +1228,165 @@ int ll_synthesis_digest(gccnmf_handle* h, const LLLayout& l, uint64_t* digest, v
   return GCCNMF_OK;
 }
 
-// ---- bank records: content digests (GCCNMF_RTREC_DIGEST_*, the real-time records' function, restated) of item 0, the dictionary
-// (W (F, K) f32 then, with inference, H0 (K, 2) f32), and items 1 .. Qe, the steering tables as stored ((F, D) complex128).  The
-// workspace holds the records' payloads, then one chunk digest per 1024-word chunk of each item, then the 1 + Qe item digests.
-static_assert(offsetof(gccnmf_llbank_record_header, config) == offsetof(gccnmf_record_header, config), "shared prefix");
-static_assert(sizeof(gccnmf_llbank_record_header) <= kRecordHeaderBytes, "record header");
-constexpr int kDigestChunk = GCCNMF_RTREC_DIGEST_CHUNK_WORDS;
-struct LLDigestItems {
-  const uint32_t *W, *H0, *E;
-  size_t nw, nh, ne;                       // words of W, of H0 (0 without inference) and of one table
-  int Qe, cd, ce;                          // chunks of the dictionary and of one table
+// ---- bank records (Qe >= 1): the content digests of the dictionaries and the steering tables.  A steering bank's state is one
+// dictionary, l.W and l.H0 with the config's K; a dictionary bank's dictionary e is dW and dH0 of entry e with K_e atoms.  The
+// workspace holds the records' payloads, then chunk slots for one dictionary of K_max atoms and for each table, then the digests:
+// [0] dictionary 0, [1 .. Qe] the tables, [Qe + e] dictionary e >= 1.  Each dictionary's digest is the llbank digest of an engine
+// built with it.
+struct LLRecordWork {
+  int cd, ce;                            // chunk slots of a dictionary and of a table
+  size_t chunks, digests, bytes;
 };
-
-LLDigestItems ll_digest_items(const LLLayout& l, bool inf) {
-  LLDigestItems d;
-  d.W = reinterpret_cast<const uint32_t*>(l.W);
-  d.H0 = reinterpret_cast<const uint32_t*>(l.H0);
-  d.E = reinterpret_cast<const uint32_t*>(l.E);
-  d.nw = (size_t)l.F * l.K;
-  d.nh = inf ? (size_t)2 * l.K : 0;
-  d.ne = (size_t)4 * l.F * l.D;
-  d.Qe = l.Qe;
-  d.cd = (int)((d.nw + d.nh + kDigestChunk - 1) / kDigestChunk);
-  d.ce = (int)((d.ne + kDigestChunk - 1) / kDigestChunk);
-  return d;
+LLRecordWork ll_record_work(const gccnmf_ll_config& c, int P, int Lh, int Qe, int Qd, int count) {
+  LLRecordWork w{};
+  w.bytes = (size_t)count * ll_record_map(c, P, Lh).payload;
+  if (!Qe) return w;
+  const size_t F = c.window_size / 2 + 1, K = c.num_atoms;
+  w.cd = digest_chunks(F * K + (c.inference_iterations > 0 ? 2 * K : 0));
+  w.ce = digest_chunks(4 * F * c.num_tdoas);
+  w.chunks = align_up(w.bytes, 256);
+  w.digests = w.chunks + align_up((size_t)(w.cd + Qe * w.ce) * sizeof(uint64_t), 256);
+  w.bytes = w.digests + (size_t)((Qd ? Qd : 1) + Qe) * sizeof(uint64_t);
+  return w;
 }
 
-// The workspace of `count` records: payloads, then (bank only) chunk digests and item digests, each 256-aligned.
-size_t ll_record_workspace_bytes(const gccnmf_ll_config& c, int P, int Lh, int Qe, int count) {
-  const size_t payloads = (size_t)count * ll_record_map(c, P, Lh).payload;
-  if (!Qe) return payloads;
-  const LLDigestItems d = ll_digest_items(ll_carve(c, P, nullptr, Lh, Qe), c.inference_iterations > 0);
-  return align_up(payloads, 256) + align_up((size_t)(d.cd + Qe * d.ce) * sizeof(uint64_t), 256) + (size_t)(1 + Qe) * sizeof(uint64_t);
-}
-
-__device__ __forceinline__ uint64_t ll_fnv(uint64_t h, uint32_t w) { return (h ^ w) * GCCNMF_RTREC_DIGEST_PRIME; }
-
-__device__ __forceinline__ void ll_digest_item(const LLDigestItems& d, int item, const uint32_t*& a, size_t& na, const uint32_t*& b, size_t& nb) {
-  if (item == 0) {
-    a = d.W; na = d.nw; b = d.H0; nb = d.nh;
-  } else {
-    a = d.E + (size_t)(item - 1) * d.ne; na = d.ne; b = nullptr; nb = 0;
-  }
-}
-
-// One thread per chunk: FNV-1a 64 over the chunk's words.
-__global__ void __launch_bounds__(128) ll_digest_chunks_kernel(LLDigestItems d, uint64_t* __restrict__ chunks) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= d.cd + d.Qe * d.ce) return;
-  const int item = t < d.cd ? 0 : 1 + (t - d.cd) / d.ce, j = t < d.cd ? t : (t - d.cd) % d.ce;
-  const uint32_t *a, *b;
-  size_t na, nb;
-  ll_digest_item(d, item, a, na, b, nb);
-  const size_t n = na + nb, w0 = (size_t)j * kDigestChunk, w1 = w0 + kDigestChunk < n ? w0 + kDigestChunk : n;
-  uint64_t h = GCCNMF_RTREC_DIGEST_BASIS;
-  for (size_t w = w0; w < (w1 < na ? w1 : na); ++w) h = ll_fnv(h, __ldg(a + w));
-  for (size_t w = w0 > na ? w0 : na; w < w1; ++w) h = ll_fnv(h, __ldg(b + (w - na)));
-  chunks[t] = h;
-}
-
-// One thread per item: FNV-1a 64 over (n_lo, n_hi, c_0 lo, c_0 hi, ...).
-__global__ void __launch_bounds__(128) ll_digest_fold_kernel(LLDigestItems d, const uint64_t* __restrict__ chunks, uint64_t* __restrict__ digest) {
-  const int item = blockIdx.x * blockDim.x + threadIdx.x;
-  if (item > d.Qe) return;
-  const size_t n = item == 0 ? d.nw + d.nh : d.ne;
-  const int c0 = item == 0 ? 0 : d.cd + (item - 1) * d.ce, nc = item == 0 ? d.cd : d.ce;
-  uint64_t h = ll_fnv(ll_fnv(GCCNMF_RTREC_DIGEST_BASIS, (uint32_t)n), (uint32_t)(n >> 32));
-  for (int j = 0; j < nc; ++j) {
-    const uint64_t c = chunks[c0 + j];
-    h = ll_fnv(ll_fnv(h, (uint32_t)c), (uint32_t)(c >> 32));
-  }
-  digest[item] = h;
-}
-
-// The dictionary digest and the Qe table digests of this state (digest[0], digest[1 ..]) into the workspace and back to the host, with
-// the entries of streams [first, first + count) when `entries` is not NULL: one wait on the stream.
-int ll_bank_digests(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l, int count, char* workspace, int first, uint64_t* digest,
-                    int32_t* entries, void* stream) {
-  const LLDigestItems d = ll_digest_items(l, cfg->inference_iterations > 0);
-  uint64_t* chunks = reinterpret_cast<uint64_t*>(workspace + align_up((size_t)count * ll_record_map(*cfg, l.P, l.Lh).payload, 256));
-  uint64_t* dev = chunks + align_up((size_t)(d.cd + l.Qe * d.ce) * sizeof(uint64_t), 256) / sizeof(uint64_t);
-  const int chunk_count = d.cd + l.Qe * d.ce;
-  GCCNMF_LAUNCH(h, ll_digest_chunks_kernel, (chunk_count + 127) / 128, 128, 0, stream, d, chunks);
-  GCCNMF_LAUNCH(h, ll_digest_fold_kernel, (l.Qe + 1 + 127) / 128, 128, 0, stream, d, chunks, dev);
+// The digests of this state's dictionaries and tables, with their K (dict_digest, K_host: max(Qd, 1); steer_digest: Qe), and when
+// the entry arrays are not NULL the entries of streams [first, first + count), back to the host.  One launch pair per dictionary,
+// the tables with the first, and one wait, after another for the K_e table of a dictionary bank.
+int ll_record_digests(gccnmf_handle* h, const gccnmf_ll_config& c, const LLLayout& l, const LLRecordWork& w, char* workspace, int first, int count,
+                      uint64_t* dict_digest, uint64_t* steer_digest, int32_t* K_host, int32_t* dict_entries, int32_t* steer_entries, void* stream) {
   cudaStream_t s = (cudaStream_t)stream;
-  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(digest, dev, (size_t)(1 + l.Qe) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
-  if (entries) GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(entries, l.assign + first, (size_t)count * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  const int nd = l.Qd ? l.Qd : 1;
+  const size_t inf = c.inference_iterations > 0 ? 2 : 0;
+  K_host[0] = l.K;
+  if (l.Qd) {
+    GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(K_host, l.dK, (size_t)nd * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    GCCNMF_CHECK_CUDA(h, cudaStreamSynchronize(s));
+  }
+  uint64_t* chunks = reinterpret_cast<uint64_t*>(workspace + w.chunks);
+  uint64_t* dev = reinterpret_cast<uint64_t*>(workspace + w.digests);
+  for (int e = 0; e < nd; ++e) {
+    GCCNMF_REQUIRE(h, K_host[e] >= 1 && K_host[e] <= l.K, "lldict: dictionary entry %d has %d atoms", e, K_host[e]);
+    DigestItems d{};
+    d.g[d.n++] = l.Qd ? DigestGroup{l.dW + (size_t)e * l.F * l.Kp, l.dH0 + (size_t)e * l.Kp * 2, 0, 0, (size_t)l.F, inf, l.dK + e, 0, 1, w.cd}
+                      : DigestGroup{l.W, l.H0, 0, 0, (size_t)l.F * l.K, inf * l.K, nullptr, l.K, 1, w.cd};
+    const size_t table = (size_t)4 * l.F * l.D;       // words of one (F, D) complex128 table
+    if (e == 0) d.g[d.n++] = DigestGroup{l.E, nullptr, table * sizeof(uint32_t), 0, table, 0, nullptr, 0, l.Qe, w.ce};
+    if (int st = record_enqueue_digests(h, d, chunks, dev + (e == 0 ? 0 : l.Qe + e), nullptr, stream)) return st;
+  }
+  uint64_t all[kLLMaxDictionaries + kLLMaxSteerings];
+  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(all, dev, (size_t)(nd + l.Qe) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+  if (dict_entries && l.Qd)
+    GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(dict_entries, l.dassign + first, (size_t)count * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  if (steer_entries) GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(steer_entries, l.assign + first, (size_t)count * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
   GCCNMF_CHECK_CUDA(h, cudaStreamSynchronize(s));
+  dict_digest[0] = all[0];
+  for (int j = 0; j < l.Qe; ++j) steer_digest[j] = all[1 + j];
+  for (int e = 1; e < nd; ++e) dict_digest[e] = all[l.Qe + e];
   return GCCNMF_OK;
 }
 
-#define LL_RECORD_ARGS_OR_FAIL(what)                                                                                               \
-  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);                                                                                                        \
-  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, what ": streams [%d, %d + %d) outside [0, %d)", \
-                 first, first, count, l.S);                                                                                          \
-  const RecordMap m = ll_record_map(*cfg, P, Lh, Qe);                                                                                \
-  const size_t rec_bytes = ll_record_bytes(*cfg, P, Lh);                                                                             \
-  GCCNMF_REQUIRE(h, record != nullptr && record_bytes >= (size_t)count * rec_bytes, what ": record needs %zu bytes for %d streams",  \
-                 (size_t)count * rec_bytes, count);                                                                                  \
-  const size_t ws_need = ll_record_workspace_bytes(*cfg, P, Lh, Qe, count);                                                          \
-  if (workspace == nullptr || workspace_bytes < ws_need || ((uintptr_t)workspace & (Qe ? 7 : 3)) != 0)                               \
-    return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, what ": workspace needs %zu bytes, %d-byte aligned", ws_need, Qe ? 8 : 4);
+// Qd >= 1 only with Qe >= 1 (ll_check); the lldict entries check Qd >= 1 themselves.
+#define LL_RECORD_ARGS_OR_FAIL(what)                                                                                                   \
+  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);                                                                                                 \
+  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "%s: streams [%d, %d + %d) outside [0, %d)", what, \
+                 first, first, count, l.S);                                                                                            \
+  const RecordMap m = ll_record_map(*cfg, P, Lh, Qe);                                                                                  \
+  const size_t rec_bytes = ll_record_bytes(*cfg, P, Lh);                                                                               \
+  GCCNMF_REQUIRE(h, record != nullptr && record_bytes >= (size_t)count * rec_bytes, "%s: record needs %zu bytes for %d streams", what,  \
+                 (size_t)count * rec_bytes, count);                                                                                    \
+  const LLRecordWork w = ll_record_work(*cfg, P, Lh, Qe, Qd, count);                                                                   \
+  if (workspace == nullptr || workspace_bytes < w.bytes || ((uintptr_t)workspace & (Qe ? 7 : 3)) != 0)                                 \
+    return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "%s: workspace needs %zu bytes, %d-byte aligned", what, w.bytes, Qe ? 8 : 4);
 
+// Every record byte a save writes is defined: the header's tail and the record's tail past the payload are zeroed here, the
+// payload's padding by the copy kernel.  The host writes its bytes while the device copies the payloads (other bytes of the same
+// records): at thousands of streams those writes miss the cache and would otherwise add to the save.
 int ll_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, int Qd, void* state, size_t state_bytes, int first, int count, void* record,
                     size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
   GCCNMF_ENTER(h);
-  LL_RECORD_ARGS_OR_FAIL("ll_save_streams");
-  gccnmf_record_header head = ll_record_header(*cfg, P, Lh, Qe);
+  const char* what = Qd ? "lldict_save_streams" : "ll_save_streams";
+  LL_RECORD_ARGS_OR_FAIL(what);
+  gccnmf_llbank_record_header head = ll_record_header(*cfg, P, Lh, Qe);
   if (int st = ll_synthesis_digest(h, l, &head.synthesis_digest, stream)) return st;
-  for (int i = 0; i < count; ++i) memcpy((char*)record + (size_t)i * rec_bytes, &head, sizeof(head));
-  if (Qe) {                              // the bank header: the dictionary's digest and that of each stream's table
-    uint64_t digest[1 + kLLMaxSteerings];
-    std::vector<int32_t> entries(count);
-    const int st = ll_bank_digests(h, cfg, l, count, (char*)workspace, first, digest, entries.data(), stream);
-    for (int i = 0; i < count && st == GCCNMF_OK; ++i) {
-      gccnmf_llbank_record_header* r = reinterpret_cast<gccnmf_llbank_record_header*>((char*)record + (size_t)i * rec_bytes);
-      r->dictionary_digest = digest[0];
-      r->steering_digest = digest[1 + entries[i]];
-    }
-    if (st) return st;
-  }
+  uint64_t dd[kLLMaxDictionaries], sd[kLLMaxSteerings];
+  int32_t Kh[kLLMaxDictionaries];
+  std::vector<int32_t> de(count, 0), se(count, 0);
+  if (Qe)
+    if (int st = ll_record_digests(h, *cfg, l, w, (char*)workspace, first, count, dd, sd, Kh, de.data(), se.data(), stream)) return st;
   GCCNMF_LAUNCH(h, ll_record_copy_kernel, dim3(count, m.n), 256, 0, stream, (char*)state, first, m, (char*)workspace, 1);
   GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync((char*)record + kRecordHeaderBytes, rec_bytes, workspace, m.payload, m.payload, count,
                                          cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  for (int i = 0; i < count; ++i) {
+    char* rec = (char*)record + (size_t)i * rec_bytes;
+    if (Qe) {                            // the bank header: the digests of the stream's dictionary and table
+      head.dictionary_digest = dd[de[i]];
+      head.steering_digest = sd[se[i]];
+      if (Qd) head.config[kConfigAtoms] = Kh[de[i]];     // the header an llbank engine built with the stream's dictionary writes
+    }
+    memcpy(rec, &head, sizeof(head));
+    memset(rec + sizeof(head), 0, kRecordHeaderBytes - sizeof(head));
+    memset(rec + kRecordHeaderBytes + m.payload, 0, rec_bytes - kRecordHeaderBytes - m.payload);
+  }
   return GCCNMF_OK;
 }
 
 int ll_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, int Qd, void* state, size_t state_bytes, int first, int count, const void* record,
                     size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
   GCCNMF_ENTER(h);
-  LL_RECORD_ARGS_OR_FAIL("ll_load_streams");
-  const gccnmf_record_header want = ll_record_header(*cfg, P, Lh, Qe);
-  for (int i = 0; i < count; ++i) {      // everything but the digests, before the device is touched
-    gccnmf_record_header got;
+  const char* what = Qd ? "lldict_load_streams" : "ll_load_streams";
+  LL_RECORD_ARGS_OR_FAIL(what);
+  const gccnmf_llbank_record_header want = ll_record_header(*cfg, P, Lh, Qe);
+  auto header = [&](int i) {
+    gccnmf_llbank_record_header got;
     memcpy(&got, (const char*)record + (size_t)i * rec_bytes, sizeof(got));
-    GCCNMF_REQUIRE(h, got.magic == want.magic, "ll_load_streams: record %d: not a stream record (magic 0x%08x)", i, got.magic);
-    GCCNMF_REQUIRE(h, got.abi_version == want.abi_version, "ll_load_streams: record %d: ABI version %d, this library is %d", i, got.abi_version,
-                   want.abi_version);
-    GCCNMF_REQUIRE(h, got.kind == want.kind, "ll_load_streams: record %d: kind %d is not a low-latency stream", i, got.kind);
-    GCCNMF_REQUIRE(h, got.num_sources == P, "ll_load_streams: record %d: %d sources, this engine has %d", i, got.num_sources, P);
-    GCCNMF_REQUIRE(h, got.config[kRecordConfigHistory] == Lh, "ll_load_streams: record %d: history length %d, this engine has %d", i,
-                   got.config[kRecordConfigHistory], Lh);
-    GCCNMF_REQUIRE(h, got.payload_bytes == want.payload_bytes, "ll_load_streams: record %d: payload of %llu bytes, expected %llu", i,
-                   (unsigned long long)got.payload_bytes, (unsigned long long)want.payload_bytes);
-    GCCNMF_REQUIRE(h, memcmp(got.config, want.config, sizeof(want.config)) == 0, "ll_load_streams: record %d: another configuration", i);
+    return got;
+  };
+  for (int i = 0; i < count; ++i) {      // everything but the digests, before the device is touched
+    gccnmf_llbank_record_header got = header(i);
+    const int K = got.config[kConfigAtoms];
+    if (Qd) {                            // a dictionary bank's records carry the stream's K_i
+      GCCNMF_REQUIRE(h, K >= 1 && K <= l.K, "%s: record %d: %d atoms, this engine holds at most %d", what, i, K, l.K);
+      got.config[kConfigAtoms] = want.config[kConfigAtoms];
+    }
+    if (int st = record_check_header(h, what, i, &got, &want, offsetof(gccnmf_record_header, config))) return st;
   }
   uint64_t digest = 0;
   if (int st = ll_synthesis_digest(h, l, &digest, stream)) return st;
-  for (int i = 0; i < count; ++i) {
-    gccnmf_record_header got;
-    memcpy(&got, (const char*)record + (size_t)i * rec_bytes, sizeof(got));
-    GCCNMF_REQUIRE(h, got.synthesis_digest == digest, "ll_load_streams: record %d: other synthesis weights or gain", i);
-  }
-  // bank: the same dictionary, and the lowest entry whose table has the record's content (only the read-only digest kernels have run
-  // when this refuses)
-  std::vector<int32_t> entries(Qe ? count : 0);
+  for (int i = 0; i < count; ++i)
+    GCCNMF_REQUIRE(h, header(i).synthesis_digest == digest, "%s: record %d: other synthesis weights or gain", what, i);
+  // bank: the lowest entries holding the record's dictionary (same content and K) and table (only the read-only digest kernels have
+  // run when this refuses)
+  std::vector<int32_t> de(count), se(count);
   if (Qe) {
-    uint64_t bank[1 + kLLMaxSteerings];
-    if (int st = ll_bank_digests(h, cfg, l, count, (char*)workspace, first, bank, nullptr, stream)) return st;
+    const int nd = Qd ? Qd : 1;
+    uint64_t dd[kLLMaxDictionaries], sd[kLLMaxSteerings];
+    int32_t Kh[kLLMaxDictionaries];
+    if (int st = ll_record_digests(h, *cfg, l, w, (char*)workspace, first, count, dd, sd, Kh, nullptr, nullptr, stream)) return st;
     for (int i = 0; i < count; ++i) {
-      gccnmf_llbank_record_header got;
-      memcpy(&got, (const char*)record + (size_t)i * rec_bytes, sizeof(got));
-      GCCNMF_REQUIRE(h, got.dictionary_digest == bank[0], "ll_load_streams: record %d: another dictionary", i);
-      int e = -1;
-      for (int j = Qe - 1; j >= 0; --j)
-        if (bank[1 + j] == got.steering_digest) e = j;
-      GCCNMF_REQUIRE(h, e >= 0, "ll_load_streams: record %d: no steering entry of this engine has the stream's table", i);
-      entries[i] = e;
+      const gccnmf_llbank_record_header got = header(i);
+      const int K = got.config[kConfigAtoms], same = record_find_entry(dd, nullptr, nd, got.dictionary_digest, 0);
+      de[i] = record_find_entry(dd, Kh, nd, got.dictionary_digest, K);
+      se[i] = record_find_entry(sd, nullptr, Qe, got.steering_digest, 0);
+      GCCNMF_REQUIRE(h, same >= 0, "%s: record %d: no dictionary entry of this engine holds the stream's dictionary", what, i);
+      GCCNMF_REQUIRE(h, de[i] >= 0, "%s: record %d: the stream's dictionary has %d atoms, the entry holding it %d", what, i, K, Kh[same]);
+      GCCNMF_REQUIRE(h, se[i] >= 0, "%s: record %d: no steering entry of this engine has the stream's table", what, i);
     }
   }
   GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync(workspace, m.payload, (const char*)record + kRecordHeaderBytes, rec_bytes, m.payload, count,
                                          cudaMemcpyHostToDevice, (cudaStream_t)stream));
   GCCNMF_LAUNCH(h, ll_record_copy_kernel, dim3(count, m.n), 256, 0, stream, (char*)state, first, m, (char*)workspace, 0);
-  if (Qe) {
+  for (int pass = Qd ? 0 : 1; Qe && pass < 2; ++pass) {    // the dictionary entries (Qd >= 1), then the tables
+    const std::vector<int32_t>& src = pass ? se : de;
     for (int i0 = 0; i0 < count; i0 += kLLParamsPerLaunch) {
       const int n = count - i0 < kLLParamsPerLaunch ? count - i0 : kLLParamsPerLaunch;
       LLAssignBatch b{};
-      memcpy(b.e, entries.data() + i0, (size_t)n * sizeof(int32_t));
-      GCCNMF_LAUNCH(h, ll_assign_kernel, 1, kLLParamsPerLaunch, 0, stream, l.assign, first + i0, n, b, 0);
+      memcpy(b.e, src.data() + i0, (size_t)n * sizeof(int32_t));
+      GCCNMF_LAUNCH(h, ll_assign_kernel, 1, kLLParamsPerLaunch, 0, stream, pass ? l.assign : l.dassign, first + i0, n, b, 0);
     }
-    GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
   }
+  if (Qe) GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
+  if (Qd) GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.dassign, l.S, Qd, l.dorder, l.dseg);
   return GCCNMF_OK;
 }
 
@@ -1510,7 +1464,6 @@ int ll_assign(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int 
 
 
 // ---- dictionary bank (gccnmf_lldict_*)
-constexpr int kConfigAtoms = offsetof(gccnmf_ll_config, num_atoms) / sizeof(int32_t);
 
 // Entry e <- W (F, K) f32 and, with inference, H0 (K, 2) f32 (device arrays), with every form derived from them; stream-ordered.
 int lld_load_entry(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l, int e, const float* W, int K, const float* H0, void* stream) {
@@ -1587,164 +1540,6 @@ int lld_assign(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int
     if (pass) GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
     else GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.dassign, l.S, Qd, l.dorder, l.dseg);
   }
-  return GCCNMF_OK;
-}
-
-// Records: the workspace holds the payloads, one chunk digest per 1024-word chunk of the largest dictionary and of each table, then
-// the Qe table digests and the Qd dictionary digests.  Each dictionary's digest is the llbank digest of an engine built with it.
-struct LLDictDigestSizes { int cd, ce; };
-LLDictDigestSizes lld_digest_sizes(const gccnmf_ll_config& c, const LLLayout& l) {
-  const size_t n = (size_t)l.F * l.K + (c.inference_iterations > 0 ? (size_t)2 * l.K : 0), ne = (size_t)4 * l.F * l.D;
-  return LLDictDigestSizes{(int)((n + kDigestChunk - 1) / kDigestChunk), (int)((ne + kDigestChunk - 1) / kDigestChunk)};
-}
-
-size_t lld_record_workspace_bytes(const gccnmf_ll_config& c, int P, int Lh, int Qd, int Qe, int count) {
-  const LLLayout l = ll_carve(c, P, nullptr, Lh, Qe, Qd);
-  const LLDictDigestSizes z = lld_digest_sizes(c, l);
-  return align_up((size_t)count * ll_record_map(c, P, Lh).payload, 256) + align_up((size_t)(z.cd + Qe * z.ce) * sizeof(uint64_t), 256) +
-         (size_t)(Qd + Qe) * sizeof(uint64_t);
-}
-
-// The Qd dictionary digests, the Qe table digests, the K_e table and (entries != NULL) the two entries of streams [first, first + count)
-// back to the host: two waits on the stream.
-int lld_digests(gccnmf_handle* h, const gccnmf_ll_config* cfg, const LLLayout& l, int count, char* workspace, int first, uint64_t* dict_digest,
-                uint64_t* steer_digest, int32_t* K_host, int32_t* dict_entries, int32_t* steer_entries, void* stream) {
-  cudaStream_t s = (cudaStream_t)stream;
-  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(K_host, l.dK, (size_t)l.Qd * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  GCCNMF_CHECK_CUDA(h, cudaStreamSynchronize(s));
-  const bool inf = cfg->inference_iterations > 0;
-  const LLDictDigestSizes z = lld_digest_sizes(*cfg, l);
-  uint64_t* chunks = reinterpret_cast<uint64_t*>(workspace + align_up((size_t)count * ll_record_map(*cfg, l.P, l.Lh).payload, 256));
-  uint64_t* dev = chunks + align_up((size_t)(z.cd + l.Qe * z.ce) * sizeof(uint64_t), 256) / sizeof(uint64_t);
-  for (int e = 0; e < l.Qd; ++e) {
-    const int K = K_host[e];
-    GCCNMF_REQUIRE(h, K >= 1 && K <= l.K, "lldict: dictionary entry %d has %d atoms", e, K);
-    LLDigestItems d = ll_digest_items(l, inf);
-    d.W = reinterpret_cast<const uint32_t*>(l.dW + (size_t)e * l.F * l.Kp);
-    d.H0 = reinterpret_cast<const uint32_t*>(l.dH0 + (size_t)e * l.Kp * 2);
-    d.nw = (size_t)l.F * K;
-    d.nh = inf ? (size_t)2 * K : 0;
-    d.cd = (int)((d.nw + d.nh + kDigestChunk - 1) / kDigestChunk);
-    d.Qe = e == 0 ? l.Qe : 0;                       // the tables once, with entry 0: dev[0] dictionary 0, dev[1 ..] the tables
-    const int n = d.cd + d.Qe * d.ce;
-    GCCNMF_LAUNCH(h, ll_digest_chunks_kernel, (n + 127) / 128, 128, 0, stream, d, chunks);
-    GCCNMF_LAUNCH(h, ll_digest_fold_kernel, (d.Qe + 1 + 127) / 128, 128, 0, stream, d, chunks, dev + (e == 0 ? 0 : l.Qe + e));
-  }
-  std::vector<uint64_t> all((size_t)l.Qd + l.Qe);
-  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(all.data(), dev, all.size() * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
-  if (dict_entries) GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(dict_entries, l.dassign + first, (size_t)count * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  if (steer_entries) GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(steer_entries, l.assign + first, (size_t)count * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-  GCCNMF_CHECK_CUDA(h, cudaStreamSynchronize(s));
-  dict_digest[0] = all[0];
-  for (int j = 0; j < l.Qe; ++j) steer_digest[j] = all[1 + j];
-  for (int e = 1; e < l.Qd; ++e) dict_digest[e] = all[l.Qe + e];
-  return GCCNMF_OK;
-}
-
-#define LLD_RECORD_ARGS_OR_FAIL(what)                                                                                              \
-  GCCNMF_REQUIRE(h, Qd >= 1, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, Qd);                    \
-  LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);                                                                                               \
-  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, what ": streams [%d, %d + %d) outside [0, %d)", \
-                 first, first, count, l.S);                                                                                          \
-  const RecordMap m = ll_record_map(*cfg, P, Lh, Qe);                                                                                \
-  const size_t rec_bytes = ll_record_bytes(*cfg, P, Lh);                                                                             \
-  GCCNMF_REQUIRE(h, record != nullptr && record_bytes >= (size_t)count * rec_bytes, what ": record needs %zu bytes for %d streams",  \
-                 (size_t)count * rec_bytes, count);                                                                                  \
-  const size_t ws_need = lld_record_workspace_bytes(*cfg, P, Lh, Qd, Qe, count);                                                     \
-  if (workspace == nullptr || workspace_bytes < ws_need || ((uintptr_t)workspace & 7) != 0)                                          \
-    return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, what ": workspace needs %zu bytes, 8-byte aligned", ws_need);
-
-int lld_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qd, int Qe, void* state, size_t state_bytes, int first, int count,
-                     void* record, size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
-  GCCNMF_ENTER(h);
-  LLD_RECORD_ARGS_OR_FAIL("lldict_save_streams");
-  gccnmf_record_header head = ll_record_header(*cfg, P, Lh, Qe);
-  if (int st = ll_synthesis_digest(h, l, &head.synthesis_digest, stream)) return st;
-  uint64_t dd[kLLMaxDictionaries], sd[kLLMaxSteerings];
-  int32_t Kh[kLLMaxDictionaries];
-  std::vector<int32_t> de(count), se(count);
-  if (int st = lld_digests(h, cfg, l, count, (char*)workspace, first, dd, sd, Kh, de.data(), se.data(), stream)) return st;
-  for (int i = 0; i < count; ++i) {
-    char* rec = (char*)record + (size_t)i * rec_bytes;
-    memcpy(rec, &head, sizeof(head));
-    gccnmf_llbank_record_header* r = reinterpret_cast<gccnmf_llbank_record_header*>(rec);
-    r->config[kConfigAtoms] = Kh[de[i]];              // the header an llbank engine built with the stream's dictionary writes
-    r->dictionary_digest = dd[de[i]];
-    r->steering_digest = sd[se[i]];
-  }
-  GCCNMF_LAUNCH(h, ll_record_copy_kernel, dim3(count, m.n), 256, 0, stream, (char*)state, first, m, (char*)workspace, 1);
-  GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync((char*)record + kRecordHeaderBytes, rec_bytes, workspace, m.payload, m.payload, count,
-                                         cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-  return GCCNMF_OK;
-}
-
-int lld_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qd, int Qe, void* state, size_t state_bytes, int first, int count,
-                     const void* record, size_t record_bytes, void* workspace, size_t workspace_bytes, void* stream) {
-  GCCNMF_ENTER(h);
-  LLD_RECORD_ARGS_OR_FAIL("lldict_load_streams");
-  const gccnmf_record_header want = ll_record_header(*cfg, P, Lh, Qe);
-  for (int i = 0; i < count; ++i) {      // everything but the digests, before the device is touched
-    gccnmf_record_header got;
-    memcpy(&got, (const char*)record + (size_t)i * rec_bytes, sizeof(got));
-    GCCNMF_REQUIRE(h, got.magic == want.magic, "lldict_load_streams: record %d: not a stream record (magic 0x%08x)", i, got.magic);
-    GCCNMF_REQUIRE(h, got.abi_version == want.abi_version, "lldict_load_streams: record %d: ABI version %d, this library is %d", i, got.abi_version,
-                   want.abi_version);
-    GCCNMF_REQUIRE(h, got.kind == want.kind, "lldict_load_streams: record %d: kind %d is not a bank stream", i, got.kind);
-    GCCNMF_REQUIRE(h, got.num_sources == P, "lldict_load_streams: record %d: %d sources, this engine has %d", i, got.num_sources, P);
-    GCCNMF_REQUIRE(h, got.config[kRecordConfigHistory] == Lh, "lldict_load_streams: record %d: history length %d, this engine has %d", i,
-                   got.config[kRecordConfigHistory], Lh);
-    GCCNMF_REQUIRE(h, got.payload_bytes == want.payload_bytes, "lldict_load_streams: record %d: payload of %llu bytes, expected %llu", i,
-                   (unsigned long long)got.payload_bytes, (unsigned long long)want.payload_bytes);
-    const int K = got.config[kConfigAtoms];
-    GCCNMF_REQUIRE(h, K >= 1 && K <= l.K, "lldict_load_streams: record %d: %d atoms, this engine holds at most %d", i, K, l.K);
-    got.config[kConfigAtoms] = want.config[kConfigAtoms];
-    GCCNMF_REQUIRE(h, memcmp(got.config, want.config, sizeof(want.config)) == 0, "lldict_load_streams: record %d: another configuration", i);
-  }
-  uint64_t digest = 0;
-  if (int st = ll_synthesis_digest(h, l, &digest, stream)) return st;
-  for (int i = 0; i < count; ++i) {
-    gccnmf_record_header got;
-    memcpy(&got, (const char*)record + (size_t)i * rec_bytes, sizeof(got));
-    GCCNMF_REQUIRE(h, got.synthesis_digest == digest, "lldict_load_streams: record %d: other synthesis weights or gain", i);
-  }
-  // the lowest entries holding the record's dictionary (same content and K) and table (only read-only kernels have run when this refuses)
-  uint64_t dd[kLLMaxDictionaries], sd[kLLMaxSteerings];
-  int32_t Kh[kLLMaxDictionaries];
-  if (int st = lld_digests(h, cfg, l, count, (char*)workspace, first, dd, sd, Kh, nullptr, nullptr, stream)) return st;
-  std::vector<int32_t> de(count), se(count);
-  for (int i = 0; i < count; ++i) {
-    gccnmf_llbank_record_header got;
-    memcpy(&got, (const char*)record + (size_t)i * rec_bytes, sizeof(got));
-    const int K = got.config[kConfigAtoms];
-    int d = -1, same_content = -1;
-    for (int e = Qd - 1; e >= 0; --e)
-      if (dd[e] == got.dictionary_digest) {
-        same_content = e;
-        if (Kh[e] == K) d = e;
-      }
-    GCCNMF_REQUIRE(h, same_content >= 0, "lldict_load_streams: record %d: no dictionary entry of this engine holds the stream's dictionary", i);
-    GCCNMF_REQUIRE(h, d >= 0, "lldict_load_streams: record %d: the stream's dictionary has %d atoms, the entry holding it %d", i, K, Kh[same_content]);
-    int e = -1;
-    for (int j = Qe - 1; j >= 0; --j)
-      if (sd[j] == got.steering_digest) e = j;
-    GCCNMF_REQUIRE(h, e >= 0, "lldict_load_streams: record %d: no steering entry of this engine has the stream's table", i);
-    de[i] = d;
-    se[i] = e;
-  }
-  GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync(workspace, m.payload, (const char*)record + kRecordHeaderBytes, rec_bytes, m.payload, count,
-                                         cudaMemcpyHostToDevice, (cudaStream_t)stream));
-  GCCNMF_LAUNCH(h, ll_record_copy_kernel, dim3(count, m.n), 256, 0, stream, (char*)state, first, m, (char*)workspace, 0);
-  for (int pass = 0; pass < 2; ++pass) {
-    const std::vector<int32_t>& src = pass ? se : de;
-    for (int i0 = 0; i0 < count; i0 += kLLParamsPerLaunch) {
-      const int n = count - i0 < kLLParamsPerLaunch ? count - i0 : kLLParamsPerLaunch;
-      LLAssignBatch b{};
-      memcpy(b.e, src.data() + i0, (size_t)n * sizeof(int32_t));
-      GCCNMF_LAUNCH(h, ll_assign_kernel, 1, kLLParamsPerLaunch, 0, stream, pass ? l.assign : l.dassign, first + i0, n, b, 0);
-    }
-  }
-  GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
-  GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.dassign, l.S, Qd, l.dorder, l.dseg);
   return GCCNMF_OK;
 }
 
@@ -1846,7 +1641,7 @@ size_t gccnmf_llrec_record_bytes(const gccnmf_ll_config* cfg, int num_sources) {
 
 size_t gccnmf_llrec_workspace_bytes(const gccnmf_ll_config* cfg, int num_sources, int count) {
   if (ll_check(nullptr, cfg, num_sources) != 0 || count < 1) return 0;
-  return (size_t)count * ll_record_map(*cfg, num_sources).payload;
+  return ll_record_work(*cfg, num_sources, 0, 0, 0, count).bytes;
 }
 
 int gccnmf_llrec_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, void* state, size_t state_bytes, int first,
@@ -1917,7 +1712,7 @@ size_t gccnmf_llhist_record_bytes(const gccnmf_ll_config* cfg, int num_sources, 
 
 size_t gccnmf_llhist_workspace_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int count) {
   if (ll_check(nullptr, cfg, num_sources, history_length) != 0 || count < 1) return 0;
-  return (size_t)count * ll_record_map(*cfg, num_sources, history_length).payload;
+  return ll_record_work(*cfg, num_sources, history_length, 0, 0, count).bytes;
 }
 
 int gccnmf_llhist_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, void* state,
@@ -2002,7 +1797,7 @@ size_t gccnmf_llbank_record_bytes(const gccnmf_ll_config* cfg, int num_sources, 
 
 size_t gccnmf_llbank_workspace_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, int count) {
   if (ll_check(nullptr, cfg, num_sources, history_length, num_steerings) != 0 || count < 1) return 0;
-  return ll_record_workspace_bytes(*cfg, num_sources, history_length, num_steerings, count);
+  return ll_record_work(*cfg, num_sources, history_length, num_steerings, 0, count).bytes;
 }
 
 int gccnmf_llbank_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_steerings, void* state,
@@ -2107,21 +1902,21 @@ size_t gccnmf_lldict_record_bytes(const gccnmf_ll_config* cfg, int num_sources, 
 size_t gccnmf_lldict_workspace_bytes(const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries, int num_steerings,
                                      int count) {
   if (num_dictionaries < 1 || ll_check(nullptr, LLD_ARGS) != 0 || count < 1) return 0;
-  return lld_record_workspace_bytes(*cfg, num_sources, history_length, num_dictionaries, num_steerings, count);
+  return ll_record_work(*cfg, num_sources, history_length, num_steerings, num_dictionaries, count).bytes;
 }
 
 int gccnmf_lldict_save_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
                                int num_steerings, void* state, size_t state_bytes, int first, int count, void* record, size_t record_bytes,
                                void* workspace, size_t workspace_bytes, void* stream) {
-  return lld_save_streams(h, cfg, num_sources, history_length, num_dictionaries, num_steerings, state, state_bytes, first, count, record, record_bytes,
-                          workspace, workspace_bytes, stream);
+  GCCNMF_REQUIRE(h, num_dictionaries >= 1, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, num_dictionaries);
+  return ll_save_streams(h, LLD_ARGS, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes, stream);
 }
 
 int gccnmf_lldict_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int num_sources, int history_length, int num_dictionaries,
                                int num_steerings, void* state, size_t state_bytes, int first, int count, const void* record, size_t record_bytes,
                                void* workspace, size_t workspace_bytes, void* stream) {
-  return lld_load_streams(h, cfg, num_sources, history_length, num_dictionaries, num_steerings, state, state_bytes, first, count, record, record_bytes,
-                          workspace, workspace_bytes, stream);
+  GCCNMF_REQUIRE(h, num_dictionaries >= 1, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, num_dictionaries);
+  return ll_load_streams(h, LLD_ARGS, state, state_bytes, first, count, record, record_bytes, workspace, workspace_bytes, stream);
 }
 #undef LLD_ARGS
 

@@ -50,6 +50,7 @@
 
 #include "common.cuh"
 #include "fft.cuh"
+#include "records.cuh"
 
 namespace {
 
@@ -1371,160 +1372,60 @@ int rt_set_targets(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout
 // scratch and stays.  Region g of slot s is [offset + s stride, + bytes) from slot 0's region; it goes to [rec_offset, + bytes)
 // of the record's payload, and [rec_offset + bytes, + span) of the record is zero.
 static_assert(sizeof(RtDev) == 44, "RtDev");
-struct RtRecordRegion { size_t offset, rec_offset, bytes, span; };
-constexpr int kRtRecordMaxRegions = 4 + kRtMaxSources + 2;
-struct RtRecordMap {
-  RtRecordRegion r[kRtRecordMaxRegions];
-  int n;
-  size_t payload;                        // payload bytes of one slot (16-aligned)
-};
 constexpr size_t kRtRecordHeaderBytes = GCCNMF_RECORD_HEADER_BYTES;
 static_assert(sizeof(gccnmf_rtrec_header) <= kRtRecordHeaderBytes, "record header");
-static_assert(offsetof(gccnmf_rtrec_header, windows_digest) == sizeof(uint64_t) + offsetof(gccnmf_record_header, payload_bytes), "shared prefix");
 
 // The state offsets follow the destination's carve (they depend on K_max through the scratch between the regions); the record
 // offsets depend only on the configuration without num_atoms and on P.
-RtRecordMap rt_record_map(const gccnmf_rt_config& c, int P, int Qd = 0, int Qe = 0) {
+RecordMap rt_record_map(const gccnmf_rt_config& c, int P, int Qd = 0, int Qe = 0) {
   const RtLayout l = rt_carve(c, 1, P, nullptr, 0, Qd, Qe);
-  const char* slot0 = reinterpret_cast<const char*>(l.dev);
-  RtRecordMap m{};
-  size_t at = 0;
-  auto add = [&](const void* p, size_t bytes) {
-    const size_t next = align_up(at + bytes, 16);
-    m.r[m.n++] = RtRecordRegion{(size_t)((const char*)p - slot0), at, bytes, next - at};
-    at = next;
-  };
-  add(l.dev, sizeof(RtDev));
-  add(l.hist, (size_t)c.num_tdoas * c.history_length * sizeof(double));
-  add(l.in_ring, (size_t)2 * l.L * sizeof(float));
-  for (int q = 0; q < (P > 0 ? P : 1); ++q) add(rt_slot(l.sout, q, l.src_stride), (size_t)2 * l.L * sizeof(float));
+  RecordMapBuilder b{l.dev, l.stride};
+  b.add(l.dev, sizeof(RtDev));
+  b.add(l.hist, (size_t)c.num_tdoas * c.history_length * sizeof(double));
+  b.add(l.in_ring, (size_t)2 * l.L * sizeof(float));
+  for (int q = 0; q < (P > 0 ? P : 1); ++q) b.add(rt_slot(l.sout, q, l.src_stride), (size_t)2 * l.L * sizeof(float));
   if (P > 0) {
-    add(l.targets, kRtMaxSources * sizeof(int32_t));
-    add(l.status, sizeof(int32_t));
+    b.add(l.targets, kRtMaxSources * sizeof(int32_t));
+    b.add(l.status, sizeof(int32_t));
   }
-  m.payload = at;
-  return m;
+  return b.m;
 }
 
 size_t rt_record_bytes(const gccnmf_rt_config& c, int P) { return kRtRecordHeaderBytes + align_up(rt_record_map(c, P).payload, 256); }
 
-// The content digests of a state: item 0 the windows, items 1 .. nd the dictionary entries, items nd + 1 .. nd + ne the steering
-// entries (nd = ne = 1 without a bank).  Each item has a fixed number of chunk slots in the workspace (cw, cd, ce: enough for
-// K_max atoms); a dictionary of fewer atoms leaves its last ones unused.
-constexpr int kRtDigestChunk = GCCNMF_RTREC_DIGEST_CHUNK_WORDS;
-struct RtDigestItems {
-  const uint32_t *win_a, *win_s, *W, *H0, *ET;
-  const int32_t* K;                      // the bank's K_i table, or NULL: one dictionary of K_fixed atoms
-  size_t dict_stride, steer_stride;      // bytes (0 without a bank)
-  int N, F, K_fixed, inf, nd, ne, et_words;
-  int cw, cd, ce;
-};
-
-__device__ __forceinline__ uint64_t rt_fnv(uint64_t h, uint32_t w) { return (h ^ w) * GCCNMF_RTREC_DIGEST_PRIME; }
-
-// Item `item` as up to two word sequences a[0 .. na) then b[0 .. nb), and its K_i (dictionaries) or 0.
-__device__ __forceinline__ int rt_digest_item(const RtDigestItems& d, int item, const uint32_t*& a, size_t& na, const uint32_t*& b, size_t& nb) {
-  if (item == 0) {
-    a = d.win_a; na = d.N; b = d.win_s; nb = d.N;
-    return 0;
-  }
-  if (item <= d.nd) {
-    const int i = item - 1, Ki = d.K ? d.K[i] : d.K_fixed;
-    a = rt_slot(d.W, i, d.dict_stride); na = (size_t)d.F * Ki;
-    b = rt_slot(d.H0, i, d.dict_stride); nb = d.inf ? (size_t)2 * Ki : 0;
-    return Ki;
-  }
-  a = rt_slot(d.ET, item - 1 - d.nd, d.steer_stride); na = d.et_words; b = nullptr; nb = 0;
-  return 0;
-}
-
-// One thread per chunk slot: c_j = FNV-1a 64 over the chunk's words (0 for an unused slot).
-__global__ void __launch_bounds__(128) rt_digest_chunks_kernel(RtDigestItems d, uint64_t* __restrict__ chunks) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x, dict_end = d.cw + d.nd * d.cd;
-  if (t >= dict_end + d.ne * d.ce) return;
-  int item, j;
-  if (t < d.cw) item = 0, j = t;
-  else if (t < dict_end) item = 1 + (t - d.cw) / d.cd, j = (t - d.cw) % d.cd;
-  else item = 1 + d.nd + (t - dict_end) / d.ce, j = (t - dict_end) % d.ce;
-  const uint32_t *a, *b;
-  size_t na, nb;
-  rt_digest_item(d, item, a, na, b, nb);
-  const size_t n = na + nb, w0 = (size_t)j * kRtDigestChunk, w1 = w0 + kRtDigestChunk < n ? w0 + kRtDigestChunk : n;
-  uint64_t h = GCCNMF_RTREC_DIGEST_BASIS;
-  if (w0 >= n) h = 0;
-#pragma unroll 8
-  for (size_t w = w0; w < (w1 < na ? w1 : na); ++w) h = rt_fnv(h, __ldg(a + w));
-  for (size_t w = w0 > na ? w0 : na; w < w1; ++w) h = rt_fnv(h, __ldg(b + (w - na)));
-  chunks[t] = h;
-}
-
-// One thread per item: the digest over (n_lo, n_hi, c_0 lo, c_0 hi, ...) and the item's K_i.
-__global__ void __launch_bounds__(128) rt_digest_fold_kernel(RtDigestItems d, const uint64_t* __restrict__ chunks, uint64_t* __restrict__ digest,
-                                                             int32_t* __restrict__ atoms) {
-  const int item = blockIdx.x * blockDim.x + threadIdx.x;
-  if (item > d.nd + d.ne) return;
-  const uint32_t *a, *b;
-  size_t na, nb;
-  const int Ki = rt_digest_item(d, item, a, na, b, nb);
-  const size_t n = na + nb;
-  const int c0 = item == 0 ? 0 : item <= d.nd ? d.cw + (item - 1) * d.cd : d.cw + d.nd * d.cd + (item - 1 - d.nd) * d.ce;
-  uint64_t h = rt_fnv(rt_fnv(GCCNMF_RTREC_DIGEST_BASIS, (uint32_t)n), (uint32_t)(n >> 32));
-  for (size_t j = 0; j < (n + kRtDigestChunk - 1) / kRtDigestChunk; ++j) {
-    const uint64_t c = chunks[c0 + j];
-    h = rt_fnv(rt_fnv(h, (uint32_t)c), (uint32_t)(c >> 32));
-  }
-  digest[item] = h;
-  atoms[item] = Ki;
-}
-
-// Grid (count, regions + 1).  CTA (i, g < regions) copies region g of slot first + i between the state and record i of the staging
-// (16-byte words where both ends and the length allow it, else 4-byte words), and on a save zeroes the record up to the next
-// region.  CTA (i, regions), the header: a save writes the header (the host part `head`, the digests and K_i of the slot's
-// entries, found through its assignment) and zeroes the header's tail and the payload's; a load maps the record's dictionary
-// (digest and K_i) and steering digest to the lowest matching entry of this state, as the host did, and writes the slot's
-// assignment (bank only).
+// Grid (count, regions + 1).  CTA (i, g < regions) copies region g of slot first + i between the state and record i of the staging.
+// CTA (i, regions), the header: a save writes the header (the host part `head`, the digests and K_i of the slot's entries, found
+// through its assignment) and zeroes the header's tail and the payload's; a load maps the record's dictionary (digest and K_i) and
+// steering digest to the lowest matching entry of this state, as the host did, and writes the slot's assignment (bank only).  The
+// digests are item 0 the windows, items 1 .. nd the dictionaries and nd + 1 .. nd + ne the steering entries.
 __global__ void __launch_bounds__(256)
-rt_record_copy_kernel(char* __restrict__ slot0, size_t stride, int first, RtRecordMap m, char* __restrict__ staging, size_t rec_bytes, int to_staging,
+rt_record_copy_kernel(char* __restrict__ slot0, size_t stride, int first, RecordMap m, char* __restrict__ staging, size_t rec_bytes, int to_staging,
                       gccnmf_rtrec_header head, const uint64_t* __restrict__ digest, const int32_t* __restrict__ atoms, int nd, int ne,
                       int32_t* __restrict__ assign0) {
   const int s = first + blockIdx.x;
   char* rec = staging + (size_t)blockIdx.x * rec_bytes;
-  if (blockIdx.y == m.n) {
-    int32_t* assign = assign0 ? rt_slot(assign0, s, stride) : nullptr;
-    if (to_staging) {
-      for (size_t i = sizeof(head) / 4 + threadIdx.x; i < kRtRecordHeaderBytes / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(rec)[i] = 0;
-      for (size_t i = (kRtRecordHeaderBytes + m.payload) / 4 + threadIdx.x; i < rec_bytes / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(rec)[i] = 0;
-      if (threadIdx.x == 0) {
-        const int di = assign ? assign[0] : 0, ej = assign ? assign[1] : 0;
-        head.windows_digest = digest[0];
-        head.dictionary_digest = digest[1 + di];
-        head.steering_digest = digest[1 + nd + ej];
-        head.dictionary_atoms = atoms[1 + di];
-        *reinterpret_cast<gccnmf_rtrec_header*>(rec) = head;
-      }
-    } else if (threadIdx.x == 0 && assign) {
-      const gccnmf_rtrec_header got = *reinterpret_cast<const gccnmf_rtrec_header*>(rec);
-      int di = -1, ej = -1;
-      for (int i = nd - 1; i >= 0; --i)
-        if (digest[1 + i] == got.dictionary_digest && atoms[1 + i] == got.dictionary_atoms) di = i;
-      for (int j = ne - 1; j >= 0; --j)
-        if (digest[1 + nd + j] == got.steering_digest) ej = j;
-      if (di >= 0 && ej >= 0) assign[0] = di, assign[1] = ej;
-    }
+  if (blockIdx.y < m.n) {
+    record_copy_region(slot0, s, m.r[blockIdx.y], rec + kRtRecordHeaderBytes, to_staging);
     return;
   }
-  const RtRecordRegion g = m.r[blockIdx.y];
-  char* slot = slot0 + g.offset + (size_t)s * stride;
-  char* payload = rec + kRtRecordHeaderBytes + g.rec_offset;
-  const char* src = to_staging ? slot : payload;
-  char* dst = to_staging ? payload : slot;
-  if ((((uintptr_t)src | (uintptr_t)dst | g.bytes) & 15) == 0) {
-    for (size_t i = threadIdx.x; i < g.bytes / 16; i += blockDim.x) reinterpret_cast<uint4*>(dst)[i] = reinterpret_cast<const uint4*>(src)[i];
-  } else {
-    for (size_t i = threadIdx.x; i < g.bytes / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(dst)[i] = reinterpret_cast<const uint32_t*>(src)[i];
+  int32_t* assign = assign0 ? rt_slot(assign0, s, stride) : nullptr;
+  if (to_staging) {
+    for (size_t i = sizeof(head) / 4 + threadIdx.x; i < kRtRecordHeaderBytes / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(rec)[i] = 0;
+    for (size_t i = (kRtRecordHeaderBytes + m.payload) / 4 + threadIdx.x; i < rec_bytes / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(rec)[i] = 0;
+    if (threadIdx.x == 0) {
+      const int di = assign ? assign[0] : 0, ej = assign ? assign[1] : 0;
+      head.windows_digest = digest[0];
+      head.dictionary_digest = digest[1 + di];
+      head.steering_digest = digest[1 + nd + ej];
+      head.dictionary_atoms = atoms[1 + di];
+      *reinterpret_cast<gccnmf_rtrec_header*>(rec) = head;
+    }
+  } else if (threadIdx.x == 0 && assign) {
+    const gccnmf_rtrec_header got = *reinterpret_cast<const gccnmf_rtrec_header*>(rec);
+    const int di = record_find_entry(digest + 1, atoms + 1, nd, got.dictionary_digest, got.dictionary_atoms);
+    const int ej = record_find_entry(digest + 1 + nd, nullptr, ne, got.steering_digest, 0);
+    if (di >= 0 && ej >= 0) assign[0] = di, assign[1] = ej;
   }
-  if (to_staging)
-    for (size_t i = g.bytes / 4 + threadIdx.x; i < g.span / 4; i += blockDim.x) reinterpret_cast<uint32_t*>(payload)[i] = 0;
 }
 
 // What a record must agree on from the host arguments alone: magic, ABI version, kind, P, payload size and the configuration
@@ -1543,47 +1444,37 @@ gccnmf_rtrec_header rt_record_header(const gccnmf_rt_config& cfg, int P) {
   return r;
 }
 
-// The workspace: count whole records, then the chunk digests, the item digests and the items' K_i.
+// The digest items of a state: the windows, its nd dictionaries (nd = ne = 1 without a bank) and its ne steering entries, each with
+// chunk slots for K_max atoms.  The workspace: count whole records, then the chunk digests, the item digests and the items' K_i.
 struct RtRecordWork {
-  RtDigestItems d;
+  DigestItems d;
+  int nd, ne;
   size_t chunks, digests, atoms, bytes;
 };
 RtRecordWork rt_record_work(const gccnmf_rt_config& c, const RtLayout& l, int count) {
   RtRecordWork w{};
-  RtDigestItems& d = w.d;
-  const int N = c.window_size, K = c.num_atoms, inf = c.inference_iterations > 0 ? 1 : 0;
-  d.win_a = reinterpret_cast<const uint32_t*>(l.win_a);
-  d.win_s = reinterpret_cast<const uint32_t*>(l.win_s);
-  d.W = reinterpret_cast<const uint32_t*>(l.W);
-  d.H0 = reinterpret_cast<const uint32_t*>(l.H0);
-  d.ET = reinterpret_cast<const uint32_t*>(l.ET);
-  d.K = l.bank_K;
-  d.dict_stride = l.bank.dict_stride;
-  d.steer_stride = l.bank.steer_stride;
-  d.N = N; d.F = l.F; d.K_fixed = K; d.inf = inf;
-  d.nd = l.Qd > 0 ? l.Qd : 1;
-  d.ne = l.Qe > 0 ? l.Qe : 1;
-  d.et_words = 2 * l.D * l.Fp;
-  auto chunks = [](size_t words) { return (int)((words + kRtDigestChunk - 1) / kRtDigestChunk); };
-  d.cw = chunks((size_t)2 * N);
-  d.cd = chunks((size_t)l.F * K + (size_t)2 * K * inf);
-  d.ce = chunks(d.et_words);
-  const int items = 1 + d.nd + d.ne, total = d.cw + d.nd * d.cd + d.ne * d.ce;
+  const size_t N = c.window_size, F = l.F, K = c.num_atoms, inf = c.inference_iterations > 0 ? 1 : 0, et_words = (size_t)2 * l.D * l.Fp;
+  w.nd = l.Qd > 0 ? l.Qd : 1;
+  w.ne = l.Qe > 0 ? l.Qe : 1;
+  const int cd = digest_chunks(F * K + 2 * K * inf);
+  w.d.g[0] = DigestGroup{l.win_a, l.win_s, 0, 0, N, N, nullptr, 0, 1, digest_chunks(2 * N)};
+  w.d.g[1] = l.bank_K ? DigestGroup{l.W, l.H0, l.bank.dict_stride, l.bank.dict_stride, F, 2 * inf, l.bank_K, 0, w.nd, cd}
+                      : DigestGroup{l.W, l.H0, 0, 0, F * K, 2 * K * inf, nullptr, (int)K, 1, cd};
+  w.d.g[2] = DigestGroup{l.ET, nullptr, l.bank.steer_stride, 0, et_words, 0, nullptr, 0, w.ne, digest_chunks(et_words)};
+  w.d.n = 3;
+  int slots = 0;
+  for (const DigestGroup& g : w.d.g) slots += g.count * g.chunks;
+  const int items = 1 + w.nd + w.ne;
   w.chunks = align_up((size_t)count * rt_record_bytes(c, l.P), 256);
-  w.digests = w.chunks + align_up((size_t)total * sizeof(uint64_t), 256);
+  w.digests = w.chunks + align_up((size_t)slots * sizeof(uint64_t), 256);
   w.atoms = w.digests + align_up((size_t)items * sizeof(uint64_t), 256);
   w.bytes = w.atoms + align_up((size_t)items * sizeof(int32_t), 256);
   return w;
 }
 
 int rt_enqueue_digests(gccnmf_handle* h, const RtRecordWork& w, char* workspace, void* stream) {
-  const RtDigestItems& d = w.d;
-  const int total = d.cw + d.nd * d.cd + d.ne * d.ce, items = 1 + d.nd + d.ne;
-  uint64_t* chunks = reinterpret_cast<uint64_t*>(workspace + w.chunks);
-  GCCNMF_LAUNCH(h, rt_digest_chunks_kernel, (total + 127) / 128, 128, 0, stream, d, chunks);
-  GCCNMF_LAUNCH(h, rt_digest_fold_kernel, (items + 127) / 128, 128, 0, stream, d, chunks, reinterpret_cast<uint64_t*>(workspace + w.digests),
-                reinterpret_cast<int32_t*>(workspace + w.atoms));
-  return 0;
+  return record_enqueue_digests(h, w.d, reinterpret_cast<uint64_t*>(workspace + w.chunks), reinterpret_cast<uint64_t*>(workspace + w.digests),
+                                reinterpret_cast<int32_t*>(workspace + w.atoms), stream);
 }
 
 #define RT_RECORD_ARGS_OR_FAIL(what)                                                                                               \
@@ -1593,7 +1484,7 @@ int rt_enqueue_digests(gccnmf_handle* h, const RtRecordWork& w, char* workspace,
   RT_CARVE_OR_FAIL_B(l, S, P, Qd, Qe);                                                                                             \
   GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < S && count <= S - first, what ": slots [%d, %d + %d) outside [0, %d)", first, \
                  first, count, S);                                                                                                 \
-  const RtRecordMap m = rt_record_map(*cfg, P, Qd, Qe);                                                                            \
+  const RecordMap m = rt_record_map(*cfg, P, Qd, Qe);                                                                              \
   const size_t rec_bytes = rt_record_bytes(*cfg, P);                                                                               \
   GCCNMF_REQUIRE(h, record != nullptr && record_bytes >= (size_t)count * rec_bytes, what ": record needs %zu bytes for %d slots",  \
                  (size_t)count * rec_bytes, count);                                                                                \
@@ -1608,8 +1499,8 @@ int rt_save_slots(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, i
   RT_RECORD_ARGS_OR_FAIL("rtrec_save_slots");
   if (int st = rt_enqueue_digests(h, w, ws, stream)) return st;
   GCCNMF_LAUNCH(h, rt_record_copy_kernel, dim3(count, m.n + 1), 256, 0, stream, reinterpret_cast<char*>(l.dev), l.stride, first, m, ws, rec_bytes, 1,
-                rt_record_header(*cfg, P), reinterpret_cast<const uint64_t*>(ws + w.digests), reinterpret_cast<const int32_t*>(ws + w.atoms), w.d.nd,
-                w.d.ne, l.assign);
+                rt_record_header(*cfg, P), reinterpret_cast<const uint64_t*>(ws + w.digests), reinterpret_cast<const int32_t*>(ws + w.atoms), w.nd,
+                w.ne, l.assign);
   GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(record, ws, (size_t)count * rec_bytes, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   return GCCNMF_OK;
 }
@@ -1622,19 +1513,12 @@ int rt_load_slots(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, i
   for (int i = 0; i < count; ++i) {      // the host fields, before the device is touched
     gccnmf_rtrec_header got;
     memcpy(&got, (const char*)record + (size_t)i * rec_bytes, sizeof(got));
-    GCCNMF_REQUIRE(h, got.magic == want.magic, "rtrec_load_slots: record %d: not a stream record (magic 0x%08x)", i, got.magic);
-    GCCNMF_REQUIRE(h, got.abi_version == want.abi_version, "rtrec_load_slots: record %d: ABI version %d, this library is %d", i, got.abi_version,
-                   want.abi_version);
-    GCCNMF_REQUIRE(h, got.kind == want.kind, "rtrec_load_slots: record %d: kind %d is not a real-time slot", i, got.kind);
-    GCCNMF_REQUIRE(h, got.num_sources == P, "rtrec_load_slots: record %d: %d sources, this engine has %d", i, got.num_sources, P);
-    GCCNMF_REQUIRE(h, got.payload_bytes == want.payload_bytes, "rtrec_load_slots: record %d: payload of %llu bytes, expected %llu", i,
-                   (unsigned long long)got.payload_bytes, (unsigned long long)want.payload_bytes);
+    if (int st = record_check_header(h, "rtrec_load_slots", i, &got, &want, offsetof(gccnmf_rtrec_header, config))) return st;
     GCCNMF_REQUIRE(h, got.reserved == 0, "rtrec_load_slots: record %d: reserved word %d", i, got.reserved);
-    GCCNMF_REQUIRE(h, memcmp(got.config, want.config, sizeof(want.config)) == 0, "rtrec_load_slots: record %d: another configuration", i);
   }
   // the destination's digests and K_i, read back once
   if (int st = rt_enqueue_digests(h, w, ws, stream)) return st;
-  const int nd = w.d.nd, ne = w.d.ne, items = 1 + nd + ne;
+  const int nd = w.nd, ne = w.ne, items = 1 + nd + ne;
   uint64_t digest[1 + 2 * kRtMaxBank];
   int32_t atoms[1 + 2 * kRtMaxBank];
   cudaStream_t s = (cudaStream_t)stream;
@@ -1645,14 +1529,10 @@ int rt_load_slots(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, i
     gccnmf_rtrec_header got;
     memcpy(&got, (const char*)record + (size_t)r * rec_bytes, sizeof(got));
     GCCNMF_REQUIRE(h, got.windows_digest == digest[0], "rtrec_load_slots: record %d: other analysis / synthesis windows", r);
-    int di = -1, ej = -1;
-    for (int i = nd - 1; i >= 0; --i)
-      if (digest[1 + i] == got.dictionary_digest && atoms[1 + i] == got.dictionary_atoms) di = i;
-    for (int j = ne - 1; j >= 0; --j)
-      if (digest[1 + nd + j] == got.steering_digest) ej = j;
-    GCCNMF_REQUIRE(h, di >= 0, "rtrec_load_slots: record %d: no dictionary entry of this engine holds its dictionary (%d atoms)", r,
-                   got.dictionary_atoms);
-    GCCNMF_REQUIRE(h, ej >= 0, "rtrec_load_slots: record %d: no steering entry of this engine holds its steering table", r);
+    GCCNMF_REQUIRE(h, record_find_entry(digest + 1, atoms + 1, nd, got.dictionary_digest, got.dictionary_atoms) >= 0,
+                   "rtrec_load_slots: record %d: no dictionary entry of this engine holds its dictionary (%d atoms)", r, got.dictionary_atoms);
+    GCCNMF_REQUIRE(h, record_find_entry(digest + 1 + nd, nullptr, ne, got.steering_digest, 0) >= 0,
+                   "rtrec_load_slots: record %d: no steering entry of this engine holds its steering table", r);
   }
   GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(ws, record, (size_t)count * rec_bytes, cudaMemcpyHostToDevice, s));
   GCCNMF_LAUNCH(h, rt_record_copy_kernel, dim3(count, m.n + 1), 256, 0, stream, reinterpret_cast<char*>(l.dev), l.stride, first, m, ws, rec_bytes, 0,

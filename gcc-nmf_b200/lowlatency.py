@@ -466,25 +466,12 @@ class LowLatencyEngine(object):
         """Bytes of one stream's record."""
         return int(self._rec('record_bytes')())
 
-    def _record_runs(self, streams):
-        """(first, count, first record row) of each run of consecutive stream indexes, in the order given."""
-        idx = self._streams(streams)
-        if len(np.unique(idx)) != len(idx):
-            raise ValueError('a stream is listed twice')
-        row = 0
-        for run in np.split(idx, np.flatnonzero(np.diff(idx) != 1) + 1):
-            yield int(run[0]), len(run), row
-            row += len(run)
-
     def _record_call(self, name, streams, rec):
-        rb = self.record_bytes
-        for first, count, row in self._record_runs(streams):
-            n = int(self._rec('workspace_bytes')(count))
-            if self._staging is None or self._staging.numel() < n:
-                self._staging = self.torch.empty(n, dtype=self.torch.uint8, device=self.h.device)
-            self._check(self._rec(name)(self.state.data_ptr(), self.state_bytes, first, count, rec.data[row].data_ptr(), count * rb,
-                                        self._staging.data_ptr(), self._staging.numel(), self.stream.cuda_stream))
-        self.stream.synchronize()
+        """One library call per run of consecutive streams, then one wait (records.call_runs)."""
+        from .records import call_runs
+        entry = self._rec(name)
+        self._staging = call_runs(lambda *a: self._check(entry(self.state.data_ptr(), self.state_bytes, *a, self.stream.cuda_stream)),
+                                  self._rec('workspace_bytes'), self._streams(streams), rec, self._staging, self.h.device, self.stream)
 
     def save_streams(self, streams=None):
         """The persistent state of `streams` (default: all, in order) between calls -> a StreamRecord, one record per stream.  The

@@ -11,7 +11,7 @@ import ctypes
 import numpy as np
 
 from .._lib import RECORD_KIND_RT, RECORD_MAGIC, ParameterError, RtConfig, RtRecordHeader
-from ..records import StreamRecord, content_digest
+from ..records import StreamRecord, call_runs, content_digest
 
 # the host mirror of a slot's settings, as a record carries it (targetTDOAIndex None travels as NaN)
 PARAM_TYPES = dict(targetTDOAIndex=np.float64, epsilon=np.float64, beta=np.float64, noiseFloor=np.float64, mode=np.int64,
@@ -79,19 +79,13 @@ class SlotRecords(object):
         return int(self.h.lib.gccnmf_rtrec_record_bytes(ctypes.byref(self.cfg), self.P))
 
     def _record_call(self, name, idx, rec):
-        """One library call per run of consecutive slots (in the order of idx), then one wait."""
-        rb = self.record_bytes
-        row = 0
-        for run in np.split(np.asarray(idx), np.flatnonzero(np.diff(idx) != 1) + 1):
-            first, count = int(run[0]), len(run)
-            n = int(self.h.lib.gccnmf_rtrec_workspace_bytes(ctypes.byref(self.cfg), *self._record_dims, count))
-            if getattr(self, '_staging', None) is None or self._staging.numel() < n:
-                self._staging = self.torch.empty(n, dtype=self.torch.uint8, device=self.h.device)
-            self.h.check(getattr(self.h.lib, 'gccnmf_rtrec_' + name)(
-                self.h.h, ctypes.byref(self.cfg), *self._record_dims, self.state.data_ptr(), self.state_bytes, first, count,
-                rec.data[row].data_ptr(), count * rb, self._staging.data_ptr(), self._staging.numel(), self.stream.cuda_stream))
-            row += count
-        self.stream.synchronize()
+        """One library call per run of consecutive slots (in the order of idx), then one wait (records.call_runs)."""
+        lib, cfg, dims = self.h.lib, ctypes.byref(self.cfg), self._record_dims
+        entry = getattr(lib, 'gccnmf_rtrec_' + name)
+        self._staging = call_runs(
+            lambda *a: self.h.check(entry(self.h.h, cfg, *dims, self.state.data_ptr(), self.state_bytes, *a, self.stream.cuda_stream)),
+            lambda count: lib.gccnmf_rtrec_workspace_bytes(cfg, *dims, count), idx, rec, getattr(self, '_staging', None), self.h.device,
+            self.stream)
 
     def _record_slots(self, slots):
         idx = self._slots(list(range(self._record_dims[0])) if slots is None else slots)

@@ -46,6 +46,26 @@ def content_digest(*arrays):
     return int(_fnv_columns(fold.reshape(1, -1))[0])
 
 
+def call_runs(entry, workspace_bytes, idx, rec, staging, device, stream):
+    """Saves or loads the records `rec` of the streams idx (in that order): one call entry(first, count, record, record bytes,
+    staging, staging bytes) per run of consecutive streams, with device staging of workspace_bytes(count) bytes, then one wait
+    on `stream`.  -> the staging buffer, grown when a run needed more, for the next call."""
+    import torch
+    idx = np.asarray(idx)
+    if len(np.unique(idx)) != len(idx):
+        raise ValueError('a stream is listed twice')
+    row, rb = 0, rec.data.shape[1]
+    for run in np.split(idx, np.flatnonzero(np.diff(idx) != 1) + 1):
+        first, count = int(run[0]), len(run)
+        n = int(workspace_bytes(count))
+        if staging is None or staging.numel() < n:
+            staging = torch.empty(n, dtype=torch.uint8, device=device)
+        entry(first, count, rec.data[row].data_ptr(), count * rb, staging.data_ptr(), staging.numel())
+        row += count
+    stream.synchronize()
+    return staging
+
+
 class StreamRecord(object):
     def __init__(self, kind, num_sources, data, mirrors):
         self.kind = int(kind)

@@ -320,3 +320,49 @@ def test_refusals_launch_nothing():
     n = b.h.launches
     assert _load_raw(b, 0, 1, rec.data) == 0                      # and the good record loads
     assert b.h.launches == n + 1
+
+
+def _payload_regions(eng):
+    """Bytes of each region of a stream's record payload, in order (the low-latency carve without history)."""
+    R = (-(-eng.N // eng.hop) - 1) * eng.hop
+    sizes = [24, 8 * eng.D, 4 * 2 * R, 4 * 2 * eng.N * max(eng.P, 1)] + ([32, 32, 4] if eng.P else [])
+    return [b for b in sizes if b]
+
+
+@pytest.mark.parametrize('form', ['llrec-P0', 'llrec-P2', 'llbank'])
+def test_saved_bytes_are_all_defined(form):
+    """A save through the C entry writes every byte of its records: the padding after each payload region, the header past its
+    struct and the record past its payload are zero, whatever the device staging and the host buffer held before, so two saves of
+    the same state are byte-identical."""
+    import torch
+    p = _setup()
+    P = 2 if form == 'llrec-P2' else 0
+    if form == 'llbank':
+        from gcc_nmf_b200 import gccNMFFunctions as fn
+        E2 = fn.getExpJOmegaTau(fn.getFrequenciesInHz(SR, p['N'] // 2 + 1), fn.getTDOAsInSeconds(0.2, p['D']))
+        eng = ll.LowLatencyEngine(p['W'], [p['E'], E2], p['win'], p['syn'], p['hop'], numStreams=3, targetTDOAEpsilon=2.5)
+        head = _lib.LLBankRecordHeader
+    else:
+        eng = _engine(p, 3, P=P)
+        head = _lib.RecordHeader
+    _feed(eng, _audio(3, 12, p['hop']), 0, 12, True)
+    rb, count = eng.record_bytes, 3
+    ws_bytes = int(eng._rec('workspace_bytes')(count))
+    saves = []
+    for staging_fill, host_fill in ((0xFF, 0xAB), (0x00, 0xCD)):
+        ws = torch.full((ws_bytes,), staging_fill, dtype=torch.uint8, device=eng.h.device)
+        rec = torch.full((count, rb), host_fill, dtype=torch.uint8).pin_memory()
+        eng._check(eng._rec('save_streams')(eng.state.data_ptr(), eng.state_bytes, 0, count, rec.data_ptr(), rec.numel(), ws.data_ptr(),
+                                            ws.numel(), eng.stream.cuda_stream))
+        eng.stream.synchronize()
+        saves.append(rec.numpy().copy())
+    assert np.array_equal(saves[0], saves[1])
+    data, H = saves[0], _lib.RECORD_HEADER_BYTES
+    assert not data[:, ctypes.sizeof(head):H].any()                              # the header past its struct
+    at = H
+    for b in _payload_regions(eng):
+        pad = -(-b // 16) * 16
+        assert not data[:, at + b:at + pad].any(), (at - H, b)                # the padding after each region
+        at += pad
+    assert at - H == eng._record_header().payload_bytes
+    assert not data[:, at:].any()                                                 # the record past its payload
