@@ -50,6 +50,8 @@ SIGNATURES = {
     'gccnmf_klnmf': (c_int, [_H, _P, c_int, c_int, _P, _P, c_int, c_int, c_float, c_float, c_int, _P, c_size_t, _S]),
     'gccnmf_klnmf_batched_workspace_bytes': (c_size_t, [c_int, c_int, c_int, c_int]),
     'gccnmf_klnmf_batched': (c_int, [_H, _P, c_int64, c_int64, c_int, c_int, c_int, _P, _P, c_int, c_int, c_float, c_float, c_int, _P, c_size_t, _S]),
+    'gccnmf_klnmf_ragged_workspace_bytes': (c_size_t, [c_int, c_int, _P, c_int]),
+    'gccnmf_klnmf_ragged': (c_int, [_H, _P, _P, _P, c_int, c_int, _P, _P, c_int, c_int, c_float, c_float, c_int, _P, c_size_t, _S]),
     'gccnmf_klnmf_begin': (c_int, [_H, _P, c_int, c_int, _P, _P, c_int, _P, c_size_t, _S]),
     'gccnmf_klnmf_step_numer': (c_int, [_H, _P, c_int, c_int, _P, _P, c_int, c_float, c_float, c_int, _P, _P, c_size_t, _S]),
     'gccnmf_klnmf_step_apply': (c_int, [_H, c_int, c_int, _P, _P, c_int, _P, _P, c_size_t, _S]),
@@ -478,6 +480,30 @@ class Handle(object):
                                                  int(iterations), float(sparsity_alpha), float(epsilon), 1 if update_W else 0, _ptr(ws),
                                                  ws.numel(), self.stream))
         return W, H
+
+    def klnmf_ragged(self, Vs, W, Hs, iterations, sparsity_alpha=0.0, epsilon=1e-16, update_W=True):
+        """B clips of different lengths in one call, in place on W (B, F, K) and Hs[b] (K, T2_b) f32 cuda.  Vs[b] (F, T2_b) f32 cuda may be
+        a strided view (unit stride along T2), e.g. a column range of one STFT output, read in place.  Clip b ends bit-identical to klnmf on
+        it alone."""
+        B = len(Vs)
+        if B < 1 or len(Hs) != B:
+            raise ParameterError('klnmf_ragged: %d V clips and %d H clips' % (B, len(Hs)))
+        F, K = W.shape[1], W.shape[2]
+        for b, (V, H) in enumerate(zip(Vs, Hs)):
+            if not V.is_cuda or V.dim() != 2 or V.stride(1) != 1 or V.shape[0] != F:
+                raise ParameterError('klnmf_ragged: V[%d] must be an (F, T2) cuda tensor with unit stride along T2' % b)
+            if tuple(H.shape) != (K, V.shape[1]) or not H.is_contiguous():
+                raise ParameterError('klnmf_ragged: H[%d] %s does not match V[%d] %s' % (b, tuple(H.shape), b, tuple(V.shape)))
+        if tuple(W.shape) != (B, F, K) or not W.is_contiguous():
+            raise ParameterError('klnmf_ragged: W %s is not a contiguous (%d, %d, %d) stack' % (tuple(W.shape), B, F, K))
+        T2 = (c_int * B)(*[int(V.shape[1]) for V in Vs])
+        Vp = (ctypes.c_void_p * B)(*[V.data_ptr() for V in Vs])
+        ld = (c_int64 * B)(*[V.stride(0) for V in Vs])
+        Hp = (ctypes.c_void_p * B)(*[H.data_ptr() for H in Hs])
+        ws = self.workspace('klnmf_ragged', self.lib.gccnmf_klnmf_ragged_workspace_bytes(B, F, T2, K))
+        self.check(self.lib.gccnmf_klnmf_ragged(self.h, Vp, ld, T2, B, F, _ptr(W), Hp, K, int(iterations), float(sparsity_alpha), float(epsilon),
+                                                1 if update_W else 0, _ptr(ws), ws.numel(), self.stream))
+        return W, Hs
 
     def _klnmf_ws(self, F, T2, K):
         return self.workspace('klnmf', self.lib.gccnmf_klnmf_workspace_bytes(F, T2, K))

@@ -11,6 +11,7 @@
 #include "gemm_simt.cuh"
 
 #include <algorithm>
+#include <vector>
 
 namespace {
 
@@ -237,6 +238,9 @@ int gccnmf_klnmf_tma_prepare(gccnmf_handle* h, const float* V, int64_t ld_v, int
 bool gccnmf_klnmf_tma_batch_supported(gccnmf_handle* h, int F, int T2, int K);
 int gccnmf_klnmf_tma_batched(gccnmf_handle* h, const float* V, int64_t ld_v, int64_t clip_stride_v, int B, int F, int T2, float* W, float* H, int K,
                              int iterations, float alpha, float eps, bool update_W, void* workspace, size_t clip_bytes, void* stream);
+size_t gccnmf_klnmf_tma_ragged_table_per_clip();
+int gccnmf_klnmf_tma_ragged(gccnmf_handle* h, int n, const float* const* V, const int64_t* ld_v, const int* T2, float* const* W, float* const* H,
+                            void* const* ws, int F, int K, int iterations, float alpha, float eps, bool update_W, void* table, void* stream);
 int gccnmf_klnmf_tma_update_H(gccnmf_handle* h, const float* V, int F, int T2, const float* W, float* H, int K, float alpha, float eps,
                               void* workspace, size_t workspace_bytes, int colsum_state, bool pending_norms, void* stream);
 int gccnmf_klnmf_tma_partial_W(gccnmf_handle* h, const float* V, int F, int T2, const float* W, const float* H, int K, void* workspace,
@@ -327,6 +331,25 @@ static size_t batch_clip_bytes(int F, int T2, int K) {
   return std::max(gccnmf_klnmf_workspace_bytes(F, T2, K), simt_workspace_bytes(F, T2, K) + align_up((size_t)F * T2 * sizeof(float), 256));
 }
 constexpr int kMaxBatchClips = 65535 / 8;     // grid z of a batched contraction = clips x k-splits (at most 8)
+
+// A ragged run's workspace: the per-call table (its size depends on B only; 256 bytes of it keep the table 128-byte aligned), then
+// clip b's region of a batched run on its shape, back to back.
+static size_t ragged_table_bytes(int B) { return (size_t)B * gccnmf_klnmf_tma_ragged_table_per_clip() + 256; }
+
+// One clip alone, on its region of a batched or ragged run's workspace: the tensor-core loop, or the float32 SIMT loop on a packed copy
+// of V when its rows are not T2 apart.
+static int klnmf_one_clip(gccnmf_handle* h, const float* V, int64_t ld_v, int F, int T2, float* W, float* H, int K, int iterations, float sparsity_alpha,
+                          float epsilon, int update_W, char* ws, size_t clip_bytes, void* stream) {
+  if (use_tc(h, F, T2, K)) return klnmf_tc(h, V, ld_v, F, T2, W, H, K, iterations, sparsity_alpha, epsilon, update_W, ws, clip_bytes, stream);
+  const size_t simt_bytes = simt_workspace_bytes(F, T2, K);
+  if (ld_v != T2) {
+    float* packed = reinterpret_cast<float*>(ws + simt_bytes);
+    GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync(packed, (size_t)T2 * sizeof(float), V, (size_t)ld_v * sizeof(float), (size_t)T2 * sizeof(float), F,
+                                           cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    V = packed;
+  }
+  return klnmf_simt(h, V, F, T2, W, H, K, iterations, sparsity_alpha, epsilon, update_W, ws, simt_bytes, stream);
+}
 
 extern "C" {
 
@@ -523,29 +546,61 @@ int gccnmf_klnmf_batched(gccnmf_handle* h, const float* V, int64_t ld_v, int64_t
   if (iterations == 0) return GCCNMF_OK;
   char* ws = static_cast<char*>(workspace);
   const int64_t fk = (int64_t)F * K, kt = (int64_t)K * T2;
-  if (use_tc(h, F, T2, K)) {
-    if (gccnmf_klnmf_tma_batch_supported(h, F, T2, K))
-      return gccnmf_klnmf_tma_batched(h, V, ld_v, clip_stride_v, B, F, T2, W, H, K, iterations, sparsity_alpha, epsilon, update_W != 0, workspace,
-                                      clip_bytes, stream);
-    for (int b = 0; b < B; ++b)       // an option the batch form leaves out: the solo path, one clip at a time
-      if (int st = klnmf_tc(h, V + b * clip_stride_v, ld_v, F, T2, W + b * fk, H + b * kt, K, iterations, sparsity_alpha, epsilon, update_W,
-                            ws + b * clip_bytes, clip_bytes, stream)) return st;
-    return GCCNMF_OK;
-  }
-  // float32 SIMT path (tiny or odd shapes, force_simt_nmf), one clip at a time
-  const size_t simt_bytes = simt_workspace_bytes(F, T2, K);
-  for (int b = 0; b < B; ++b) {
-    const float* Vb = V + b * clip_stride_v;
-    if (ld_v != T2) {
-      float* packed = reinterpret_cast<float*>(ws + b * clip_bytes + simt_bytes);
-      GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync(packed, (size_t)T2 * sizeof(float), Vb, (size_t)ld_v * sizeof(float), (size_t)T2 * sizeof(float), F,
-                                             cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-      Vb = packed;
-    }
-    if (int st = klnmf_simt(h, Vb, F, T2, W + b * fk, H + b * kt, K, iterations, sparsity_alpha, epsilon, update_W, ws + b * clip_bytes, simt_bytes,
-                            stream)) return st;
-  }
+  if (use_tc(h, F, T2, K) && gccnmf_klnmf_tma_batch_supported(h, F, T2, K))
+    return gccnmf_klnmf_tma_batched(h, V, ld_v, clip_stride_v, B, F, T2, W, H, K, iterations, sparsity_alpha, epsilon, update_W != 0, workspace,
+                                    clip_bytes, stream);
+  // an option the batch form leaves out, or the float32 SIMT path (tiny or odd shapes, force_simt_nmf): one clip at a time
+  for (int b = 0; b < B; ++b)
+    if (int st = klnmf_one_clip(h, V + b * clip_stride_v, ld_v, F, T2, W + b * fk, H + b * kt, K, iterations, sparsity_alpha, epsilon, update_W,
+                                ws + b * clip_bytes, clip_bytes, stream)) return st;
   return GCCNMF_OK;
+}
+
+size_t gccnmf_klnmf_ragged_workspace_bytes(int B, int F, const int* T2, int K) {
+  if (B < 1 || B > kMaxBatchClips || F <= 0 || K <= 0 || !T2) return 0;
+  size_t n = ragged_table_bytes(B);
+  for (int b = 0; b < B; ++b) {
+    if (T2[b] <= 0) return 0;
+    n += batch_clip_bytes(F, T2[b], K);
+  }
+  return n;
+}
+
+int gccnmf_klnmf_ragged(gccnmf_handle* h, const float* const* V, const int64_t* ld_v, const int* T2, int B, int F, float* W, float* const* H, int K,
+                        int iterations, float sparsity_alpha, float epsilon, int update_W, void* workspace, size_t workspace_bytes, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, B >= 1 && B <= kMaxBatchClips, "klnmf_ragged: B must be 1 .. %d (got %d)", kMaxBatchClips, B);
+  GCCNMF_REQUIRE(h, V && ld_v && T2 && W && H, "klnmf_ragged: NULL V, ld_v, T2, W or H");
+  for (int b = 0; b < B; ++b) {
+    if (int st = check_dims(h, F, T2[b], K)) return st;
+    GCCNMF_REQUIRE(h, V[b] && H[b], "klnmf_ragged: NULL V or H of clip %d", b);
+    GCCNMF_REQUIRE(h, ld_v[b] >= T2[b], "klnmf_ragged: V pitch %lld < T2 %d of clip %d", (long long)ld_v[b], T2[b], b);
+  }
+  GCCNMF_REQUIRE(h, iterations >= 0, "klnmf_ragged: iterations must be >= 0 (got %d)", iterations);
+  const size_t need = gccnmf_klnmf_ragged_workspace_bytes(B, F, T2, K);
+  if (!workspace || workspace_bytes < need) return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "klnmf_ragged workspace too small: need %zu bytes", need);
+  if (iterations == 0) return GCCNMF_OK;
+  char* table = reinterpret_cast<char*>(align_up(reinterpret_cast<uintptr_t>(workspace), 128));
+  char* ws = static_cast<char*>(workspace) + ragged_table_bytes(B);
+  const int64_t fk = (int64_t)F * K;
+  // the clips the tensor-core batch form takes run as one ragged loop; the others one at a time, as gccnmf_klnmf_batched runs them
+  std::vector<const float*> tv;
+  std::vector<int64_t> tld;
+  std::vector<int> tt;
+  std::vector<float*> tw, th;
+  std::vector<void*> tws;
+  for (int b = 0; b < B; ++b) {
+    if (use_tc(h, F, T2[b], K) && gccnmf_klnmf_tma_batch_supported(h, F, T2[b], K)) {
+      tv.push_back(V[b]); tld.push_back(ld_v[b]); tt.push_back(T2[b]); tw.push_back(W + b * fk); th.push_back(H[b]); tws.push_back(ws);
+    } else if (int st = klnmf_one_clip(h, V[b], ld_v[b], F, T2[b], W + b * fk, H[b], K, iterations, sparsity_alpha, epsilon, update_W, ws,
+                                       batch_clip_bytes(F, T2[b], K), stream)) {
+      return st;
+    }
+    ws += batch_clip_bytes(F, T2[b], K);
+  }
+  if (tt.empty()) return GCCNMF_OK;
+  return gccnmf_klnmf_tma_ragged(h, (int)tt.size(), tv.data(), tld.data(), tt.data(), tw.data(), th.data(), tws.data(), F, K, iterations, sparsity_alpha,
+                                 epsilon, update_W != 0, table, stream);
 }
 
 }  // extern "C"

@@ -27,6 +27,7 @@
 // epilogue warps while the main loop runs.
 // Tile widths are chosen per contraction by a cost model over the SM count of the device (make_plan).
 #include <algorithm>
+#include <cstring>
 #include <mutex>
 #include <utility>
 #include <vector>
@@ -48,10 +49,20 @@ constexpr int kApplyTile = 32;
 // ------------------------------------------------------------------------------------------------ epilogues
 // (concept: tma_gemm.cuh)  A warp owns column n; the lane holds rows m .. m + 3, contiguous in every output below.
 // at_offset(bytes): the same functor with every buffer pointer moved `bytes` on (the clip of a batched launch, tgemm::Clips).
+// at_clip(table, c): the same functor with clip c's buffers and length from a ragged run's per-clip table (tgemm::Ragged).
 template <class T>
 __device__ __forceinline__ T* byte_offset(T* p, int64_t bytes) {
   return p ? reinterpret_cast<T*>(reinterpret_cast<typename std::conditional<std::is_const<T>::value, const char, char>::type*>(p) + bytes) : p;
 }
+// One clip of a ragged run (gccnmf_klnmf_ragged), in the call's workspace table: its V, W and H, its own workspace carve, and the
+// k-splits and row-sum slots of its solo plan.
+struct RaggedClip {
+  const float* V; int64_t ld_v; float* W; float* H;
+  float *HT, *VT, *partial, *colsum, *sumsq_part, *rowsum_part;
+  bf16 *HTp, *Wp, *RTp;
+  int64_t plane_ht, plane_rt;
+  int T2, splits, rowsum_slots;
+};
 struct EpiStoreT {   // DT[z][n][m] = acc.  G4 partials (m = atom, n = f) and the test entry.
   struct State {};
   struct Loaded {};
@@ -68,6 +79,7 @@ struct EpiStoreT {   // DT[z][n][m] = acc.  G4 partials (m = atom, n = f) and th
   __device__ void row_total(int, int, float) const {}
   __device__ void elem(int m, int n, float acc, int z) const { DT[(int64_t)z * slab + (int64_t)n * ld + m] = acc; }
   __device__ EpiStoreT at_offset(int64_t bytes) const { EpiStoreT e = *this; e.DT = byte_offset(DT, bytes); return e; }
+  __device__ EpiStoreT at_clip(const void* table, int c) const { EpiStoreT e = *this; e.DT = static_cast<const RaggedClip*>(table)[c].partial; return e; }
   __device__ Loaded load(int, int) const { return Loaded{}; }
   __device__ void store(int m, int n, const float4& acc, const Loaded&, int z, State&) const {
     const int valid = min(4, M - m);
@@ -93,6 +105,13 @@ struct EpiRatioPlanes {   // RT[n][m] = split(VT[n][m] / acc)     G1 / G3 (m = f
     EpiRatioPlanes e;
     e.VT = byte_offset(VT, bytes); e.RT = byte_offset(RT, bytes);
     e.ld = ld; e.plane = plane; e.M = M; e.N = N; e.vec = vec;
+    return e;
+  }
+  __device__ EpiRatioPlanes at_clip(const void* table, int c) const {
+    const RaggedClip& r = static_cast<const RaggedClip*>(table)[c];
+    EpiRatioPlanes e;
+    e.VT = r.VT; e.RT = r.RTp;
+    e.ld = ld; e.plane = r.plane_rt; e.M = M; e.N = r.T2; e.vec = vec;
     return e;
   }
   int64_t operand_ld() const { return ld; }
@@ -137,6 +156,14 @@ struct EpiUpdateH {
     EpiUpdateH e = *this;
     e.HT = byte_offset(HT, bytes); e.HTp = byte_offset(HTp, bytes); e.colsum_part = byte_offset(colsum_part, bytes);
     e.sumsq_part = byte_offset(sumsq_part, bytes); e.rowsum_part = byte_offset(rowsum_part, bytes);
+    return e;
+  }
+  __device__ EpiUpdateH at_clip(const void* table, int c) const {     // (sumsq_part: non-NULL once the W update has left the clip's)
+    const RaggedClip& r = static_cast<const RaggedClip*>(table)[c];
+    EpiUpdateH e = *this;
+    e.HT = r.HT; e.HTp = r.HTp; e.colsum_part = r.colsum;
+    e.sumsq_part = sumsq_part ? r.sumsq_part : nullptr; e.rowsum_part = r.rowsum_part;
+    e.plane = r.plane_ht; e.N = r.T2;
     return e;
   }
   __device__ void row_values(int m, float* v) const {
@@ -617,6 +644,40 @@ __global__ void tma_finish_h_clips_kernel(const float* __restrict__ HT, int T2, 
                                           float* __restrict__ H, int64_t ws_clip_bytes) {
   const int64_t c = blockIdx.z, o = c * ws_clip_bytes;
   finish_h(byte_offset(HT, o), T2, K, byte_offset(sumsq_part, o), row_blocks, H + c * K * T2);
+}
+
+// Ragged forms (gccnmf_klnmf_ragged): the clip is the last grid index, its buffers and length come from the table; a grid sized for
+// the longest clip returns at once in the frame blocks past a shorter clip's end.
+__global__ void tma_prepare_v_ragged_kernel(const RaggedClip* clips, int F, int64_t Fp) {
+  const RaggedClip& c = clips[blockIdx.z];
+  if ((int)blockIdx.x * 32 >= c.T2) return;
+  transpose_split(c.V, F, c.T2, c.ld_v, c.VT, Fp, nullptr, 0, 0);
+}
+__global__ void tma_prepare_h_ragged_kernel(const RaggedClip* clips, int K) {
+  const RaggedClip& c = clips[blockIdx.z];
+  if ((int)blockIdx.x * 32 >= c.T2) return;
+  transpose_split(c.H, K, c.T2, c.T2, c.HT, K, c.HTp, K, c.plane_ht);
+}
+__global__ void tma_split_ragged_kernel(const RaggedClip* clips, int64_t n) {
+  const RaggedClip& c = clips[blockIdx.y];
+  split_planes(c.W, n, c.Wp, n);
+}
+__global__ void tma_colsum_ragged_kernel(const RaggedClip* clips, int F, int K) {
+  const RaggedClip& c = clips[blockIdx.y];
+  column_sums(c.W, F, K, c.colsum);
+}
+__global__ void __launch_bounds__(256) tma_apply_w_ragged_kernel(const RaggedClip* clips, int F, int K) {
+  const RaggedClip& c = clips[blockIdx.z];
+  apply_w<kApplyLocal>(c.W, c.Wp, (int64_t)F * K, c.partial, c.splits, c.rowsum_part, c.rowsum_slots, F, K, c.sumsq_part, c.colsum, nullptr, 0u,
+                       nullptr, PeerSet{});
+}
+__global__ void tma_finish_h_ragged_kernel(const RaggedClip* clips, int K, int row_blocks, int normalise) {
+  const RaggedClip& c = clips[blockIdx.z];
+  if ((int)blockIdx.y * 32 >= c.T2) return;
+  finish_h(c.HT, c.T2, K, normalise ? c.sumsq_part : nullptr, row_blocks, c.H);
+}
+__global__ void tma_finish_w_ragged_kernel(const RaggedClip* clips, int F, int K, int row_blocks) {
+  finish_w(clips[blockIdx.z].W, F, K, clips[blockIdx.z].sumsq_part, row_blocks);
 }
 
 // numer = [sum_z partial[z] (F*K) | sum_s rowsum_part[s] (K)] for the cross-rank sum.
@@ -1251,6 +1312,117 @@ int gccnmf_klnmf_tma_batched(gccnmf_handle* h, const float* V, int64_t ld_v, int
                 update_W ? (const float*)w.sumsq_part : (const float*)nullptr, w.row_blocks, H, cb);
   if (update_W)
     GCCNMF_LAUNCH(h, tma_finish_w_clips_kernel, dim3((K + 127) / 128, std::min(F, 64), B), 128, 0, stream, W, F, K, (const float*)w.sumsq_part, w.row_blocks, cb);
+  return 0;
+}
+
+// ---- ragged runs (gccnmf_klnmf_ragged): n clips of different lengths T2[i], each on its own workspace carve ws[i] and its solo plan.
+// Each plane-GEMM contraction is launched once per distinct tile width among the clips' plans (tgemm::Ragged: a flat grid of the
+// clips' own tiles), every small kernel once for all clips; so each clip computes what gccnmf_klnmf computes on it alone.  The W-update
+// numerator is written as k-split slabs, as in batched runs.  The per-call table (the clips' tensor maps, RaggedClip records and
+// the launches' RaggedTile lists) is built on the host and copied into `table` (kRaggedTablePerClip bytes per clip, 128-byte
+// aligned) by one stream-ordered copy before the first launch.
+constexpr size_t kRaggedTablePerClip = 1280;
+constexpr int kRaggedMaps = 6;              // per clip: A and B of G1 / G3, of G2 and of G4
+static_assert(kRaggedMaps * sizeof(CUtensorMap) + sizeof(RaggedClip) + 3 * sizeof(tgemm::RaggedTile) + 3 * 16 <= kRaggedTablePerClip,
+              "ragged table entry");
+size_t gccnmf_klnmf_tma_ragged_table_per_clip() { return kRaggedTablePerClip; }
+
+int gccnmf_klnmf_tma_ragged(gccnmf_handle* h, int n, const float* const* V, const int64_t* ld_v, const int* T2, float* const* W, float* const* H,
+                            void* const* ws, int F, int K, int iterations, float alpha, float eps, bool update_W, void* table, void* stream) {
+  enum { kWH, kH, kW, kContractions };
+  std::vector<RaggedClip> clips(n);
+  std::vector<CUtensorMap> maps((size_t)n * kRaggedMaps);
+  std::vector<tgemm::RaggedTile> tiles[kContractions];
+  std::vector<int> width[kContractions];
+  const int64_t Fp = (F + 7) & ~7, fk = (int64_t)F * K;
+  const int row_blocks = (F + kApplyTile - 1) / kApplyTile;
+  int max_T2 = 0;
+  unsigned char* dev = static_cast<unsigned char*>(table);
+  const CUtensorMap* maps_d = reinterpret_cast<const CUtensorMap*>(dev);
+  const size_t clips_off = (size_t)n * kRaggedMaps * sizeof(CUtensorMap);
+  const size_t tiles_off = align_up(clips_off + (size_t)n * sizeof(RaggedClip), 16);
+  std::vector<Plan> plans(n);
+  for (int i = 0; i < n; ++i) {
+    const TmaWorkspace w = tma_carve(ws[i], tma_workspace_bytes(F, T2[i], K), F, T2[i], K);
+    const Plan p = plans[i] = make_plan(h, F, T2[i], K);
+    clips[i] = RaggedClip{V[i], ld_v[i], W[i], H[i], w.HT, w.VT, w.partial, w.colsum, w.sumsq_part, w.rowsum_part, w.HTp, w.Wp, w.RTp,
+                          w.plane_ht, w.plane_rt, T2[i], p.w.splits, p.rowsum_slots};
+    max_T2 = std::max(max_T2, T2[i]);
+    const Operand Wk{w.Wp, (int64_t)K, w.plane_w, false}, Wmn{w.Wp, (int64_t)K, w.plane_w, true};
+    const Operand HTk{w.HTp, (int64_t)K, w.plane_ht, false}, HTmn{w.HTp, (int64_t)K, w.plane_ht, true};
+    const Operand RTk{w.RTp, w.Fp, w.plane_rt, false}, RTmn{w.RTp, w.Fp, w.plane_rt, true};
+    CUtensorMap* m = &maps[(size_t)i * kRaggedMaps];
+    if (int st = ragged_maps<false, false>(h, Wk, HTk, F, T2[i], K, p.bn_wh, m)) return st;
+    if (int st = ragged_maps<true, false>(h, Wmn, RTk, K, T2[i], F, p.bn_h, m + 2)) return st;
+    if (int st = ragged_maps<true, true>(h, HTmn, RTmn, K, F, T2[i], p.w.bn, m + 4)) return st;
+    const int kb_k = (K + kKB - 1) / kKB, kb_f = (F + kKB - 1) / kKB, kb_t = (T2[i] + kKB - 1) / kKB;
+    const tgemm::RaggedTile t[kContractions] = {
+        {0, i, T2[i], K, (T2[i] + p.bn_wh - 1) / p.bn_wh, kb_k, maps_d + i * kRaggedMaps, maps_d + i * kRaggedMaps + 1, w.Wp, w.HTp, w.plane_w, w.plane_ht},
+        {0, i, T2[i], F, (T2[i] + p.bn_h - 1) / p.bn_h, kb_f, maps_d + i * kRaggedMaps + 2, maps_d + i * kRaggedMaps + 3, nullptr, nullptr, 0, 0},
+        {0, i, F, T2[i], (F + p.w.bn - 1) / p.w.bn, (kb_t + p.w.splits - 1) / p.w.splits, maps_d + i * kRaggedMaps + 4, maps_d + i * kRaggedMaps + 5,
+         nullptr, nullptr, 0, 0}};
+    const int widths[kContractions] = {p.bn_wh, p.bn_h, p.w.bn};
+    for (int c = 0; c < kContractions; ++c) { tiles[c].push_back(t[c]); width[c].push_back(widths[c]); }
+  }
+  // Each contraction's clips ordered by tile width (stable): one launch per run of equal widths, CTAs numbered along the run.
+  struct Launch { int bn, begin, count, ctas; };
+  std::vector<Launch> launches[kContractions];
+  std::vector<unsigned char> host(tiles_off + (size_t)kContractions * n * sizeof(tgemm::RaggedTile));
+  for (int c = 0; c < kContractions; ++c) {
+    std::vector<int> order(n);
+    for (int i = 0; i < n; ++i) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return width[c][a] < width[c][b]; });
+    const int M = c == kWH ? F : K;
+    tgemm::RaggedTile* out = reinterpret_cast<tgemm::RaggedTile*>(host.data() + tiles_off) + (size_t)c * n;
+    for (int j = 0; j < n; ++j) {
+      const int i = order[j], bn = width[c][i];
+      if (launches[c].empty() || launches[c].back().bn != bn) launches[c].push_back(Launch{bn, j, 0, 0});
+      Launch& l = launches[c].back();
+      tgemm::RaggedTile t = tiles[c][i];
+      t.cta_begin = l.ctas;
+      l.ctas += t.n_tiles * m_tiles_of(M, c == kWH, bn) * (c == kW ? plans[i].w.splits : 1);
+      l.count++;
+      std::memcpy(out + j, &t, sizeof(t));
+    }
+  }
+  std::memcpy(host.data(), maps.data(), maps.size() * sizeof(CUtensorMap));
+  std::memcpy(host.data() + clips_off, clips.data(), clips.size() * sizeof(RaggedClip));
+  GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(table, host.data(), host.size(), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  const RaggedClip* clips_d = reinterpret_cast<const RaggedClip*>(dev + clips_off);
+  const tgemm::RaggedTile* tiles_d = reinterpret_cast<const tgemm::RaggedTile*>(dev + tiles_off);
+
+  const dim3 block(32, 8);
+  GCCNMF_LAUNCH(h, tma_prepare_v_ragged_kernel, dim3((max_T2 + 31) / 32, (unsigned)((Fp + 31) / 32), n), block, 0, stream, clips_d, F, Fp);
+  GCCNMF_LAUNCH(h, tma_split_ragged_kernel, dim3((unsigned)((fk + 255) / 256), n), 256, 0, stream, clips_d, fk);
+  GCCNMF_LAUNCH(h, tma_prepare_h_ragged_kernel, dim3((max_T2 + 31) / 32, (K + 31) / 32, n), block, 0, stream, clips_d, K);
+  auto contraction = [&](int c, auto epi, auto launch) -> int {
+    for (const Launch& l : launches[c]) {
+      epi.tiles = tiles_d + (size_t)c * n + l.begin;
+      epi.count = l.count;
+      if (int st = launch(l.bn, l.ctas, epi)) return st;
+    }
+    return 0;
+  };
+  const tgemm::Ragged<EpiRatioPlanes> ratio{EpiRatioPlanes{nullptr, nullptr, Fp, 0, F, 0, true}, nullptr, 0, clips_d};
+  const tgemm::Ragged<EpiStoreT> numer{EpiStoreT{nullptr, (int64_t)K, fk, K, F, true, h->gemm_streaming != 0}, nullptr, 0, clips_d};
+  auto wh = [&](int bn, int ctas, const tgemm::Ragged<EpiRatioPlanes>& e) { return plane_gemm_ragged<false, false>(h, bn, F, ctas, true, K, K, e, stream); };
+  auto upd_h = [&](int bn, int ctas, const tgemm::Ragged<EpiUpdateH>& e) { return plane_gemm_ragged<true, false>(h, bn, K, ctas, false, 0, 0, e, stream); };
+  auto num_w = [&](int bn, int ctas, const tgemm::Ragged<EpiStoreT>& e) { return plane_gemm_ragged<true, true>(h, bn, K, ctas, false, 0, 0, e, stream); };
+  for (int it = 0; it < iterations; ++it) {
+    const int colsum_state = it == 0 ? 0 : (update_W ? 2 : 1);     // (as in gccnmf_klnmf_tma_batched)
+    if (int st = contraction(kWH, ratio, wh)) return st;                                                               // G1
+    if (colsum_state == 0) GCCNMF_LAUNCH(h, tma_colsum_ragged_kernel, dim3((K + 127) / 128, n), 128, 0, stream, clips_d, F, K);
+    const tgemm::Ragged<EpiUpdateH> upd{EpiUpdateH{nullptr, nullptr, nullptr, colsum_state == 2 ? clips[0].sumsq_part : nullptr, nullptr, alpha, eps,
+                                                   (int64_t)K, 0, K, 0, colsum_state == 2 ? row_blocks : 1, true}, nullptr, 0, clips_d};
+    if (int st = contraction(kH, upd, upd_h)) return st;                                                               // G2
+    if (!update_W) continue;
+    if (int st = contraction(kWH, ratio, wh)) return st;                                                               // G3
+    if (int st = contraction(kW, numer, num_w)) return st;                                                             // G4
+    if (int st = launch_ex(h, "tma_apply_w_ragged_kernel", tma_apply_w_ragged_kernel, dim3((K + kApplyAtoms - 1) / kApplyAtoms, row_blocks, n), block, 0,
+                           stream, h->nmf_pdl, dim3(1, 1, 1), clips_d, F, K)) return st;
+  }
+  GCCNMF_LAUNCH(h, tma_finish_h_ragged_kernel, dim3((K + 31) / 32, (max_T2 + 31) / 32, n), block, 0, stream, clips_d, K, row_blocks, update_W ? 1 : 0);
+  if (update_W) GCCNMF_LAUNCH(h, tma_finish_w_ragged_kernel, dim3((K + 127) / 128, std::min(F, 64), n), 128, 0, stream, clips_d, F, K, row_blocks);
   return 0;
 }
 

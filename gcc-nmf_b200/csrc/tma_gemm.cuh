@@ -297,6 +297,67 @@ template <class E> __device__ __forceinline__ int split_of(const E&) { return bl
 template <class E> __device__ __forceinline__ int split_of(const Clips<E>& c) { return (int)blockIdx.z % c.splits; }
 template <class E> __device__ __forceinline__ int64_t clip_offset(const E&, int) { return 0; }
 template <class E> __device__ __forceinline__ int64_t clip_offset(const Clips<E>& c, int clip) { return c.clip_bytes * clip; }
+// Ragged launch of a by-column epilogue E over clips of different lengths that share one tile width: the grid is flat, the
+// concatenation of each clip's own (n tiles x m tiles x splits) CTAs, so a short clip launches only its own tiles.  A CTA finds its
+// clip in `tiles` (sorted by cta_begin) and takes from it everything that differs between clips: the extents N and Kc, the k-split
+// ranges, the clip's own operand tensor maps (encoded on the host with the clip's exact extents, so TMA zero-fills its edges exactly as
+// in a solo launch, and read through their global address) and the SIMT-tail operands.  The functor it runs is
+// E::at_clip(clips, clip): E with the clip's buffers and lengths from the functor's per-clip table.  1 x 1 clusters, k-splits as
+// slabs, epilogue operands from global memory, as in Clips.  A separate instantiation of plane_gemm_kernel.
+struct RaggedTile {
+  int cta_begin;                 // first CTA of the clip in the flat grid
+  int clip;                      // index into the functor's per-clip table
+  int N, Kc, n_tiles, kblocks_per_split;
+  const CUtensorMap* map_a;      // in global memory
+  const CUtensorMap* map_b;
+  const __nv_bfloat16* tail_a;   // SIMT tail rows: the clip's A and B planes and plane strides (lda, ldb are the launch's)
+  const __nv_bfloat16* tail_b;
+  int64_t a_plane, b_plane;
+};
+template <class E>
+struct Ragged {
+  static constexpr bool kRowReduce = E::kRowReduce;
+  static constexpr int kRowValues = E::kRowValues;
+  static constexpr bool kPrefetch = E::kPrefetch;
+  static constexpr bool kDualN = wants_dual_n<E>::value;
+  static constexpr bool kPreloadOperands = wants_preload<E>::value;
+  using State = typename E::State;
+  using Loaded = typename E::Loaded;
+  E e;                           // the fields every clip shares
+  const RaggedTile* tiles;
+  int count;
+  const void* clips;             // the functor's per-clip table
+};
+template <class E>
+struct is_ragged { static constexpr bool value = false; };
+template <class E>
+struct is_ragged<Ragged<E>> { static constexpr bool value = true; };
+
+// Index of the entry of `tiles` that holds this CTA: a 32-way search by warp 0 (three rounds of loads for 8191 clips), published
+// to the CTA through shared memory.  Called by every thread.
+__device__ __forceinline__ int ragged_find(const RaggedTile* tiles, int count) {
+  __shared__ int found;
+  if (threadIdx.x < 32) {
+    const int me = (int)blockIdx.x;
+    int lo = 0, hi = count;                   // tiles[lo].cta_begin <= me < tiles[hi].cta_begin
+    while (hi - lo > 1) {
+      const int step = (hi - lo + 31) / 32;
+      const int i = lo + (int)threadIdx.x * step;
+      const unsigned le = __ballot_sync(0xffffffffu, i < hi && tiles[i].cta_begin <= me);
+      lo += (31 - __clz(le)) * step;          // (lane 0 always qualifies)
+      hi = min(hi, lo + step);
+    }
+    if (threadIdx.x == 0) found = lo;
+  }
+  __syncthreads();
+  return found;
+}
+// A tensor map written to global memory by a copy before the launch is read by the tensormap proxy: acquire it first.
+__device__ __forceinline__ void tensormap_acquire(const CUtensorMap* map) {
+  asm volatile("fence.proxy.tensormap::generic.acquire.sys [%0], 128;" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
+}
+template <class E> __device__ __forceinline__ E clip_epilogue(const Ragged<E>& r, int clip) { return r.e.at_clip(r.clips, clip); }
+
 template <bool BATCHED, bool MULTICAST>
 __device__ __forceinline__ void tma_load_operand(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int clip, uint16_t mask) {
   if constexpr (BATCHED) tma_load_4d(dst, map, bar, c0, c1, c2, clip);
@@ -322,7 +383,8 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   constexpr bool OPERAND = C::kOperandBytes > 0;     // the epilogue's operand tile comes into shared memory by TMA
   constexpr int kCluster = CN * CM;
   constexpr bool BATCHED = is_batched<Epilogue>::value;
-  static_assert(!BATCHED || kCluster == 1, "a batched launch runs 1 x 1 clusters");
+  constexpr bool RAGGED = is_ragged<Epilogue>::value;
+  static_assert((!BATCHED && !RAGGED) || kCluster == 1, "a batched or ragged launch runs 1 x 1 clusters");
   static_assert((CN == 1 || CN == 2) && (CM == 1 || CM == 2), "cluster of CN n-tiles x CM m-tiles");
   static_assert(A_MN || (kBM / CN) % 8 == 0, "A row slices keep the swizzle atoms whole");
   static_assert(B_MN || (BN / CM) % 8 == 0, "B row slices keep the swizzle atoms whole");
@@ -331,15 +393,31 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const bool mf = args.m_fastest != 0;
-  const int tile_n = mf ? (int)blockIdx.y : (int)blockIdx.x;
-  const int tile_m = mf ? (int)blockIdx.x : (int)blockIdx.y;
-  const int z = split_of(epi);
-  const int clip = clip_of(epi);
+  // my tile, k-split and clip, and the extents, k-split length and operand maps of my clip
+  int tile_n, tile_m, z, clip, N = args.N, Kc = args.Kc, kblocks_per_split = args.kblocks_per_split;
+  const CUtensorMap* tmap_a = &map_a;
+  const CUtensorMap* tmap_b = &map_b;
+  const RaggedTile* rt = nullptr;
+  if constexpr (RAGGED) {
+    rt = epi.tiles + ragged_find(epi.tiles, epi.count);
+    const int local = (int)blockIdx.x - rt->cta_begin, per_split = rt->n_tiles * args.m_tiles;
+    tile_n = local % rt->n_tiles;
+    tile_m = (local % per_split) / rt->n_tiles;
+    z = local / per_split;
+    clip = rt->clip;
+    N = rt->N; Kc = rt->Kc; kblocks_per_split = rt->kblocks_per_split;
+    tmap_a = rt->map_a; tmap_b = rt->map_b;
+  } else {
+    tile_n = mf ? (int)blockIdx.y : (int)blockIdx.x;
+    tile_m = mf ? (int)blockIdx.x : (int)blockIdx.y;
+    z = split_of(epi);
+    clip = clip_of(epi);
+  }
   auto&& ep = clip_epilogue(epi, clip);     // the functor of my clip
   const int n0 = tile_n * BN;
-  const int total_kblocks = (args.Kc + KB - 1) / KB;
-  const int kb_begin = z * args.kblocks_per_split;
-  const int kb_end = min(total_kblocks, kb_begin + args.kblocks_per_split);
+  const int total_kblocks = (Kc + KB - 1) / KB;
+  const int kb_begin = z * kblocks_per_split;
+  const int kb_end = min(total_kblocks, kb_begin + kblocks_per_split);
   const int num_kb = max(0, kb_end - kb_begin);
   // position inside the cluster (x = n tile, y = m tile); rank = x + CN y (%cluster_ctarank)
   const int cx = (!mf && CN > 1) ? (int)(blockIdx.x % CN) : 0;     // (the m-fastest grid is used with CN == 1 only)
@@ -372,8 +450,12 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     }
     if constexpr (OPERAND) mbar_init(smem_u32(operand_full), 1);
     gmma::fence_barrier_init();
-    tma_prefetch_descriptor(&map_a);
-    tma_prefetch_descriptor(&map_b);
+    if constexpr (RAGGED) {
+      tensormap_acquire(tmap_a);
+      tensormap_acquire(tmap_b);
+    }
+    tma_prefetch_descriptor(tmap_a);
+    tma_prefetch_descriptor(tmap_b);
     if constexpr (OPERAND) tma_prefetch_descriptor(&epi.operand_map);
   }
   if (kCluster > 1) cluster_sync();     // no peer may signal my barriers or write my stages before they are initialised
@@ -395,7 +477,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   auto preload = [&]() {
     if constexpr (kPre > 0) {
       if (!args.preload) return;
-      const int n_valid = min(BN, args.N - n0);
+      const int n_valid = min(BN, N - n0);
 #pragma unroll
       for (int u = 0; u < kPre; ++u) {
         const int cc = warp + kWarpsAll * u;
@@ -418,22 +500,22 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         if (A_MN) {
 #pragma unroll
           for (int a = 0; a < C::kAAtoms; ++a)
-            if (a % CN == cx) tma_load_operand<BATCHED, (CN > 1)>(a_dst + a * C::kAtomBytes, &map_a, bar, m0 + 64 * a, k0, 0, clip, mask_row);
+            if (a % CN == cx) tma_load_operand<BATCHED, (CN > 1)>(a_dst + a * C::kAtomBytes, tmap_a, bar, m0 + 64 * a, k0, 0, clip, mask_row);
         } else {
           constexpr int kRows = kBM / CN;      // my row slice of the A tile, one box per plane
 #pragma unroll
           for (int p = 0; p < 2; ++p)
-            tma_load_operand<BATCHED, (CN > 1)>(a_dst + p * (kBM * KB * 2) + cx * (kRows * KB * 2), &map_a, bar, k0, m0 + cx * kRows, p, clip, mask_row);
+            tma_load_operand<BATCHED, (CN > 1)>(a_dst + p * (kBM * KB * 2) + cx * (kRows * KB * 2), tmap_a, bar, k0, m0 + cx * kRows, p, clip, mask_row);
         }
         if (B_MN) {
 #pragma unroll
           for (int a = 0; a < C::kBAtoms; ++a)
-            if (a % CM == cy) tma_load_operand<BATCHED, (CM > 1)>(b_dst + a * C::kAtomBytes, &map_b, bar, n0 + 64 * a, k0, 0, clip, mask_col);
+            if (a % CM == cy) tma_load_operand<BATCHED, (CM > 1)>(b_dst + a * C::kAtomBytes, tmap_b, bar, n0 + 64 * a, k0, 0, clip, mask_col);
         } else {
           constexpr int kRows = BN / CM;
 #pragma unroll
           for (int p = 0; p < 2; ++p)
-            tma_load_operand<BATCHED, (CM > 1)>(b_dst + p * (BN * KB * 2) + cy * (kRows * KB * 2), &map_b, bar, k0, n0 + cy * kRows, p, clip, mask_col);
+            tma_load_operand<BATCHED, (CM > 1)>(b_dst + p * (BN * KB * 2) + cy * (kRows * KB * 2), tmap_b, bar, k0, n0 + cy * kRows, p, clip, mask_col);
         }
       }
       if constexpr (OPERAND) {
@@ -460,7 +542,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     if (Epilogue::kPrefetch) {
       // pull the epilogue's global operands of this tile towards L2 while the main loop runs (they were last touched an
       // iteration ago and have partly been evicted to HBM since): one prefetch per 128-byte line, 4 lines per column
-      const int n_valid = min(BN, args.N - n0);
+      const int n_valid = min(BN, N - n0);
       if ((lane & 7) == 0)
         for (int c = e; c < n_valid; c += kAuxWarps) ep.prefetch(m0 + 4 * lane, n0 + c);
     }
@@ -472,16 +554,21 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       // (k-splits summed inside a cluster, z_cluster > 1: the functor is not linear in the accumulator, so the tail rows are computed
       // over the WHOLE contraction, each split taking its share of the tile's tail columns)
       const bool z_red = kCluster == 1 && args.z_cluster > 1;
-      const int k_begin = z_red ? 0 : kb_begin * KB, k_end = z_red ? args.Kc : min(args.Kc, kb_end * KB);
+      const int k_begin = z_red ? 0 : kb_begin * KB, k_end = z_red ? Kc : min(Kc, kb_end * KB);
       const int tcols = z_red ? (((args.tail_cols + args.z_cluster - 1) / args.z_cluster) + 1) & ~1 : args.tail_cols;
       const int c_begin = n0 + (z_red ? tile_m * args.z_cluster + z : tile_m) * tcols;
-      const int c_end = min(min(args.N, n0 + BN), c_begin + tcols);
+      const int c_end = min(min(N, n0 + BN), c_begin + tcols);
       constexpr int kRound = 32 * kAuxWarps;             // columns per round: 16 steps of 2 columns per warp
       const __nv_bfloat16* tail_a = reinterpret_cast<const __nv_bfloat16*>(reinterpret_cast<const char*>(args.A) + clip_offset(epi, clip));
       const __nv_bfloat16* tail_b = reinterpret_cast<const __nv_bfloat16*>(reinterpret_cast<const char*>(args.B) + clip_offset(epi, clip));
+      int64_t a_plane = args.a_plane, b_plane = args.b_plane;
+      if constexpr (RAGGED) {
+        tail_a = rt->tail_a; tail_b = rt->tail_b;
+        a_plane = rt->a_plane; b_plane = rt->b_plane;
+      }
       for (int m = args.m_tiles * kBM; m < args.M; ++m) {
         const __nv_bfloat16* a_hi = tail_a + (int64_t)m * args.lda;
-        const __nv_bfloat16* a_lo = a_hi + args.a_plane;
+        const __nv_bfloat16* a_lo = a_hi + a_plane;
 #pragma unroll 1
         for (int c_round = c_begin; c_round < c_end; c_round += kRound) {
           float keep = 0.f;
@@ -491,7 +578,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
             if (n >= c_end) break;
             const bool two = n + 1 < c_end;
             const __nv_bfloat16* b_hi = tail_b + (int64_t)n * args.ldb;
-            const __nv_bfloat16* b_lo = b_hi + args.b_plane;
+            const __nv_bfloat16* b_lo = b_hi + b_plane;
             const int64_t next = two ? args.ldb : 0;
             float acc0 = 0.f, acc1 = 0.f;
 #pragma unroll 4
@@ -583,7 +670,7 @@ plane_gemm_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     const int m_first = m0 + 4 * lane;
     typename Epilogue::State st;
     ep.init(st, m_first, rowvals + 4 * lane);
-    int n_valid = min(BN, args.N - n0);
+    int n_valid = min(BN, N - n0);
     constexpr int U = kColumnsInFlight;
     int c_first = warp;
     if constexpr (OPERAND) mbar_wait(smem_u32(operand_full), 0);

@@ -60,25 +60,31 @@ namespace tgemm_host {
 // Tensor map over a plane pair [2][rows][pitch] of bf16: dims (inner, rows, 2), box (box_inner, box_rows, box_planes).
 // box_inner * 2 bytes = 64 -> SWIZZLE_64B (K-major k-blocks of 32), 128 -> SWIZZLE_128B (MN-major atoms of 64).
 // clips > 0: `clips` such pairs clip_bytes apart, dims (inner, rows, 2, clips), box of one clip.
+// encode_tmap encodes the map of `key` (byte strides); get_tmap looks it up in the handle's cache first.
+inline int encode_tmap(gccnmf_handle* h, const TmapKey& key, CUtensorMap* out) {
+  EncodeTiledFn encode = encode_tiled_fn();
+  if (!encode) return gccnmf_fail(h, GCCNMF_ERR_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
+  if ((reinterpret_cast<uintptr_t>(key.base) & 15) || (key.pitch_bytes & 15) || (key.plane_bytes & 15) || (key.clip_bytes & 15))
+    return gccnmf_fail(h, GCCNMF_ERR_INVALID_ARGUMENT, "tensor map: base / pitch / plane / clip stride must be 16-byte aligned");
+  const cuuint64_t dims[4] = {key.inner, key.rows, 2, key.clips};
+  const cuuint64_t strides[3] = {key.pitch_bytes, key.plane_bytes, key.clip_bytes};
+  const cuuint32_t box[4] = {key.box_inner, key.box_rows, key.box_planes, 1};
+  const cuuint32_t elem_strides[4] = {1, 1, 1, 1};
+  const CUtensorMapSwizzle swz = (key.box_inner * 2 == 128) ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+  const CUresult r = encode(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, key.clips ? 4 : 3, const_cast<void*>(key.base), dims, strides, box, elem_strides,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return gccnmf_fail(h, GCCNMF_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
+  return 0;
+}
+
 inline int get_tmap(gccnmf_handle* h, const bf16* base, uint64_t inner, uint64_t rows, uint64_t pitch_elems, uint64_t plane_elems,
              uint32_t box_inner, uint32_t box_rows, uint32_t box_planes, CUtensorMap* out, uint64_t clips = 0, uint64_t clip_bytes = 0) {
   if (!h->tmaps) h->tmaps = new gccnmf_tmap_cache();
   const TmapKey key{base, inner, rows, pitch_elems * 2, plane_elems * 2, box_inner, box_rows, box_planes, clips, clips ? clip_bytes : 0};
   for (auto& e : h->tmaps->entries)
     if (e.first == key) { *out = e.second; return 0; }
-  EncodeTiledFn encode = encode_tiled_fn();
-  if (!encode) return gccnmf_fail(h, GCCNMF_ERR_CUDA, "cuTensorMapEncodeTiled is not available from the driver");
-  if ((reinterpret_cast<uintptr_t>(base) & 15) || (key.pitch_bytes & 15) || (key.plane_bytes & 15) || (key.clip_bytes & 15))
-    return gccnmf_fail(h, GCCNMF_ERR_INVALID_ARGUMENT, "tensor map: base / pitch / plane / clip stride must be 16-byte aligned");
-  const cuuint64_t dims[4] = {inner, rows, 2, clips};
-  const cuuint64_t strides[3] = {key.pitch_bytes, key.plane_bytes, key.clip_bytes};
-  const cuuint32_t box[4] = {box_inner, box_rows, box_planes, 1};
-  const cuuint32_t elem_strides[4] = {1, 1, 1, 1};
-  const CUtensorMapSwizzle swz = (box_inner * 2 == 128) ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   CUtensorMap m;
-  const CUresult r = encode(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, clips ? 4 : 3, const_cast<bf16*>(base), dims, strides, box, elem_strides,
-                            CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return gccnmf_fail(h, GCCNMF_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
+  if (int st = encode_tmap(h, key, &m)) return st;
   if (h->tmaps->entries.size() > 256) h->tmaps->entries.clear();
   h->tmaps->entries.emplace_back(key, m);
   *out = m;
@@ -431,6 +437,57 @@ int plane_gemm_clips(gccnmf_handle* h, int bn, const Operand& A, const Operand& 
     case 256: return launch_plane_gemm_clips<256, A_MN, B_MN>(h, A, B, M, N, Kc, splits, simt_tail, epi, clips, stream);
   }
   return gccnmf_fail(h, GCCNMF_ERR_UNSUPPORTED, "plane gemm (batched): tile width %d", bn);
+}
+
+// Ragged launches (tgemm::Ragged).  ragged_maps encodes the two operand maps of one clip as launch() encodes them for a 1 x 1
+// cluster of `bn`-column tiles, with the clip's own extents; the caller copies them into the launch's table.
+template <bool A_MN, bool B_MN>
+int ragged_maps(gccnmf_handle* h, const Operand& A, const Operand& B, int M, int N, int Kc, int bn, CUtensorMap* out) {
+  auto key = [](const Operand& o, bool mn, int rows, int kc, uint32_t box_rows) {
+    return mn ? TmapKey{o.planes, (uint64_t)rows, (uint64_t)kc, (uint64_t)o.pitch * 2, (uint64_t)o.plane * 2, 64, kKB, 2, 0, 0}
+              : TmapKey{o.planes, (uint64_t)kc, (uint64_t)rows, (uint64_t)o.pitch * 2, (uint64_t)o.plane * 2, kKB, box_rows, 1, 0, 0};
+  };
+  if (int st = encode_tmap(h, key(A, A_MN, M, Kc, tgemm::kBM), &out[0])) return st;
+  return encode_tmap(h, key(B, B_MN, N, Kc, (uint32_t)bn), &out[1]);
+}
+// One launch of `bn`-column tiles over the clips of epi.tiles (ctas = the sum of their tiles x splits); M, the SIMT tail rule and
+// the tail operands' row pitches are the launch's.
+template <int BN, bool A_MN, bool B_MN, class Epi>
+int launch_plane_gemm_ragged(gccnmf_handle* h, int M, int ctas, bool simt_tail, int64_t lda, int64_t ldb, const tgemm::Ragged<Epi>& epi, void* stream) {
+  using I = PlaneGemmInstance<BN, A_MN, B_MN, 1, 1, tgemm::Ragged<Epi>>;
+  int unused;
+  if (int st = I::max_clusters(h, &unused)) return st;     // (sets the shared-memory attribute on first use)
+  const int tail = M % tgemm::kBM;
+  const bool use_tail = simt_tail && !A_MN && !B_MN && tail != 0 && tail <= kTailRowsMax && M > tgemm::kBM && (M / tgemm::kBM) * 128 >= BN;
+  PlaneGemmArgs args{};
+  args.M = M;
+  args.m_tiles = use_tail ? M / tgemm::kBM : (M + tgemm::kBM - 1) / tgemm::kBM;
+  args.tail_rows = use_tail ? tail : 0;
+  args.tail_cols = (((BN + args.m_tiles - 1) / args.m_tiles) + 1) & ~1;
+  args.lda = lda;
+  args.ldb = ldb;
+  args.preload = h->gemm_preload & 1;
+  const CUtensorMap none{};         // (the maps come from the table)
+  return launch_ex(h, "plane_gemm_kernel", tgemm::plane_gemm_kernel<BN, kKB, A_MN, B_MN, 1, 1, tgemm::Ragged<Epi>>, dim3(ctas), dim3(tgemm::kThreads),
+                   (size_t)I::C::kTotal, stream, h->nmf_pdl, dim3(1, 1, 1), none, none, args, epi);
+}
+template <bool A_MN, bool B_MN, class Epi>
+int plane_gemm_ragged(gccnmf_handle* h, int bn, int M, int ctas, bool simt_tail, int64_t lda, int64_t ldb, const tgemm::Ragged<Epi>& epi, void* stream) {
+  switch (bn) {
+    case 104:
+      if constexpr (tgemm::wants_dual_n<Epi>::value && !B_MN) return launch_plane_gemm_ragged<104, A_MN, B_MN>(h, M, ctas, simt_tail, lda, ldb, epi, stream);
+      break;
+    case 120:
+      if constexpr (tgemm::wants_dual_n<Epi>::value && !B_MN) return launch_plane_gemm_ragged<120, A_MN, B_MN>(h, M, ctas, simt_tail, lda, ldb, epi, stream);
+      break;
+    case 112: return launch_plane_gemm_ragged<112, A_MN, B_MN>(h, M, ctas, simt_tail, lda, ldb, epi, stream);
+    case 128: return launch_plane_gemm_ragged<128, A_MN, B_MN>(h, M, ctas, simt_tail, lda, ldb, epi, stream);
+    case 176: return launch_plane_gemm_ragged<176, A_MN, B_MN>(h, M, ctas, simt_tail, lda, ldb, epi, stream);
+    case 208: return launch_plane_gemm_ragged<208, A_MN, B_MN>(h, M, ctas, simt_tail, lda, ldb, epi, stream);
+    case 240: return launch_plane_gemm_ragged<240, A_MN, B_MN>(h, M, ctas, simt_tail, lda, ldb, epi, stream);
+    case 256: return launch_plane_gemm_ragged<256, A_MN, B_MN>(h, M, ctas, simt_tail, lda, ldb, epi, stream);
+  }
+  return gccnmf_fail(h, GCCNMF_ERR_UNSUPPORTED, "plane gemm (ragged): tile width %d", bn);
 }
 
 // k-splits reduced inside (1, 1, splits) clusters (no slabs): query how many such clusters are resident at once / launch.

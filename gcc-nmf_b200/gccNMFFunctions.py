@@ -89,8 +89,22 @@ def performKLNMF(V, dictionarySize, numIterations, sparsityAlpha, epsilon=1e-16,
 
 
 def performKLNMFBatch(Vs, dictionarySize, numIterations, sparsityAlpha, epsilon=1e-16, seedValue=0):
-    """performKLNMF on B equal-shape clips in one batched call: Vs (B, F, T2) -> W (B, F, K), H (B, K, T2), clip b equal to
-    performKLNMF(Vs[b], ...).  The reference re-seeds on every call, so every clip starts from the same draw: drawn once here."""
+    """performKLNMF on B clips in one batched call, clip b equal to performKLNMF(Vs[b], ...).  Vs (B, F, T2) -> W (B, F, K),
+    H (B, K, T2); a list of (F, T2_b) arrays of any lengths -> W (B, F, K), [H_b (K, T2_b)].  The reference re-seeds on every call,
+    so every clip starts from the same draw: drawn once here.  W0 does not depend on T2 and H0 for T2 frames is the first K T2
+    values drawn after W0, so one draw at the longest clip serves every clip of a list."""
+    if isinstance(Vs, (list, tuple)):
+        Vs = [np.asarray(V) for V in Vs]
+        if not Vs or any(V.ndim != 2 or V.shape[0] != Vs[0].shape[0] for V in Vs):
+            raise ParameterError('performKLNMFBatch: Vs must be a non-empty list of (F, T2_b) arrays of one F')
+        F, K = Vs[0].shape[0], dictionarySize
+        W0, Hmax = _seededInit(F, max(V.shape[1] for V in Vs), K, epsilon, seedValue)
+        h = default_handle()
+        W = h.to_device(np.ascontiguousarray(np.broadcast_to(W0, (len(Vs),) + W0.shape)))
+        Hs = [h.to_device(np.ascontiguousarray(Hmax.reshape(-1)[:K * V.shape[1]].reshape(K, V.shape[1]))) for V in Vs]
+        h.klnmf_ragged([h.to_device(np.ascontiguousarray(V, dtype=np.float32)) for V in Vs], W, Hs, numIterations, sparsityAlpha, epsilon,
+                       update_W=True)
+        return W.cpu().numpy(), [H.cpu().numpy() for H in Hs]
     Vs = np.asarray(Vs)
     if Vs.ndim != 3:
         raise ParameterError('performKLNMFBatch: Vs must be (B, F, T2), got shape %s' % (Vs.shape,))

@@ -56,14 +56,16 @@ class GCCNMFPipeline(object):
         return 1 + (numSamples - self.N) // self.hop
 
     def nmf_init(self, T2):
-        """Seeded initial (W0, H0) on the device, drawn once per shape (gccNMFFunctions.py:70-73)."""
-        key = (self.F, T2, self.K, self.seed, self.eps)
-        if key not in self._init:
-            while len(self._init) >= 2:                 # clips of varying length: keep the two most recent shapes
-                self._init.pop(next(iter(self._init)))
+        """Seeded initial (W0, H0) on the device (gccNMFFunctions.py:70-73).  W0 does not depend on T2, and H0 for T2 frames is the
+        first K T2 values the seeded stream draws after W0, so one draw at the longest T2 seen so far serves every shorter clip:
+        clips of any mix of lengths never redraw it."""
+        key = (self.F, self.K, self.seed, self.eps)
+        entry = self._init.get(key)
+        if entry is None or entry[2] < T2:
             W0, H0 = fn._seededInit(self.F, T2, self.K, self.eps, self.seed)
-            self._init[key] = (self.h.to_device(W0), self.h.to_device(H0))
-        return self._init[key]
+            entry = (self.h.to_device(W0), self.h.to_device(H0).reshape(-1), T2)
+            self._init = {key: entry}
+        return entry[0], entry[1][:self.K * T2].view(self.K, T2)
 
     # ------------------------------------------------------------------ timing hooks
     def _mark(self, name):
@@ -108,37 +110,65 @@ class GCCNMFPipeline(object):
     def _front_batch(self, samples):
         """_front for B clips (B, 2, n): the STFT of each clip into one (2B, F, T) spectrogram and one (B, F, 2T) V stack (the
         STFT entry takes one stereo pair per call), the angular spectrum per clip with one event for all B means, one batched
-        KL-NMF over the stack.  Returns one _front dict per clip (views of batch buffers)."""
+        KL-NMF over the stack.  A list of (2, n_b) recordings of any lengths: each clip's STFT into its own buffers, one ragged
+        KL-NMF over them.  Returns one _front dict per clip (views of batch buffers)."""
         h, torch = self.h, self.torch
-        B, C, n = samples.shape
-        if C != 2:
-            raise ValueError('samples must be (B, 2, n), got %s' % (tuple(samples.shape),))
+        ragged = isinstance(samples, (list, tuple))
+        if ragged and not samples:
+            return []
+        for x in (samples if ragged else [samples[0]] if len(samples) else []):
+            if x.dim() != 2 or x.shape[0] != 2:
+                raise ValueError('samples must be (B, 2, n) or a list of (2, n_b), got a clip of shape %s' % (tuple(x.shape),))
+        B = len(samples)
         self._mark('start')
         key = self._token
-        F, T = self.F, self.num_frames(n)
-        X = h.buffer((key, 'batch', 'X'), (2 * B, F, T), torch.complex64)
-        Vs = h.buffer((key, 'batch', 'V'), (B, F, 2 * T), torch.float32)
-        for b in range(B):
-            h.stft(samples[b], self.window, self.N, self.hop, conjugate=True, want_V=True, out=(X[2 * b:2 * b + 2], Vs[b]))
+        F = self.F
+        if ragged:
+            Xs, Vs = [], []
+            for b, x in enumerate(samples):
+                T = self.num_frames(x.shape[1])
+                Xb = h.buffer((key, 'clip', b, 'X'), (2, F, T), torch.complex64)
+                Vb = h.buffer((key, 'clip', b, 'V'), (F, 2 * T), torch.float32)
+                h.stft(x, self.window, self.N, self.hop, conjugate=True, want_V=True, out=(Xb, Vb))
+                Xs.append(Xb)
+                Vs.append(Vb)
+        else:
+            T = self.num_frames(samples.shape[2])
+            X = h.buffer((key, 'batch', 'X'), (2 * B, F, T), torch.complex64)
+            Vs = h.buffer((key, 'batch', 'V'), (B, F, 2 * T), torch.float32)
+            for b in range(B):
+                h.stft(samples[b], self.window, self.N, self.hop, conjugate=True, want_V=True, out=(X[2 * b:2 * b + 2], Vs[b]))
+            Xs = [X[2 * b:2 * b + 2] for b in range(B)]
         self._mark('stft')
         means_host = getattr(self, '_means_host', None)
         if means_host is None or means_host.shape[0] != B:
             means_host = self._means_host = torch.empty((B, self.D), dtype=torch.float64, pin_memory=True)
         rs = []
         for b in range(B):
-            Xb = X[2 * b:2 * b + 2]
+            Xb = Xs[b]
             coh, ang, mean = h.phat_angspec(Xb, self.E, out_key=(key, 'clip', b))
             means_host[b].copy_(mean, non_blocking=True)
             rs.append(dict(X=Xb, coherence=coh, angularSpectrogram=ang, meanAngularSpectrum=mean, _mean_host=means_host[b]))
         means_ready = torch.cuda.Event()
         means_ready.record()
         self._mark('angular')
-        W0, H0 = self.nmf_init(2 * T)
-        W = h.buffer((key, 'batch', 'W'), (B,) + tuple(W0.shape), W0.dtype)
-        H = h.buffer((key, 'batch', 'H'), (B,) + tuple(H0.shape), H0.dtype)
-        W.copy_(W0.expand_as(W))
-        H.copy_(H0.expand_as(H))
-        h.klnmf_batched(Vs, W, H, self.I, self.alpha, self.eps, update_W=True)
+        if ragged:
+            W0, _ = self.nmf_init(max(V.shape[1] for V in Vs))
+            W = h.buffer((key, 'batch', 'W'), (B,) + tuple(W0.shape), W0.dtype)
+            W.copy_(W0.expand_as(W))
+            H = []
+            for b, V in enumerate(Vs):
+                Hb = h.buffer((key, 'clip', b, 'H'), (self.K, V.shape[1]), torch.float32)
+                Hb.copy_(self.nmf_init(V.shape[1])[1])
+                H.append(Hb)
+            h.klnmf_ragged(Vs, W, H, self.I, self.alpha, self.eps, update_W=True)
+        else:
+            W0, H0 = self.nmf_init(2 * T)
+            W = h.buffer((key, 'batch', 'W'), (B,) + tuple(W0.shape), W0.dtype)
+            H = h.buffer((key, 'batch', 'H'), (B,) + tuple(H0.shape), H0.dtype)
+            W.copy_(W0.expand_as(W))
+            H.copy_(H0.expand_as(H))
+            h.klnmf_batched(Vs, W, H, self.I, self.alpha, self.eps, update_W=True)
         self._mark('nmf')
         for b, r in enumerate(rs):
             r.update(V=Vs[b], W=W[b], H=H[b], _mean_ready=means_ready)
@@ -204,10 +234,11 @@ class GCCNMFPipeline(object):
         r['_all_nan_flag'] = flag
         return self._back(r, masks, key)
 
-    # ------------------------------------------------------------------ batches of equal-length clips
+    # ------------------------------------------------------------------ batches of clips
     def enhance_batch(self, samples, collect_stage_times=False):
-        """samples (B, 2, n) f32 cuda -> list of B dicts, clip b's bit-identical to enhance(samples[b]).  The STFT and the
-        KL-NMF run once for the whole batch; the later stages run per clip.  Valid until the next batch call."""
+        """samples (B, 2, n) f32 cuda, or a list of B (2, n_b) f32 cuda recordings of any lengths -> list of B dicts, clip b's
+        bit-identical to enhance(samples[b]).  The KL-NMF runs once for the whole batch; the other stages run per clip.  Valid
+        until the next batch call."""
         self.stage_events = [] if collect_stage_times else None
         rs = self._front_batch(samples)
         if rs:
@@ -215,7 +246,8 @@ class GCCNMFPipeline(object):
         return [self._enhance_back(r, (self._token, 'clip', b)) for b, r in enumerate(rs)]
 
     def separate_batch(self, samples, numTargets, collect_stage_times=False):
-        """samples (B, 2, n) f32 cuda -> list of B dicts, clip b's bit-identical to separate(samples[b], numTargets)."""
+        """samples (B, 2, n) f32 cuda or a list of (2, n_b) recordings -> list of B dicts, clip b's bit-identical to
+        separate(samples[b], numTargets)."""
         self.stage_events = [] if collect_stage_times else None
         rs = self._front_batch(samples)
         if rs:

@@ -135,6 +135,24 @@ GCCNMF_API int gccnmf_klnmf_batched(gccnmf_handle* h, const float* V, int64_t ld
                          float* W, float* H, int K, int iterations, float sparsity_alpha, float epsilon, int update_W,
                          void* workspace, size_t workspace_bytes, void* stream);
 /*
+ * B clips of different lengths in one call: clip b's W and H come out bit for bit as gccnmf_klnmf on that clip alone would leave
+ * them (same handle, same options).  V, ld_v, T2 and H are HOST arrays of B entries, read only during the call (no pointer to them
+ * is kept): clip b's V is (F, T2[b]) at V[b] with row pitch ld_v[b] >= T2[b], read in place (an STFT output view works); its H is
+ * (K, T2[b]) contiguous at H[b].  W is a contiguous (B, F, K) stack.  W and H hold the initial values on entry and the results on
+ * return.  On the tensor-core path each contraction of an iteration is launched once per distinct tile width among the clips' solo
+ * plans, and each other kernel once for all clips; the launch count does not grow with B.  Clips the float32 SIMT path takes, and
+ * clips under an option the batch form leaves out, run one at a time as gccnmf_klnmf_batched runs them.
+ * Workspace (gccnmf_klnmf_ragged_workspace_bytes): a per-call table of 1280 B + 256 bytes, then clip b's region of a batched run on
+ * its shape (gccnmf_klnmf_batched_workspace_bytes(1, F, T2[b], K), which is gccnmf_klnmf_workspace_bytes(F, T2[b], K) at
+ * tensor-core shapes); nothing is padded to the longest clip.  The table is written by a stream-ordered copy from host memory
+ * that the call owns.  B is 1 .. 8191; B, null pointers, T2[b] <= 0, ld_v[b] < T2[b], negative iterations and a short workspace
+ * are refused before anything is enqueued.  The size function returns 0 for such arguments.
+ */
+GCCNMF_API size_t gccnmf_klnmf_ragged_workspace_bytes(int B, int F, const int* T2, int K);
+GCCNMF_API int gccnmf_klnmf_ragged(gccnmf_handle* h, const float* const* V, const int64_t* ld_v, const int* T2, int B, int F,
+                         float* W, float* const* H, int K, int iterations, float sparsity_alpha, float epsilon, int update_W,
+                         void* workspace, size_t workspace_bytes, void* stream);
+/*
  * Frame-sharded dictionary learning (multi-GPU; SURVEY.md section 8e).  A rank holds the columns V_s
  * (F, T2s), H_s (K, T2s) of its frames and a replica of W.  The loop of gccNMFFunctions.py:75-81 becomes
  *
