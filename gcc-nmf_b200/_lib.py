@@ -105,6 +105,11 @@ SIGNATURES.update({
     'gccnmf_pipeline_workspace_bytes': (c_size_t, [_PC, c_int64]),
     'gccnmf_pick_targets': (c_int, [_H, _P, c_int, c_int, _P, _P, _S]),
     'gccnmf_separate': (c_int, [_H, _PC, _P, c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_size_t, _S]),
+    'gccnmf_window_targets': (c_int, [_H, _P, c_int, c_int, c_int, c_int, _P, _P, _P, _S]),
+    'gccnmf_target_gccnmf': (c_int, [_H, _P, c_int, c_int, _P, c_int, _P, c_int, _P, c_int, _P, _S]),
+    'gccnmf_argmax_mask_frames': (c_int, [_H, _P, c_int, c_int, _P, c_int, _P, c_double, _P, _P, _S]),
+    'gccnmf_pipeline_tracked_workspace_bytes': (c_size_t, [_PC, c_int, c_int64]),
+    'gccnmf_separate_tracked': (c_int, [_H, _PC, c_int, _P, c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_size_t, _S]),
     'gccnmf_wiener_apply_h': (c_int, [_H, _P, _P, _P, _P, c_int, c_int, c_int, _P, _P, _S]),
     'gccnmf_rt_state_bytes': (c_size_t, [_C]),
     'gccnmf_rt_init': (c_int, [_H, _C, _P, _P, _P, _P, _P, _P, c_size_t, _S]),
@@ -626,6 +631,41 @@ class Handle(object):
         K, T = argmax.shape
         mask = self._out(out_key, 'mask', (K, T), torch.float32)
         self.check(self.lib.gccnmf_argmax_mask(self.h, _ptr(argmax), K, T, _ptr(lut), lut.numel(), _ptr(mask), self.stream))
+        return mask
+
+    def window_targets(self, angular, window, P, want_means=True, out_key=None):
+        """angular (D, T) f64 -> (targets (T, P) i32, means (D, T) f64 | None, status (1) i32): each frame's P targets from the
+        nanmean of its newest `window` frames (gccnmf_window_targets); status bit 0 when a frame held earlier targets."""
+        torch = self.torch
+        D, T = angular.shape
+        means = self._out(out_key, 'window_means', (D, T), torch.float64) if want_means else None
+        targets = self._out(out_key, 'frame_targets', (T, int(P)), torch.int32)
+        status = self._out(out_key, 'window_status', (1,), torch.int32)
+        status.zero_()
+        self.check(self.lib.gccnmf_window_targets(self.h, _ptr(angular), D, T, int(window), int(P), _ptr(means), _ptr(targets), _ptr(status),
+                                                  self.stream))
+        return targets, means, status
+
+    def target_gccnmf(self, coherence, E, W, targets, out_key=None):
+        """coherence (F, T) c64, E (F, D) c128, W (F, K) f32, targets (T, P) i32 -> values (P, K, T) f32 at each frame's targets.
+        Every target must be in [0, D): the kernel indexes E with them unchecked (gccnmf_target_gccnmf), as window_targets writes them."""
+        torch = self.torch
+        F, T = coherence.shape
+        D, K, P = E.shape[1], W.shape[1], targets.shape[1]
+        values = self._out(out_key, 'target_values', (P, K, T), torch.float32)
+        self.check(self.lib.gccnmf_target_gccnmf(self.h, _ptr(coherence), F, T, _ptr(E), D, _ptr(W), K, _ptr(targets), P, _ptr(values),
+                                                 self.stream))
+        return values
+
+    def argmax_mask_frames(self, argmax, tdoas, targets, window_seconds, out_key=None):
+        """argmax (K, T) i32, tdoas (D) f64, targets (T) i32 -> mask (K, T) f32 = |tdoa[argmax] - tdoa[target of the frame]| < window."""
+        torch = self.torch
+        K, T = argmax.shape
+        D = tdoas.numel()
+        table = self.workspace('tdoa_table', D * D)
+        mask = self._out(out_key, 'mask', (K, T), torch.float32)
+        self.check(self.lib.gccnmf_argmax_mask_frames(self.h, _ptr(argmax), K, T, _ptr(tdoas), D, _ptr(targets), float(window_seconds), _ptr(table),
+                                                      _ptr(mask), self.stream))
         return mask
 
     def online_targets(self, angular):

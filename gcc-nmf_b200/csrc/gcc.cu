@@ -858,6 +858,7 @@ int gccnmf_tdoa_gccnmf_gated(gccnmf_handle* h, const float* coherence, int F, in
 // wide tiles would leave SMs idle.
 int gccnmf_target_gccnmf(gccnmf_handle* h, const float* coherence, int F, int T, const double* E, int D, const float* W, int K,
                          const int32_t* targets, int P, float* values, void* stream) {
+  GCCNMF_ENTER(h);
   GCCNMF_REQUIRE(h, F > 0 && T > 0 && D > 0 && K > 0 && P > 0 && coherence && E && W && targets && values, "target_gccnmf: bad arguments");
   GCCNMF_REQUIRE(h, (int64_t)T * P < (int64_t)1 << 31 && (int64_t)P * K * T < (int64_t)1 << 31, "target_gccnmf: T x P or P x K x T overflows int32");
   const int N = T * P;

@@ -44,8 +44,6 @@ int gccnmf_stft_segments(gccnmf_handle* h, const float* samples, int64_t sample_
 int gccnmf_istft_frames(gccnmf_handle* h, const float* spec, int batch, int n_fft, int T, int conjugate, float* frames, void* stream);
 int gccnmf_tdoa_gccnmf_gated(gccnmf_handle* h, const float* coherence, int F, int T, const double* E, int D, const float* W, int K,
                              int32_t* argmax, const int32_t* gate, int capacity, int32_t* ran, void* stream);
-int gccnmf_target_gccnmf(gccnmf_handle* h, const float* coherence, int F, int T, const double* E, int D, const float* W, int K,
-                         const int32_t* targets, int P, float* values, void* stream);
 int gccnmf_phat_angspec_bank(gccnmf_handle* h, const float* X, int F, int T, const SteerBank& bank, int D, float* coherence, double* angular,
                              void* stream);
 int gccnmf_tdoa_argmax_bank(gccnmf_handle* h, const float* coherence, int F, int T, const SteerBank& bank, int D, const float* W, int K,

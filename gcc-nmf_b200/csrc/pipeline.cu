@@ -8,6 +8,7 @@
 // indexes, the gathered steering columns and the TDOA look-up table stay on the device.  Conditions the reference turns into Python
 // exceptions are reported through a device-side status word the caller reads after the call (bit 0: fewer peaks than targets,
 // bit 1: an all-NaN mask column, bit 2: more near-tie argmax decisions than the float64 refinement list holds).
+// gccnmf_separate_tracked is the same flow with targets per frame (tracking.cu) in place of the one pick over the whole clip.
 #include <cmath>
 
 #include "common.cuh"
@@ -52,13 +53,16 @@ struct PipeLayout {
   double *mean, *E_sel;
   int32_t *argmax, *flags;
   uint8_t* lut;
+  double *angular, *means;       // tracked flow only: the angular spectrogram and its window means (D, T)
+  uint8_t* table;                // tracked enhancement: the (D, D) TDOA table
   void *ws_nmf, *ws_ang, *ws_argmax, *ws_recon, *ws_istft;
   size_t n_nmf, n_ang, n_argmax, n_recon, n_istft, bytes;
   int F, T;
   bool ok;
 };
 
-PipeLayout pipe_carve(const gccnmf_pipeline_config& c, int64_t num_samples, void* ws, size_t ws_bytes) {
+// tracked: the gccnmf_separate_tracked layout, the gccnmf_separate one followed by its own buffers.
+PipeLayout pipe_carve(const gccnmf_pipeline_config& c, int64_t num_samples, void* ws, size_t ws_bytes, bool tracked = false) {
   PipeLayout l{};
   const int N = c.window_size, K = c.num_atoms, D = c.num_tdoas;
   const int S = c.num_targets > 0 ? c.num_targets : 1;
@@ -88,6 +92,11 @@ PipeLayout pipe_carve(const gccnmf_pipeline_config& c, int64_t num_samples, void
   l.ws_argmax = w.take<char>(l.n_argmax);
   l.ws_recon = w.take<char>(l.n_recon);
   l.ws_istft = w.take<char>(l.n_istft);
+  if (tracked) {
+    l.angular = w.take<double>((size_t)D * T);
+    l.means = w.take<double>((size_t)D * T);
+    l.table = w.take<uint8_t>((size_t)D * D);
+  }
   l.bytes = align_up(w.used, 256);
   l.ok = ws != nullptr && w.ok();
   return l;
@@ -152,6 +161,55 @@ int gccnmf_separate(gccnmf_handle* h, const gccnmf_pipeline_config* cfg, const f
     GCCNMF_LAUNCH(h, or_status_kernel, 1, 1, 0, stream, l.flags + 2, 0, 2, status);
   }
   // a8 + a9
+  if (int st = gccnmf_masked_recon_phase(h, l.masks, l.X, W, H, S, F, T, K, l.est, l.ws_recon, l.n_recon, stream)) return st;
+  return gccnmf_istft_ola(h, l.est, S * 2, N, hop, T, window, (float)((double)hop / (double)N * 2.0), 1, 1, signals, l.ws_istft, l.n_istft, stream);
+}
+
+size_t gccnmf_pipeline_tracked_workspace_bytes(const gccnmf_pipeline_config* cfg, int localization_window, int64_t num_samples) {
+  if (!cfg || localization_window < 1 || cfg->window_size < 2 || cfg->hop_size < 1 || cfg->num_atoms < 1 || cfg->num_tdoas < 1) return 0;
+  const PipeLayout l = pipe_carve(*cfg, num_samples, nullptr, 0, true);
+  return l.T >= 1 ? l.bytes : 0;
+}
+
+// gccnmf_separate with targets per frame: the window targets of the angular spectrogram (tracking.cu) in place of the one pick
+// over the whole clip.  frame_targets (T, S) i32 and status are device outputs; window_means (D, T) f64 may be NULL.  Status bit
+// 0 means that some frame held the targets of an earlier one (or the defaults), not that the flow failed.
+int gccnmf_separate_tracked(gccnmf_handle* h, const gccnmf_pipeline_config* cfg, int localization_window, const float* samples,
+                            int64_t num_samples, const double* window, const double* E, const double* tdoas, float* W, float* H,
+                            float* signals, int32_t* frame_targets, double* window_means, int32_t* status, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+  GCCNMF_ENTER(h);
+  GCCNMF_REQUIRE(h, cfg && samples && window && E && tdoas && W && H && signals && frame_targets && status, "separate_tracked: NULL pointer");
+  GCCNMF_REQUIRE(h, localization_window >= 1, "separate_tracked: localization window must be >= 1 (got %d)", localization_window);
+  GCCNMF_REQUIRE(h, cfg->num_targets >= 0 && cfg->num_iterations >= 0 && cfg->num_tdoas >= 3 && cfg->num_tdoas <= kPickMaxD &&
+                        cfg->num_targets <= cfg->num_tdoas && cfg->num_atoms >= 1,
+                 "separate_tracked: bad configuration");
+  PipeLayout l = pipe_carve(*cfg, num_samples, workspace, workspace_bytes, true);
+  GCCNMF_REQUIRE(h, l.T >= 1, "Buffer is too short (n=%lld) for frame_length=%d", (long long)num_samples, cfg->window_size);
+  const int N = cfg->window_size, hop = cfg->hop_size, K = cfg->num_atoms, D = cfg->num_tdoas, F = l.F, T = l.T;
+  const bool enhancement = cfg->num_targets == 0;
+  const int S = enhancement ? 1 : cfg->num_targets;
+  GCCNMF_REQUIRE(h, (int64_t)T * S < (int64_t)1 << 31 && (int64_t)S * K * T < (int64_t)1 << 31,
+                 "separate_tracked: T x S or S x K x T overflows int32");
+  if (!l.ok) return gccnmf_fail(h, GCCNMF_ERR_WORKSPACE, "separate_tracked: workspace too small: need %zu bytes", l.bytes);
+  double* means = window_means ? window_means : l.means;
+  cudaStream_t s = (cudaStream_t)stream;
+  GCCNMF_CHECK_CUDA(h, cudaMemsetAsync(status, 0, sizeof(int32_t), s));
+  GCCNMF_CHECK_CUDA(h, cudaMemsetAsync(l.flags, 0, 8 * sizeof(int32_t), s));
+  if (int st = gccnmf_stft(h, samples, num_samples, 2, num_samples, window, N, hop, 1, l.X, l.V, stream)) return st;
+  if (int st = gccnmf_phat_angspec(h, l.X, F, T, 0, E, D, l.coh, l.angular, nullptr, l.ws_ang, l.n_ang, stream)) return st;
+  if (int st = gccnmf_window_targets(h, l.angular, D, T, localization_window, S, means, frame_targets, status, stream)) return st;
+  if (int st = gccnmf_klnmf(h, l.V, F, 2 * T, W, H, K, cfg->num_iterations, cfg->sparsity_alpha, cfg->epsilon, 1, l.ws_nmf, l.n_nmf, stream)) return st;
+  if (enhancement) {
+    if (int st = gccnmf_tdoa_argmax(h, l.coh, F, T, E, D, W, K, l.argmax, l.flags + 1, l.ws_argmax, l.n_argmax, stream)) return st;
+    GCCNMF_LAUNCH(h, or_status_kernel, 1, 1, 0, stream, l.flags + 1, gccnmf_tdoa_argmax_refine_capacity(K, T), 4, status);
+    if (int st = gccnmf_argmax_mask_frames(h, l.argmax, K, T, tdoas, D, frame_targets, (double)cfg->target_window_seconds, l.table, l.masks, stream))
+      return st;
+  } else {
+    if (int st = gccnmf_target_gccnmf(h, l.coh, F, T, E, D, W, K, frame_targets, S, l.values, stream)) return st;
+    if (int st = gccnmf_coeff_mask(h, l.values, S, K, T, l.masks, l.flags + 2, stream)) return st;
+    GCCNMF_LAUNCH(h, or_status_kernel, 1, 1, 0, stream, l.flags + 2, 0, 2, status);
+  }
   if (int st = gccnmf_masked_recon_phase(h, l.masks, l.X, W, H, S, F, T, K, l.est, l.ws_recon, l.n_recon, stream)) return st;
   return gccnmf_istft_ola(h, l.est, S * 2, N, hop, T, window, (float)((double)hop / (double)N * 2.0), 1, 1, signals, l.ws_istft, l.n_istft, stream);
 }

@@ -13,6 +13,10 @@ next call on the same pipeline.  Steady-state calls therefore never enter the CU
 Only two things happen on the host, as in gccNMFFunctions.py: the D-element peak picking
 (scipy.signal.argrelmax) and the plan-time constants (window, exp(-2 pi i f tau) table in float64,
 seeded numpy draw of the NMF initial values -- a function of shape and seed only, gccNMFFunctions.py:70-73).
+
+With localizationWindow=w every flow follows a moving talker instead: each frame takes its targets from the nanmean of the
+angular spectrogram over its newest w frames (gccnmf_window_targets, on the device, no host wait), and the result gains
+frameTargetTDOAIndexes (T, S), windowMeans (D, T) and status (bit 0: some frame held earlier targets; information, not an error).
 """
 import weakref
 
@@ -197,36 +201,59 @@ class GCCNMFPipeline(object):
         return r['targetTDOAIndexes']
 
     # ------------------------------------------------------------------ flows
-    def enhance(self, samples, collect_stage_times=False):
-        """samples (2, n) f32 cuda -> dict of device tensors (enhancement flow, one target)."""
+    def enhance(self, samples, collect_stage_times=False, localizationWindow=None):
+        """samples (2, n) f32 cuda -> dict of device tensors (enhancement flow, one target; per frame with a localizationWindow)."""
         self.stage_events = [] if collect_stage_times else None
-        return self._enhance_back(self._front(samples), self._token)
+        return self._enhance_back(self._front(samples), self._token, localizationWindow)
 
-    def _enhance_back(self, r, key):
+    def _window_targets(self, r, numTargets, localizationWindow, key):
+        """Each frame's targets from the window means of the clip's angular spectrogram, on the device."""
+        targets, means, status = self.h.window_targets(r['angularSpectrogram'], localizationWindow, numTargets, out_key=key)
+        self._mark('localize')
+        r.update(frameTargetTDOAIndexes=targets, windowMeans=means, status=status)
+        return targets
+
+    def _tdoas_device(self):
+        if getattr(self, '_tdoas_dev', None) is None:
+            self._tdoas_dev = self.h.to_device(np.ascontiguousarray(self.hypothesisTDOAs, dtype=np.float64))
+        return self._tdoas_dev
+
+    def _enhance_back(self, r, key, localizationWindow=None):
         h = self.h
+        if localizationWindow is not None:
+            targets = self._window_targets(r, 1, localizationWindow, key)
         argmax, refined = h.tdoa_argmax(r['coherence'], self.E, r['W'], out_key=key)
         self._mark('gccnmf')
-        target = self._pick_targets(r, 1)[0]
+        if localizationWindow is None:
+            target = self._pick_targets(r, 1)[0]
         r['refinedDecisions'] = int(refined.item())
         if r['refinedDecisions'] > h.lib.gccnmf_tdoa_argmax_refine_capacity(self.K, argmax.shape[1]):
             _, argmax = h.tdoa_gccnmf(r['coherence'], self.E, r['W'], want_values=False, want_argmax=True)   # exact float64 kernel
         window = (self.hypothesisTDOAs[-1] - self.hypothesisTDOAs[0]) * self.windowPercent
-        lut = fn.getTargetTDOALookup(self.hypothesisTDOAs, target, window)
-        mask = h.argmax_mask(argmax, h.to_device(lut.astype(np.uint8)), out_key=key)
+        if localizationWindow is None:
+            lut = fn.getTargetTDOALookup(self.hypothesisTDOAs, target, window)
+            mask = h.argmax_mask(argmax, h.to_device(lut.astype(np.uint8)), out_key=key)
+        else:
+            mask = h.argmax_mask_frames(argmax, self._tdoas_device(), targets.reshape(-1), window, out_key=key)
         self._mark('mask')
         r['argMaxGCCNMF'] = argmax
         return self._back(r, mask[None], key)
 
-    def separate(self, samples, numTargets, collect_stage_times=False):
-        """samples (2, n) f32 cuda -> dict of device tensors (runGCCNMF.py flow, numTargets sources)."""
+    def separate(self, samples, numTargets, collect_stage_times=False, localizationWindow=None):
+        """samples (2, n) f32 cuda -> dict of device tensors (runGCCNMF.py flow, numTargets sources; source q is the q-th target
+        from the left in each frame with a localizationWindow)."""
         self.stage_events = [] if collect_stage_times else None
-        return self._separate_back(self._front(samples), numTargets, self._token)
+        return self._separate_back(self._front(samples), numTargets, self._token, localizationWindow)
 
-    def _separate_back(self, r, numTargets, key):
+    def _separate_back(self, r, numTargets, key, localizationWindow=None):
         h = self.h
-        idx = self._pick_targets(r, numTargets)
-        E_sel = h.to_device(np.ascontiguousarray(self.E_host[:, idx]))
-        values, _ = h.tdoa_gccnmf(r['coherence'], E_sel, r['W'], want_values=True, want_argmax=False)
+        if localizationWindow is None:
+            idx = self._pick_targets(r, numTargets)
+            E_sel = h.to_device(np.ascontiguousarray(self.E_host[:, idx]))
+            values, _ = h.tdoa_gccnmf(r['coherence'], E_sel, r['W'], want_values=True, want_argmax=False)
+        else:
+            targets = self._window_targets(r, numTargets, localizationWindow, key)
+            values = h.target_gccnmf(r['coherence'], self.E, r['W'], targets, out_key=key)
         self._mark('gccnmf')
         masks, flag = h.coeff_mask(values)
         self._mark('mask')
@@ -235,30 +262,32 @@ class GCCNMFPipeline(object):
         return self._back(r, masks, key)
 
     # ------------------------------------------------------------------ batches of clips
-    def enhance_batch(self, samples, collect_stage_times=False):
+    def enhance_batch(self, samples, collect_stage_times=False, localizationWindow=None):
         """samples (B, 2, n) f32 cuda, or a list of B (2, n_b) f32 cuda recordings of any lengths -> list of B dicts, clip b's
-        bit-identical to enhance(samples[b]).  The KL-NMF runs once for the whole batch; the other stages run per clip.  Valid
-        until the next batch call."""
+        bit-identical to enhance(samples[b], localizationWindow=localizationWindow).  The KL-NMF runs once for the whole batch;
+        the other stages run per clip.  Valid until the next batch call."""
         self.stage_events = [] if collect_stage_times else None
         rs = self._front_batch(samples)
-        if rs:
+        if rs and localizationWindow is None:
             rs[0]['_mean_ready'].synchronize()          # one host wait for all B means before peak picking
-        return [self._enhance_back(r, (self._token, 'clip', b)) for b, r in enumerate(rs)]
+        return [self._enhance_back(r, (self._token, 'clip', b), localizationWindow) for b, r in enumerate(rs)]
 
-    def separate_batch(self, samples, numTargets, collect_stage_times=False):
+    def separate_batch(self, samples, numTargets, collect_stage_times=False, localizationWindow=None):
         """samples (B, 2, n) f32 cuda or a list of (2, n_b) recordings -> list of B dicts, clip b's bit-identical to
-        separate(samples[b], numTargets)."""
+        separate(samples[b], numTargets, localizationWindow=localizationWindow)."""
         self.stage_events = [] if collect_stage_times else None
         rs = self._front_batch(samples)
-        if rs:
+        if rs and localizationWindow is None:
             rs[0]['_mean_ready'].synchronize()
-        return [self._separate_back(r, numTargets, (self._token, 'clip', b)) for b, r in enumerate(rs)]
+        return [self._separate_back(r, numTargets, (self._token, 'clip', b), localizationWindow) for b, r in enumerate(rs)]
 
     # ------------------------------------------------------------------ the whole flow as ONE C-ABI call
-    def run_fused(self, samples, numTargets=0):
+    def run_fused(self, samples, numTargets=0, localizationWindow=None):
         """gccnmf_separate: every stage enqueued by one library call, target picking on the device, no host synchronisation
         until the caller reads a result.  numTargets = 0: enhancement flow (one target); >= 1: runGCCNMF.py separation.
-        Returns dict(W, H, targetSignalEstimates (S, 2, n_out), targetTDOAIndexes (device i32), status (device i32))."""
+        Returns dict(W, H, targetSignalEstimates (S, 2, n_out), targetTDOAIndexes (device i32), status (device i32)).
+        With a localizationWindow, gccnmf_separate_tracked: targets per frame, and the dict has frameTargetTDOAIndexes (T, S) and
+        windowMeans (D, T) in place of targetTDOAIndexes."""
         import ctypes
         from ._lib import PipelineConfig, _ptr
         h, torch = self.h, self.torch
@@ -272,22 +301,30 @@ class GCCNMFPipeline(object):
         W, H = h.buffer((key, 'W'), W0.shape, W0.dtype), h.buffer((key, 'H'), H0.shape, H0.dtype)
         W.copy_(W0)
         H.copy_(H0)
-        if getattr(self, '_tdoas_dev', None) is None:
-            self._tdoas_dev = h.to_device(np.ascontiguousarray(self.hypothesisTDOAs, dtype=np.float64))
+        tdoas = self._tdoas_device()
         length = int(h.lib.gccnmf_istft_length(self.N, self.hop, T, 1))
         y = h.buffer((key, 'y'), (S, 2, length), torch.float32)
-        targets = h.buffer((key, 'targets'), (S,), torch.int32)
         status = h.buffer((key, 'status'), (1,), torch.int32)
+        if localizationWindow is not None:
+            w = int(localizationWindow)
+            frame_targets = h.buffer((key, 'frame_targets'), (T, S), torch.int32)
+            means = h.buffer((key, 'window_means'), (self.D, T), torch.float64)
+            ws = h.workspace('pipeline', h.lib.gccnmf_pipeline_tracked_workspace_bytes(ctypes.byref(cfg), w, n))
+            h.check(h.lib.gccnmf_separate_tracked(h.h, ctypes.byref(cfg), w, _ptr(samples), n, _ptr(self.window), _ptr(self.E), _ptr(tdoas), _ptr(W),
+                                                  _ptr(H), _ptr(y), _ptr(frame_targets), _ptr(means), _ptr(status), _ptr(ws), ws.numel(), h.stream))
+            return dict(W=W, H=H, targetSignalEstimates=y, frameTargetTDOAIndexes=frame_targets, windowMeans=means, status=status)
+        targets = h.buffer((key, 'targets'), (S,), torch.int32)
         ws = h.workspace('pipeline', h.lib.gccnmf_pipeline_workspace_bytes(ctypes.byref(cfg), n))
-        h.check(h.lib.gccnmf_separate(h.h, ctypes.byref(cfg), _ptr(samples), n, _ptr(self.window), _ptr(self.E), _ptr(self._tdoas_dev), _ptr(W), _ptr(H),
+        h.check(h.lib.gccnmf_separate(h.h, ctypes.byref(cfg), _ptr(samples), n, _ptr(self.window), _ptr(self.E), _ptr(tdoas), _ptr(W), _ptr(H),
                                       _ptr(y), _ptr(targets), _ptr(status), _ptr(ws), ws.numel(), h.stream))
         return dict(W=W, H=H, targetSignalEstimates=y, targetTDOAIndexes=targets, status=status)
 
     @staticmethod
-    def raise_on_status(status):
-        """The conditions the reference turns into exceptions (call after synchronising)."""
+    def raise_on_status(status, tracked=False):
+        """The conditions the reference turns into exceptions (call after synchronising).  tracked: bit 0 of a tracked flow (a
+        frame held earlier targets) is not one of them."""
         st = int(status.item())
-        if st & 1:
+        if st & 1 and not tracked:
             raise ValueError('did not find enough peaks in the angular spectrum')          # gccNMFFunctions.py:102-104
         if st & 2:
             raise ValueError('All-NaN slice encountered')                                  # numpy.nanargmax, :138
@@ -295,12 +332,13 @@ class GCCNMFPipeline(object):
             raise RuntimeError('all-TDOA argmax: more near-tie decisions than the refinement list holds; use enhance(), which falls '
                                'back to the exact float64 kernel')
 
-    def run_fused_host(self, samples_host, numTargets=0, out_host=None, check=True):
+    def run_fused_host(self, samples_host, numTargets=0, out_host=None, check=True, localizationWindow=None):
         """Pinned (or pageable) host samples in -> host float32 (S, 2, n_out) signal estimates out, through ONE library call
-        (gccnmf_separate): H2D copy, the whole flow enqueued without host synchronisation, D2H copy, one stream synchronise."""
+        (gccnmf_separate, or gccnmf_separate_tracked with a localizationWindow): H2D copy, the whole flow enqueued without host
+        synchronisation, D2H copy, one stream synchronise."""
         torch = self.torch
         s = samples_host if isinstance(samples_host, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(samples_host, dtype=np.float32))
-        r = self.run_fused(s.to(self.h.device, non_blocking=True), numTargets)
+        r = self.run_fused(s.to(self.h.device, non_blocking=True), numTargets, localizationWindow)
         y = r['targetSignalEstimates']
         if out_host is None:
             out_host = torch.empty(y.shape, dtype=torch.float32, pin_memory=True)
@@ -310,7 +348,7 @@ class GCCNMFPipeline(object):
         self._status_host.copy_(r['status'], non_blocking=True)
         torch.cuda.current_stream(self.h.device).synchronize()
         if check:
-            self.raise_on_status(self._status_host)
+            self.raise_on_status(self._status_host, tracked=localizationWindow is not None)
         return out_host
 
     # ------------------------------------------------------------------ host-buffer entry (what e2e times)

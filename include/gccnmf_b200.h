@@ -346,6 +346,44 @@ GCCNMF_API int gccnmf_separate(gccnmf_handle* h, const gccnmf_pipeline_config* c
                     const double* window, const double* E, const double* tdoas, float* W, float* H, float* signals,
                     int32_t* target_indexes, int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- the offline path following a moving talker: targets per frame from a sliding window of the angular spectrogram -------
+ * The sliding-window rule of realtime/gccNMFProcessor.py:219-226 (the real-time and low-latency engines' window), per frame of a
+ * whole clip.  With A the (D, T) f64 angular spectrogram of gccnmf_phat_angspec and a window of w >= 1 frames:
+ * - means[d][t] = the nanmean of A[d][t], A[d][t - 1], ..., A[d][max(0, t - w + 1)]: summed in float64 newest first, skipping
+ *   NaN, divided by the number of non-NaN terms; NaN when all are NaN.  The window is cut at the start of the clip.  It is
+ *   causal, so a target lags a move by up to w frames.
+ * - targets[t] = the P largest strict interior local maxima of means[:, t], ascending (gccnmf_pick_targets' rule).  A frame with
+ *   fewer than P peaks holds the targets of the latest earlier frame that had P, or floor((2 q + 1) D / (2 P)) before any such
+ *   frame, and sets *status bit 0 (ORed in; the status is not cleared).
+ * w < 1, P outside [1, D], D outside [3, 1024], T P >= 2^31 and NULL pointers are refused before anything is enqueued.
+ * means may be NULL: the call then keeps them in a stream-ordered allocation (cudaMallocAsync) for its duration. */
+GCCNMF_API int gccnmf_window_targets(gccnmf_handle* h, const double* angular, int D, int T, int window, int P, double* means,
+                          int32_t* targets, int32_t* status, void* stream);
+/* values (P, K, T) f32 = the float64 GCC-NMF contraction at P target TDOAs per frame, targets (T, P) i32 each in [0, D);
+ * values[q][k][t] has the bits gccnmf_tdoa_gccnmf writes at (targets[t][q], k, t).  T P or P K T >= 2^31 is refused.
+ * The targets are device data the call does not read on the host, and the kernel indexes E with them unchecked: a target outside
+ * [0, D) is undefined behaviour (an out-of-bounds read of E).  gccnmf_window_targets only writes targets in [0, D). */
+GCCNMF_API int gccnmf_target_gccnmf(gccnmf_handle* h, const float* coherence, int F, int T, const double* E, int D, const float* W,
+                         int K, const int32_t* targets, int P, float* values, void* stream);
+/* The enhancement mask with a target per frame: mask[k][t] = |tdoa[argmax[k][t]] - tdoa[targets[t]]| < window_seconds, in
+ * float64 through a (D, D) u8 table built in lut_workspace (D * D bytes), whose row tau is the LUT of gccnmf_separate's
+ * enhancement flow for target tau.  targets (T) i32; D <= 1024. */
+GCCNMF_API int gccnmf_argmax_mask_frames(gccnmf_handle* h, const int32_t* argmax, int K, int T, const double* tdoas, int D,
+                              const int32_t* targets, double window_seconds, uint8_t* lut_workspace, float* mask, void* stream);
+/* gccnmf_separate with the targets of gccnmf_window_targets (P = num_targets, or 1 for the enhancement flow): one call, no host
+ * synchronisation.  Separation: values at each frame's targets (gccnmf_target_gccnmf), then gccnmf_coeff_mask; source q is the
+ * q-th target from the left in each frame.  Enhancement: gccnmf_argmax_mask_frames on the all-TDOA argmax.  frame_targets (T, S)
+ * i32 and status (1) i32 are device outputs, window_means (D, T) f64 a device output that may be NULL.  Status bits as
+ * gccnmf_separate's, except that bit 0 means a frame held earlier targets: information, not an error.  When every frame's targets
+ * are gccnmf_separate's, the signals are gccnmf_separate's, byte for byte.  A window < 1, num_targets > num_tdoas, T S or S K T
+ * >= 2^31, NULL pointers and a workspace smaller than gccnmf_pipeline_tracked_workspace_bytes are refused before anything is
+ * enqueued.  The workspace size is 0 for a window < 1 or an invalid configuration. */
+GCCNMF_API size_t gccnmf_pipeline_tracked_workspace_bytes(const gccnmf_pipeline_config* cfg, int localization_window, int64_t num_samples);
+GCCNMF_API int gccnmf_separate_tracked(gccnmf_handle* h, const gccnmf_pipeline_config* cfg, int localization_window,
+                            const float* samples, int64_t num_samples, const double* window, const double* E,
+                            const double* tdoas, float* W, float* H, float* signals, int32_t* frame_targets,
+                            double* window_means, int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- a13 + f-2: the real-time block path as one stream-ordered unit ----------------------------------
  * GCCNMFProcessor.processFrames (realtime/gccNMFProcessor.py:201-231 and the Theano graph of :245-270) with the
  * OverlapAddProcessor rings around it (realtime/utils.py:72-116) and, optionally, the per-frame coefficient inference of
