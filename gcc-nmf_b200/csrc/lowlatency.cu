@@ -38,6 +38,7 @@
 
 #include "common.cuh"
 #include "records.cuh"
+#include "streams.cuh"
 
 int gccnmf_stft_segments(gccnmf_handle* h, const float* samples, int64_t sample_stride, int channels, int segments, int frames_per_seg,
                          int64_t seg_stride, const double* window, int n_fft, int hop, int conjugate, float* X, float* V, void* stream);
@@ -131,6 +132,7 @@ constexpr int kLLInferMaxSmem = 227 * 1024;   // the H100's opt-in dynamic share
 constexpr int kLLMaxHistory = 1024;
 constexpr int kLLMaxSteerings = 64;
 constexpr int kLLMaxDictionaries = 64;
+static_assert(kLLMaxSteerings <= kStreamMaxEntries && kLLMaxDictionaries <= kStreamMaxEntries, "sort_by_entry_kernel");
 
 int ll_check(gccnmf_handle* h, const gccnmf_ll_config* cfg) {
   GCCNMF_REQUIRE(h, cfg != nullptr, "ll: NULL config");
@@ -542,51 +544,6 @@ __global__ void ll_hist_reset_kernel(char* __restrict__ hist, size_t hist_stride
   for (size_t i = threadIdx.x; i < hist_stride / 16; i += blockDim.x) b[i] = make_uint4(0, 0, 0, 0);
 }
 
-struct LLWindowBatch { int32_t w[kLLParamsPerLaunch]; };
-
-__global__ void ll_hist_window_kernel(char* __restrict__ hist, size_t hist_stride, size_t window_offset, int first, int count, LLWindowBatch b) {
-  const int i = threadIdx.x;
-  if (i >= count) return;
-  *reinterpret_cast<int32_t*>(hist + (size_t)(first + i) * hist_stride + window_offset) = b.w[i];
-}
-
-// Bank: stable counting sort of the S streams by entry, by one warp over chunks of 32 streams: order lists the streams of entry 0
-// in stream order, then those of entry 1, ...; seg[e] is entry e's first position and seg[Qe] = S.
-__global__ void __launch_bounds__(32) ll_sort_streams_kernel(const int32_t* __restrict__ assign, int S, int Qe, int32_t* __restrict__ order,
-                                                            int32_t* __restrict__ seg) {
-  __shared__ int base[kLLMaxSteerings];
-  const int lane = threadIdx.x;
-  for (int i = lane; i < Qe; i += 32) base[i] = 0;
-  __syncwarp();
-  for (int pass = 0; pass < 2; ++pass) {               // 0: count per entry, 1: place
-    for (int s0 = 0; s0 < S; s0 += 32) {
-      const int s = s0 + lane;
-      const int e = s < S ? assign[s] : -1;
-      const unsigned peers = __match_any_sync(0xffffffffu, e);
-      const bool leader = lane == __ffs(peers) - 1;
-      if (pass == 1 && e >= 0) order[base[e] + __popc(peers & ((1u << lane) - 1u))] = s;
-      __syncwarp();
-      if (leader && e >= 0) base[e] += __popc(peers);
-      __syncwarp();
-    }
-    if (pass == 0 && lane == 0)                        // counts -> first positions
-      for (int i = 0, sum = 0; i < Qe; ++i) {
-        const int n = base[i];
-        base[i] = seg[i] = sum;
-        sum += n;
-      }
-    __syncwarp();
-  }
-  if (lane == 0) seg[Qe] = S;
-}
-
-struct LLAssignBatch { int32_t e[kLLParamsPerLaunch]; };
-
-// Bank: streams [first, first + count) onto the entries of the batch, or all of them onto entry 0 (set_zero: init, reset).
-__global__ void ll_assign_kernel(int32_t* __restrict__ assign, int first, int count, LLAssignBatch b, int set_zero) {
-  for (int i = threadIdx.x; i < count; i += blockDim.x) assign[first + i] = set_zero ? 0 : b.e[i];
-}
-
 // mask[k][t] = |argmax[k][t] - target[t]| < epsilon of t's stream   (atom_mask_kernel mode 0)
 __global__ void ll_mask_kernel(const LLStream* __restrict__ streams, const int32_t* __restrict__ argmax, const int32_t* __restrict__ targets, int K,
                                int T, int hops, float* __restrict__ mask) {
@@ -735,14 +692,6 @@ __global__ void ll_src_reset_kernel(int first, int count, int P, int D, int N, f
   if (threadIdx.x == 0) src_status[s] = 0;
 }
 
-struct LLTargetsBatch { int32_t t[kLLParamsPerLaunch * kLLMaxSources]; };
-
-__global__ void ll_src_override_kernel(int32_t* __restrict__ src_override, int first, int count, int P, LLTargetsBatch b) {
-  const int i = threadIdx.x;
-  if (i >= count) return;
-  for (int q = 0; q < P; ++q) src_override[(int64_t)(first + i) * kLLMaxSources + q] = b.t[i * P + q];
-}
-
 // ---- dictionary bank (gccnmf_lldict_*): column t is on entry dassign[t / hops] with K_e atoms
 // ll_mask_kernel's mask on rows k < K_e; rows [K_e, Kmax) get 0
 __global__ void ll_dict_mask_kernel(const LLStream* __restrict__ streams, const int32_t* __restrict__ argmax, const int32_t* __restrict__ targets,
@@ -808,12 +757,6 @@ __global__ void ll_dict_fill_kernel(const int32_t* __restrict__ dK, const int32_
     H[(int64_t)k * 2 * T + t] = 0.f;
     H[(int64_t)k * 2 * T + T + t] = 0.f;
   }
-}
-
-// streams [first, first + count) onto the batch's entries where they are >= 0 (-1 keeps a stream's entry)
-__global__ void ll_dict_assign_kernel(int32_t* __restrict__ assign, int first, int count, LLAssignBatch b) {
-  for (int i = threadIdx.x; i < count; i += blockDim.x)
-    if (b.e[i] >= 0) assign[first + i] = b.e[i];
 }
 
 __global__ void ll_set_int_kernel(int32_t* p, int v) { *p = v; }
@@ -974,7 +917,7 @@ int ll_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe
   for (int j = 0; j < Qe; ++j)
     if (int st = gccnmf_steering_transpose(h, l.E + (size_t)j * 2 * l.F * l.D, l.F, l.D, l.ET + (size_t)j * 2 * l.D * l.Fp, l.Fp, stream)) return st;
   // with a bank every stream is on entry 0 (the memset above): sorted in stream order
-  if (Qe) GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
+  if (Qe) GCCNMF_LAUNCH(h, sort_by_entry_kernel, 1, 32, 0, stream, l.assign, sizeof(int32_t), l.S, Qe, l.order, l.seg);
   if (!Qd) GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.W, W, (size_t)l.F * l.K * sizeof(float), cudaMemcpyDeviceToDevice, s));
   if (!Qd && cfg->inference_iterations > 0) {
     GCCNMF_CHECK_CUDA(h, cudaMemcpyAsync(l.H0, H0, (size_t)l.K * 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
@@ -993,19 +936,18 @@ int ll_reset_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int L
                      void* stream) {
   GCCNMF_ENTER(h);
   LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
-  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "ll_reset_streams: streams [%d, %d + %d) outside [0, %d)", first,
-                 first, count, l.S);
+  if (int st = stream_range_check(h, "ll_reset_streams", l.S, first, count)) return st;
   GCCNMF_LAUNCH(h, ll_reset_kernel, count, 256, 0, stream, l.streams, first, count, l.in_ring, l.out_ring, l.carry, l.R, P ? 0 : l.N, l.D, 0);
   if (P)
     GCCNMF_LAUNCH(h, ll_src_reset_kernel, count, 256, 0, stream, first, count, P, l.D, l.N, l.out_ring, l.src_targets, l.src_override, l.src_status, 0);
   if (Lh) GCCNMF_LAUNCH(h, ll_hist_reset_kernel, count, 256, 0, stream, l.hist, l.hist_stride, first, count);
   if (Qe) {
-    GCCNMF_LAUNCH(h, ll_assign_kernel, 1, 256, 0, stream, l.assign, first, count, LLAssignBatch{}, 1);
-    GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
+    if (int st = enqueue_stream_fill(h, l.assign, sizeof(int32_t), first, count, 0, stream)) return st;
+    GCCNMF_LAUNCH(h, sort_by_entry_kernel, 1, 32, 0, stream, l.assign, sizeof(int32_t), l.S, Qe, l.order, l.seg);
   }
   if (Qd) {
-    GCCNMF_LAUNCH(h, ll_assign_kernel, 1, 256, 0, stream, l.dassign, first, count, LLAssignBatch{}, 1);
-    GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.dassign, l.S, Qd, l.dorder, l.dseg);
+    if (int st = enqueue_stream_fill(h, l.dassign, sizeof(int32_t), first, count, 0, stream)) return st;
+    GCCNMF_LAUNCH(h, sort_by_entry_kernel, 1, 32, 0, stream, l.dassign, sizeof(int32_t), l.S, Qd, l.dorder, l.dseg);
   }
   return GCCNMF_OK;
 }
@@ -1014,8 +956,7 @@ int ll_set_params(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, 
                   const gccnmf_ll_stream_params* params_host, void* stream) {
   GCCNMF_ENTER(h);
   LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
-  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "ll_set_params: streams [%d, %d + %d) outside [0, %d)", first,
-                 first, count, l.S);
+  if (int st = stream_range_check(h, "ll_set_params", l.S, first, count)) return st;
   GCCNMF_REQUIRE(h, params_host != nullptr, "ll_set_params: NULL parameters");
   for (int i = 0; i < count; ++i) {
     GCCNMF_REQUIRE(h, !std::isnan(params_host[i].epsilon), "ll_set_params: stream %d: epsilon is NaN", first + i);
@@ -1040,27 +981,9 @@ int ll_graph_create(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh
   GCCNMF_REQUIRE(h, hops >= 1 && hops <= l.C, "ll_graph_create: hops must be in [1, %d] (got %d)", l.C, hops);
   GCCNMF_REQUIRE(h, in && out, "ll_graph_create: NULL pointer");
   if (int st = gccnmf_get_twiddles(h, l.N, nullptr, nullptr)) return st;
-  cudaStream_t s = (cudaStream_t)stream;
   const size_t bytes = (size_t)l.S * 2 * hops * l.hop * sizeof(float);
-  const size_t out_bytes = bytes * (P ? P : 1);
-  GCCNMF_CHECK_CUDA(h, cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-  int st = GCCNMF_OK;
-  if (in_host && cudaMemcpyAsync(in, in_host, bytes, cudaMemcpyHostToDevice, s) != cudaSuccess) st = GCCNMF_ERR_CUDA;
-  if (st == GCCNMF_OK) st = ll_enqueue(h, cfg, l, hops, in, out, stream);
-  if (st == GCCNMF_OK && out_host && cudaMemcpyAsync(out_host, out, out_bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess) st = GCCNMF_ERR_CUDA;
-  cudaGraph_t graph = nullptr;
-  const cudaError_t end = cudaStreamEndCapture(s, &graph);
-  if (st != GCCNMF_OK || end != cudaSuccess) {
-    if (graph) cudaGraphDestroy(graph);
-    if (st == GCCNMF_OK) return gccnmf_fail(h, GCCNMF_ERR_CUDA, "ll_graph_create: stream capture failed: %s", cudaGetErrorString(end));
-    return st;
-  }
-  cudaGraphExec_t exec = nullptr;
-  const cudaError_t inst = cudaGraphInstantiate(&exec, graph, 0);
-  cudaGraphDestroy(graph);
-  if (inst != cudaSuccess) return gccnmf_fail(h, GCCNMF_ERR_CUDA, "ll_graph_create: cudaGraphInstantiate failed: %s", cudaGetErrorString(inst));
-  *graph_exec = exec;
-  return GCCNMF_OK;
+  return capture_graph(h, "ll_graph_create", stream, in, in_host, bytes, out, out_host, bytes * (P ? P : 1),
+                       [&] { return ll_enqueue(h, cfg, l, hops, in, out, stream); }, graph_exec);
 }
 
 int ll_export(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, int Qd, void* state, size_t state_bytes, int hops, int what, void* dst,
@@ -1287,8 +1210,7 @@ int ll_record_digests(gccnmf_handle* h, const gccnmf_ll_config& c, const LLLayou
 // Qd >= 1 only with Qe >= 1 (ll_check); the lldict entries check Qd >= 1 themselves.
 #define LL_RECORD_ARGS_OR_FAIL(what)                                                                                                   \
   LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);                                                                                                 \
-  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "%s: streams [%d, %d + %d) outside [0, %d)", what, \
-                 first, first, count, l.S);                                                                                            \
+  if (int st__ = stream_range_check(h, what, l.S, first, count)) return st__;                                                          \
   const RecordMap m = ll_record_map(*cfg, P, Lh, Qe);                                                                                  \
   const size_t rec_bytes = ll_record_bytes(*cfg, P, Lh);                                                                               \
   GCCNMF_REQUIRE(h, record != nullptr && record_bytes >= (size_t)count * rec_bytes, "%s: record needs %zu bytes for %d streams", what,  \
@@ -1374,17 +1296,11 @@ int ll_load_streams(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh
   GCCNMF_CHECK_CUDA(h, cudaMemcpy2DAsync(workspace, m.payload, (const char*)record + kRecordHeaderBytes, rec_bytes, m.payload, count,
                                          cudaMemcpyHostToDevice, (cudaStream_t)stream));
   GCCNMF_LAUNCH(h, ll_record_copy_kernel, dim3(count, m.n), 256, 0, stream, (char*)state, first, m, (char*)workspace, 0);
-  for (int pass = Qd ? 0 : 1; Qe && pass < 2; ++pass) {    // the dictionary entries (Qd >= 1), then the tables
-    const std::vector<int32_t>& src = pass ? se : de;
-    for (int i0 = 0; i0 < count; i0 += kLLParamsPerLaunch) {
-      const int n = count - i0 < kLLParamsPerLaunch ? count - i0 : kLLParamsPerLaunch;
-      LLAssignBatch b{};
-      memcpy(b.e, src.data() + i0, (size_t)n * sizeof(int32_t));
-      GCCNMF_LAUNCH(h, ll_assign_kernel, 1, kLLParamsPerLaunch, 0, stream, pass ? l.assign : l.dassign, first + i0, n, b, 0);
-    }
-  }
-  if (Qe) GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
-  if (Qd) GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.dassign, l.S, Qd, l.dorder, l.dseg);
+  for (int pass = Qd ? 0 : 1; Qe && pass < 2; ++pass)      // the dictionary entries (Qd >= 1), then the tables
+    if (int st = enqueue_stream_rows(h, pass ? l.assign : l.dassign, sizeof(int32_t), 0, first, count, 1, (pass ? se : de).data(), false, stream))
+      return st;
+  if (Qe) GCCNMF_LAUNCH(h, sort_by_entry_kernel, 1, 32, 0, stream, l.assign, sizeof(int32_t), l.S, Qe, l.order, l.seg);
+  if (Qd) GCCNMF_LAUNCH(h, sort_by_entry_kernel, 1, 32, 0, stream, l.dassign, sizeof(int32_t), l.S, Qd, l.dorder, l.dseg);
   return GCCNMF_OK;
 }
 
@@ -1392,19 +1308,12 @@ int ll_set_targets(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh,
                    const int32_t* targets_host, void* stream) {
   GCCNMF_ENTER(h);
   LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
-  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "llsep_set_targets: streams [%d, %d + %d) outside [0, %d)",
-                 first, first, count, l.S);
+  if (int st = stream_range_check(h, "llsep_set_targets", l.S, first, count)) return st;
   GCCNMF_REQUIRE(h, targets_host != nullptr, "llsep_set_targets: NULL targets");
   for (int i = 0; i < count * P; ++i)
     GCCNMF_REQUIRE(h, targets_host[i] >= -1 && targets_host[i] < l.D, "llsep_set_targets: stream %d source %d: target %d outside [0, %d) (or -1)",
                    first + i / P, i % P, targets_host[i], l.D);
-  for (int i0 = 0; i0 < count; i0 += kLLParamsPerLaunch) {
-    const int n = count - i0 < kLLParamsPerLaunch ? count - i0 : kLLParamsPerLaunch;
-    LLTargetsBatch b{};
-    memcpy(b.t, targets_host + (size_t)i0 * P, (size_t)n * P * sizeof(int32_t));
-    GCCNMF_LAUNCH(h, ll_src_override_kernel, 1, kLLParamsPerLaunch, 0, stream, l.src_override, first + i0, n, P, b);
-  }
-  return GCCNMF_OK;
+  return enqueue_stream_rows(h, l.src_override, kLLMaxSources * sizeof(int32_t), 0, first, count, P, targets_host, false, stream);
 }
 
 int ll_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Qe, int Qd, void* state, size_t state_bytes, int first, int count,
@@ -1412,20 +1321,12 @@ int ll_set_window(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, 
   GCCNMF_ENTER(h);
   LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
   GCCNMF_REQUIRE(h, Lh > 0, "llhist_set_window: needs history_length > 0");
-  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "llhist_set_window: streams [%d, %d + %d) outside [0, %d)",
-                 first, first, count, l.S);
+  if (int st = stream_range_check(h, "llhist_set_window", l.S, first, count)) return st;
   GCCNMF_REQUIRE(h, windows_host != nullptr, "llhist_set_window: NULL windows");
   for (int i = 0; i < count; ++i)
     GCCNMF_REQUIRE(h, windows_host[i] >= 0 && windows_host[i] <= Lh, "llhist_set_window: stream %d: window %d outside [0, %d]", first + i,
                    windows_host[i], Lh);
-  for (int i0 = 0; i0 < count; i0 += kLLParamsPerLaunch) {
-    const int n = count - i0 < kLLParamsPerLaunch ? count - i0 : kLLParamsPerLaunch;
-    LLWindowBatch b{};
-    memcpy(b.w, windows_host + i0, (size_t)n * sizeof(int32_t));
-    GCCNMF_LAUNCH(h, ll_hist_window_kernel, 1, kLLParamsPerLaunch, 0, stream, l.hist, l.hist_stride, (size_t)l.D * Lh * sizeof(double) + 4,
-                  first + i0, n, b);
-  }
-  return GCCNMF_OK;
+  return enqueue_stream_rows(h, l.hist, l.hist_stride, (size_t)l.D * Lh * sizeof(double) + 4, first, count, 1, windows_host, false, stream);
 }
 
 // Bank: table j <- E (F, D) complex128 on the device, and its transpose; stream-ordered, from the next call on.
@@ -1445,18 +1346,12 @@ int ll_assign(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int 
               const int32_t* entries_host, void* stream) {
   GCCNMF_ENTER(h);
   LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
-  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "llbank_assign: streams [%d, %d + %d) outside [0, %d)", first,
-                 first, count, l.S);
+  if (int st = stream_range_check(h, "llbank_assign", l.S, first, count)) return st;
   GCCNMF_REQUIRE(h, entries_host != nullptr, "llbank_assign: NULL entries");
   for (int i = 0; i < count; ++i)
     GCCNMF_REQUIRE(h, entries_host[i] >= 0 && entries_host[i] < Qe, "llbank_assign: stream %d: entry %d outside [0, %d)", first + i, entries_host[i], Qe);
-  for (int i0 = 0; i0 < count; i0 += kLLParamsPerLaunch) {
-    const int n = count - i0 < kLLParamsPerLaunch ? count - i0 : kLLParamsPerLaunch;
-    LLAssignBatch b{};
-    memcpy(b.e, entries_host + i0, (size_t)n * sizeof(int32_t));
-    GCCNMF_LAUNCH(h, ll_assign_kernel, 1, kLLParamsPerLaunch, 0, stream, l.assign, first + i0, n, b, 0);
-  }
-  GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
+  if (int st = enqueue_stream_rows(h, l.assign, sizeof(int32_t), 0, first, count, 1, entries_host, false, stream)) return st;
+  GCCNMF_LAUNCH(h, sort_by_entry_kernel, 1, 32, 0, stream, l.assign, sizeof(int32_t), l.S, Qe, l.order, l.seg);
   return GCCNMF_OK;
 }
 
@@ -1499,7 +1394,7 @@ int lld_init(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int Q
   if (int st = ll_init(h, cfg, P, Lh, Qe, Qd, nullptr, E, analysis_window, synthesis_weights, gain, nullptr, state, state_bytes, stream)) return st;
   for (int e = 0; e < Qd; ++e)
     if (int st = lld_load_entry(h, cfg, l, e, W[e], num_atoms[e], H0 ? H0[e] : nullptr, stream)) return st;
-  GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.dassign, l.S, Qd, l.dorder, l.dseg);     // every stream on entry 0
+  GCCNMF_LAUNCH(h, sort_by_entry_kernel, 1, 32, 0, stream, l.dassign, sizeof(int32_t), l.S, Qd, l.dorder, l.dseg);     // every stream on entry 0
   return GCCNMF_OK;
 }
 
@@ -1518,8 +1413,7 @@ int lld_assign(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int
   GCCNMF_ENTER(h);
   GCCNMF_REQUIRE(h, Qd >= 1, "lldict: num_dictionaries must be in [1, %d] (got %d)", kLLMaxDictionaries, Qd);
   LLD_CARVE_OR_FAIL(l, P, Lh, Qe, Qd);
-  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < l.S && count <= l.S - first, "lldict_assign: streams [%d, %d + %d) outside [0, %d)", first,
-                 first, count, l.S);
+  if (int st = stream_range_check(h, "lldict_assign", l.S, first, count)) return st;
   for (int i = 0; i < count; ++i) {
     const int d = dictionary_host ? dictionary_host[i] : -1, e = steering_host ? steering_host[i] : -1;
     GCCNMF_REQUIRE(h, d >= -1 && d < Qd, "lldict_assign: stream %d: dictionary entry %d outside [0, %d) (or -1)", first + i, d, Qd);
@@ -1528,15 +1422,9 @@ int lld_assign(gccnmf_handle* h, const gccnmf_ll_config* cfg, int P, int Lh, int
   for (int pass = 0; pass < 2; ++pass) {
     const int32_t* src = pass ? steering_host : dictionary_host;
     if (!src) continue;
-    int32_t* assign = pass ? l.assign : l.dassign;
-    for (int i0 = 0; i0 < count; i0 += kLLParamsPerLaunch) {
-      const int n = count - i0 < kLLParamsPerLaunch ? count - i0 : kLLParamsPerLaunch;
-      LLAssignBatch b{};
-      memcpy(b.e, src + i0, (size_t)n * sizeof(int32_t));
-      GCCNMF_LAUNCH(h, ll_dict_assign_kernel, 1, kLLParamsPerLaunch, 0, stream, assign, first + i0, n, b);
-    }
-    if (pass) GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.assign, l.S, Qe, l.order, l.seg);
-    else GCCNMF_LAUNCH(h, ll_sort_streams_kernel, 1, 32, 0, stream, l.dassign, l.S, Qd, l.dorder, l.dseg);
+    if (int st = enqueue_stream_rows(h, pass ? l.assign : l.dassign, sizeof(int32_t), 0, first, count, 1, src, true, stream)) return st;
+    if (pass) GCCNMF_LAUNCH(h, sort_by_entry_kernel, 1, 32, 0, stream, l.assign, sizeof(int32_t), l.S, Qe, l.order, l.seg);
+    else GCCNMF_LAUNCH(h, sort_by_entry_kernel, 1, 32, 0, stream, l.dassign, sizeof(int32_t), l.S, Qd, l.dorder, l.dseg);
   }
   return GCCNMF_OK;
 }

@@ -47,10 +47,12 @@
 // (slot, frame) pairs in dictionary order, so a CTA spans more than one entry only where the sorted order changes entry, and
 // then runs its f loop once per entry.
 #include <cmath>
+#include <vector>
 
 #include "common.cuh"
 #include "fft.cuh"
 #include "records.cuh"
+#include "streams.cuh"
 
 namespace {
 
@@ -284,58 +286,6 @@ __global__ void rt_default_params_kernel(RtDev* dev0, size_t stride, int first, 
   dev->mode = 1; dev->separation = 1; dev->localization = 0; dev->loc_window = 6;
   dev->active = 1;
   for (int q = 0; q < P; ++q) rt_slot(targets0, first + i, stride)[q] = (2 * q + 1) * D / (2 * P);
-}
-
-// Target TDOA indexes of up to kRtParamsPerLaunch slots, P per slot, by value; -1 keeps a source's target.
-struct RtTargetsBatch {
-  int32_t t[kRtParamsPerLaunch * kRtMaxSources];
-};
-__global__ void rt_set_targets_kernel(int32_t* targets0, size_t stride, int first, int count, int P, RtTargetsBatch b) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= count) return;
-  int32_t* t = rt_slot(targets0, first + i, stride);
-  for (int q = 0; q < P; ++q)
-    if (b.t[i * P + q] >= 0) t[q] = b.t[i * P + q];
-}
-
-// (dictionary, steering) entries of up to kRtParamsPerLaunch slots, by value; -1 keeps the slot's entry.
-struct RtAssignBatch {
-  int32_t d[kRtParamsPerLaunch], e[kRtParamsPerLaunch];
-};
-__global__ void rt_assign_kernel(int32_t* assign0, size_t stride, int first, int count, RtAssignBatch b) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= count) return;
-  int32_t* a = rt_slot(assign0, first + i, stride);
-  if (b.d[i] >= 0) a[0] = b.d[i];
-  if (b.e[i] >= 0) a[1] = b.e[i];
-}
-
-// Stable counting sort of the S slots by dictionary index, by one warp over chunks of 32 slots: order lists the slots of entry 0
-// in slot order, then those of entry 1, ...  Inactive slots are listed too (the kernels skip them).
-__global__ void __launch_bounds__(32) rt_sort_slots_kernel(const int32_t* __restrict__ assign0, size_t stride, int S, int Qd, int32_t* __restrict__ order) {
-  __shared__ int base[kRtMaxBank];
-  const int lane = threadIdx.x;
-  for (int i = lane; i < Qd; i += 32) base[i] = 0;
-  __syncwarp();
-  for (int pass = 0; pass < 2; ++pass) {               // 0: count per entry, 1: place
-    for (int s0 = 0; s0 < S; s0 += 32) {
-      const int s = s0 + lane;
-      const int d = s < S ? rt_slot(assign0, s, stride)[0] : -1;
-      const unsigned peers = __match_any_sync(0xffffffffu, d);
-      const bool leader = lane == __ffs(peers) - 1;
-      if (pass == 1 && d >= 0) order[base[d] + __popc(peers & ((1u << lane) - 1u))] = s;
-      __syncwarp();
-      if (leader && d >= 0) base[d] += __popc(peers);
-      __syncwarp();
-    }
-    if (pass == 0 && lane == 0)                        // counts -> first positions
-      for (int i = 0, sum = 0; i < Qd; ++i) {
-        const int n = base[i];
-        base[i] = sum;
-        sum += n;
-      }
-    __syncwarp();
-  }
 }
 
 // ---------------------------------------------------------------------------------------------- numerics shared with gcc.cu
@@ -1132,7 +1082,7 @@ int rt_enqueue_params(gccnmf_handle* h, const RtLayout& l, int first, int count,
 
 // A bank's slots in dictionary order, after every change of an assignment (stream-ordered, like the changes themselves).
 int rt_enqueue_sort(gccnmf_handle* h, const RtLayout& l, void* stream) {
-  if (l.Qd > 0) GCCNMF_LAUNCH(h, rt_sort_slots_kernel, 1, 32, 0, stream, l.assign, l.stride, l.S, l.Qd, l.order);
+  if (l.Qd > 0) GCCNMF_LAUNCH(h, sort_by_entry_kernel, 1, 32, 0, stream, l.assign, l.stride, l.S, l.Qd, l.order, nullptr);
   return 0;
 }
 
@@ -1237,26 +1187,10 @@ int rt_graph_create(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P,
   *graph_exec = nullptr;
   RT_CARVE_OR_FAIL_B(l, S, P, Qd, Qe);
   GCCNMF_REQUIRE(h, in_blocks && out_blocks, "rt_graph_create: NULL pointer");
-  cudaStream_t s = (cudaStream_t)stream;
-  const size_t block_bytes = (size_t)S * 2 * cfg->block_size * sizeof(float), out_bytes = block_bytes * rt_sources_grid(l);
-  GCCNMF_CHECK_CUDA(h, cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-  int st = GCCNMF_OK;
-  if (in_host && cudaMemcpyAsync(in_blocks, in_host, block_bytes, cudaMemcpyHostToDevice, s) != cudaSuccess) st = GCCNMF_ERR_CUDA;
-  if (st == GCCNMF_OK) st = rt_process_block(h, cfg, S, P, state, state_bytes, in_blocks, out_blocks, nullptr, stream, Qd, Qe);
-  if (st == GCCNMF_OK && out_host && cudaMemcpyAsync(out_host, out_blocks, out_bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess) st = GCCNMF_ERR_CUDA;
-  cudaGraph_t graph = nullptr;
-  const cudaError_t end = cudaStreamEndCapture(s, &graph);
-  if (st != GCCNMF_OK || end != cudaSuccess) {
-    if (graph) cudaGraphDestroy(graph);
-    if (st == GCCNMF_OK) return gccnmf_fail(h, GCCNMF_ERR_CUDA, "rt_graph_create: stream capture failed: %s", cudaGetErrorString(end));
-    return st;
-  }
-  cudaGraphExec_t exec = nullptr;
-  const cudaError_t inst = cudaGraphInstantiate(&exec, graph, 0);
-  cudaGraphDestroy(graph);
-  if (inst != cudaSuccess) return gccnmf_fail(h, GCCNMF_ERR_CUDA, "rt_graph_create: cudaGraphInstantiate failed: %s", cudaGetErrorString(inst));
-  *graph_exec = exec;
-  return GCCNMF_OK;
+  const size_t block_bytes = (size_t)S * 2 * cfg->block_size * sizeof(float);
+  auto enqueue = [&] { return rt_process_block(h, cfg, S, P, state, state_bytes, in_blocks, out_blocks, nullptr, stream, Qd, Qe); };
+  return capture_graph(h, "rt_graph_create", stream, in_blocks, in_host, block_bytes, out_blocks, out_host, block_bytes * rt_sources_grid(l), enqueue,
+                       graph_exec);
 }
 
 // Items 2 and 4 are source 0's with P > 0; items 9 .. 13 exist only with P > 0, item 14 only with a bank.  With a bank the
@@ -1308,17 +1242,12 @@ int rt_export(gccnmf_handle* h, const gccnmf_rt_config* cfg, int S, int P, void*
   return GCCNMF_OK;
 }
 
-int rt_check_range(gccnmf_handle* h, int S, int first, int count) {
-  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < S && count <= S - first, "rtm: slots [%d, %d + %d) outside [0, %d)", first, first, count, S);
-  return 0;
-}
-
 // Per-slot parameters of slots [first_slot, first_slot + count): as given without sources; with P sources mode, target_index and
 // set_target are ignored (the masks are one-hot, the targets come from set_targets or the localisation).
 int rt_slot_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout& l, int first_slot, int count, const gccnmf_rtm_slot_params* params,
                    void* stream) {
-  if (int st = rt_check_range(h, l.S, first_slot, count)) return st;
   const char* name = l.P > 0 ? "rtsep_set_params" : "rtm_set_params";
+  if (int st = stream_range_check(h, name, l.S, first_slot, count)) return st;
   GCCNMF_REQUIRE(h, params != nullptr, "%s: NULL parameters", name);
   for (int i = 0; i < count; ++i) {
     GCCNMF_REQUIRE(h, l.P > 0 || params[i].mode == 0 || params[i].mode == 1, "%s: slot %d: mode must be 0 (boxcar) or 1 (window)", name, first_slot + i);
@@ -1344,19 +1273,13 @@ int rt_slot_params(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout
 
 int rt_set_targets(gccnmf_handle* h, const gccnmf_rt_config* cfg, const RtLayout& l, int first_slot, int count, const int32_t* targets_host,
                    void* stream) {
-  if (int st = rt_check_range(h, l.S, first_slot, count)) return st;
+  if (int st = stream_range_check(h, "rtsep_set_targets", l.S, first_slot, count)) return st;
   GCCNMF_REQUIRE(h, targets_host != nullptr, "rtsep_set_targets: NULL targets");
   const int P = l.P;
   for (int i = 0; i < count * P; ++i)
     GCCNMF_REQUIRE(h, targets_host[i] >= -1 && targets_host[i] < cfg->num_tdoas, "rtsep_set_targets: slot %d source %d: target %d outside [0, %d) (or -1)",
                    first_slot + i / P, i % P, targets_host[i], cfg->num_tdoas);
-  for (int i0 = 0; i0 < count; i0 += kRtParamsPerLaunch) {
-    const int n = count - i0 < kRtParamsPerLaunch ? count - i0 : kRtParamsPerLaunch;
-    RtTargetsBatch b{};
-    memcpy(b.t, targets_host + (size_t)i0 * P, (size_t)n * P * sizeof(int32_t));
-    GCCNMF_LAUNCH(h, rt_set_targets_kernel, 1, kRtParamsPerLaunch, 0, stream, l.targets, l.stride, first_slot + i0, n, P, b);
-  }
-  return GCCNMF_OK;
+  return enqueue_stream_rows(h, l.targets, l.stride, 0, first_slot, count, P, targets_host, true, stream);
 }
 
 // ---------------------------------------------------------------------------------------------- stream records
@@ -1482,8 +1405,7 @@ int rt_enqueue_digests(gccnmf_handle* h, const RtRecordWork& w, char* workspace,
   if (!empty__)                                                                                                                    \
     if (int st__ = rt_check_bank(h, Qd, Qe)) return st__;                                                                          \
   RT_CARVE_OR_FAIL_B(l, S, P, Qd, Qe);                                                                                             \
-  GCCNMF_REQUIRE(h, first >= 0 && count >= 1 && first < S && count <= S - first, what ": slots [%d, %d + %d) outside [0, %d)", first, \
-                 first, count, S);                                                                                                 \
+  if (int st__ = stream_range_check(h, what, S, first, count)) return st__;                                                      \
   const RecordMap m = rt_record_map(*cfg, P, Qd, Qe);                                                                              \
   const size_t rec_bytes = rt_record_bytes(*cfg, P);                                                                               \
   GCCNMF_REQUIRE(h, record != nullptr && record_bytes >= (size_t)count * rec_bytes, what ": record needs %zu bytes for %d slots",  \
@@ -1636,7 +1558,7 @@ int gccnmf_rtm_reset_slots(gccnmf_handle* h, const gccnmf_rt_config* cfg, int nu
                            void* stream) {
   GCCNMF_ENTER(h);
   RT_CARVE_OR_FAIL(l, num_streams);
-  if (int st = rt_check_range(h, num_streams, first_slot, count)) return st;
+  if (int st = stream_range_check(h, "rtm_reset_slots", num_streams, first_slot, count)) return st;
   return rt_enqueue_reset(h, l, first_slot, count, stream);
 }
 
@@ -1689,7 +1611,7 @@ int gccnmf_rtsep_reset_slots(gccnmf_handle* h, const gccnmf_rt_config* cfg, int 
   GCCNMF_ENTER(h);
   GCCNMF_REQUIRE(h, num_sources != 0, "rtsep: num_sources must be in [2, %d] (got 0)", kRtMaxSources);
   RT_CARVE_OR_FAIL_P(l, num_streams, num_sources);
-  if (int st = rt_check_range(h, num_streams, first_slot, count)) return st;
+  if (int st = stream_range_check(h, "rtsep_reset_slots", num_streams, first_slot, count)) return st;
   return rt_enqueue_reset(h, l, first_slot, count, stream);
 }
 
@@ -1788,22 +1710,19 @@ int gccnmf_rtbank_assign(gccnmf_handle* h, const gccnmf_rt_config* cfg, int num_
                          void* state, size_t state_bytes, int first_slot, int count, const int32_t* dictionary, const int32_t* steering, void* stream) {
   GCCNMF_ENTER(h);
   RT_BANK_OR_FAIL(l);
-  if (int st = rt_check_range(h, num_streams, first_slot, count)) return st;
+  if (int st = stream_range_check(h, "rtbank_assign", num_streams, first_slot, count)) return st;
   for (int i = 0; i < count; ++i) {
     GCCNMF_REQUIRE(h, !dictionary || (dictionary[i] >= -1 && dictionary[i] < num_dictionaries),
                    "rtbank_assign: slot %d: dictionary %d outside [0, %d) (or -1)", first_slot + i, dictionary[i], num_dictionaries);
     GCCNMF_REQUIRE(h, !steering || (steering[i] >= -1 && steering[i] < num_steerings), "rtbank_assign: slot %d: steering %d outside [0, %d) (or -1)",
                    first_slot + i, steering[i], num_steerings);
   }
-  for (int i0 = 0; i0 < count; i0 += kRtParamsPerLaunch) {
-    const int n = count - i0 < kRtParamsPerLaunch ? count - i0 : kRtParamsPerLaunch;
-    RtAssignBatch b{};
-    for (int i = 0; i < n; ++i) {
-      b.d[i] = dictionary ? dictionary[i0 + i] : -1;
-      b.e[i] = steering ? steering[i0 + i] : -1;
-    }
-    GCCNMF_LAUNCH(h, rt_assign_kernel, 1, kRtParamsPerLaunch, 0, stream, l.assign, l.stride, first_slot + i0, n, b);
+  std::vector<int32_t> rows(2 * (size_t)count);         // (dictionary, steering) per slot; a NULL array keeps
+  for (int i = 0; i < count; ++i) {
+    rows[2 * i] = dictionary ? dictionary[i] : -1;
+    rows[2 * i + 1] = steering ? steering[i] : -1;
   }
+  if (int st = enqueue_stream_rows(h, l.assign, l.stride, 0, first_slot, count, 2, rows.data(), true, stream)) return st;
   return rt_enqueue_sort(h, l, stream);
 }
 
@@ -1811,7 +1730,7 @@ int gccnmf_rtbank_reset_slots(gccnmf_handle* h, const gccnmf_rt_config* cfg, int
                               void* state, size_t state_bytes, int first_slot, int count, void* stream) {
   GCCNMF_ENTER(h);
   RT_BANK_OR_FAIL(l);
-  if (int st = rt_check_range(h, num_streams, first_slot, count)) return st;
+  if (int st = stream_range_check(h, "rtbank_reset_slots", num_streams, first_slot, count)) return st;
   return rt_enqueue_reset(h, l, first_slot, count, stream);
 }
 

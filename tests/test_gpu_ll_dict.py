@@ -6,6 +6,7 @@ columns and rows < K_i, and the fill of the rows past K_i.
     (grouped tensor-core GEMM), hops per call 1 and 3, mixed schedules, graph and kernel-by-kernel runs of the same case.  K_i = 24
     and 100 make the plain engine take the float64 argmax while the bank takes the tensor path with refinement;
   - 1056 streams over 64 dictionaries and 4 tables;
+  - every per-stream setting on 130 streams in one call, against the host mirror;
   - assign_dictionary and load_dictionary between launches of a kept graph;
   - the gated float64 fallback on mono input;
   - records: lldict <-> llbank, permuted and duplicated entries, the lowest matching entry, refusals that leave every stream as it
@@ -210,6 +211,27 @@ def test_1056_streams_over_64_dictionaries_and_4_tables():
         _eq(am[:atoms[i]][:, streams], ref.export(ll.EXPORT_ARGMAX))
         assert (am[atoms[i]:][:, streams] == -1).all()
         ref.close()
+    bank.close()
+
+
+def test_settings_of_130_streams_in_one_call():
+    """set_targets (-1 included), set_localization, assign_dictionary and assign_steering on 130 streams, each in one call that
+    takes three launches of at most 64 streams: after one call of the engine its exports equal the host mirror."""
+    p = _setup(16, atoms=[24, 64])
+    S, P, Lh = 130, 3, 8
+    rng = np.random.RandomState(130)
+    bank = _engine(p, p['Ws'], p['E'], S, numSources=P, historyLength=Lh)
+    bank.set_targets(None, rng.randint(-1, p['D'], (S, P)))
+    bank.set_localization(None, rng.randint(0, Lh + 1, S))
+    bank.assign_dictionary(None, rng.randint(0, 2, S))
+    bank.assign_steering(None, rng.randint(0, len(p['E']), S))
+    assert (bank._targets == -1).any() and (bank._targets >= 0).any()
+    bank.process(_audio(S, 1, p['hop']))
+    _eq(bank.export(ll.EXPORT_WINDOWS), bank._window)
+    _eq(bank.export(ll.EXPORT_DICTIONARY_ASSIGNMENT), bank._dassign)
+    _eq(bank.export(ll.EXPORT_ASSIGNMENT), bank._assign)
+    # one hop per call: column s is stream s, on its override where one is set, else on its carried target
+    _eq(bank.export(ll.EXPORT_SOURCE_TARGETS), np.where(bank._targets >= 0, bank._targets, bank.export(ll.EXPORT_CARRIED_TARGETS)))
     bank.close()
 
 

@@ -212,6 +212,28 @@ def test_reset_and_activation_keep_or_restore_entries():
         assert np.array_equal(y[0], ref.process_blocks(x[b][:1])[0]), b
 
 
+def test_settings_of_130_slots_in_one_call():
+    """assign and set_targets on 130 slots, each in one call that takes three launches of at most 64 slots, with a mix of -1
+    (keep) and values, twice: every slot's EXPORT_ASSIGNMENT and EXPORT_TARGETS equal the host's expectation."""
+    N, D, P, S = 256, 16, 3, 130
+    hop = N // 4
+    Ws = _dicts(N, [32, 64, 48], seed=6)
+    Es = [_steering(N, D, 0.1), _steering(N, D, 0.2)]
+    bank = _engine(Ws, Es, N, hop, hop, 1, S, 0, P)
+    rng = np.random.default_rng(130)
+    entries = np.zeros((S, 2), np.int64)
+    targets = np.tile([(2 * q + 1) * D // (2 * P) for q in range(P)], (S, 1))
+    for _ in range(2):
+        d, e, t = rng.integers(-1, 3, S), rng.integers(-1, 2, S), rng.integers(-1, D, (S, P))
+        bank.assign(range(S), d, e)
+        bank.set_targets(range(S), t)
+        entries = np.where(np.stack([d, e], 1) >= 0, np.stack([d, e], 1), entries)
+        targets = np.where(t >= 0, t, targets)
+    for s in range(S):
+        assert tuple(bank.export(s, 14)) == tuple(entries[s]) == bank.assignment(s), s
+        assert np.array_equal(bank.export(s, 9), targets[s]), s
+
+
 @pytest.mark.parametrize('P', [0, 2])
 def test_bank_of_one_entry_equals_multi_stream_engine(P):
     N, D, nT, S, blocks = 512, 64, 1, 5, 6

@@ -62,7 +62,7 @@ def _split(eng, S, rec, ws, n):
                 continue
             t = evt.device_time if hasattr(evt, 'device_time') else evt.cuda_time
             key = ('digest kernels' if 'rt_digest' in evt.name else 'copy kernel' if 'rt_record_copy' in evt.name
-                   else 'sort' if 'rt_sort_slots' in evt.name else 'copies' if 'Memcpy' in evt.name or 'memcpy' in evt.name else evt.name)
+                   else 'sort' if 'sort_by_entry' in evt.name else 'copies' if 'Memcpy' in evt.name or 'memcpy' in evt.name else evt.name)
             split[key] = round(split.get(key, 0.0) + t, 2)
     return out
 
